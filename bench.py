@@ -1,6 +1,6 @@
-"""Benchmarks of the B200 hot path: the SigLIP two-tower training step (BASELINE.json metric:
-image-text pairs/sec; config 4 at weak scaling: 1024 pairs per GPU, global batch 1024*N) and the
-other BASELINE.json configurations as `--workload`s.
+"""Benchmarks of the H100 hot path: the SigLIP two-tower training step (BASELINE.json metric:
+image-text pairs/sec; config 4 at weak scaling: 768 pairs per GPU, global batch 768*N, the largest
+round batch whose activations fit in 80 GB) and the other BASELINE.json configurations as `--workload`s.
 
   python bench.py --gpus 1 --steps 8 --warmup 3                       # config 4 (the headline)
   python bench.py --workload vit_b16_cls | mixer_b16 | vit_s16 | siglip_l14_336
@@ -29,10 +29,11 @@ OPT_CONFIG = dict(optax_name="scale_by_adam", optax=dict(b2=0.95, mu_dtype="bflo
 TXT_LEN = 64
 
 # BASELINE.json configs -> workloads.  flops = algorithmic training FLOPs per sample (3 x forward;
-# SURVEY.md 8d / BASELINE.md 3).  per_gpu_batch is the weak-scaling shard (config 4: 8192 / 8).
+# SURVEY.md 8d / BASELINE.md 3).  per_gpu_batch is the weak-scaling shard, sized so that one step's
+# activations fit in an H100's 80 GB (config 4: 768, ~61 GiB peak; config 5 with recompute: 512).
 WORKLOADS = {
     "siglip_b16": dict(          # config 4 -- the headline metric
-        kind="siglip", metric="siglip_vit_b16_pairs_per_sec", unit="pairs/s", res=224, per_gpu_batch=1024,
+        kind="siglip", metric="siglip_vit_b16_pairs_per_sec", unit="pairs/s", res=224, per_gpu_batch=768,
         flops=139.3e9, model_kw=dict(image=dict(variant="B/16", pool_type="map"),
                                      text=dict(variant="B", vocab_size=32_000),
                                      out_dim=(None, 768), temperature_init=10.0, bias_init=-10.0),
@@ -42,7 +43,7 @@ WORKLOADS = {
         desc="SigLIP two_towers ViT-B/16 (map pool) + text-B (64 tok, vocab 32000), 224x224, full update_fn "
              "(fwd, sigmoid loss over gathered ztxt, bwd, grad all-reduce, Adam)"),
     "siglip_l14_336": dict(      # config 5
-        kind="siglip", metric="siglip_vit_l14_336_pairs_per_sec", unit="pairs/s", res=336, per_gpu_batch=2048,
+        kind="siglip", metric="siglip_vit_l14_336_pairs_per_sec", unit="pairs/s", res=336, per_gpu_batch=512,
         flops=1268e9, remat=True,
         model_kw=dict(image=dict(variant="L/14", pool_type="map"), text=dict(variant="L", vocab_size=32_000),
                       out_dim=(None, 1024), temperature_init=10.0, bias_init=-10.0),
@@ -71,11 +72,6 @@ WORKLOADS = {
         desc="ViT-S/16 (configs/vit_s16_i1k.py: gap, sincos2d, rep_size, softmax_xent), 224x224, batch 8, "
              "full update_fn"),
 }
-# ncu-measured DRAM traffic per GEMM launch (all GEMM launches of one siglip_b16 bench run)
-NCU_GEMM_DRAM_BYTES_PER_LAUNCH = 0.929e9
-NCU_GEMM_DRAM_SOURCE = ("profiles/r02/ncu/launch_summary_siglip_b16_n1024.md (ncu dram__bytes_read.sum + "
-                        "dram__bytes_write.sum over the 1244 GEMM launches of this workload on the final round-2 "
-                        "tree: 1156.1 GB); round 1 measured 0.927 GB (profiles/r01_final_launch_summary.md)")
 
 
 def measured_peaks():
@@ -84,7 +80,8 @@ def measured_peaks():
     with open(p) as f:
       d = json.load(f)
     return d, "measured"
-  return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+  # NVIDIA's H100 SXM data sheet (dense bf16, HBM3, 700 W card): a ceiling, not a measured rate
+  return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -456,6 +453,8 @@ def measure_ours(args, wl, world, rank, local_rank):
   ev1.record()
   barrier()
   launches = L.LAUNCHES[0] - launches0
+  if args.dump_outputs and rank == 0:
+    dump_outputs(args.dump_outputs, state, m)
   # (2) the same K steps again with a CUDA-event pair around every GEMM launch (the roofline's
   # `achieved`); kept apart from (1) so that the event records are not inside the headline number
   ops.gemm = timed_gemm
@@ -542,6 +541,27 @@ def measure_ours(args, wl, world, rank, local_rank):
   return R
 
 
+DUMP_SAMPLE = 1 << 22      # elements sampled from the parameter and gradient buffers (16 MB each)
+
+
+def dump_outputs(out_dir, state, measurements):
+  """Writes what the last timed step returned to its caller: every measurement (scalars) and a fixed,
+  seeded sample of the updated fp32 parameters and of the gradients the step computed, as float32
+  .npy files.  The sample positions depend only on the parameter count, so two builds run with the
+  same arguments can be compared file by file."""
+  import numpy as np
+  import torch
+  os.makedirs(out_dir, exist_ok=True)
+  P = state["params"]
+  n = P.flat.numel()
+  idx = np.sort(np.random.default_rng(0).choice(n, size=min(n, DUMP_SAMPLE), replace=False))
+  idx_dev = torch.from_numpy(idx).to(P.flat.device)
+  for name, buf in (("params_sample", P.flat), ("grads_sample", P.grad)):
+    np.save(os.path.join(out_dir, f"{name}.npy"), buf[idx_dev].float().cpu().numpy())
+  for k, v in measurements.items():
+    np.save(os.path.join(out_dir, f"{k}.npy"), np.asarray(v.float().cpu().numpy(), dtype=np.float32).reshape(-1))
+
+
 def run_ours(args):
   import torch
   import torch.distributed as dist
@@ -556,7 +576,7 @@ def run_ours(args):
   if world > 1:
     dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
   if L.load().bv_device_supported() != 1:
-    raise SystemExit("bench.py needs a compute-capability 10.x device")
+    raise SystemExit("bench.py needs a compute-capability 9.x device")
   R = measure_ours(args, wl, world, rank, local_rank)
   gc.collect()
   torch.cuda.empty_cache()
@@ -603,22 +623,21 @@ def run_ours(args):
                    "seq_len": seq.get(wl["kind"], (wl["res"] // 16) ** 2),
                    "parallelism": f"dp{world}", "image_input": args.input,
                    "l2_policy": f"inputs ({R['h2d'] / 1e6:.0f} MB/step) and activations (GBs) exceed the "
-                                "126 MB L2; no explicit flush",
+                                "50 MB L2; no explicit flush",
                    "final_loss": R["loss"], "peak_mem_gib": R["peak_mem_gib"]},
         "clocks": R["clocks"],
         "e2e": {"value": e2e_val, "unit": wl["unit"], "ms_per_step": R["ms_e2e"] / args.steps,
                 "h2d_bytes_per_step": R["h2d"], "d2h_bytes_per_step": 4},
         "gpu_launches": R["launches"],
-        "roofline": {"bound": "tensor", "kernel": "gemm_kernel (tcgen05 persistent GEMM)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_kernel (wgmma + TMA GEMM)",
                      "achieved": gemm_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": gemm_tf / peak_tf,
-                     "peak_source": f"{peak_src} bf16_tflops_sustained",
+                     "peak_source": f"{peak_src} " + ("bf16_tflops_sustained" if "bf16_tflops_sustained" in peaks
+                                                      else "bf16_tflops"),
                      # per launch, averaged over the step's GEMM launches (shapes differ)
                      "launches_per_step": R["gemm_launches"] // args.steps,
                      "flop_per_launch": R["gemm_flops"] / R["gemm_launches"],
                      "algorithmic_bytes_per_launch": R["gemm_bytes"] / R["gemm_launches"],
-                     "traffic": NCU_GEMM_DRAM_BYTES_PER_LAUNCH if args.workload == "siglip_b16" else None,
-                     "traffic_source": ("NOT measured in this run: constant from " + NCU_GEMM_DRAM_SOURCE
-                                        if args.workload == "siglip_b16" else None),
+                     "traffic": None, "traffic_source": "not measured",
                      # measured in a second pass of the same K steps with an event pair per GEMM launch
                      "gemm_share_of_step": R["gemm_ms"] / R["ms_instrumented"],
                      "ms_per_step_instrumented": R["ms_instrumented"] / args.steps,
@@ -646,6 +665,9 @@ def main():
   ap.add_argument("--no-gpu-baseline", action="store_true")
   ap.add_argument("--profile-calls", action="store_true",
                   help="time every C-ABI call of one extra step with CUDA events; breakdown on stderr")
+  ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                  help="after the timed steps, write the last step's outputs (measurements, seeded samples of "
+                       "the updated parameters and of the gradients) to DIR/<name>.npy")
   args = ap.parse_args()
   if args.impl == "reference":
     run_reference(args)

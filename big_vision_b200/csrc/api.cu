@@ -18,7 +18,7 @@ int bv_device_supported(void) {
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   int major = 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 10 ? 1 : 0;
+  return major == 9 ? 1 : 0;
 }
 
 int bv_gemm(const bv_gemm_args* a, void* stream) {
@@ -72,11 +72,6 @@ int bv_attention_bwd(const bv_attn_bwd_args* a, void* stream) {
   g.delta = a->delta; g.dq_accum = a->dq_accum;
   return launch_attention_bwd(g, S(stream));
 }
-
-/* bring-up aid (not in the public header): copies the BV_ATTN_DBG=1 timeline of the last
- * attention forward launch (clock64 per event, first 32 tiles of CTA 0) to host memory */
-int bv_debug_attn_timeline(long long* host, int n) { return attn_debug_read(host, n); }
-int bv_debug_gemm_timeline(long long* host, int n) { return gemm_debug_read(host, n); }
 
 int bv_patchify(const float* image, void* patches, int64_t n, int32_t H, int32_t W, int32_t C,
                 int32_t P, void* stream) {

@@ -1,1074 +1,432 @@
-// Scaled-dot-product attention forward / backward on tcgen05 (K5, and the MAP
-// head's 1-query attention, K10) for sequences whose keys fit on chip.  Reference:
-// flax.linen.MultiHeadDotProductAttention as called at models/vit.py:93-98 (self-attention, no
-// mask, no dropout) and models/vit.py:176-178 (MAPHead probe attention): q is scaled by
-// 1/sqrt(dh), softmax over keys, weights times v.  Head dim is fixed at 64 (every ViT variant in
-// models/vit.py:297-300 has width/heads == 64 except "mu" and So400m).
+// Scaled-dot-product attention forward / backward on sm_90a wgmma (K5, and the MAP head's
+// 1-query attention, K10).  Reference: flax.linen.MultiHeadDotProductAttention as called at
+// models/vit.py:93-98 (self-attention, no mask, no dropout) and models/vit.py:176-178 (MAPHead
+// probe attention): q is scaled by 1/sqrt(dh), softmax over keys, weights times v.  Head dim is
+// fixed at 64 (every ViT variant in models/vit.py:297-300 has width/heads == 64 except "mu" and
+// So400m).
 //
-// These are the RESIDENT kernels: all keys of one (image, head) fit on chip (N <= 256: 196/197
-// image tokens, 64 text tokens), so scores for a 128-query tile live in TMEM as a single
-// [128 x Nk] fp32 tile and the softmax is exact (no online rescaling).  Longer sequences (config 5:
-// 576 keys) go to the key-block streaming kernels of attention_stream.cu; the launchers here
-// dispatch.  64-token items (the text tower) are packed two per 128-row tile with block-diagonal
-// scores (can_pack / launch_attention_fwd).
+// q/k/v/o are strided views into the fused QKV GEMM output: element (b, t, h*64+j) at
+// base + b*batch_stride + t*row_stride + h*64 + j; 3-D TMA descriptors read them in place (no head
+// transpose, no padding copies; rows past N are zero-filled).
 //
-// q/k/v/o are strided views into the fused QKV GEMM output: element (b, t, h*64+j)
-// at base + b*batch_stride + t*row_stride + h*64 + j; 3-D TMA descriptors read them
-// in place (no head transpose, no padding copies; rows past N are zero-filled).
+// Both kernels run one warpgroup per CTA on 64-row tiles and stream the other operand in 64-row
+// blocks through a two-slot TMA ring, so any sequence length works with the same code:
+//   forward   (b, h, 64 queries):  S = Q K^T (smem x smem), online softmax in registers,
+//             O += P V with P as the register A operand of wgmma.
+//   backward  (b, h, 64 keys):     S^T = K Q^T, dP^T = V dO^T, P^T and dS^T in registers,
+//             dV += P^T dO, dK += dS^T Q (register A operands), dQ_kt = dS K through a swizzled
+//             shared-memory copy of dS^T, stored per key block in fp32; a second kernel sums the
+//             key blocks in a fixed order (bit-reproducible) and converts to bf16.
 #include "common.cuh"
 #include "host_utils.h"
 #include "kernels.h"
-#include "attn_common.cuh"
-
-#include <stdlib.h>
 
 namespace bv {
+
 namespace {
 
-using namespace attn;
+constexpr int DH = 64;
+constexpr int T = 64;                      // rows per tile (queries or keys)
+constexpr int TILE_BYTES = T * DH * 2;     // 8 KB: 64 rows x 128 B, 128B-swizzled
+constexpr float LOG2E = 1.4426950408889634f;
+constexpr float LN2 = 0.6931471805599453f;
+constexpr int THREADS = 128;
+// shared memory: 1024-aligned 8 KB tiles, then three mbarriers (+ alignment slack)
+constexpr int FWD_TILES = 5, BWD_TILES = 7;
+constexpr int FWD_SMEM = FWD_TILES * TILE_BYTES + 1024 + 64;
+constexpr int BWD_SMEM = BWD_TILES * TILE_BYTES + 1024 + 64;
+
+__device__ __forceinline__ float ex2(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+
+int make_tmap_bnd(CUtensorMap* m, const void* ptr, int cols, int64_t N, int64_t B, int64_t ld, int64_t bs) {
+  uint64_t dims[3] = {static_cast<uint64_t>(cols), static_cast<uint64_t>(N), static_cast<uint64_t>(B)};
+  uint64_t strides[2] = {static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(bs) * 2};
+  uint32_t box[3] = {64, T, 1};
+  return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, ptr, dims, strides, box, true);
+}
+
+// Descriptors of a 64 x 64 bf16 tile: K-major (rows = M|N, the 64 columns are the contraction) or
+// MN-major (rows = the contraction, the 64 columns are M|N).  One k step of 16 is 32 B or 16 rows.
+__device__ __forceinline__ uint64_t desc_k(uint32_t tile) { return wgmma_desc_sw128(tile, 16u, 1024u); }
+__device__ __forceinline__ uint64_t desc_mn(uint32_t tile) { return wgmma_desc_sw128(tile, 8192u, 1024u); }
+constexpr uint64_t KSTEP_K = 32 >> 4, KSTEP_MN = 2048 >> 4;
+
+// S[64 x 64] = A B^T over the 64-wide head dimension, both tiles K-major
+__device__ __forceinline__ void mma_tile_kk(float (&d)[32], uint32_t a_tile, uint32_t b_tile) {
+  const uint64_t a = desc_k(a_tile), b = desc_k(b_tile);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) wgmma_ss_n64<0, 0>(d, a + k * KSTEP_K, b + k * KSTEP_K, k > 0 ? 1 : 0);
+}
+// D[64 x 64] += P[64 x 64] (register fragments) * B, B an MN-major tile (rows = contraction)
+__device__ __forceinline__ void mma_tile_rs(float (&d)[32], const uint32_t (&p)[4][4], uint32_t b_tile) {
+  const uint64_t b = desc_mn(b_tile);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) wgmma_rs_n64<1>(d, p[k], b + k * KSTEP_MN, 1);
+}
+
+// accumulator element 4j + e of lane l in warp w: row 16w + l/4 + 8*(e >> 1), column 8j + 2*(l%4) + (e & 1).
+// The register A fragment of k step kk (columns 16kk..16kk+15) is then {j = 2kk: e01, e23; j = 2kk+1: e01, e23}.
+__device__ __forceinline__ void to_frags(const float (&s)[32], uint32_t (&p)[4][4]) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    p[kk][0] = pack_bf16(s[8 * kk + 0], s[8 * kk + 1]);
+    p[kk][1] = pack_bf16(s[8 * kk + 2], s[8 * kk + 3]);
+    p[kk][2] = pack_bf16(s[8 * kk + 4], s[8 * kk + 5]);
+    p[kk][3] = pack_bf16(s[8 * kk + 6], s[8 * kk + 7]);
+  }
+}
+
+__device__ __forceinline__ void zero(float (&d)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) d[i] = 0.f;
+}
 
 // ============================================================================
 // forward
 // ============================================================================
-constexpr int FWD_THREADS = 512;   // WG0,1 softmax; WG2: TMA / S issue / PV issue; WG3: O epilogue
-
 struct FwdDev {
-  int tiles;          // B * H * QT
-  int H, QT, Nq, Nk, NKP;
-  int nstage, nbuf;
-  float scale_log2;   // scale * log2(e)
-  float* lse;         // [B, H, Nq]
-  long long* dbg;     // optional timeline of CTA 0 (bring-up aid, BV_ATTN_DBG=1), else null
-  int sm_var;         // softmax tuning variant (BV_ATTN_SM, bit 0 = independent max / sum chains)
-  int pack;           // 1: every 128-row tile holds TWO 64-token items (block-diagonal scores), see launcher
-};
-
-// dbg[(tile_i * 16 + event)] = clock64() for the first 32 tiles of CTA 0
-#define ATTN_DBG(ev, i)                                                       \
-  do {                                                                        \
-    if (p.dbg != nullptr && blockIdx.x == 0 && (i) < 32)                      \
-      p.dbg[(i) * 16 + (ev)] = clock64();                                     \
-  } while (0)
-
-struct FwdSmem {
-  // byte offsets from the 1024-aligned base
-  int stage_bytes, kv_bytes, p_off, o_off, x_off, bar_off, total;
-};
-
-__host__ __device__ inline FwdSmem fwd_smem_layout(int NKP, int nstage) {
-  FwdSmem L;
-  L.kv_bytes = NKP * 128;
-  L.stage_bytes = TILE_BYTES + 2 * L.kv_bytes;
-  L.p_off = nstage * L.stage_bytes;
-  const int nblk = (NKP + 63) / 64;
-  L.o_off = L.p_off + nblk * TILE_BYTES;
-  L.x_off = L.o_off + TILE_BYTES;
-  L.bar_off = L.x_off + 6 * 128 * 4;
-  L.total = L.bar_off + 160 + 1024;
-  return L;
-}
-
-// Everything the softmax warpgroups need, copied into registers once (kernel parameters live in
-// constant memory; re-reading them inside the unrolled per-unit code costs an LDCU round trip each
-// time and was the dominant stall of the first version).
-struct SoftmaxCtx {
-  uint32_t tmem_base, p_s, bar, s_full0, s_empty0, p_full, p_empty, inv_full0, inv_empty0;
-  float* xch;
-  float* lse;
-  long long* dbg;
-  int my_tiles, NKP, Nk, Nq, QT, nbuf, pack, H;
+  int H, Nq, Nk, QT, NB;
   float scale_log2;
+  float* lse;
+  bf16* o;
+  long long ldo, bso;
 };
 
-#define SM_DBG(ev, i)                                                         \
-  do {                                                                        \
-    if (c.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0 && (i) < 32)  \
-      c.dbg[(i) * 16 + (ev)] = clock64();                                     \
-  } while (0)
-
-// NU = number of 8-column units per thread (compile time; 0 = run time, up to 16)
-// ALL_MUFU: every exponential on MUFU.EX2 (BV_ATTN_SM >> 2 == 2, the default) instead of alternating
-// 8-column units with the FMA-pipe polynomial.  (Independent max / sum chains were tried on the
-// streaming kernel and measured no different; the ILP switch is kept off.)
-template <int NU, bool ALL_MUFU>
-__device__ __forceinline__ void softmax_warpgroups(const SoftmaxCtx c) {
-  constexpr bool ILP = false;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int quarter = warp & 3, hf = warp >> 2;
-  const int row = quarter * 32 + lane;
-  const uint32_t sw = static_cast<uint32_t>(row & 7);
-  const int nunits = NU ? NU : (c.NKP >> 4);
-  const int half_cols = nunits * 8;
-  const int kbase = hf * nunits;                    // first 8-column unit of this warp's half
-  const int valid = pin_reg(c.Nk - hf * half_cols);  // columns of this half that are real keys
-  const uint32_t lane_addr = static_cast<uint32_t>(quarter * 32) << 16;
-  const uint32_t p_row = c.p_s + row * 128;
-  const float scale_log2 = pin_reg(c.scale_log2);
-  float* xch = pin_reg(c.xch);
-  const int nbuf = pin_reg(c.nbuf), NKP = pin_reg(c.NKP), QT = pin_reg(c.QT), Nq = pin_reg(c.Nq);
-  // packed tiles (two 64-token items, block-diagonal scores): rows 0..63 own key columns 0..63 (this
-  // thread's half iff hf == 0), rows 64..127 own columns 64..127 (hf == 1); the other half of the row is
-  // masked: probability 0, no contribution to max / sum.  Warp-uniform (a warp is 32 rows of one half).
-  const bool dead = pin_reg(c.pack) != 0 && ((row < 64) != (hf == 0));
-  const int pH = pin_reg(c.H);
-#define UNIT_ON(u) (NU ? ((u) < NU) : ((u) < nunits))
-  for (int i = 0; i < c.my_tiles; ++i) {
-    const int tile = blockIdx.x + i * gridDim.x;
-    const int qt = tile % QT;
-    const int bh = tile / QT;
-    const int bf = i % nbuf;
-    // no real query row in this warp's 32 rows of the tile (the second tile of a 196-token item holds
-    // 68 rows): nothing to exponentiate; the rows it would produce are clipped by the output store
-#ifdef BV_NO_DEAD_SKIP      // A/B build (python -m big_vision_b200.build --variant BV_NO_DEAD_SKIP noskip)
-    const bool dead_t = dead;
-#else
-    const bool dead_t = dead || (qt * TQ + quarter * 32 >= Nq);
-#endif
-    mbar_wait(c.s_full0 + 8u * bf, static_cast<uint32_t>(i / nbuf) & 1u);
-    tc_fence_after();
-    SM_DBG(3, i);
-    uint32_t sv[16][8];
-    const uint32_t s_addr = c.tmem_base + lane_addr + bf * NKP + hf * half_cols;
-#pragma unroll
-    for (int u = 0; u < 16; ++u)
-      if (UNIT_ON(u)) tmem_ld_x8(s_addr + u * 8, sv[u]);
-    tmem_ld_wait();
-    SM_DBG(12, i);
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(c.s_empty0 + 8u * bf);
-
-    // row maximum of the raw scores (scale > 0, so max commutes with the scaling)
-    float mxa[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-    for (int u = 0; u < 16; ++u) {
-      if (UNIT_ON(u)) {
-        if (dead_t) {
-          // masked half of a packed tile, or rows past Nq
-        } else if (u * 8 + 8 <= valid) {
-          // every column of this unit is a real key (warp-uniform test): no per-element masking
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float& m = mxa[ILP ? (j & 3) : 0];
-            m = fmaxf(m, __uint_as_float(sv[u][j]));
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float sc = __uint_as_float(sv[u][j]);
-            if (u * 8 + j >= valid) sc = -INFINITY;     // padded key columns
-            sv[u][j] = __float_as_uint(sc);
-            float& m = mxa[ILP ? (j & 3) : 0];
-            m = fmaxf(m, sc);
-          }
-        }
-      }
-    }
-    float mx = fmaxf(fmaxf(mxa[0], mxa[1]), fmaxf(mxa[2], mxa[3]));
-    xch[hf * 128 + row] = mx;
-    SM_DBG(13, i);
-    named_bar_sync(2, 256);
-    mx = fmaxf(mx, xch[(hf ^ 1) * 128 + row]);
-    SM_DBG(4, i);
-    const float mxs = mx * scale_log2;
-    float sma[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int u = 0; u < 16; ++u) {
-      if (UNIT_ON(u)) {
-        float e[8];
-        // exp2(scale * s - scale * max); ALL_MUFU (default since round 2: measured faster, the FMA
-        // pipe is the co-bottleneck) or units alternating between MUFU and the FMA-pipe polynomial
-        if (dead_t) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) e[j] = 0.f;
-        } else if (!ALL_MUFU && (u & 1)) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) e[j] = ex2_poly(fmaf(__uint_as_float(sv[u][j]), scale_log2, -mxs));
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) e[j] = ex2_mufu(fmaf(__uint_as_float(sv[u][j]), scale_log2, -mxs));
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) sma[ILP ? (j & 3) : 0] += e[j];
-        // packed in place: sv[u][0..3] now hold the 8 bf16 probabilities of this unit
-        sv[u][0] = pack_bf16(e[0], e[1]); sv[u][1] = pack_bf16(e[2], e[3]);
-        sv[u][2] = pack_bf16(e[4], e[5]); sv[u][3] = pack_bf16(e[6], e[7]);
-      }
-    }
-    SM_DBG(14, i);
-    // the P buffer is free once the previous tile's P V product has retired
-    mbar_wait(c.p_empty, (static_cast<uint32_t>(i) & 1u) ^ 1u);
-    SM_DBG(5, i);
-#pragma unroll
-    for (int u = 0; u < 16; ++u) {
-      if (UNIT_ON(u)) {
-        const uint32_t k = static_cast<uint32_t>(kbase + u);      // global 8-column unit index
-        const uint32_t addr = p_row + (k >> 3) * TILE_BYTES + (((k & 7u) ^ sw) << 4);
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(sv[u][0]),
-                     "r"(sv[u][1]), "r"(sv[u][2]), "r"(sv[u][3]) : "memory");
-      }
-    }
-    float sum = (sma[0] + sma[1]) + (sma[2] + sma[3]);
-    xch[256 + hf * 128 + row] = sum;
-    SM_DBG(15, i);
-    fence_proxy_async();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(c.p_full);
-    SM_DBG(6, i);
-    named_bar_sync(2, 256);
-    sum += xch[256 + (hf ^ 1) * 128 + row];
-    // hand 1/rowsum to the epilogue warpgroup (double-buffered slot) and write the log-sum-exp
-    mbar_wait(c.inv_empty0 + 8u * (i & 1), (static_cast<uint32_t>(i >> 1) & 1u) ^ 1u);
-    if (hf == 0) {
-      xch[512 + (i & 1) * 128 + row] = 1.0f / sum;
-      const int qrow = qt * TQ + row;
-      if (qrow < Nq && c.lse != nullptr) {
-        // packed: tile bh = (b', h) holds images 2b' (rows 0..63) and 2b'+1 (rows 64..127); lse stays in
-        // the caller's [B, H, 64] layout
-        const int64_t li = c.pack ? (static_cast<int64_t>(bh + (bh / pH) * pH + (row >> 6) * pH) * 64 + (row & 63))
-                                  : (static_cast<int64_t>(bh) * Nq + qrow);
-        c.lse[li] = (mxs + log2f(sum)) * LN2;
-      }
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(c.inv_full0 + 8u * (i & 1));
-  }
-#undef UNIT_ON
-}
-
-__global__ void __launch_bounds__(FWD_THREADS, 1)
+__global__ void __launch_bounds__(THREADS)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmO,
-                const FwdDev p) {
+                const __grid_constant__ CUtensorMap tmV, const FwdDev p) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  const uint32_t base = (raw_addr + 1023u) & ~1023u;
-  uint8_t* base_ptr = smem_raw + (base - raw_addr);
-  const FwdSmem L = fwd_smem_layout(p.NKP, p.nstage);
+  const uint32_t q_s = (smem_u32(smem_raw) + 1023u) & ~1023u, k_s = q_s + TILE_BYTES, v_s = q_s + 3 * TILE_BYTES;
+  const uint32_t q_bar = q_s + FWD_TILES * TILE_BYTES;
+  auto kv_bar = [&](int s) { return q_bar + 8u * (1 + s); };
 
-  const uint32_t bar = base + L.bar_off;
-  auto in_full = [&](int s) { return bar + 8u * s; };
-  auto in_empty = [&](int s) { return bar + 8u * (2 + s); };
-  auto s_full = [&](int b) { return bar + 8u * (4 + b); };
-  auto s_empty = [&](int b) { return bar + 8u * (6 + b); };
-  const uint32_t p_full = bar + 64, p_empty = bar + 72, o_full = bar + 80, o_empty = bar + 88;
-  auto inv_full = [&](int b) { return bar + 96u + 8u * b; };
-  auto inv_empty = [&](int b) { return bar + 112u + 8u * b; };
-  const uint32_t tmem_slot = bar + 128;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(base_ptr + L.bar_off + 128);
-  float* xch = reinterpret_cast<float*>(base_ptr + L.x_off);   // [max0|max1|sum0|sum1|inv0|inv1][128]
+  const int qt = static_cast<int>(blockIdx.x % p.QT);
+  const int bh = static_cast<int>(blockIdx.x / p.QT);
+  const int h = bh % p.H, b = bh / p.H;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmO);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(in_full(s), 1); mbar_init(in_empty(s), 1);
-      mbar_init(s_full(s), 1);  mbar_init(s_empty(s), 8);
-      mbar_init(inv_full(s), 8); mbar_init(inv_empty(s), 4);
-    }
-    mbar_init(p_full, 8); mbar_init(p_empty, 1);
-    mbar_init(o_full, 1); mbar_init(o_empty, 4);
+  auto load_kv = [&](int j) {
+    const int s = j & 1;
+    mbar_expect_tx(kv_bar(s), 2 * TILE_BYTES);
+    tma_load_3d(k_s + s * TILE_BYTES, &tmK, kv_bar(s), h * DH, j * T, b);
+    tma_load_3d(v_s + s * TILE_BYTES, &tmV, kv_bar(s), h * DH, j * T, b);
+  };
+  if (tid == 0) {
+    mbar_init(q_bar, 1);
+    mbar_init(kv_bar(0), 1);
+    mbar_init(kv_bar(1), 1);
     fence_barrier_init();
+    mbar_expect_tx(q_bar, TILE_BYTES);
+    tma_load_3d(q_s, &tmQ, q_bar, h * DH, qt * T, b);
+    load_kv(0);
+    if (p.NB > 1) load_kv(1);
   }
-  if (warp == 9) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  const uint32_t O_COL = 448;
 
-  const int my_tiles = (p.tiles - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) /
-                       static_cast<int>(gridDim.x);
-
-  if (warp >= 8 && warp < 12) {
-    // ======================= warpgroup 2: TMA producer, S issuer, PV issuer =======================
-    reg_dec<40>();
-    if (warp == 8) {
-      if (lane == 0) {
-        for (int i = 0; i < my_tiles; ++i) {
-          const int tile = blockIdx.x + i * gridDim.x;
-          const int qt = tile % p.QT;
-          const int bh = tile / p.QT;
-          const int h = bh % p.H, b = bh / p.H;
-          const int st = i % p.nstage;
-          const uint32_t ph = static_cast<uint32_t>(i / p.nstage) & 1u;
-          mbar_wait(in_empty(st), ph ^ 1u);
-          const uint32_t q_s = base + st * L.stage_bytes;
-          const uint32_t k_s = q_s + TILE_BYTES;
-          const uint32_t v_s = k_s + L.kv_bytes;
-          mbar_expect_tx(in_full(st), L.stage_bytes);
-          tma_load_3d(q_s, &tmQ, in_full(st), h * DH, qt * TQ, b);
-          tma_load_3d(k_s, &tmK, in_full(st), h * DH, 0, b);
-          tma_load_3d(v_s, &tmV, in_full(st), h * DH, 0, b);
-          ATTN_DBG(0, i);
-        }
-      }
-    } else if (warp == 9) {
-      // ---------------- S = Q K^T issuer ----------------
-      // The MMA issuers run as whole, converged warps and one elected lane executes the tcgen05
-      // instructions: inside a single-lane branch the compiler cannot prove the descriptors
-      // warp-uniform and wraps EVERY tcgen05.mma in an elect loop with four R2UR broadcasts, which
-      // makes the issue (not the tensor pipe) the limit for these small MMAs.
-      {
-        const uint32_t idesc_s = umma_idesc_bf16(128, p.NKP, 0, 0);   // both operands K-major
-        for (int i = 0; i < my_tiles; ++i) {
-          const int st = i % p.nstage, bf = i % p.nbuf;
-          mbar_wait(in_full(st), static_cast<uint32_t>(i / p.nstage) & 1u);
-          mbar_wait(s_empty(bf), (static_cast<uint32_t>(i / p.nbuf) & 1u) ^ 1u);
-          tc_fence_after();
-          if (lane == 0) ATTN_DBG(1, i);
-          const uint32_t q_s = base + st * L.stage_bytes;
-          const uint32_t k_s = q_s + TILE_BYTES;
-          const uint32_t d = tmem_base + bf * p.NKP;
-          const uint64_t dq = umma_smem_desc_sw128(q_s, 16, 1024), dk = umma_smem_desc_sw128(k_s, 16, 1024);
-          if (elect_one()) {
+  float o[32], s[32];
+  zero(o);
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  mbar_wait(q_bar, 0);
+  for (int j = 0; j < p.NB; ++j) {
+    const int slot = j & 1;
+    mbar_wait(kv_bar(slot), (j >> 1) & 1);
+    wgmma_fence();
+    mma_tile_kk(s, q_s, k_s + slot * TILE_BYTES);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    // online softmax in base 2 over this key block; keys past Nk get probability 0
+    const int kbase = j * T + 2 * (lane & 3);
+    float mx[2] = {m[0], m[1]};
 #pragma unroll
-            for (int k = 0; k < DH / 16; ++k) umma_bf16_ss(d, dq + k * 2, dk + k * 2, idesc_s, k > 0 ? 1u : 0u);
-            umma_commit(s_full(bf));
-          }
-          __syncwarp();
-          if (lane == 0) ATTN_DBG(2, i);
-        }
-      }
-    } else if (warp == 10) {
-      // ---------------- O = P V issuer (its own warp: never blocked behind a TMA wait) --------
-      {
-        const uint32_t idesc_o = umma_idesc_bf16(128, DH, 0, 1);      // V is MN-major
-        const int ksteps = p.NKP / 16;
-        for (int i = 0; i < my_tiles; ++i) {
-          const int st = i % p.nstage;
-          mbar_wait(p_full, static_cast<uint32_t>(i) & 1u);
-          mbar_wait(o_empty, (static_cast<uint32_t>(i) & 1u) ^ 1u);
-          tc_fence_after();
-          if (lane == 0) ATTN_DBG(7, i);
-          const uint32_t v_s = base + st * L.stage_bytes + TILE_BYTES + L.kv_bytes;
-          const uint32_t p_s = base + L.p_off;
-          const uint64_t dpd = umma_smem_desc_sw128(p_s, 16, 1024), dvd = umma_smem_desc_sw128(v_s, 8192, 1024);
-          if (elect_one()) {
-            for (int j = 0; j < ksteps; ++j)
-              umma_bf16_ss(tmem_base + O_COL, dpd + (j >> 2) * (TILE_BYTES / 16) + (j & 3) * 2, dvd + j * 128,
-                           idesc_o, j > 0 ? 1u : 0u);
-            umma_commit(o_full);
-            umma_commit(p_empty);
-            umma_commit(in_empty(st));   // Q/K were consumed by S(i) long before (softmax(i) waited on it)
-          }
-          __syncwarp();
-          if (lane == 0) ATTN_DBG(8, i);
-        }
-      }
+    for (int i = 0; i < 32; ++i) {
+      const int key = kbase + 8 * (i >> 2) + (i & 1);
+      s[i] = key < p.Nk ? s[i] * p.scale_log2 : -INFINITY;
+      mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
     }
-  } else if (warp >= 12) {
-    // ======================= warpgroup 3: O epilogue =======================
-    // TMEM -> registers -> (1/rowsum) -> bf16 -> swizzled smem -> TMA store, concurrently with the
-    // softmax warps working on the next tile.
-    reg_dec<96>();
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const int etid = threadIdx.x - 384;     // 0..127
-    const uint32_t sw = static_cast<uint32_t>(row & 7);
-    const uint32_t lane_addr = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t o_s = base + L.o_off;
-    for (int i = 0; i < my_tiles; ++i) {
-      const int tile = blockIdx.x + i * gridDim.x;
-      const int qt = tile % p.QT;
-      const int bh = tile / p.QT;
-      const int h = bh % p.H, b = bh / p.H;
-      mbar_wait(o_full, static_cast<uint32_t>(i) & 1u);
-      tc_fence_after();
-      if (etid == 0) ATTN_DBG(9, i);
-      uint32_t ov[64];
-      tmem_ld_32x32b_x32(tmem_base + lane_addr + O_COL, *reinterpret_cast<uint32_t(*)[32]>(&ov[0]));
-      tmem_ld_32x32b_x32(tmem_base + lane_addr + O_COL + 32, *reinterpret_cast<uint32_t(*)[32]>(&ov[32]));
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(o_empty);
-      mbar_wait(inv_full(i & 1), static_cast<uint32_t>(i >> 1) & 1u);
-      const float inv = xch[512 + (i & 1) * 128 + row];
-      __syncwarp();
-      if (lane == 0) mbar_arrive(inv_empty(i & 1));
-      if (etid == 0) tma_store_wait_read<0>();
-      named_bar_sync(3, 128);
-      if (etid == 0) ATTN_DBG(10, i);
+    float corr[2];
 #pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        const uint32_t addr = o_s + row * 128 + ((static_cast<uint32_t>(g) ^ sw) << 4);
-        float f[8];
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      corr[r] = ex2(m[r] - mx[r]);       // 0 on the first block (m = -inf)
+      m[r] = mx[r];
+      l[r] *= corr[r];
+    }
 #pragma unroll
-        for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(ov[g * 8 + j]) * inv;
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr),
-                     "r"(pack_bf16(f[0], f[1])), "r"(pack_bf16(f[2], f[3])),
-                     "r"(pack_bf16(f[4], f[5])), "r"(pack_bf16(f[6], f[7])) : "memory");
-      }
-      fence_proxy_async();
-      named_bar_sync(3, 128);
-      if (etid == 0) {
-        tma_store_3d(&tmO, o_s, h * DH, qt * TQ, b);
-        tma_store_commit();
-        ATTN_DBG(11, i);
-      }
+    for (int i = 0; i < 32; ++i) {
+      const int r = (i >> 1) & 1;
+      s[i] = ex2(s[i] - m[r]);
+      l[r] += s[i];
+      o[i] *= corr[r];
     }
-    if (etid == 0) tma_store_wait<0>();
-  } else {
-    // ======================= warpgroups 0,1: softmax =======================
-    reg_inc<184>();
-    SoftmaxCtx c;
-    c.tmem_base = tmem_base; c.p_s = base + L.p_off; c.xch = xch; c.bar = bar; c.my_tiles = my_tiles;
-    c.s_full0 = s_full(0); c.s_empty0 = s_empty(0); c.p_full = p_full; c.p_empty = p_empty;
-    c.inv_full0 = inv_full(0); c.inv_empty0 = inv_empty(0);
-    c.NKP = p.NKP; c.Nk = p.Nk; c.Nq = p.Nq; c.QT = p.QT; c.nbuf = p.nbuf; c.scale_log2 = p.scale_log2;
-    c.pack = p.pack; c.H = p.H;
-    c.lse = p.lse; c.dbg = p.dbg;
-    const int nunits = p.NKP >> 4;
-    if (p.sm_var >> 2 == 2) {
-      if (nunits == 13) softmax_warpgroups<13, true>(c);
-      else if (nunits == 8) softmax_warpgroups<8, true>(c);     // 128 keys: two packed 64-token items
-      else if (nunits == 4) softmax_warpgroups<4, true>(c);
-      else if (nunits == 16) softmax_warpgroups<16, true>(c);
-      else softmax_warpgroups<0, true>(c);
-    } else {
-      if (nunits == 13) softmax_warpgroups<13, false>(c);
-      else if (nunits == 8) softmax_warpgroups<8, false>(c);
-      else if (nunits == 4) softmax_warpgroups<4, false>(c);
-      else if (nunits == 16) softmax_warpgroups<16, false>(c);
-      else softmax_warpgroups<0, false>(c);
-    }
+    uint32_t pf[4][4];
+    to_frags(s, pf);
+    wgmma_fence_regs(o);
+    wgmma_fence();
+    mma_tile_rs(o, pf, v_s + slot * TILE_BYTES);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    __syncthreads();                     // every warp is done with this slot
+    if (tid == 0 && j + 2 < p.NB) load_kv(j + 2);
   }
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  // normalise, store O (bf16) and the log-sum-exp (natural log of the scaled scores)
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
+  }
+  const float inv[2] = {1.f / l[0], 1.f / l[1]};
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int q = qt * T + 16 * warp + (lane >> 2) + 8 * r;
+    if (q >= p.Nq) continue;
+    bf16* orow = p.o + b * p.bso + static_cast<long long>(q) * p.ldo + h * DH + 2 * (lane & 3);
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+      *reinterpret_cast<uint32_t*>(orow + 8 * jj) = pack_bf16(o[4 * jj + 2 * r] * inv[r], o[4 * jj + 2 * r + 1] * inv[r]);
+    if ((lane & 3) == 0) p.lse[(static_cast<long long>(b) * p.H + h) * p.Nq + q] = (m[r] + __log2f(l[r])) * LN2;
   }
 }
 
 // ============================================================================
 // backward
 // ============================================================================
-// One CTA per (image, head).  Queries and keys are cut into 128-wide tiles; for each
-// (key tile kt, query tile qt):
-//   S  = Q_qt K_kt^T           dP = dO_qt V_kt^T                  (TMEM, fp32)
-//   P  = exp(scale S - lse)    dS = scale * P o (dP - delta)      (registers -> smem bf16)
-//   dV_kt += P^T dO_qt         dK_kt += dS^T Q_qt      dQ_qt += dS K_kt     (TMEM)
-// delta_i = sum_j O_ij dO_ij is computed in the prologue from the O tile.
-constexpr int BWD_THREADS = 512;   // WG0,1 compute; WG2: warp 8 TMA, 9 MMA; WG3: gradient write-out
-constexpr int BWD_ROWS = 256;                       // smem rows per operand (zero-filled past N)
-constexpr int OP_BYTES = BWD_ROWS * 128;            // 32 KB
 struct BwdDev {
-  int BH, H, Nq, Nk, QT, KT;
+  int H, Nq, Nk, QT, KT;
+  long long B;
   float scale, scale_log2;
   const float* lse;
-  const bf16* o;     // forward output and its gradient, read straight from global memory for
-  const bf16* d_o;   // delta = rowsum(O o dO) (element (b,t,h*64+j) at b*bs + t*ld + h*64 + j)
-  long long ldo, bso, lddo, bsdo;
-  float* dq_colsum; float* dk_colsum; float* dv_colsum;   // optional [H*64] bias gradients
-  int variant;       // BV_BWD_VARIANT (bring-up experiments; 0 = default)
-  int in_bytes;      // bytes the four operand boxes of one item bring in (boxes are 128 rows when N <= 128)
-  int pack;          // 1: every item is TWO 64-token (image, head) items in one 128 x 128 pair (block-diagonal)
-  long long* dbg;    // optional timeline of CTA 0 (BV_ATTN_DBG=1)
+  const float* delta;
+  float* dq_accum;                        // [KT, B, Nq, H*64] fp32: one dQ slice per key block
+  bf16* dk; bf16* dv;
+  long long lddk, bsdk, lddv, bsdv;
+  float* dk_colsum; float* dv_colsum;
 };
-// dbg[256 + slot] : per-pair events (16 per pair, first 12 pairs) of CTA 0
-#define BWD_DBG(ev, pr)                                                       \
-  do {                                                                        \
-    if (p.dbg != nullptr && blockIdx.x == 0 && (pr) < 12)                     \
-      p.dbg[256 + (pr) * 16 + (ev)] = clock64();                              \
-  } while (0)
-constexpr int BWD_P_OFF = 4 * OP_BYTES;                       // P  [128 x 128] bf16 (2 blocks)
-constexpr int BWD_DS_OFF = BWD_P_OFF + 2 * TILE_BYTES;        // dS [128 x 128]
-constexpr int BWD_STG_OFF = BWD_DS_OFF + 2 * TILE_BYTES;      // 16 KB output staging
-constexpr int BWD_STAT_OFF = BWD_STG_OFF + TILE_BYTES;        // lse2[256], delta[256]
-constexpr int BWD_BAR_OFF = BWD_STAT_OFF + 4 * BWD_ROWS * 4;   // lse2 / delta, double-buffered per item
-constexpr int BWD_SMEM = BWD_BAR_OFF + 128 + 1024;
-constexpr int BWD_SMEM_PIPE = BWD_SMEM + 128;      // + per-tile operand barriers
 
-// PIPE = true (BV_ATTN_BWD_PIPE=1, bring-up; NOT yet validated on hardware): operands are loaded
-// and released per 128-row tile instead of per item, so the next item's K/V (and then Q/dO) tiles
-// stream in while the current item still works on its last key tile; single-tile items (the text
-// tower) alternate between the two tile slots of each operand, i.e. are double-buffered; S/dP of the
-// next item's first pair are issued ahead of the last gradient products when its operands have
-// landed; and delta / lse of item i+1 are fetched at the start of item i.
-template <bool PIPE>
-__global__ void __launch_bounds__(BWD_THREADS, 1)
+// column sums of a [64 x 64] accumulator tile's stored (bf16-rounded) rows < nvalid: the eight lanes
+// that share a column pair are summed with shuffles, then one atomic per warp and column
+__device__ __forceinline__ void tile_colsum(const float (&d)[32], float mul, int row0, int nvalid, float* colsum,
+                                            int lane) {
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj) {
+    float c[2] = {0.f, 0.f};
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      if (row0 + 8 * r >= nvalid) continue;
+      c[0] += round_bf16(d[4 * jj + 2 * r] * mul);
+      c[1] += round_bf16(d[4 * jj + 2 * r + 1] * mul);
+    }
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      c[e] += __shfl_xor_sync(0xffffffffu, c[e], 4);
+      c[e] += __shfl_xor_sync(0xffffffffu, c[e], 8);
+      c[e] += __shfl_xor_sync(0xffffffffu, c[e], 16);
+    }
+    if (lane < 4) {
+      atomicAdd(colsum + 8 * jj + 2 * lane, c[0]);
+      atomicAdd(colsum + 8 * jj + 2 * lane + 1, c[1]);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(THREADS)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmO,
-                const __grid_constant__ CUtensorMap tmdO, const __grid_constant__ CUtensorMap tmdQ,
-                const __grid_constant__ CUtensorMap tmdK, const __grid_constant__ CUtensorMap tmdV,
-                const BwdDev p) {
+                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const BwdDev p) {
+  // K, V (this CTA's key block), Q / dO ring of two, dS^T staging tile
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  const uint32_t base = (raw_addr + 1023u) & ~1023u;
-  uint8_t* base_ptr = smem_raw + (base - raw_addr);
-  const uint32_t q_s = base, k_s = base + OP_BYTES, v_s = base + 2 * OP_BYTES, do_s = base + 3 * OP_BYTES;
-  const uint32_t p_s = base + BWD_P_OFF, ds_s = base + BWD_DS_OFF, stg_s = base + BWD_STG_OFF;
-  float* lse2_s = reinterpret_cast<float*>(base_ptr + BWD_STAT_OFF);
-  float* delta_s = lse2_s + 2 * BWD_ROWS;
-  const uint32_t bar = base + BWD_BAR_OFF;
-  const uint32_t in_full = bar, in_empty = bar + 8, o_in_full = bar + 16, stat_ready = bar + 24;
-  const uint32_t sdp_full = bar + 32, sdp_empty = bar + 40, pds_full = bar + 48, pds_empty = bar + 56;
-  const uint32_t dkv_full = bar + 64, dkv_empty = bar + 72, dq_full = bar + 80, dq_empty = bar + 88;
-  const uint32_t tmem_slot = bar + 96;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(base_ptr + BWD_BAR_OFF + 96);
-  // PIPE: operand tile slots.  K and V tile t travel together (slot barrier "kv"), Q and dO too ("q")
-  auto full_kv = [&](int sl) { return bar + 128u + 8u * sl; };
-  auto empty_kv = [&](int sl) { return bar + 144u + 8u * sl; };
-  auto full_q = [&](int sl) { return bar + 160u + 8u * sl; };
-  auto empty_q = [&](int sl) { return bar + 176u + 8u * sl; };
+  const uint32_t k_s = (smem_u32(smem_raw) + 1023u) & ~1023u, v_s = k_s + TILE_BYTES, q_s = k_s + 2 * TILE_BYTES,
+                 do_s = k_s + 4 * TILE_BYTES, ds_s = k_s + 6 * TILE_BYTES;
+  const uint32_t kv_bar = k_s + BWD_TILES * TILE_BYTES;
+  auto q_bar = [&](int s) { return kv_bar + 8u * (1 + s); };
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
-    tma_prefetch_desc(&tmO); tma_prefetch_desc(&tmdO);
-    mbar_init(in_full, 1);   mbar_init(in_empty, 1);
-    mbar_init(o_in_full, 1); mbar_init(stat_ready, 8);
-    mbar_init(sdp_full, 1);  mbar_init(sdp_empty, 8);
-    mbar_init(pds_full, 8);  mbar_init(pds_empty, 1);
-    mbar_init(dkv_full, 1);  mbar_init(dkv_empty, 4);   // *_empty: one arrive per write-out warp
-    mbar_init(dq_full, 1);   mbar_init(dq_empty, 4);
-    if constexpr (PIPE) {
-      for (int sl = 0; sl < 2; ++sl) {
-        mbar_init(full_kv(sl), 1); mbar_init(empty_kv(sl), 1);
-        mbar_init(full_q(sl), 1);  mbar_init(empty_q(sl), 1);
-      }
-    }
+  const int kt = static_cast<int>(blockIdx.x % p.KT);
+  const int bh = static_cast<int>(blockIdx.x / p.KT);
+  const int h = bh % p.H, b = bh / p.H;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+
+  auto load_q = [&](int i) {
+    const int s = i & 1;
+    mbar_expect_tx(q_bar(s), 2 * TILE_BYTES);
+    tma_load_3d(q_s + s * TILE_BYTES, &tmQ, q_bar(s), h * DH, i * T, b);
+    tma_load_3d(do_s + s * TILE_BYTES, &tmdO, q_bar(s), h * DH, i * T, b);
+  };
+  if (tid == 0) {
+    mbar_init(kv_bar, 1);
+    mbar_init(q_bar(0), 1);
+    mbar_init(q_bar(1), 1);
     fence_barrier_init();
+    mbar_expect_tx(kv_bar, 2 * TILE_BYTES);
+    tma_load_3d(k_s, &tmK, kv_bar, h * DH, kt * T, b);
+    tma_load_3d(v_s, &tmV, kv_bar, h * DH, kt * T, b);
+    load_q(0);
+    if (p.QT > 1) load_q(1);
   }
-  if (warp == 9) { tmem_alloc(tmem_slot, 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  constexpr uint32_t S_COL = 0, DP_COL = 128, DV_COL = 256, DK_COL = 320, DQ_COL = 384;
 
-  const int my_items = (p.BH - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) /
-                       static_cast<int>(gridDim.x);
-
-  if (warp >= 12) {
-    // ---------------- gradient write-out warpgroup ----------------
-    // dV/dK (once per key tile) and dQ (once per item): TMEM -> bf16 -> swizzled staging -> TMA
-    // store, concurrently with the compute warps working on the next (key, query) tile pair.
-    reg_dec<112>();
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const int etid = threadIdx.x - 384;
-    const uint32_t sw = static_cast<uint32_t>(row & 7);
-    const uint32_t lane_addr = static_cast<uint32_t>(quarter * 32) << 16;
-    const int pH = pin_reg(p.H), pQT = pin_reg(p.QT), pKT = pin_reg(p.KT);
-    uint32_t kt_cnt = 0;
-    const int wmode = pin_reg(p.variant) & 3;
-    const int pNq = pin_reg(p.Nq), pNk = pin_reg(p.Nk);
-    // release != 0: this is the last tile of an accumulator group; the MMA warp may overwrite the
-    // group as soon as the tile is in registers (staging, column sums and the store are off its
-    // critical path)
-    auto write_tile = [&](uint32_t tcol, const CUtensorMap* tm, int h, int r0, int b, float* colsum, int nvalid,
-                          uint32_t release) {
-      uint32_t a[64];
-      tmem_ld_32x32b_x32(tmem_base + lane_addr + tcol, *reinterpret_cast<uint32_t(*)[32]>(&a[0]));
-      tmem_ld_32x32b_x32(tmem_base + lane_addr + tcol + 32, *reinterpret_cast<uint32_t(*)[32]>(&a[32]));
-      tmem_ld_wait();
-      if (release != 0u) {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(release);
-      }
-      if (etid == 0) tma_store_wait_read<0>();
-      named_bar_sync(3, 128);
+  float dk[32], dv[32];
+  zero(dk);
+  zero(dv);
+  const long long bhq = (static_cast<long long>(b) * p.H + h) * p.Nq;
+  const int cols = p.H * DH;
+  const int key_row = 16 * warp + (lane >> 2);      // + 8r: this thread's rows of the key block
+  mbar_wait(kv_bar, 0);
+  for (int i = 0; i < p.QT; ++i) {
+    const int slot = i & 1;
+    mbar_wait(q_bar(slot), (i >> 1) & 1);
+    const uint32_t qi = q_s + slot * TILE_BYTES, doi = do_s + slot * TILE_BYTES;
+    float st[32], dpt[32];
+    wgmma_fence();
+    mma_tile_kk(st, k_s, qi);            // S^T  = K Q^T
+    mma_tile_kk(dpt, v_s, doi);          // dP^T = V dO^T
+    wgmma_commit();
+    // this thread's 16 queries: lse / delta, fetched while the MMAs run
+    float lse2[16], dl[16];
 #pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        const uint32_t addr = stg_s + row * 128 + ((static_cast<uint32_t>(g) ^ sw) << 4);
-        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr),
-                     "r"(pack_bf16(__uint_as_float(a[g * 8 + 0]), __uint_as_float(a[g * 8 + 1]))),
-                     "r"(pack_bf16(__uint_as_float(a[g * 8 + 2]), __uint_as_float(a[g * 8 + 3]))),
-                     "r"(pack_bf16(__uint_as_float(a[g * 8 + 4]), __uint_as_float(a[g * 8 + 5]))),
-                     "r"(pack_bf16(__uint_as_float(a[g * 8 + 6]), __uint_as_float(a[g * 8 + 7]))) : "memory");
-      }
-      fence_proxy_async();
-      named_bar_sync(3, 128);
-      if (colsum != nullptr) {
-        // bias gradient of the projection that produced q/k/v: column sums of the staged tile over
-        // its valid rows (thread t: column t % 64, half of the rows)
-        // warp w sums rows 32w..32w+31, lane l the column pair (2l, 2l+1): every load is one
-        // conflict-free 128-byte row, all 32 loads independent
-        const int r_lo = (etid >> 5) * 32;
-        const uint32_t cp = static_cast<uint32_t>(etid & 31);
-        const uint32_t cbase = stg_s + (cp & 3) * 4;
-        float s0[2] = {0.f, 0.f}, s1[2] = {0.f, 0.f};
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int r = r_lo + i;
-          uint32_t w;
-          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w)
-                       : "r"(cbase + r * 128 + (((cp >> 2) ^ static_cast<uint32_t>(r & 7)) << 4)));
-          if (r0 + r >= nvalid) w = 0u;
-          s0[i & 1] += bf16_lo(w);
-          s1[i & 1] += bf16_hi(w);
-        }
-        atomicAdd(colsum + h * DH + 2 * cp, s0[0] + s0[1]);
-        atomicAdd(colsum + h * DH + 2 * cp + 1, s1[0] + s1[1]);
-      }
-      if (etid == 0) {
-        tma_store_3d(tm, stg_s, h * DH, r0, b);
-        tma_store_commit();
-      }
-    };
-    for (int it = 0; it < my_items; ++it) {
-      const int bh = blockIdx.x + it * gridDim.x;
-      const int h = bh % pH, b = bh / pH;
-      const uint32_t ph = static_cast<uint32_t>(it) & 1u;
-      for (int kt = 0; kt < pKT; ++kt, ++kt_cnt) {
-        mbar_wait_mode(dkv_full, kt_cnt & 1u, wmode);
-        tc_fence_after();
-        write_tile(DV_COL, &tmdV, h, kt * TQ, b, p.dv_colsum, pNk, 0u);
-        write_tile(DK_COL, &tmdK, h, kt * TQ, b, p.dk_colsum, pNk, dkv_empty);
-      }
-      mbar_wait_mode(dq_full, ph, wmode);
-      tc_fence_after();
-      for (int qt = 0; qt < pQT; ++qt)
-        write_tile(DQ_COL + qt * DH, &tmdQ, h, qt * TQ, b, p.dq_colsum, pNq, qt == pQT - 1 ? dq_empty : 0u);
+    for (int c = 0; c < 16; ++c) {
+      const int q = i * T + 8 * (c >> 1) + 2 * (lane & 3) + (c & 1);
+      lse2[c] = q < p.Nq ? p.lse[bhq + q] * LOG2E : INFINITY;   // +inf -> P = 0 for queries past Nq
+      dl[c] = q < p.Nq ? p.delta[bhq + q] : 0.f;
     }
-    if (etid == 0) tma_store_wait<0>();
-  } else if (warp >= 8) {
-    // PIPE: the issuer keeps more state (slot parities, next-item look-ahead): 64 registers, taken
-    // from the compute warps (168 instead of 176)
-    if constexpr (PIPE) reg_dec<64>(); else reg_dec<48>();
-  }
-  if (warp == 8) {
-    // ---------------- TMA producer ----------------
-    if (PIPE) {
-      if (lane == 0) {
-        // need-order of an item: K/V tile 0, Q/dO tiles, then K/V tile 1.  A slot is refilled as soon
-        // as the MMAs of its last use retired (empty_*), which for tile 0 of a two-tile operand is
-        // long before the item ends.  fills_* hold the parity of each slot's fill count.
-        uint32_t fills_kv = 0u, fills_q = 0u;      // bit sl = parity of the number of fills of slot sl
-        for (int it = 0; it < my_items; ++it) {
-          const int bh = blockIdx.x + it * gridDim.x;
-          const int h = bh % p.H, b = bh / p.H;
-          auto load_kv = [&](int t) {
-            const int sl = p.KT == 1 ? (it & 1) : t;
-            mbar_wait(empty_kv(sl), ((fills_kv >> sl) & 1u) ^ 1u);
-            fills_kv ^= 1u << sl;
-            mbar_expect_tx(full_kv(sl), 2 * TILE_BYTES);
-            tma_load_3d(k_s + sl * TILE_BYTES, &tmK, full_kv(sl), h * DH, t * TQ, b);
-            tma_load_3d(v_s + sl * TILE_BYTES, &tmV, full_kv(sl), h * DH, t * TQ, b);
-          };
-          auto load_q = [&](int t) {
-            const int sl = p.QT == 1 ? (it & 1) : t;
-            mbar_wait(empty_q(sl), ((fills_q >> sl) & 1u) ^ 1u);
-            fills_q ^= 1u << sl;
-            mbar_expect_tx(full_q(sl), 2 * TILE_BYTES);
-            tma_load_3d(do_s + sl * TILE_BYTES, &tmdO, full_q(sl), h * DH, t * TQ, b);
-            tma_load_3d(q_s + sl * TILE_BYTES, &tmQ, full_q(sl), h * DH, t * TQ, b);
-          };
-          load_kv(0);
-          for (int t = 0; t < p.QT; ++t) load_q(t);
-          if (p.KT > 1) load_kv(1);
-          BWD_DBG(13, it * 4);
-        }
-      }
-    } else if (lane == 0) {
-      // Operands are single-buffered (shared memory is full), so every CTA alternates between an
-      // HBM-bound load phase and a compute phase.  Left alone, all 148 CTAs fall into the same
-      // phase and the loads of one burst share the HBM bandwidth.  Starting the odd CTAs half an
-      // item late puts the two halves of the chip in anti-phase: one half loads while the other
-      // computes.
-      if ((blockIdx.x & 1) && my_items > 1) {
-        const long long t_start = clock64();
-        while (clock64() - t_start < 13000) { }
-      }
-      for (int it = 0; it < my_items; ++it) {
-        const int bh = blockIdx.x + it * gridDim.x;
-        const int h = bh % p.H, b = bh / p.H;
-        const uint32_t ph = static_cast<uint32_t>(it) & 1u;
-        // operands are free once every MMA of the previous item retired
-        mbar_wait(in_empty, ph ^ 1u);
-        mbar_expect_tx(in_full, static_cast<uint32_t>(p.in_bytes));
-        tma_load_3d(do_s, &tmdO, in_full, h * DH, 0, b);
-        tma_load_3d(q_s, &tmQ, in_full, h * DH, 0, b);
-        tma_load_3d(k_s, &tmK, in_full, h * DH, 0, b);
-        tma_load_3d(v_s, &tmV, in_full, h * DH, 0, b);
-        BWD_DBG(13, it * 4);
+    wgmma_wait<0>();
+    wgmma_fence_regs(st);
+    wgmma_fence_regs(dpt);
+    // P^T = exp(scale S^T - lse), dS^T = P^T o (dP^T - delta)   (the scale of dS is applied at the end)
+#pragma unroll
+    for (int e = 0; e < 32; ++e) {
+      const int c = 2 * (e >> 2) + (e & 1);
+      st[e] = ex2(st[e] * p.scale_log2 - lse2[c]);
+      dpt[e] = st[e] * (dpt[e] - dl[c]);
+    }
+    uint32_t pf[4][4], sf[4][4];
+    to_frags(st, pf);
+    to_frags(dpt, sf);
+    // dS^T -> shared memory (rows = keys, 128B swizzle), the MN-major A operand of dQ = dS K
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+      for (int f = 0; f < 4; ++f) {
+        const int r = key_row + 8 * (f & 1);
+        const int chunk = 2 * kk + (f >> 1);
+        const uint32_t addr = ds_s + r * 128 + ((chunk ^ (r & 7)) << 4) + 4 * (lane & 3);
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(sf[kk][f]) : "memory");
       }
     }
-  } else if (warp == 9) {
-    // ---------------- MMA issuer (whole warp converged, one elected lane issues; see the forward) ----
+    fence_proxy_async();
+    __syncthreads();
+    float dq[32];
+    wgmma_fence_regs(dv);
+    wgmma_fence_regs(dk);
+    wgmma_fence();
+    mma_tile_rs(dv, pf, doi);            // dV += P^T dO
+    mma_tile_rs(dk, sf, qi);             // dK += dS^T Q
     {
-      const uint32_t id_kk = umma_idesc_bf16(128, 128, 0, 0);   // S, dP
-      const uint32_t id_mm = umma_idesc_bf16(128, DH, 1, 1);    // dV, dK : A^T (MN) x B (MN)
-      const uint32_t id_km = umma_idesc_bf16(128, DH, 0, 1);    // dQ     : A (K)  x B (MN)
-      uint32_t sdp_cnt = 0, grad_cnt = 0, kt_cnt = 0;
-      const int pairs = p.KT * p.QT;
-      // S = Q K^T and dP = dO V^T of pair j (kt outer, qt inner) into TMEM
-      auto issue_sdp = [&](int j) {
-        const int kt = j / p.QT, qt = j % p.QT;
-        mbar_wait(sdp_empty, (sdp_cnt & 1u) ^ 1u);
-        ++sdp_cnt;
-        tc_fence_after();
-        uint32_t qa = q_s + qt * TILE_BYTES, ka = k_s + kt * TILE_BYTES;
-        uint32_t va = v_s + kt * TILE_BYTES, da = do_s + qt * TILE_BYTES;
-        // The addresses are made opaque per call: otherwise the compiler hoists every descriptor
-        // variant of every (kt, qt) out of the item loop and SPILLS them (this thread has few
-        // registers); a spill reload that misses L1 costs more than the MMAs it feeds.
-        asm volatile("" : "+r"(qa), "+r"(ka), "+r"(va), "+r"(da));
-        // descriptors are built once per tile; stepping along K only bumps the 16-byte-granular
-        // start-address field (this thread issues 32 MMAs per pair -- its instruction count matters)
-        const uint64_t dq_k = umma_smem_desc_sw128(qa, 16, 1024), dk_k = umma_smem_desc_sw128(ka, 16, 1024);
-        const uint64_t ddo_k = umma_smem_desc_sw128(da, 16, 1024), dv_k = umma_smem_desc_sw128(va, 16, 1024);
-        // S and dP are independent accumulators: interleaving their K steps keeps two dependent
-        // chains in flight (an MMA that accumulates into the tile of the previous one waits for it)
-        if (elect_one()) {
+      const uint64_t a = desc_mn(ds_s), bk = desc_mn(k_s);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            umma_bf16_ss(tmem_base + S_COL, dq_k + k * 2, dk_k + k * 2, id_kk, k > 0 ? 1u : 0u);
-            umma_bf16_ss(tmem_base + DP_COL, ddo_k + k * 2, dv_k + k * 2, id_kk, k > 0 ? 1u : 0u);
-          }
-          umma_commit(sdp_full);
-        }
-        __syncwarp();
-        if (lane == 0) BWD_DBG(5, sdp_cnt - 1);
-      };
-      // dV, dK, dQ contributions of pair j from the P / dS tiles the compute warps wrote
-      auto issue_grads = [&](int j, uint32_t ph) {
-        const int kt = j / p.QT, qt = j % p.QT;
-        uint32_t qa = q_s + qt * TILE_BYTES, ka = k_s + kt * TILE_BYTES;
-        uint32_t da = do_s + qt * TILE_BYTES, pa = p_s, dsa = ds_s;
-        asm volatile("" : "+r"(qa), "+r"(ka), "+r"(da), "+r"(pa), "+r"(dsa));   // see issue_sdp
-        if (lane == 0) BWD_DBG(10, grad_cnt);
-        mbar_wait(pds_full, grad_cnt & 1u);
-        if (lane == 0) BWD_DBG(8, grad_cnt);
-        ++grad_cnt;
-        if (qt == 0) mbar_wait(dkv_empty, (kt_cnt & 1u) ^ 1u);
-        if (kt == 0 && qt == 0) mbar_wait(dq_empty, ph ^ 1u);
-        if (lane == 0) BWD_DBG(9, grad_cnt - 1);
-        tc_fence_after();
-        const uint64_t dp_mn = umma_smem_desc_sw128(pa, TILE_BYTES, 1024);
-        const uint64_t dds_mn = umma_smem_desc_sw128(dsa, TILE_BYTES, 1024);
-        const uint64_t dds_k = umma_smem_desc_sw128(dsa, 16, 1024);
-        const uint64_t ddo_mn = umma_smem_desc_sw128(da, 8192, 1024);
-        const uint64_t dq_mn = umma_smem_desc_sw128(qa, 8192, 1024);
-        const uint64_t dk_mn = umma_smem_desc_sw128(ka, 8192, 1024);
-        // three independent accumulation chains (dV, dK, dQ) issued round-robin
-        const bool last_q = (qt == p.QT - 1);
-        if (elect_one()) {
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            const uint32_t accv = (qt > 0 || jj > 0) ? 1u : 0u;
-            // dV, dK: contraction over the 128 query rows, 16 per step (2048 B in the MN-major tiles)
-            umma_bf16_ss(tmem_base + DV_COL, dp_mn + jj * 128, ddo_mn + jj * 128, id_mm, accv);
-            umma_bf16_ss(tmem_base + DK_COL, dds_mn + jj * 128, dq_mn + jj * 128, id_mm, accv);
-            // dQ: contraction over the 128 keys
-            umma_bf16_ss(tmem_base + DQ_COL + qt * DH, dds_k + (jj >> 2) * (TILE_BYTES / 16) + (jj & 3) * 2,
-                         dk_mn + jj * 128, id_km, (kt > 0 || jj > 0) ? 1u : 0u);
-          }
-          umma_commit(pds_empty);
-          if (last_q) umma_commit(dkv_full);
-        }
-        __syncwarp();
-        if (lane == 0) BWD_DBG(6, grad_cnt - 1);
-        if (last_q) ++kt_cnt;
-      };
-      if constexpr (PIPE) {
-        // per-slot parity of the releases so far (== fills consumed; parity of the slot's full barrier),
-        // one bit per slot: indexed arrays would live in local memory
-        uint32_t use_kv = 0u, use_q = 0u;
-        auto slot_kv = [&](int it, int kt) { return p.KT == 1 ? (it & 1) : kt; };
-        auto slot_q = [&](int it, int qt) { return p.QT == 1 ? (it & 1) : qt; };
-        // have the operands of pair 0 of item `it` landed?  (non-blocking)
-        auto first_pair_ready = [&](int it) {
-          const int skv = slot_kv(it, 0), sq = slot_q(it, 0);
-          const int ok = (mbar_test(full_kv(skv), (use_kv >> skv) & 1u) && mbar_test(full_q(sq), (use_q >> sq) & 1u)) ? 1 : 0;
-          return __shfl_sync(0xffffffffu, ok, 0) != 0;      // one answer for the whole warp
-        };
-        auto sdp_pipe = [&](int it, int j) {
-          const int kt = j / p.QT, qt = j % p.QT;
-          const int skv = slot_kv(it, kt), sq = slot_q(it, qt);
-          if (qt == 0) mbar_wait(full_kv(skv), (use_kv >> skv) & 1u);   // first use of this K/V tile
-          if (kt == 0) mbar_wait(full_q(sq), (use_q >> sq) & 1u);       // first use of this Q/dO tile
-          mbar_wait(sdp_empty, (sdp_cnt & 1u) ^ 1u);
-          ++sdp_cnt;
-          tc_fence_after();
-          uint32_t qa = q_s + sq * TILE_BYTES, ka = k_s + skv * TILE_BYTES;
-          uint32_t va = v_s + skv * TILE_BYTES, da = do_s + sq * TILE_BYTES;
-          asm volatile("" : "+r"(qa), "+r"(ka), "+r"(va), "+r"(da));
-          const uint64_t dq_k = umma_smem_desc_sw128(qa, 16, 1024), dk_k = umma_smem_desc_sw128(ka, 16, 1024);
-          const uint64_t ddo_k = umma_smem_desc_sw128(da, 16, 1024), dv_k = umma_smem_desc_sw128(va, 16, 1024);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              umma_bf16_ss(tmem_base + S_COL, dq_k + k * 2, dk_k + k * 2, id_kk, k > 0 ? 1u : 0u);
-              umma_bf16_ss(tmem_base + DP_COL, ddo_k + k * 2, dv_k + k * 2, id_kk, k > 0 ? 1u : 0u);
-            }
-            umma_commit(sdp_full);
-          }
-          __syncwarp();
-          if (lane == 0) BWD_DBG(5, sdp_cnt - 1);
-        };
-        auto grads_pipe = [&](int it, int j) {
-          const int kt = j / p.QT, qt = j % p.QT;
-          const int skv = slot_kv(it, kt), sq = slot_q(it, qt);
-          const uint32_t ph = static_cast<uint32_t>(it) & 1u;
-          uint32_t qa = q_s + sq * TILE_BYTES, ka = k_s + skv * TILE_BYTES;
-          uint32_t da = do_s + sq * TILE_BYTES, pa = p_s, dsa = ds_s;
-          asm volatile("" : "+r"(qa), "+r"(ka), "+r"(da), "+r"(pa), "+r"(dsa));
-          mbar_wait(pds_full, grad_cnt & 1u);
-          ++grad_cnt;
-          if (qt == 0) mbar_wait(dkv_empty, (kt_cnt & 1u) ^ 1u);
-          if (kt == 0 && qt == 0) mbar_wait(dq_empty, ph ^ 1u);
-          tc_fence_after();
-          const uint64_t dp_mn = umma_smem_desc_sw128(pa, TILE_BYTES, 1024);
-          const uint64_t dds_mn = umma_smem_desc_sw128(dsa, TILE_BYTES, 1024);
-          const uint64_t dds_k = umma_smem_desc_sw128(dsa, 16, 1024);
-          const uint64_t ddo_mn = umma_smem_desc_sw128(da, 8192, 1024);
-          const uint64_t dq_mn = umma_smem_desc_sw128(qa, 8192, 1024);
-          const uint64_t dk_mn = umma_smem_desc_sw128(ka, 8192, 1024);
-          const bool last_q = (qt == p.QT - 1), last_k = (kt == p.KT - 1);
-          if (elect_one()) {
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-              const uint32_t accv = (qt > 0 || jj > 0) ? 1u : 0u;
-              umma_bf16_ss(tmem_base + DV_COL, dp_mn + jj * 128, ddo_mn + jj * 128, id_mm, accv);
-              umma_bf16_ss(tmem_base + DK_COL, dds_mn + jj * 128, dq_mn + jj * 128, id_mm, accv);
-              umma_bf16_ss(tmem_base + DQ_COL + qt * DH, dds_k + (jj >> 2) * (TILE_BYTES / 16) + (jj & 3) * 2,
-                           dk_mn + jj * 128, id_km, (kt > 0 || jj > 0) ? 1u : 0u);
-            }
-            umma_commit(pds_empty);
-            if (last_q) { umma_commit(dkv_full); umma_commit(empty_kv(skv)); }   // K/V tile kt done
-            if (last_k) umma_commit(empty_q(sq));                                // Q/dO tile qt done
-            if (last_q && last_k) umma_commit(dq_full);                          // item done
-          }
-          __syncwarp();
-          if (lane == 0) BWD_DBG(6, grad_cnt - 1);
-          if (last_q) { ++kt_cnt; use_kv ^= 1u << skv; }
-          if (last_k) use_q ^= 1u << sq;
-        };
-        if (my_items > 0) sdp_pipe(0, 0);
-        for (int it = 0; it < my_items; ++it) {
-          for (int j = 0; j < pairs; ++j) {
-            bool deferred = false;
-            if (j + 1 < pairs) {
-              sdp_pipe(it, j + 1);
-            } else if (it + 1 < my_items) {
-              // S/dP of the next item go ahead of this item's last gradient products only if its
-              // first tiles are already in shared memory; otherwise they follow them
-              if (first_pair_ready(it + 1)) sdp_pipe(it + 1, 0); else deferred = true;
-            }
-            grads_pipe(it, j);
-            if (deferred) sdp_pipe(it + 1, 0);
-          }
-        }
-      } else
-      for (int it = 0; it < my_items; ++it) {
-        const uint32_t ph = static_cast<uint32_t>(it) & 1u;
-        mbar_wait(in_full, ph);
-        // software pipeline: S/dP of pair j+1 are issued BEFORE the gradient products of pair j,
-        // so the compute warps can start on pair j+1 while the tensor core finishes pair j
-        issue_sdp(0);
-        for (int j = 0; j < pairs; ++j) {
-          if (j + 1 < pairs) issue_sdp(j + 1);
-          issue_grads(j, ph);
-        }
-        if (elect_one()) {
-          umma_commit(dq_full);
-          umma_commit(in_empty);
-        }
-        __syncwarp();
-      }
+      for (int k = 0; k < 4; ++k) wgmma_ss_n64<1, 1>(dq, a + k * KSTEP_MN, bk + k * KSTEP_MN, k > 0 ? 1 : 0);
     }
-  } else if (warp < 8) {
-    // ---------------- compute warps ----------------
-    if constexpr (PIPE) reg_inc<168>(); else reg_inc<176>();
-    const int quarter = warp & 3, hf = warp >> 2;
-    const int row = quarter * 32 + lane;
-    const int tid = threadIdx.x;
-    const uint32_t sw = static_cast<uint32_t>(row & 7);
-    const uint32_t lane_addr = static_cast<uint32_t>(quarter * 32) << 16;
-    uint32_t pair_cnt = 0;
-    // kernel parameters copied to registers once (see SoftmaxCtx)
-    const int pH = pin_reg(p.H), pNq = pin_reg(p.Nq), pNk = pin_reg(p.Nk), pQT = pin_reg(p.QT),
-              pKT = pin_reg(p.KT);
-    const float p_scale = pin_reg(p.scale), p_scale_log2 = pin_reg(p.scale_log2);
-    const float* __restrict__ p_lse = pin_reg(p.lse);
-    const bf16* __restrict__ p_o = pin_reg(p.o);
-    const bf16* __restrict__ p_do = pin_reg(p.d_o);
-    const long long p_ldo = p.ldo, p_bso = p.bso, p_lddo = p.lddo, p_bsdo = p.bsdo;
-    const int wmode = pin_reg(p.variant) & 3;
-    const bool mixed_exp = (pin_reg(p.variant) & 4) != 0;
-    const int p_pack = pin_reg(p.pack);
-    // packed items: this thread's 64 key columns belong to the other image -> P = dS = 0 (warp-uniform)
-    const bool dead = p_pack != 0 && ((row < 64) != (hf == 0));
-    // ---- prologue of item `pit`: delta = rowsum(O o dO) and lse (log2 units) for its 256 row slots,
-    // straight from global memory while the TMA loads are in flight; buffers alternate per item
-    auto prologue = [&](int pit) {
-      const int bh = blockIdx.x + pit * gridDim.x;
-      const int h = bh % pH, b = bh / pH;
-      float* lse2_i = lse2_s + (pit & 1) * BWD_ROWS;
-      float* delta_i = delta_s + (pit & 1) * BWD_ROWS;
-      // Eight lanes share a row (16 B each), so one warp-wide load touches four full 128-byte
-      // lines: 8x fewer L1 wavefronts than a row per thread.  That matters beyond this loop -- a
-      // congested load pipe also delays the tcgen05.mma issue of the other warps (measured).
-      {
-        const int chunk = tid & 7;
-        const bf16* po = p_o + b * p_bso + h * DH + chunk * 8;
-        const bf16* pd = p_do + b * p_bsdo + h * DH + chunk * 8;
-        uint4 ao[8], ad[8];
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(dv);
+    wgmma_fence_regs(dk);
+    wgmma_fence_regs(dq);
+    // dQ rows of this query block (rows = queries here) from this key block: this CTA's slice
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int r = (tid >> 3) + 32 * i;
-          if (r < pNq) {
-            ao[i] = ld_nc_na(reinterpret_cast<const uint4*>(po + r * p_ldo));
-            ad[i] = ld_nc_na(reinterpret_cast<const uint4*>(pd + r * p_lddo));
-          } else {
-            ao[i] = make_uint4(0u, 0u, 0u, 0u);
-            ad[i] = ao[i];
-          }
-        }
+    for (int r = 0; r < 2; ++r) {
+      const int q = i * T + 16 * warp + (lane >> 2) + 8 * r;
+      if (q >= p.Nq) continue;
+      float* dst = p.dq_accum + ((static_cast<long long>(kt) * p.B + b) * p.Nq + q) * cols + h * DH + 2 * (lane & 3);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          float acc = bf16_lo(ao[i].x) * bf16_lo(ad[i].x) + bf16_hi(ao[i].x) * bf16_hi(ad[i].x);
-          acc += bf16_lo(ao[i].y) * bf16_lo(ad[i].y) + bf16_hi(ao[i].y) * bf16_hi(ad[i].y);
-          acc += bf16_lo(ao[i].z) * bf16_lo(ad[i].z) + bf16_hi(ao[i].z) * bf16_hi(ad[i].z);
-          acc += bf16_lo(ao[i].w) * bf16_lo(ad[i].w) + bf16_hi(ao[i].w) * bf16_hi(ad[i].w);
-          acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-          acc += __shfl_xor_sync(0xffffffffu, acc, 2);
-          acc += __shfl_xor_sync(0xffffffffu, acc, 4);
-          if (chunk == 0) delta_i[(tid >> 3) + 32 * i] = acc;
-        }
-        // packed items: rows 0..63 = image 2b', rows 64..127 = image 2b'+1, lse in the caller's [B,H,64] layout
-        const int64_t li = p_pack ? (static_cast<int64_t>(bh + (bh / pH) * pH + (tid >> 6) * pH) * 64 + (tid & 63))
-                                  : (static_cast<int64_t>(bh) * pNq + tid);
-        lse2_i[tid] = tid < pNq ? p_lse[li] * LOG2E : INFINITY;
-      }
-    };
-    if constexpr (PIPE) {
-      if (my_items > 0) prologue(0);
+      for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<float2*>(dst + 8 * jj) = make_float2(dq[4 * jj + 2 * r] * p.scale,
+                                                               dq[4 * jj + 2 * r + 1] * p.scale);
     }
-    for (int it = 0; it < my_items; ++it) {
-      if constexpr (PIPE) {
-        // item i+1's statistics are fetched now, a whole item ahead of their use: the barrier
-        // orders them (written during item i-1) before this item's reads, and this item's reads of
-        // the other buffer (finished with item i-1's pairs) before the writes below
-        named_bar_sync(2, 256);
-        if (it + 1 < my_items) prologue(it + 1);
-      } else {
-        prologue(it);
-        named_bar_sync(2, 256);
-      }
-      const float* lse2_i = lse2_s + (it & 1) * BWD_ROWS;
-      const float* delta_i = delta_s + (it & 1) * BWD_ROWS;
-      if (tid == 0) BWD_DBG(7, pair_cnt);
-
-      for (int kt = 0; kt < pKT; ++kt) {
-        for (int qt = 0; qt < pQT; ++qt, ++pair_cnt) {
-          const uint32_t pp = pair_cnt & 1u;
-          mbar_wait_mode(sdp_full, pp, wmode);
-          if (tid == 0) BWD_DBG(0, pair_cnt);
-          tc_fence_after();
-          const int qrow = qt * TQ + row;
-          const bool row_ok = qrow < pNq;
-          const float l2 = lse2_i[qrow], dl = delta_i[qrow];
-          float pe[64];
-          {
-            uint32_t t0[32], t1[32];
-            tmem_ld_32x32b_x32(tmem_base + lane_addr + S_COL + hf * 64, t0);
-            tmem_ld_32x32b_x32(tmem_base + lane_addr + S_COL + hf * 64 + 32, t1);
-            tmem_ld_wait();
-            // No masking is needed here: padded query rows have lse = +inf (so P ~ 0), zero dO and
-            // zero Q rows; padded key columns only feed dV/dK rows that the TMA store clips and a
-            // dQ product against zero-filled K rows.  Everything stays finite.
-            // Exponentials: all on MUFU (BV_BWD_VARIANT bit 2 clear, the default since round 2) or
-            // alternating between MUFU and the FMA-pipe polynomial (see ex2_poly).
-            // live key columns of this thread's 64-column half in this key tile, and whether the warp's
-            // 32 query rows hold any real query: P = dS = 0 elsewhere costs nothing to produce (the
-            // 196-token items leave 68 rows / columns in their second tile)
-#ifdef BV_NO_DEAD_SKIP
-            const int ncl = 64;
-            const bool dead_p = dead;
-#else
-            int ncl = pNk - kt * TQ - hf * 64;
-            ncl = ncl > 64 ? 64 : ncl;
-            const bool dead_p = dead || ncl <= 0 || (qt * TQ + quarter * 32 >= pNq);
-#endif
-            if (dead_p) {
+    __syncthreads();                     // the Q / dO slot and the dS^T tile are free again
+    if (tid == 0 && i + 2 < p.QT) load_q(i + 2);
+  }
+  // dK (scaled), dV for the keys of this block, and their fused column sums
+  const int k0 = kt * T + key_row;
 #pragma unroll
-              for (int j = 0; j < 64; ++j) pe[j] = 0.f;
-            } else if (ncl < 64) {
+  for (int r = 0; r < 2; ++r) {
+    const int key = k0 + 8 * r;
+    if (key >= p.Nk) continue;
+    bf16* kr = p.dk + b * p.bsdk + static_cast<long long>(key) * p.lddk + h * DH + 2 * (lane & 3);
+    bf16* vr = p.dv + b * p.bsdv + static_cast<long long>(key) * p.lddv + h * DH + 2 * (lane & 3);
 #pragma unroll
-              for (int u8 = 0; u8 < 8; ++u8) {
-                if (u8 * 8 < ncl) {
-#pragma unroll
-                  for (int jj = 0; jj < 8; ++jj) {
-                    const int j = u8 * 8 + jj;
-                    const float sj = __uint_as_float(j < 32 ? t0[j & 31] : t1[j & 31]);
-                    pe[j] = ex2_mufu(fmaf(sj, p_scale_log2, -l2));
-                  }
-                } else {
-#pragma unroll
-                  for (int jj = 0; jj < 8; ++jj) pe[u8 * 8 + jj] = 0.f;
-                }
-              }
-            } else if (!mixed_exp) {
-#pragma unroll
-              for (int j = 0; j < 64; ++j) {
-                const float sj = __uint_as_float(j < 32 ? t0[j & 31] : t1[j & 31]);
-                pe[j] = ex2_mufu(fmaf(sj, p_scale_log2, -l2));
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 64; ++j) {
-                const float sj = __uint_as_float(j < 32 ? t0[j & 31] : t1[j & 31]);
-                const float xa = fmaf(sj, p_scale_log2, -l2);
-                pe[j] = (j & 2) ? ex2_poly(xa) : ex2_mufu(xa);
-              }
-            }
-          }
-          if (tid == 0) BWD_DBG(1, pair_cnt);
-          mbar_wait_mode(pds_empty, pp ^ 1u, wmode);
-          if (tid == 0) BWD_DBG(2, pair_cnt);
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t dv[32];
-            tmem_ld_32x32b_x32(tmem_base + lane_addr + DP_COL + hf * 64 + c * 32, dv);
-            tmem_ld_wait();
-            if (c == 1) {
-              tc_fence_before();
-              __syncwarp();
-              if (lane == 0) mbar_arrive(sdp_empty);
-            }
-#pragma unroll
-            for (int uu = 0; uu < 4; ++uu) {
-              const int u = c * 4 + uu;
-              uint32_t pk[4], dk[4];
-#pragma unroll
-              for (int j2 = 0; j2 < 4; ++j2) {
-                const int j = u * 8 + j2 * 2;
-                const float d0 = p_scale * pe[j] * (__uint_as_float(dv[(j & 31)]) - dl);
-                const float d1 = p_scale * pe[j + 1] * (__uint_as_float(dv[(j & 31) + 1]) - dl);
-                pk[j2] = pack_bf16(pe[j], pe[j + 1]);
-                dk[j2] = pack_bf16(d0, d1);
-              }
-              const uint32_t off = hf * TILE_BYTES + row * 128 + ((static_cast<uint32_t>(u) ^ sw) << 4);
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(p_s + off), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]), "r"(pk[3]) : "memory");
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(ds_s + off), "r"(dk[0]), "r"(dk[1]), "r"(dk[2]), "r"(dk[3]) : "memory");
-            }
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(pds_full);
-          if (tid == 0) BWD_DBG(4, pair_cnt);
-          if (tid == 224) BWD_DBG(11, pair_cnt);
-
-        }
-      }
+    for (int jj = 0; jj < 8; ++jj) {
+      *reinterpret_cast<uint32_t*>(kr + 8 * jj) = pack_bf16(dk[4 * jj + 2 * r] * p.scale, dk[4 * jj + 2 * r + 1] * p.scale);
+      *reinterpret_cast<uint32_t*>(vr + 8 * jj) = pack_bf16(dv[4 * jj + 2 * r], dv[4 * jj + 2 * r + 1]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  if (p.dk_colsum != nullptr) tile_colsum(dk, p.scale, k0, p.Nk, p.dk_colsum + h * DH, lane);
+  if (p.dv_colsum != nullptr) tile_colsum(dv, 1.f, k0, p.Nk, p.dv_colsum + h * DH, lane);
+}
+
+// delta[b,h,t] = sum_j O[b,t,h*64+j] * dO[b,t,h*64+j]: eight lanes per (b, t, h) row of 64
+__global__ void __launch_bounds__(256)
+attn_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ d_o, float* __restrict__ delta,
+                  int64_t B, int H, int N, int64_t ldo, int64_t bso, int64_t lddo, int64_t bsdo) {
+  const int64_t total = B * N * H;                    // head rows
+  const int chunk = threadIdx.x & 7;
+  for (int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 3; r < total;
+       r += (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 3) {
+    const int h = static_cast<int>(r % H);
+    const int64_t bt = r / H;
+    const int t = static_cast<int>(bt % N);
+    const int64_t b = bt / N;
+    const uint4 ao = ld_nc_na(reinterpret_cast<const uint4*>(o + b * bso + t * ldo + h * DH + chunk * 8));
+    const uint4 ad = ld_nc_na(reinterpret_cast<const uint4*>(d_o + b * bsdo + t * lddo + h * DH + chunk * 8));
+    float acc = bf16_lo(ao.x) * bf16_lo(ad.x) + bf16_hi(ao.x) * bf16_hi(ad.x);
+    acc += bf16_lo(ao.y) * bf16_lo(ad.y) + bf16_hi(ao.y) * bf16_hi(ad.y);
+    acc += bf16_lo(ao.z) * bf16_lo(ad.z) + bf16_hi(ao.z) * bf16_hi(ad.z);
+    acc += bf16_lo(ao.w) * bf16_lo(ad.w) + bf16_hi(ao.w) * bf16_hi(ad.w);
+    acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+    acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+    acc += __shfl_xor_sync(0xffffffffu, acc, 4);
+    if (chunk == 0) delta[(b * H + h) * N + t] = acc;
+  }
+}
+
+// dq[b,t,c] = bf16(sum_kt acc[kt,b,t,c]) summed in kt order; optional colsum[c] += sum over (b,t) of the
+// ROUNDED values (the bias gradient of the query projection, same definition as the fused column sums
+// of dk / dv).
+// Block = 256 threads: thread (rl, cg) walks rows rl, rl+R, ... of its row chunk for column group cg.
+__global__ void __launch_bounds__(256)
+attn_dq_convert_kernel(const float* __restrict__ acc, int KT, bf16* __restrict__ dq, float* __restrict__ colsum,
+                       int64_t rows_total, int N, int cols, int64_t lddq, int64_t bsdq, int rows_per_block) {
+  const int groups = cols / 8;                        // 8-column groups
+  const int rlanes = 256 / groups > 0 ? 256 / groups : 1;
+  const int cg = threadIdx.x % groups, rl = threadIdx.x / groups;
+  const int64_t r0 = static_cast<int64_t>(blockIdx.x) * rows_per_block;
+  float cs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  if (rl < rlanes) {
+    for (int64_t r = r0 + rl; r < r0 + rows_per_block && r < rows_total; r += rlanes) {
+      float4 a = *reinterpret_cast<const float4*>(acc + r * cols + cg * 8);
+      float4 c = *reinterpret_cast<const float4*>(acc + r * cols + cg * 8 + 4);
+      for (int kt = 1; kt < KT; ++kt) {
+        const float* src = acc + (kt * rows_total + r) * cols + cg * 8;
+        const float4 a2 = *reinterpret_cast<const float4*>(src), c2 = *reinterpret_cast<const float4*>(src + 4);
+        a.x += a2.x; a.y += a2.y; a.z += a2.z; a.w += a2.w;
+        c.x += c2.x; c.y += c2.y; c.z += c2.z; c.w += c2.w;
+      }
+      uint4 q;
+      q.x = pack_bf16(a.x, a.y); q.y = pack_bf16(a.z, a.w);
+      q.z = pack_bf16(c.x, c.y); q.w = pack_bf16(c.z, c.w);
+      const int64_t b = r / N;
+      const int t = static_cast<int>(r % N);
+      *reinterpret_cast<uint4*>(dq + b * bsdq + t * lddq + cg * 8) = q;
+      cs[0] += bf16_lo(q.x); cs[1] += bf16_hi(q.x); cs[2] += bf16_lo(q.y); cs[3] += bf16_hi(q.y);
+      cs[4] += bf16_lo(q.z); cs[5] += bf16_hi(q.z); cs[6] += bf16_lo(q.w); cs[7] += bf16_hi(q.w);
+    }
+    if (colsum != nullptr) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) atomicAdd(colsum + cg * 8 + k, cs[k]);
+    }
   }
 }
 
@@ -1078,175 +436,112 @@ int check_attn(const AttnArgs& a, const char* who) {
               (long long)a.B, a.H, a.Nq, a.Nk);
     return BV_ERR_INVALID;
   }
-  if (a.B * a.H * ((a.Nq + TQ - 1) / TQ) > 0x7fffffffLL) {
-    set_error("%s: too many (batch, head, query tile) work units", who);
+  const int64_t tiles = ((a.Nq > a.Nk ? a.Nq : a.Nk) + T - 1) / T;
+  if (a.B * a.H * tiles > 0x7fffffffLL) {
+    set_error("%s: too many (batch, head, tile) work units", who);
+    return BV_ERR_INVALID;
+  }
+  if ((reinterpret_cast<uintptr_t>(a.o) & 15) || (a.ldo % 8) || (a.bso % 8)) {
+    set_error("%s: o must be 16B aligned with strides that are multiples of 8", who);
     return BV_ERR_INVALID;
   }
   return BV_OK;
 }
 
-// Two 64-token items per 128-row tile (see launch_attention_fwd): needs self-attention over exactly 64
-// tokens, an even batch, and every operand's images back to back (batch stride == 64 row strides).
-// BV_ATTN_PACK=0 switches it off (A/B measurements, tests).
-bool can_pack(const AttnArgs& a, const void* extra, int64_t ld_extra, int64_t bs_extra) {
-  const char* e = getenv("BV_ATTN_PACK");
-  if (e && e[0] == '0') return false;
-  if (a.Nq != 64 || a.Nk != 64 || (a.B & 1)) return false;
-  (void)extra;
-  return a.bsq == 64 * a.ldq && a.bsk == 64 * a.ldk && a.bsv == 64 * a.ldv && bs_extra == 64 * ld_extra;
-}
-
-// Which forward kernel: sequences whose scores fit in TMEM (Nk <= 256) can use the whole-key-range
-// kernel of this file; longer ones need the key-block streaming kernel (attention_stream.cu), which
-// also handles the short ones.  BV_ATTN_FWD = "resident" | "stream" forces one for A/B measurements.
-bool use_stream_fwd(const AttnArgs& a) {
-  const char* e = getenv("BV_ATTN_FWD");     // read per call: tests flip it between launches
-  const int mode = (e && e[0] == 'r') ? 1 : (e && e[0] == 's') ? 2 : 0;
-  if (a.Nk > 256) return true;
-  if (mode == 1) return false;
-  if (mode == 2) return true;
-  return false;
-}
-
 }  // namespace
 
-static long long* g_attn_dbg = nullptr;
-
-long long* attn_debug_buffer() {
-  static const bool on = [] { const char* e = getenv("BV_ATTN_DBG"); return e && e[0] == '1'; }();
-  if (!on) return nullptr;
-  if (g_attn_dbg == nullptr) {
-    if (cudaMalloc(&g_attn_dbg, 32 * 16 * sizeof(long long)) != cudaSuccess) return nullptr;
-  }
-  cudaMemset(g_attn_dbg, 0, 32 * 16 * sizeof(long long));
-  return g_attn_dbg;
-}
-int attn_debug_read(long long* host, int n) {
-  if (g_attn_dbg == nullptr) return 0;
-  if (n > 32 * 16) n = 32 * 16;
-  cudaDeviceSynchronize();
-  cudaMemcpy(host, g_attn_dbg, n * sizeof(long long), cudaMemcpyDeviceToHost);
-  return n;
-}
-
-int launch_attention_fwd(const AttnArgs& a_in, cudaStream_t s) {
-  int rc = check_attn(a_in, "bv_attention_fwd");
+int launch_attention_fwd(const AttnArgs& a, cudaStream_t s) {
+  int rc = check_attn(a, "bv_attention_fwd");
   if (rc) return rc;
-  if (use_stream_fwd(a_in)) return launch_attention_fwd_stream(a_in, s);
   FwdDev p;
-  p.dbg = attn_debug_buffer();
-  { const char* e = getenv("BV_ATTN_SM"); p.sm_var = e ? atoi(e) : 8; }   // bits 2..: 2 = all exponentials on MUFU
-  // Packing: a 64-token item (the text tower) fills half of a 128-row tile.  When the images lie back
-  // to back in memory (batch stride == 64 rows, true for the fused QKV buffer) two consecutive images
-  // are ONE box of 128 rows: the kernel runs on B/2 items of 128 tokens with block-diagonal scores
-  // (the cross-image quarter tiles are masked to probability 0).  Half the tiles, no padded rows.
-  AttnArgs a = a_in;
-  p.pack = can_pack(a_in, a_in.o, a_in.ldo, a_in.bso) ? 1 : 0;
-  if (p.pack) { a.B = a_in.B / 2; a.Nq = a.Nk = 128; a.bsq *= 2; a.bsk *= 2; a.bsv *= 2; a.bso *= 2; }
   p.H = a.H; p.Nq = a.Nq; p.Nk = a.Nk;
-  p.QT = (a.Nq + TQ - 1) / TQ;
-  p.NKP = (a.Nk + 15) / 16 * 16;
-  p.tiles = static_cast<int>(a.B * a.H * p.QT);
-  p.nbuf = (2 * p.NKP <= 448) ? 2 : 1;
-  p.nstage = 2;
-  FwdSmem L = fwd_smem_layout(p.NKP, 2);
-  if (L.total > 232448) { p.nstage = 1; L = fwd_smem_layout(p.NKP, 1); }
+  p.QT = (a.Nq + T - 1) / T;
+  p.NB = (a.Nk + T - 1) / T;
   p.scale_log2 = a.scale * LOG2E;
   p.lse = a.lse;
+  p.o = static_cast<bf16*>(a.o);
+  p.ldo = a.ldo; p.bso = a.bso;
   const int cols = a.H * DH;
-  CUtensorMap tmQ, tmK, tmV, tmO;
-  if ((rc = make_tmap_bnd(&tmQ, a.q, cols, a.Nq, a.B, a.ldq, a.bsq, TQ))) return rc;
-  if ((rc = make_tmap_bnd(&tmK, a.k, cols, a.Nk, a.B, a.ldk, a.bsk, p.NKP))) return rc;
-  if ((rc = make_tmap_bnd(&tmV, a.v, cols, a.Nk, a.B, a.ldv, a.bsv, p.NKP))) return rc;
-  if ((rc = make_tmap_bnd(&tmO, a.o, cols, a.Nq, a.B, a.ldo, a.bso, TQ))) return rc;
-  rc = check_cuda(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       L.total), "cudaFuncSetAttribute(attn_fwd)");
+  CUtensorMap tmQ, tmK, tmV;
+  if ((rc = make_tmap_bnd(&tmQ, a.q, cols, a.Nq, a.B, a.ldq, a.bsq))) return rc;
+  if ((rc = make_tmap_bnd(&tmK, a.k, cols, a.Nk, a.B, a.ldk, a.bsk))) return rc;
+  if ((rc = make_tmap_bnd(&tmV, a.v, cols, a.Nk, a.B, a.ldv, a.bsv))) return rc;
+  const long long grid = a.B * a.H * p.QT;
+  rc = check_cuda(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM),
+                  "cudaFuncSetAttribute(attn_fwd)");
   if (rc) return rc;
-  const int sms = num_sms();
-  const int grid = p.tiles < sms ? p.tiles : sms;
-  attn_fwd_kernel<<<grid, FWD_THREADS, L.total, s>>>(tmQ, tmK, tmV, tmO, p);
+  attn_fwd_kernel<<<static_cast<unsigned>(grid), THREADS, FWD_SMEM, s>>>(tmQ, tmK, tmV, p);
   return check_cuda(cudaGetLastError(), "attn_fwd_kernel launch");
 }
 
-int launch_attention_bwd(const AttnBwdArgs& g_in, cudaStream_t s) {
-  int rc = check_attn(g_in.f, "bv_attention_bwd");
+int launch_attention_bwd(const AttnBwdArgs& g, cudaStream_t s) {
+  const AttnArgs& a = g.f;
+  int rc = check_attn(a, "bv_attention_bwd");
   if (rc) return rc;
-  if (g_in.f.lse == nullptr) { set_error("bv_attention_bwd: lse required"); return BV_ERR_INVALID; }
-  {
-    // long sequences stream 128-key tiles (attention_stream.cu); BV_ATTN_BWD=stream forces that kernel
-    // for short ones too when its workspaces were passed (A/B measurements, tests)
-    const char* e = getenv("BV_ATTN_BWD");
-    const bool force = e && e[0] == 's' && g_in.dq_accum != nullptr && g_in.delta != nullptr;
-    if (g_in.f.Nq > 256 || g_in.f.Nk > 256 || force) return launch_attention_bwd_stream(g_in, s);
+  if (a.lse == nullptr) { set_error("bv_attention_bwd: lse required"); return BV_ERR_INVALID; }
+  if (g.dq_accum == nullptr || g.delta == nullptr) {
+    set_error("bv_attention_bwd: needs the dq_accum [ceil(Nk/64),B,Nq,H*64] and delta [B,H,Nq] fp32 workspaces");
+    return BV_ERR_INVALID;
   }
-  BwdDev p;
-  // two 64-token items per 128 x 128 pair (see launch_attention_fwd); every tensor must have its images
-  // back to back
-  AttnBwdArgs gp = g_in;
-  {
-    const AttnArgs& f = g_in.f;
-    const bool ok = can_pack(f, f.o, f.ldo, f.bso) && g_in.bsdo == 64 * g_in.lddo && g_in.bsdq == 64 * g_in.lddq &&
-                    g_in.bsdk == 64 * g_in.lddk && g_in.bsdv == 64 * g_in.lddv &&
-                    !([] { const char* e = getenv("BV_ATTN_BWD_PIPE"); return e && e[0] == '1'; }());
-    p.pack = ok ? 1 : 0;
-    if (ok) {
-      gp.f.B = f.B / 2; gp.f.Nq = gp.f.Nk = 128;
-      gp.f.bsq *= 2; gp.f.bsk *= 2; gp.f.bsv *= 2; gp.f.bso *= 2;
-      gp.bsdo *= 2; gp.bsdq *= 2; gp.bsdk *= 2; gp.bsdv *= 2;
+  if ((reinterpret_cast<uintptr_t>(g.d_o) & 15) || (g.lddo % 8) || (g.bsdo % 8)) {
+    set_error("bv_attention_bwd: d_o must be 16B aligned with strides that are multiples of 8");
+    return BV_ERR_INVALID;
+  }
+  // dq / dk / dv are written with 16-byte / 4-byte vector stores
+  const void* grads[3] = {g.dq, g.dk, g.dv};
+  const int64_t lds[3] = {g.lddq, g.lddk, g.lddv}, bss[3] = {g.bsdq, g.bsdk, g.bsdv};
+  for (int i = 0; i < 3; ++i) {
+    if (grads[i] == nullptr || (reinterpret_cast<uintptr_t>(grads[i]) & 15) || (lds[i] % 8) || (bss[i] % 8)) {
+      set_error("bv_attention_bwd: dq / dk / dv must be non-null, 16B aligned, with strides that are multiples of 8");
+      return BV_ERR_INVALID;
     }
   }
-  const AttnBwdArgs& g = gp;
-  const AttnArgs& a = gp.f;
-  p.BH = static_cast<int>(a.B * a.H);
-  p.H = a.H; p.Nq = a.Nq; p.Nk = a.Nk;
-  p.QT = (a.Nq + TQ - 1) / TQ;
-  p.KT = (a.Nk + TQ - 1) / TQ;
+  if (a.H * DH > 2048) { set_error("bv_attention_bwd: H*64 must be <= 2048"); return BV_ERR_INVALID; }
+  const int cols = a.H * DH;
+  // delta = rowsum(O o dO)
+  {
+    const int64_t head_rows = a.B * a.Nq * a.H;
+    int64_t blocks = (head_rows * 8 + 255) / 256;
+    const int64_t cap = static_cast<int64_t>(num_sms()) * 16;
+    if (blocks > cap) blocks = cap;
+    attn_delta_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(
+        reinterpret_cast<const bf16*>(a.o), reinterpret_cast<const bf16*>(g.d_o), g.delta, a.B, a.H, a.Nq,
+        a.ldo, a.bso, g.lddo, g.bsdo);
+    if ((rc = check_cuda(cudaGetLastError(), "attn_delta_kernel launch"))) return rc;
+  }
+  BwdDev p;
+  p.H = a.H; p.Nq = a.Nq; p.Nk = a.Nk; p.B = a.B;
+  p.QT = (a.Nq + T - 1) / T;
+  p.KT = (a.Nk + T - 1) / T;
   p.scale = a.scale;
   p.scale_log2 = a.scale * LOG2E;
   p.lse = a.lse;
-  p.o = reinterpret_cast<const bf16*>(a.o);
-  p.d_o = reinterpret_cast<const bf16*>(g.d_o);
-  p.ldo = a.ldo; p.bso = a.bso; p.lddo = g.lddo; p.bsdo = g.bsdo;
-  p.dq_colsum = g.dq_colsum; p.dk_colsum = g.dk_colsum; p.dv_colsum = g.dv_colsum;
-  if ((reinterpret_cast<uintptr_t>(a.o) & 15) || (reinterpret_cast<uintptr_t>(g.d_o) & 15) ||
-      (a.ldo % 8) || (g.lddo % 8) || (a.bso % 8) || (g.bsdo % 8)) {
-    set_error("bv_attention_bwd: o / d_o must be 16B aligned with strides that are multiples of 8");
-    return BV_ERR_INVALID;
-  }
-  p.dbg = attn_debug_buffer();
-  { const char* e = getenv("BV_BWD_VARIANT"); p.variant = e ? atoi(e) : 0; }
-  const int cols = a.H * DH;
-  CUtensorMap tmQ, tmK, tmV, tmO, tmdO, tmdQ, tmdK, tmdV;
-  // BV_ATTN_BWD_PIPE=1: per-tile operand pipeline (bring-up switch, see attn_bwd_kernel<PIPE>)
-  const bool pipe = [] { const char* e = getenv("BV_ATTN_BWD_PIPE"); return e && e[0] == '1'; }();
-  // operand boxes: one tile (PIPE), or the whole item -- 128 rows are enough for a single-tile operand
-  // (the 64-token text tower, the 1-query MAP head): a 256-row box would spend half of its shared-memory
-  // writes on TMA zero-fill
-  const uint32_t q_rows = pipe ? TQ : (a.Nq <= TQ ? TQ : BWD_ROWS);
-  const uint32_t k_rows = pipe ? TQ : (a.Nk <= TQ ? TQ : BWD_ROWS);
-  p.in_bytes = static_cast<int>(2 * q_rows * 128 + 2 * k_rows * 128);
-  if ((rc = make_tmap_bnd(&tmQ, a.q, cols, a.Nq, a.B, a.ldq, a.bsq, q_rows))) return rc;
-  if ((rc = make_tmap_bnd(&tmK, a.k, cols, a.Nk, a.B, a.ldk, a.bsk, k_rows))) return rc;
-  if ((rc = make_tmap_bnd(&tmV, a.v, cols, a.Nk, a.B, a.ldv, a.bsv, k_rows))) return rc;
-  if ((rc = make_tmap_bnd(&tmO, a.o, cols, a.Nq, a.B, a.ldo, a.bso, q_rows))) return rc;
-  if ((rc = make_tmap_bnd(&tmdO, g.d_o, cols, a.Nq, a.B, g.lddo, g.bsdo, q_rows))) return rc;
-  if ((rc = make_tmap_bnd(&tmdQ, g.dq, cols, a.Nq, a.B, g.lddq, g.bsdq, TQ))) return rc;
-  if ((rc = make_tmap_bnd(&tmdK, g.dk, cols, a.Nk, a.B, g.lddk, g.bsdk, TQ))) return rc;
-  if ((rc = make_tmap_bnd(&tmdV, g.dv, cols, a.Nk, a.B, g.lddv, g.bsdv, TQ))) return rc;
-  const int sms = num_sms();
-  const int grid = p.BH < sms ? p.BH : sms;
-  if (pipe) {
-    rc = check_cuda(cudaFuncSetAttribute(attn_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         BWD_SMEM_PIPE), "cudaFuncSetAttribute(attn_bwd pipe)");
-    if (rc) return rc;
-    attn_bwd_kernel<true><<<grid, BWD_THREADS, BWD_SMEM_PIPE, s>>>(tmQ, tmK, tmV, tmO, tmdO, tmdQ, tmdK, tmdV, p);
-    return check_cuda(cudaGetLastError(), "attn_bwd_kernel<pipe> launch");
-  }
-  rc = check_cuda(cudaFuncSetAttribute(attn_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       BWD_SMEM), "cudaFuncSetAttribute(attn_bwd)");
+  p.delta = g.delta;
+  p.dq_accum = g.dq_accum;
+  p.dk = static_cast<bf16*>(g.dk); p.dv = static_cast<bf16*>(g.dv);
+  p.lddk = g.lddk; p.bsdk = g.bsdk; p.lddv = g.lddv; p.bsdv = g.bsdv;
+  p.dk_colsum = g.dk_colsum; p.dv_colsum = g.dv_colsum;
+  CUtensorMap tmQ, tmK, tmV, tmdO;
+  if ((rc = make_tmap_bnd(&tmQ, a.q, cols, a.Nq, a.B, a.ldq, a.bsq))) return rc;
+  if ((rc = make_tmap_bnd(&tmK, a.k, cols, a.Nk, a.B, a.ldk, a.bsk))) return rc;
+  if ((rc = make_tmap_bnd(&tmV, a.v, cols, a.Nk, a.B, a.ldv, a.bsv))) return rc;
+  if ((rc = make_tmap_bnd(&tmdO, g.d_o, cols, a.Nq, a.B, g.lddo, g.bsdo))) return rc;
+  const long long grid = a.B * a.H * p.KT;
+  rc = check_cuda(cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM),
+                  "cudaFuncSetAttribute(attn_bwd)");
   if (rc) return rc;
-  attn_bwd_kernel<false><<<grid, BWD_THREADS, BWD_SMEM, s>>>(tmQ, tmK, tmV, tmO, tmdO, tmdQ, tmdK, tmdV, p);
-  return check_cuda(cudaGetLastError(), "attn_bwd_kernel launch");
+  attn_bwd_kernel<<<static_cast<unsigned>(grid), THREADS, BWD_SMEM, s>>>(tmQ, tmK, tmV, tmdO, p);
+  if ((rc = check_cuda(cudaGetLastError(), "attn_bwd_kernel launch"))) return rc;
+  {
+    const int64_t rows = a.B * a.Nq;
+    const int rows_per_block = 256;
+    const int64_t blocks = (rows + rows_per_block - 1) / rows_per_block;
+    attn_dq_convert_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(
+        g.dq_accum, p.KT, reinterpret_cast<bf16*>(g.dq), g.dq_colsum, rows, a.Nq, cols, g.lddq, g.bsdq,
+        rows_per_block);
+    rc = check_cuda(cudaGetLastError(), "attn_dq_convert_kernel launch");
+  }
+  return rc;
 }
 
 }  // namespace bv

@@ -520,7 +520,7 @@ int launch_patchify(const float* img, void* out, int64_t n, int H, int W, int C,
   }
   const int Kp = (P * P * C + 7) / 8 * 8;
   const int64_t total = n * (H / P) * (W / P) * (Kp / 8);
-  patchify_kernel<<<grid_for(total, 256, 148 * 16), 256, 0, s>>>(img, reinterpret_cast<bf16*>(out),
+  patchify_kernel<<<grid_for(total, 256, num_sms() * 16), 256, 0, s>>>(img, reinterpret_cast<bf16*>(out),
                                                                 n, H, W, C, P, Kp);
   return check_launch("patchify_kernel");
 }
@@ -546,20 +546,20 @@ int launch_patchify_u8(const uint8_t* img, void* out, int64_t n, int H, int W, i
 int launch_embed_fwd(const int32_t* ids, const float* table, const float* pos, void* out,
                      int out_dtype, int64_t n, int L, int d, int vocab, cudaStream_t s) {
   if (d % 4) { set_error("bv_embed_fwd: d %% 4 != 0"); return BV_ERR_INVALID; }
-  embed_fwd_kernel<<<grid_for(n * L * (d / 4), 256, 148 * 16), 256, 0, s>>>(ids, table, pos, out,
+  embed_fwd_kernel<<<grid_for(n * L * (d / 4), 256, num_sms() * 16), 256, 0, s>>>(ids, table, pos, out,
                                                                          out_dtype, n, L, d, vocab);
   return check_launch("embed_fwd_kernel");
 }
 int launch_embed_bwd(const int32_t* ids, const void* dy, int dy_dtype, float* dtable, float* dpos,
                      int64_t n, int L, int d, int vocab, cudaStream_t s) {
   if (dtable) {
-    embed_bwd_table_kernel<<<grid_for(n * L * d, 256, 148 * 16), 256, 0, s>>>(ids, dy, dy_dtype,
+    embed_bwd_table_kernel<<<grid_for(n * L * d, 256, num_sms() * 16), 256, 0, s>>>(ids, dy, dy_dtype,
                                                                            dtable, n, L, d, vocab);
     int rc = check_launch("embed_bwd_table_kernel");
     if (rc) return rc;
   }
   if (dpos) {
-    embed_bwd_pos_kernel<<<grid_for(static_cast<int64_t>(L) * d, 128, 148 * 16), 128, 0, s>>>(
+    embed_bwd_pos_kernel<<<grid_for(static_cast<int64_t>(L) * d, 128, num_sms() * 16), 128, 0, s>>>(
         dy, dy_dtype, dpos, n, L, d);
     return check_launch("embed_bwd_pos_kernel");
   }
@@ -581,7 +581,7 @@ int launch_colsum(const void* x, int x_dtype, float* out, int64_t rows, int64_t 
 
 int launch_cast(const void* src, int sdt, void* dst, int ddt, int64_t n, cudaStream_t s) {
   if (n <= 0) return BV_OK;
-  cast_kernel<<<grid_for(n / 4 + 1, 256, 148 * 16), 256, 0, s>>>(src, sdt, dst, ddt, n);
+  cast_kernel<<<grid_for(n / 4 + 1, 256, num_sms() * 16), 256, 0, s>>>(src, sdt, dst, ddt, n);
   return check_launch("cast_kernel");
 }
 
@@ -602,45 +602,45 @@ int launch_pool(const void* x, int xdt, void* y, int ydt, int64_t n, int N, int 
                 int tok, cudaStream_t s) {
   if (mode < 0 || mode > 2) { set_error("bv_pool: mode must be 0 (mean), 1 (token) or 2 (max)"); return BV_ERR_INVALID; }
   if (mode == 1 && (tok < 0 || tok >= N)) { set_error("bv_pool: token index out of range"); return BV_ERR_INVALID; }
-  pool_fwd_kernel<<<grid_for(n * d, 256, 148 * 16), 256, 0, s>>>(x, xdt, y, ydt, n, N, d, mode, tok);
+  pool_fwd_kernel<<<grid_for(n * d, 256, num_sms() * 16), 256, 0, s>>>(x, xdt, y, ydt, n, N, d, mode, tok);
   return check_launch("pool_fwd_kernel");
 }
 int launch_pool_bwd(const void* dy, int ydt, void* dx, int xdt, int64_t n, int N, int d, int mode,
                     int tok, cudaStream_t s) {
   if (mode == 2) { set_error("bv_pool_bwd: the max pool needs its input, use bv_pool_max_bwd"); return BV_ERR_INVALID; }
   if (mode != 0 && (tok < 0 || tok >= N)) { set_error("bv_pool_bwd: token index out of range"); return BV_ERR_INVALID; }
-  pool_bwd_kernel<<<grid_for(n * N * d, 256, 148 * 16), 256, 0, s>>>(dy, ydt, dx, xdt, n, N, d, mode, tok);
+  pool_bwd_kernel<<<grid_for(n * N * d, 256, num_sms() * 16), 256, 0, s>>>(dy, ydt, dx, xdt, n, N, d, mode, tok);
   return check_launch("pool_bwd_kernel");
 }
 int launch_pool_max_bwd(const void* dy, int ydt, const void* x, int xdt, void* dx, int dxdt, int64_t n,
                         int N, int d, cudaStream_t s) {
   if (n <= 0 || N <= 0 || d <= 0) { set_error("bv_pool_max_bwd: empty problem"); return BV_ERR_INVALID; }
-  pool_max_bwd_kernel<<<grid_for(n * d, 256, 148 * 16), 256, 0, s>>>(dy, ydt, x, xdt, dx, dxdt, n, N, d);
+  pool_max_bwd_kernel<<<grid_for(n * d, 256, num_sms() * 16), 256, 0, s>>>(dy, ydt, x, xdt, dx, dxdt, n, N, d);
   return check_launch("pool_max_bwd_kernel");
 }
 
 int launch_add_rows(const void* x, int xdt, const float* row, void* y, int ydt, int64_t rows,
                     int d, cudaStream_t s) {
   // x holds a single row that is broadcast to `rows` rows (src_rows = 1)
-  add_rows_kernel<<<grid_for(rows * d, 256, 148 * 16), 256, 0, s>>>(x, xdt, row, y, ydt, rows, d, 1);
+  add_rows_kernel<<<grid_for(rows * d, 256, num_sms() * 16), 256, 0, s>>>(x, xdt, row, y, ydt, rows, d, 1);
   return check_launch("add_rows_kernel");
 }
 
 int launch_tanh_fwd(const void* x, void* y, int dt, int64_t n, cudaStream_t s) {
-  map_kernel<MAP_TANH><<<grid_for(n, 256, 148 * 16), 256, 0, s>>>(x, nullptr, y, dt, 0.f, 0.f, n);
+  map_kernel<MAP_TANH><<<grid_for(n, 256, num_sms() * 16), 256, 0, s>>>(x, nullptr, y, dt, 0.f, 0.f, n);
   return check_launch("tanh_fwd");
 }
 int launch_tanh_bwd(const void* dy, const void* y, void* dx, int dt, int64_t n, cudaStream_t s) {
-  map_kernel<MAP_TANH_BWD><<<grid_for(n, 256, 148 * 16), 256, 0, s>>>(dy, y, dx, dt, 0.f, 0.f, n);
+  map_kernel<MAP_TANH_BWD><<<grid_for(n, 256, num_sms() * 16), 256, 0, s>>>(dy, y, dx, dt, 0.f, 0.f, n);
   return check_launch("tanh_bwd");
 }
 int launch_gelu_fwd(const void* x, void* y, int dt, int64_t n, cudaStream_t s) {
-  map_kernel<MAP_GELU><<<grid_for(n, 256, 148 * 16), 256, 0, s>>>(x, nullptr, y, dt, 0.f, 0.f, n);
+  map_kernel<MAP_GELU><<<grid_for(n, 256, num_sms() * 16), 256, 0, s>>>(x, nullptr, y, dt, 0.f, 0.f, n);
   return check_launch("gelu_fwd");
 }
 int launch_axpby(const void* x, const void* y, void* out, int dt, float a, float b, int64_t n,
                  cudaStream_t s) {
-  map_kernel<MAP_AXPBY><<<grid_for(n, 256, 148 * 16), 256, 0, s>>>(x, y, out, dt, a, b, n);
+  map_kernel<MAP_AXPBY><<<grid_for(n, 256, num_sms() * 16), 256, 0, s>>>(x, y, out, dt, a, b, n);
   return check_launch("axpby");
 }
 int launch_transpose_tokens(const void* x, void* y, int64_t n, int N, int d, cudaStream_t s) {
@@ -676,13 +676,13 @@ int launch_row_select(const void* a, const void* b, const float* mask, void* out
 int launch_concat_cls(const void* x, const float* cls, void* out, int64_t n, int N0, int d,
                       cudaStream_t s) {
   if (d % 8) { set_error("bv_concat_cls: d %% 8 != 0"); return BV_ERR_INVALID; }
-  concat_cls_kernel<<<grid_for(n * (N0 + 1) * (d / 8), 256, 148 * 16), 256, 0, s>>>(
+  concat_cls_kernel<<<grid_for(n * (N0 + 1) * (d / 8), 256, num_sms() * 16), 256, 0, s>>>(
       reinterpret_cast<const bf16*>(x), cls, reinterpret_cast<bf16*>(out), n, N0, d);
   return check_launch("concat_cls_kernel");
 }
 int launch_drop_cls(const void* x, void* out, int64_t n, int N0, int d, cudaStream_t s) {
   if (d % 8) { set_error("bv_drop_cls: d %% 8 != 0"); return BV_ERR_INVALID; }
-  drop_cls_kernel<<<grid_for(n * N0 * (d / 8), 256, 148 * 16), 256, 0, s>>>(
+  drop_cls_kernel<<<grid_for(n * N0 * (d / 8), 256, num_sms() * 16), 256, 0, s>>>(
       reinterpret_cast<const bf16*>(x), reinterpret_cast<bf16*>(out), n, N0, d);
   return check_launch("drop_cls_kernel");
 }

@@ -1,27 +1,22 @@
-// Persistent warp-specialised tcgen05 GEMM for sm_100a.
+// Warp-specialised wgmma GEMM for sm_90a.
 //
 //   D[M,N] = epilogue( alpha * sum_k A(m,k) * B(n,k) )
 //
 // A and B are bf16 and each may be stored K-major (rows = M/N, K contiguous) or
 // MN-major (rows = K, M/N contiguous); both go HBM -> smem by TMA (128B swizzle)
-// and smem -> tensor core by UMMA descriptors, accumulating fp32 in TMEM.  This
-// one kernel serves every dense contraction of the hot path:
+// and smem -> tensor core by wgmma descriptors (the transpose bits select the
+// major-ness), accumulating fp32 in registers.  This one kernel serves every dense
+// contraction of the hot path:
 //   forward  Y  = X  W      A = X  (K-major),  B = W  [K,N] (MN-major)    K1,K4,K6,K7,K8,K11
 //   dgrad    dX = dY W^T    A = dY (K-major),  B = W  [K,N] (K-major)
 //   wgrad    dW = X^T dY    A = X  (MN-major), B = dY (MN-major), split-K, fp32 reduce-add
 // (reference call sites: flax Dense/DenseGeneral under models/vit.py:72-77,93-98,
 //  176-178,212-214,261,272; models/mlp_mixer.py:35-37,72,82).
 //
-// CTA pair (cta_group::2): two CTAs of a cluster own one 256 x BN output tile.  Each CTA
-// TMA-loads its 128 rows of A and its BN/2 rows of B per k-block; the leader CTA issues
-// UMMA 256 x BN x 16 instructions that read both CTAs' shared memory and write each
-// CTA's 128 x BN half of the accumulator into that CTA's TMEM.  Per SM this halves the
-// shared-memory traffic of the B operand (fill + MMA read), which is what bounds the
-// single-CTA 128 x 256 tile at ~2/3 of the tensor peak.
-//
-// Roles (320 threads per CTA): warp 0 = TMA producer, warp 1 = TMEM alloc (+ MMA issue in
-// the leader), warps 2..9 = epilogue (TMEM -> regs -> swizzled smem -> TMA store / reduce).
-// Two TMEM accumulator stages so the epilogue of tile i overlaps the mainloop of i+1.
+// One CTA owns one 128 x BN output tile (x one K split).  Roles (384 threads): warpgroup 0 is the
+// TMA producer (one thread issues, the rest give their registers back with setmaxnreg), warpgroups
+// 1 and 2 each run m64 x BN x 16 wgmma on their half of the rows from a STAGES-deep ring of shared
+// memory, then apply the epilogue straight from the accumulator registers.
 #include "common.cuh"
 #include "host_utils.h"
 #include "kernels.h"
@@ -34,628 +29,279 @@ namespace bv {
 
 namespace {
 
-constexpr int BM = 128;          // rows per CTA
+constexpr int BM = 128;          // rows per CTA (two consumer warpgroups of 64)
 constexpr int BK = 64;           // 64 bf16 = 128 B = one swizzle row
-constexpr int UMMA_K = 16;
 constexpr int A_STAGE_BYTES = BM * BK * 2;   // 16 KB
-// epilogue warps: two per TMEM lane quarter, each taking one half of the tile's columns
-constexpr int EPI_PARTS = 2;
-constexpr int EPI_WARPS = 4 * EPI_PARTS;
-constexpr int NUM_THREADS = 64 + EPI_WARPS * 32;
+constexpr int NUM_THREADS = 384;
 
 // epilogue families (template parameter)
 enum : int { EF_BIAS = 0, EF_GELU = 1, EF_RESID = 2, EF_DGELU = 3 };
 
-// Epilogue staging: every epilogue warp owns private 4 KB slabs (32 rows x 128 B, 128B-swizzled)
-// and issues its own TMA loads / stores on them, so the eight warps never synchronise with each
-// other.  Slabs per warp: 1 (plain), 2 (gelu: activation + pre-activation), 3 (ring of the
-// residual / gelu' operand, which is overwritten in place by the result and stored from there).
-constexpr int SLAB_BYTES = 32 * 128;
-
-template <int BN, int CTAS, bool DUAL_OUT, bool AUX_TMA>
+template <int BN>
 struct Cfg {
-  static constexpr int B_ROWS = BN / CTAS;                 // rows of B this CTA loads
-  static constexpr int B_STAGE_BYTES = B_ROWS * BK * 2;
+  static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int SLABS = AUX_TMA ? 3 : (DUAL_OUT ? 2 : 1);
-  static constexpr int EPI_BYTES = EPI_WARPS * SLABS * SLAB_BYTES;
-  static constexpr int SMEM_LIMIT = 232448 - 1536;         // 227 KB minus barriers / align slack
-  static constexpr int STAGES_FIT = (SMEM_LIMIT - EPI_BYTES) / STAGE_BYTES;
+  static constexpr int SMEM_LIMIT = 232448 - 2048;         // 227 KB minus barriers / align slack
+  static constexpr int STAGES_FIT = SMEM_LIMIT / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
-  static constexpr int TMEM_COLS = 2 * BN;                 // 512 or 256 (power of two)
-  static constexpr int EPI_OFFSET = STAGES * STAGE_BYTES;
-  static constexpr int BAR_OFFSET = EPI_OFFSET + EPI_BYTES;
-  static constexpr int SMEM_BYTES = BAR_OFFSET + 512 + 1024;  // + barriers + align slack
-};
-
-// (n tile, m tile, k split) of a persistent CTA's current tile, advanced without divisions
-struct TileIter {
-  int n_tile, m_tile, split;
-  int dn, dm, ds, nn, nm;
-  __device__ __forceinline__ void init(int t0, int step, int num_n, int num_m) {
-    nn = num_n; nm = num_m;
-    n_tile = t0 % nn; int r = t0 / nn; m_tile = r % nm; split = r / nm;
-    dn = step % nn; r = step / nn; dm = r % nm; ds = r / nm;
-  }
-  __device__ __forceinline__ void next() {
-    n_tile += dn;
-    int c = n_tile >= nn ? 1 : 0;
-    n_tile -= c ? nn : 0;
-    m_tile += dm + c;
-    c = m_tile >= nm ? 1 : 0;
-    m_tile -= c ? nm : 0;
-    split += ds + c;
-  }
+  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int SMEM_BYTES = BAR_OFFSET + 256 + 1024;  // + barriers + align slack
 };
 
 struct GemmDev {
   int M, N, K;
-  int num_m_tiles, num_n_tiles, total_tiles;   // m tiles count CTA-pair tiles when CTAS == 2
   int kblocks_total, kblocks_per_split;
   int a_mn, b_mn;        // 1 = MN-major
-  int reduce_out;        // 1 = TMA reduce-add into D (split-K / grad accumulation)
+  int reduce_out;        // 1 = atomic add into D (split-K / grad accumulation)
   float alpha;
   const float* bias;
   const bf16* aux;
+  void* d; void* d2;
+  long long ldd, ldd2, ldaux;
   float* colsum;         // optional bias-gradient accumulator (bf16 outputs only)
-  long long* dbg;        // optional per-tile timeline of CTA 0 (BV_GEMM_DBG=1)
-  long long ldaux;
   int aux_row_mod;
 };
 
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_cta(uint32_t addr, uint32_t cta) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(cta));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  // default (.release.cta) semantics, as CUTLASS' ClusterBarrier::arrive(cta_id): the explicit
-  // .release.cluster form costs a MEMBAR.ALL + ERRBAR per arrival (6% of the gelu GEMM's samples)
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load whose completion may be signalled on the CTA-pair leader's mbarrier.
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* m, uint32_t bar,
-                                                 int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ss_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                                  uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(bar), "h"(static_cast<uint16_t>(3)) : "memory");
+// The consumer warpgroup's main loop.  The transpose bits of wgmma are immediates, so each operand
+// layout pair is its own instantiation (a branch between wgmma issues would make ptxas serialise them).
+template <int BN, int STAGES, int STAGE_BYTES, int TA, int TB>
+__device__ __forceinline__ void mainloop(float (&acc)[BN / 2], uint32_t base, uint32_t bar_base, int cw, int kb0,
+                                         int kb1) {
+  // 128B-swizzled operand tiles: K-major rows of 128 B (8-row groups 1024 B apart, K step 32 B);
+  // MN-major boxes of 64 (M|N) x 64 (K), 8 KB each (K step 16 rows = 2048 B)
+  constexpr uint32_t a_lbo = TA ? 8192u : 16u, b_lbo = TB ? 8192u : 16u;
+  constexpr uint32_t a_kstep = TA ? 2048u : 32u, b_kstep = TB ? 2048u : 32u;
+  int stage = 0;
+  uint32_t phase = 0;
+  int prev_stage = -1;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(bar_base + 8u * stage, phase);
+    const uint32_t a_s = base + stage * STAGE_BYTES + cw * 8192;
+    const uint32_t b_s = base + stage * STAGE_BYTES + A_STAGE_BYTES;
+    const uint64_t adesc = wgmma_desc_sw128(a_s, a_lbo, 1024u), bdesc = wgmma_desc_sw128(b_s, b_lbo, 1024u);
+    wgmma_fence_regs(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+      const uint64_t a = adesc + k * (a_kstep >> 4), b = bdesc + k * (b_kstep >> 4);
+      const int accumulate = (kb > kb0 || k > 0) ? 1 : 0;    // the first MMA overwrites the registers
+      if constexpr (BN == 256) wgmma_ss_n256<TA, TB>(acc, a, b, accumulate);
+      else wgmma_ss_n128<TA, TB>(acc, a, b, accumulate);
+    }
+    wgmma_commit();
+    wgmma_fence_regs(acc);
+    // keep this k block's MMAs in flight; the previous one has retired -> its slot is free
+    wgmma_wait<1>();
+    if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_base + 8u * (STAGES + prev_stage));
+    prev_stage = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+  if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_base + 8u * (STAGES + prev_stage));
 }
 
-// AUXM: how the epilogue's second operand arrives: 0 none, 1 per-thread global loads (row-modulo
-// position embeddings, fp32 outputs), 2 TMA ring in shared memory (residual / gelu' operands)
-// per-tile timeline of CTA 0 (bring-up aid): dbg[tile * 16 + ev] = clock64, first 32 tiles
-#define GEMM_DBG(ev, ti)                                                        \
-  do {                                                                          \
-    if (p.dbg != nullptr && blockIdx.x == 0 && (ti) < 32)                       \
-      p.dbg[(ti) * 16 + (ev)] = clock64();                                      \
-  } while (0)
-
-template <int BN, bool OUT_F32, int EF, int CTAS, int AUXM>
+template <int BN, bool OUT_F32, int EF>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmD2,
-            const __grid_constant__ CUtensorMap tmAux, const GemmDev p) {
-  using C = Cfg<BN, CTAS, EF == EF_GELU, AUXM == 2>;
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
+  using C = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t base = (raw_addr + 1023u) & ~1023u;
-  uint8_t* base_ptr = smem_raw + (base - raw_addr);
-
-  const uint32_t epi_base = base + C::EPI_OFFSET;
   const uint32_t bar_base = base + C::BAR_OFFSET;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * C::STAGES + 4);
-  // per-warp ring of "operand tile landed" barriers (AUXM == 2): warp w, slab b
-  auto aux_full = [&](int w, int b) { return bar_base + 8u * (2 * C::STAGES + 5 + w * 3 + b); };
-  static_assert(8 * (2 * 8 + 5 + EPI_WARPS * 3) <= 512, "barrier region too small");
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(base_ptr + C::BAR_OFFSET + 8 * (2 * C::STAGES + 4));
 
-  // broadcast from lane 0 so the compiler can treat the role dispatch as warp-uniform
-  const int warp_idx = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
-  const int lane = threadIdx.x & 31;
-  const uint32_t cta_rank = (CTAS == 2) ? cluster_ctarank() : 0u;
-  const bool leader = cta_rank == 0;
+  const int wg = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 7), 0);
+  const int n0 = static_cast<int>(blockIdx.x) * BN;
+  const int m0 = static_cast<int>(blockIdx.y) * BM;
+  const int kb0 = static_cast<int>(blockIdx.z) * p.kblocks_per_split;
+  const int kb1 = min(kb0 + p.kblocks_per_split, p.kblocks_total);
 
-  if (warp_idx == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmD);
-    if (EF == EF_GELU) tma_prefetch_desc(&tmD2);
-    if (AUXM == 2) tma_prefetch_desc(&tmAux);
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int w = 0; w < EPI_WARPS; ++w)
-      for (int b = 0; b < 3; ++b) mbar_init(aux_full(w, b), 1);
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), EPI_WARPS * CTAS);   // one arrive per epilogue warp of each CTA
+      mbar_init(empty_bar(s), 2);     // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp_idx == 1) {
-    if (CTAS == 2) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;"
-                   ::"r"(tmem_slot), "r"(static_cast<uint32_t>(C::TMEM_COLS)) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      tmem_alloc(tmem_slot, C::TMEM_COLS);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  if (CTAS == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
+  __syncthreads();
 
-  const int tile_start = (CTAS == 2) ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int tile_step = (CTAS == 2) ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-
-  auto tile_coords = [&](const TileIter& it, int& m0, int& n0, int& kb0, int& kb1) {
-    m0 = it.m_tile * (BM * CTAS) + static_cast<int>(cta_rank) * BM;   // this CTA's first row
-    n0 = it.n_tile * BN;
-    kb0 = it.split * p.kblocks_per_split;
-    kb1 = min(kb0 + p.kblocks_per_split, p.kblocks_total);
-  };
-
-  if (warp_idx == 0) {
-    // ========================= TMA producer (every CTA) =========================
-    if (lane == 0) {
+  if (wg == 0) {
+    // ========================= TMA producer =========================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      TileIter it;
-      it.init(tile_start, tile_step, p.num_n_tiles, p.num_m_tiles);
-      int ti = 0;
-      for (int tile = tile_start; tile < p.total_tiles; tile += tile_step, it.next(), ++ti) {
-        int m0, n0, kb0, kb1;
-        tile_coords(it, m0, n0, kb0, kb1);
-        const int nb0 = n0 + static_cast<int>(cta_rank) * C::B_ROWS;   // this CTA's slice of B
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);
-          if (kb == kb0) GEMM_DBG(3, ti);
-          if (kb == kb1 - 1) GEMM_DBG(4, ti);
-          const uint32_t a_s = base + stage * C::STAGE_BYTES;
-          const uint32_t b_s = a_s + A_STAGE_BYTES;
-          // the pair leader's barrier collects the bytes of both CTAs
-          uint32_t fb = full_bar(stage);
-          if (CTAS == 2) {
-            if (leader) mbar_expect_tx(fb, 2 * C::STAGE_BYTES);
-            else fb = mapa_cta(fb, 0);
-          } else {
-            mbar_expect_tx(fb, C::STAGE_BYTES);
-          }
-          const int k0 = kb * BK;
-          if (p.a_mn) {
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(empty_bar(stage), phase ^ 1u);
+        const uint32_t a_s = base + stage * C::STAGE_BYTES;
+        const uint32_t b_s = a_s + A_STAGE_BYTES;
+        const uint32_t fb = full_bar(stage);
+        mbar_expect_tx(fb, C::STAGE_BYTES);
+        const int k0 = kb * BK;
+        if (p.a_mn) {
 #pragma unroll
-            for (int j = 0; j < BM / 64; ++j) {
-              if (CTAS == 2) tma_load_2d_pair(a_s + j * 8192, &tmA, fb, m0 + 64 * j, k0);
-              else tma_load_2d(a_s + j * 8192, &tmA, fb, m0 + 64 * j, k0);
-            }
-          } else {
-            if (CTAS == 2) tma_load_2d_pair(a_s, &tmA, fb, k0, m0);
-            else tma_load_2d(a_s, &tmA, fb, k0, m0);
-          }
-          if (p.b_mn) {
-#pragma unroll
-            for (int j = 0; j < C::B_ROWS / 64; ++j) {
-              if (CTAS == 2) tma_load_2d_pair(b_s + j * 8192, &tmB, fb, nb0 + 64 * j, k0);
-              else tma_load_2d(b_s + j * 8192, &tmB, fb, nb0 + 64 * j, k0);
-            }
-          } else {
-            if (CTAS == 2) tma_load_2d_pair(b_s, &tmB, fb, k0, nb0);
-            else tma_load_2d(b_s, &tmB, fb, k0, nb0);
-          }
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp_idx == 1) {
-    // ========================= MMA issuer (pair leader only) =========================
-    // The whole warp runs this loop convergently and one elected lane issues the tcgen05
-    // instructions (as CUTLASS does).  Inside a single-lane branch the compiler cannot prove the
-    // descriptors warp-uniform and builds them in vector registers with five R2UR broadcasts per
-    // MMA; convergent code keeps them on the uniform datapath.  It matters: issuing one MMA takes
-    // about as long as the 256 x BN x 16 MMA runs, so this instruction stream IS the tensor pipe's
-    // feed, and everything else it does per tile is kept to a few instructions.
-    if (leader) {
-      const uint32_t idesc = umma_idesc_bf16(BM * CTAS, BN, p.a_mn, p.b_mn);
-      const uint32_t a_lbo = p.a_mn ? 8192u : 16u, b_lbo = p.b_mn ? 8192u : 16u;
-      const uint32_t a_kstep = p.a_mn ? 2048u : 32u, b_kstep = p.b_mn ? 2048u : 32u;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      // only the k range of a tile is needed here, and that without divisions
-      const int tiles_mn = p.num_m_tiles * p.num_n_tiles;
-      int split = tile_start / tiles_mn, mn = tile_start % tiles_mn;
-      const int dsplit = tile_step / tiles_mn, dmn = tile_step % tiles_mn;
-      int ti = 0;
-      for (int tile = tile_start; tile < p.total_tiles; tile += tile_step, ++ti) {
-        const int kb0 = split * p.kblocks_per_split;
-        const int kb1 = min(kb0 + p.kblocks_per_split, p.kblocks_total);
-        mn += dmn; split += dsplit;
-        if (mn >= tiles_mn) { mn -= tiles_mn; ++split; }
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        if (lane == 0) GEMM_DBG(0, ti);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          if (kb == kb0 && lane == 0) GEMM_DBG(1, ti);
-          tc_fence_after();
-          const uint32_t a_s = base + stage * C::STAGE_BYTES;
-          const uint32_t b_s = a_s + A_STAGE_BYTES;
-          const uint64_t adesc0 = umma_smem_desc_sw128(a_s, a_lbo, 1024u);
-          const uint64_t bdesc0 = umma_smem_desc_sw128(b_s, b_lbo, 1024u);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              // stepping along K only bumps the 16-byte-granular start-address field
-              const uint64_t adesc = adesc0 + k * (a_kstep >> 4);
-              const uint64_t bdesc = bdesc0 + k * (b_kstep >> 4);
-              const uint32_t accf = (kb > kb0 || k > 0) ? 1u : 0u;
-              if (CTAS == 2) umma_bf16_ss_pair(d_tmem, adesc, bdesc, idesc, accf);
-              else umma_bf16_ss(d_tmem, adesc, bdesc, idesc, accf);
-            }
-            // smem slot free (in both CTAs) once these MMAs retire
-            if (CTAS == 2) umma_commit_pair(empty_bar(stage)); else umma_commit(empty_bar(stage));
-          }
-          __syncwarp();
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
-        }
-        // accumulator complete: wake the epilogue warps of both CTAs
-        if (elect_one()) {
-          if (CTAS == 2) umma_commit_pair(tfull_bar(acc)); else umma_commit(tfull_bar(acc));
-        }
-        __syncwarp();
-        if (lane == 0) GEMM_DBG(2, ti);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
-  } else {
-    // ========================= epilogue (8 independent warps, every CTA) =========================
-    // Warp (quarter q, half h) owns rows 32q..32q+31 (its TMEM lanes) x columns [h*BN/2, (h+1)*BN/2)
-    // of the tile, processed in chunks of one 128-byte row (64 bf16 / 32 fp32 columns).  Each chunk:
-    // tcgen05.ld (the next chunk's load is already in flight) -> math in registers -> swizzled
-    // store into the warp's own slab -> TMA store by lane 0.  No CTA-wide barriers: the warps drift
-    // apart and overlap each other's TMEM / MUFU / FMA / shared-memory phases.
-    const int ew = warp_idx - 2;                    // 0..7
-    const int quarter = warp_idx & 3;               // TMEM lanes this warp may access
-    const int half = ew >> 2;                       // which half of the tile's columns
-    const uint32_t sw = static_cast<uint32_t>(lane & 7);
-    constexpr bool DUAL = (EF == EF_GELU);
-    constexpr int CH = OUT_F32 ? 32 : 64;           // columns per chunk (one 128-byte row)
-    constexpr int WCOLS = BN / EPI_PARTS;           // columns per warp
-    constexpr int NCH = WCOLS / CH;                 // chunks per warp per tile
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    // kernel parameters used per element are copied to registers once (constant-bank reads inside
-    // the unrolled column loop would put an LDCU round trip on every group's dependency chain)
-    const int pM = pin_reg(p.M), pN = pin_reg(p.N), p_mod = pin_reg(p.aux_row_mod),
-              p_reduce = pin_reg(p.reduce_out);
-    const float p_alpha = pin_reg(p.alpha);
-    const float* __restrict__ p_bias = pin_reg(p.bias);
-    const bf16* __restrict__ p_aux = pin_reg(p.aux);
-    float* __restrict__ p_colsum = pin_reg(p.colsum);
-    const long long p_ldaux = p.ldaux;
-    const bool unit_alpha = (p_alpha == 1.0f);
-    constexpr bool HAS_AUX = (EF == EF_RESID || EF == EF_DGELU);
-    static_assert(!(AUXM == 2) || (HAS_AUX && !OUT_F32), "TMA aux ring is for bf16 residual/gelu' tiles");
-    static_assert(HAS_AUX == (AUXM != 0), "aux mode must match the epilogue family");
-    const uint32_t slab0 = epi_base + static_cast<uint32_t>(ew) * (C::SLABS * SLAB_BYTES);
-    const uint32_t my_row = static_cast<uint32_t>(lane) * 128u;
-
-    TileIter it;
-    it.init(tile_start, tile_step, p.num_n_tiles, p.num_m_tiles);
-    // --- AUXM == 2: lane 0 keeps the operand box of the NEXT chunk in flight (ring of 3 slabs)
-    uint32_t aux_q = 0;                    // chunks consumed so far by this warp
-    TileIter it_nx = it;                   // tile of chunk aux_q + 1
-    int c_nx = 0, tile_nx = tile_start;
-    auto aux_issue_next = [&]() {          // lane 0: load the box of chunk (tile_nx, c_nx) into slab (aux_q+1)%3
-      if (tile_nx >= p.total_tiles) return;
-      int m0, n0, kb0, kb1;
-      tile_coords(it_nx, m0, n0, kb0, kb1);
-      const uint32_t b = (aux_q + 1u) % 3u;
-      mbar_expect_tx(aux_full(ew, b), SLAB_BYTES);
-      tma_load_2d(slab0 + b * SLAB_BYTES, &tmAux, aux_full(ew, b), n0 + half * WCOLS + c_nx * CH,
-                  m0 + quarter * 32);
-    };
-    auto aux_advance = [&]() {             // move (tile_nx, c_nx) one chunk forward
-      if (++c_nx == NCH) { c_nx = 0; tile_nx += tile_step; it_nx.next(); }
-    };
-    if (AUXM == 2 && lane == 0) {
-      // chunk 0 goes to slab 0: same code path with aux_q "= -1"
-      int m0, n0, kb0, kb1;
-      tile_coords(it_nx, m0, n0, kb0, kb1);
-      if (tile_nx < p.total_tiles) {
-        mbar_expect_tx(aux_full(ew, 0), SLAB_BYTES);
-        tma_load_2d(slab0, &tmAux, aux_full(ew, 0), n0 + half * WCOLS, m0 + quarter * 32);
-      }
-    }
-    if (AUXM == 2) aux_advance();
-
-    int ti = 0;
-    for (int tile = tile_start; tile < p.total_tiles; tile += tile_step, it.next(), ++ti) {
-      int m0, n0, kb0, kb1;
-      tile_coords(it, m0, n0, kb0, kb1);
-      const int grow0 = m0 + quarter * 32;          // first row of this warp's boxes
-      const int grow = grow0 + lane;
-      const bool row_ok = grow < pM;
-      const int wcol0 = n0 + half * WCOLS;          // first column of this warp
-      const bf16* aux_row = nullptr;                // AUXM == 1: this thread's row of the operand
-      if (AUXM == 1 && row_ok) {
-        const long long ar = p_mod > 0 ? (grow % p_mod) : grow;
-        aux_row = p_aux + ar * p_ldaux;
-      }
-      if (ew == 0 && lane == 0) GEMM_DBG(8, ti);
-      mbar_wait(tfull_bar(acc), acc_phase);
-      if (ew == 0 && lane == 0) GEMM_DBG(5, ti);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN + half * WCOLS;
-
-      // TMEM is read in units of 32 columns, double-buffered in registers: unit u+1 is in flight
-      // while unit u is processed
-      constexpr int UPC = CH / 32;                  // units per chunk (2 for bf16, 1 for fp32)
-      constexpr int NU = NCH * UPC;                 // units per tile
-      constexpr int GPU_ = 4;                       // 8-column groups per unit
-      uint32_t rbuf[2][32];
-      tmem_ld_32x32b_x32(t_row, rbuf[0]);
-      uint32_t slab = slab0;
-#pragma unroll
-      for (int u = 0; u < NU; ++u) {
-        const int c = u / UPC, uc = u % UPC;        // chunk, unit within the chunk
-        uint32_t (&r)[32] = rbuf[u & 1];
-        const int ncol0 = wcol0 + c * CH;           // first column of the chunk
-        // AUXM == 1: fetch this unit's operand before blocking on the accumulator
-        uint4 aq[(AUXM == 1) ? GPU_ : 1];
-        if (AUXM == 1) {
-#pragma unroll
-          for (int g = 0; g < GPU_; ++g) {
-            const int nc = ncol0 + uc * 32 + g * 8;
-            aq[g] = make_uint4(0u, 0u, 0u, 0u);
-            if (aux_row != nullptr && nc < pN) aq[g] = *reinterpret_cast<const uint4*>(aux_row + nc);
-          }
-        }
-        tmem_ld_wait();
-        if (u + 1 < NU) {
-          tmem_ld_32x32b_x32(t_row + (u + 1) * 32, rbuf[(u + 1) & 1]);
+          for (int j = 0; j < BM / 64; ++j) tma_load_2d(a_s + j * 8192, &tmA, fb, m0 + 64 * j, k0);
         } else {
-          // accumulator fully drained into registers -> hand TMEM back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if (CTAS == 2 && !leader) mbar_arrive_cluster(mapa_cta(tempty_bar(acc), 0));
-            else mbar_arrive(tempty_bar(acc));
-          }
-          if (ew == 0 && lane == 0) GEMM_DBG(6, ti);
+          tma_load_2d(a_s, &tmA, fb, k0, m0);
         }
-        if (uc == 0 && AUXM == 2) {
-          // chunk start: which slab holds this chunk's operand (the result overwrites it in place)
-          if (lane == 0) {
-            // slab (aux_q+1)%3 was last stored from two chunks ago: allow only the newest store
-            // to be still reading, then refill it with the next chunk's operand
-            tma_store_wait_read<1>();
-            aux_issue_next();
-          }
-          aux_advance();
-          slab = slab0 + (aux_q % 3u) * SLAB_BYTES;
-          mbar_wait(aux_full(ew, aux_q % 3u), (aux_q / 3u) & 1u);
-          ++aux_q;
+        if (p.b_mn) {
+#pragma unroll
+          for (int j = 0; j < BN / 64; ++j) tma_load_2d(b_s + j * 8192, &tmB, fb, n0 + 64 * j, k0);
+        } else {
+          tma_load_2d(b_s, &tmB, fb, k0, n0);
         }
-        uint32_t ow[DUAL ? 2 : 1][OUT_F32 ? 32 : 16];   // packed results of this unit
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
+      }
+    }
+    return;
+  }
+
+  // ========================= consumers: warpgroups 1, 2 =========================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int cw = wg - 1;                        // which 64-row half of the tile
+  float acc[BN / 2];
+  constexpr int S = C::STAGES, SB = C::STAGE_BYTES;
+  if (p.a_mn) {
+    if (p.b_mn) mainloop<BN, S, SB, 1, 1>(acc, base, bar_base, cw, kb0, kb1);
+    else mainloop<BN, S, SB, 1, 0>(acc, base, bar_base, cw, kb0, kb1);
+  } else {
+    if (p.b_mn) mainloop<BN, S, SB, 0, 1>(acc, base, bar_base, cw, kb0, kb1);
+    else mainloop<BN, S, SB, 0, 0>(acc, base, bar_base, cw, kb0, kb1);
+  }
+
+  // ========================= epilogue from registers =========================
+  // Accumulator layout (per warp w of the warpgroup, lane l): element 4j + e sits at row
+  // 16w + l/4 + 8*(e >> 1), column 8j + 2*(l%4) + (e & 1).
+  const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
+  const int row0 = m0 + cw * 64 + warp * 16 + (lane >> 2);
+  const int pM = p.M, pN = p.N;
+  const float alpha = p.alpha;
+  const bool reduce = p.reduce_out != 0;
+  constexpr bool HAS_AUX = (EF == EF_RESID || EF == EF_DGELU);
+  float cs[BN / 8][2];
 #pragma unroll
-        for (int g = 0; g < GPU_; ++g) {    // 8 columns per group
-          const int nc = ncol0 + uc * 32 + g * 8;
-          float v[8];
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = n0 + 8 * j + 2 * (lane & 3);
+    cs[j][0] = cs[j][1] = 0.f;
+    if (col >= pN) continue;
+    const bool pair = col + 1 < pN;
+    float b0 = 0.f, b1 = 0.f;
+    if (p.bias != nullptr) {
+      b0 = __ldg(p.bias + col);
+      if (pair) b1 = __ldg(p.bias + col + 1);
+    }
 #pragma unroll
-          for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[g * 8 + i]);
-          if (!unit_alpha) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] *= p_alpha;
-          }
-          const bool col_ok = nc < pN;
-          if (p_bias != nullptr && col_ok) {
-            const float4 b0 = __ldg(reinterpret_cast<const float4*>(p_bias + nc));
-            const float4 b1 = __ldg(reinterpret_cast<const float4*>(p_bias + nc + 4));
-            v[0] += b0.x; v[1] += b0.y; v[2] += b0.z; v[3] += b0.w;
-            v[4] += b1.x; v[5] += b1.y; v[6] += b1.z; v[7] += b1.w;
-          }
-          float v2[8];
-          if (EF == EF_GELU) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              v2[i] = round_bf16(v[i]);
-              v[i] = gelu_tanh_fast(v2[i]);
-            }
-          } else if (EF == EF_RESID || EF == EF_DGELU) {
-            uint4 q;
-            if (AUXM == 2) {
-              const uint32_t piece = static_cast<uint32_t>(uc * 4 + g);
-              asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
-                           : "=r"(q.x), "=r"(q.y), "=r"(q.z), "=r"(q.w)
-                           : "r"(slab + my_row + ((piece ^ sw) << 4)));
-            } else {
-              q = aq[(AUXM == 1) ? g : 0];
-            }
-            const float a[8] = {bf16_lo(q.x), bf16_hi(q.x), bf16_lo(q.y), bf16_hi(q.y),
-                                bf16_lo(q.z), bf16_hi(q.z), bf16_lo(q.w), bf16_hi(q.w)};
-            if (EF == EF_RESID) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) v[i] = (OUT_F32 ? v[i] : round_bf16(v[i])) + a[i];
-            } else {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) v[i] *= gelu_tanh_grad_fast(a[i]);
-            }
-          }
-          if (OUT_F32) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) ow[0][(OUT_F32 ? g * 8 : 0) + i] = __float_as_uint(v[i]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) ow[0][g * 4 + i] = pack_bf16(v[2 * i], v[2 * i + 1]);
-            if (DUAL) {
-#pragma unroll
-              for (int i = 0; i < 4; ++i) ow[DUAL ? 1 : 0][g * 4 + i] = pack_bf16(v2[2 * i], v2[2 * i + 1]);
-            }
-          }
-        }
-        // the slab must have been read by the TMA store of the previous chunk (the math above has
-        // given it time); the AUXM == 2 ring was already checked when its operand was requested
-        if (uc == 0 && AUXM != 2) {
-          if (lane == 0) tma_store_wait_read<0>();
-          __syncwarp();
-        }
-        constexpr int PIECES = OUT_F32 ? 8 : 4;     // 16-byte pieces this unit contributes to the row
-#pragma unroll
-        for (int j = 0; j < PIECES; ++j) {
-          const uint32_t piece = static_cast<uint32_t>(uc * PIECES + j);
-          const uint32_t a0 = slab + my_row + ((piece ^ sw) << 4);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a0), "r"(ow[0][j * 4]),
-                       "r"(ow[0][j * 4 + 1]), "r"(ow[0][j * 4 + 2]), "r"(ow[0][j * 4 + 3]) : "memory");
-          if (DUAL) {
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a0 + SLAB_BYTES),
-                         "r"(ow[DUAL ? 1 : 0][j * 4]), "r"(ow[DUAL ? 1 : 0][j * 4 + 1]),
-                         "r"(ow[DUAL ? 1 : 0][j * 4 + 2]), "r"(ow[DUAL ? 1 : 0][j * 4 + 3]) : "memory");
-          }
-        }
-        if (uc == UPC - 1) {
-          // chunk complete: publish the slab to the async proxy and store it
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) {
-            if (ncol0 < pN) {
-              if (p_reduce) tma_reduce_add_2d(&tmD, slab, ncol0, grow0);
-              else tma_store_2d(&tmD, slab, ncol0, grow0);
-              if (DUAL) tma_store_2d(&tmD2, slab + SLAB_BYTES, ncol0, grow0);
-            }
-            tma_store_commit();
-            if (ew == 0 && u == NU - 1) GEMM_DBG(7, ti);
-          }
-          if (!OUT_F32 && p_colsum != nullptr) {
-            // bias gradient fused into the producer: column sums of the staged (bf16-rounded) slab.
-            // Lane l sums the column pair (2l, 2l+1) over the warp's 32 rows: every load is one
-            // conflict-free 128-byte row and all 32 are independent.  Rows past M hold exact zeros.
-            const uint32_t cp = static_cast<uint32_t>(lane);
-            const uint32_t cbase = slab + (cp & 3) * 4;
-            float s0[2] = {0.f, 0.f}, s1[2] = {0.f, 0.f};
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              uint32_t w;
-              asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w)
-                           : "r"(cbase + i * 128 + (((cp >> 2) ^ static_cast<uint32_t>(i & 7)) << 4)));
-              s0[i & 1] += bf16_lo(w);
-              s1[i & 1] += bf16_hi(w);
-            }
-            const int ncol = ncol0 + 2 * lane;
-            if (ncol < pN) atomicAdd(p_colsum + ncol, s0[0] + s0[1]);
-            if (ncol + 1 < pN) atomicAdd(p_colsum + ncol + 1, s1[0] + s1[1]);
-          }
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 8 * h;
+      if (row >= pM) continue;
+      float v0 = acc[4 * j + 2 * h] * alpha + b0, v1 = acc[4 * j + 2 * h + 1] * alpha + b1;
+      float a0 = 0.f, a1 = 0.f;
+      if (HAS_AUX) {
+        const long long ar = p.aux_row_mod > 0 ? (row % p.aux_row_mod) : row;
+        const bf16* ap = p.aux + ar * p.ldaux + col;
+        if (pair) {
+          const uint32_t q = *reinterpret_cast<const uint32_t*>(ap);
+          a0 = bf16_lo(q); a1 = bf16_hi(q);
+        } else {
+          a0 = __bfloat162float(*ap);
         }
       }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
+      float pre0 = 0.f, pre1 = 0.f;
+      if (EF == EF_GELU) {
+        pre0 = round_bf16(v0); pre1 = round_bf16(v1);
+        v0 = gelu_tanh_fast(pre0); v1 = gelu_tanh_fast(pre1);
+      } else if (EF == EF_RESID) {
+        v0 = (OUT_F32 ? v0 : round_bf16(v0)) + a0;
+        v1 = (OUT_F32 ? v1 : round_bf16(v1)) + a1;
+      } else if (EF == EF_DGELU) {
+        v0 *= gelu_tanh_grad_fast(a0);
+        v1 *= gelu_tanh_grad_fast(a1);
+      }
+      if (OUT_F32) {
+        float* dp = static_cast<float*>(p.d) + row * p.ldd + col;
+        if (reduce) {
+          atomicAdd(dp, v0);
+          if (pair) atomicAdd(dp + 1, v1);
+        } else if (pair) {
+          *reinterpret_cast<float2*>(dp) = make_float2(v0, v1);
+        } else {
+          *dp = v0;
+        }
+      } else {
+        bf16* dp = static_cast<bf16*>(p.d) + row * p.ldd + col;
+        const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
+        if (reduce) {
+          if (pair) atomicAdd(reinterpret_cast<__nv_bfloat162*>(dp), o);
+          else atomicAdd(dp, o.x);
+        } else if (pair) {
+          *reinterpret_cast<__nv_bfloat162*>(dp) = o;
+        } else {
+          *dp = o.x;
+        }
+        cs[j][0] += __low2float(o);
+        cs[j][1] += pair ? __high2float(o) : 0.f;
+        if (EF == EF_GELU) {
+          bf16* d2 = static_cast<bf16*>(p.d2) + row * p.ldd2 + col;
+          const __nv_bfloat162 q = __floats2bfloat162_rn(pre0, pre1);
+          if (pair) *reinterpret_cast<__nv_bfloat162*>(d2) = q;
+          else *d2 = q.x;
+        }
+      }
     }
-    if (lane == 0) tma_store_wait<0>();
   }
-
-  __syncwarp();
-  tc_fence_before();
-  if (CTAS == 2) cluster_sync_all(); else __syncthreads();
-  if (warp_idx == 1) {
-    __syncwarp();
-    tc_fence_after();
-    if (CTAS == 2) {
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;"
-                   ::"r"(tmem_base), "r"(static_cast<uint32_t>(C::TMEM_COLS)) : "memory");
-    } else {
-      tmem_dealloc(tmem_base, C::TMEM_COLS);
+  if (!OUT_F32 && p.colsum != nullptr) {
+    // bias gradient fused into the producer: column sums of the stored (bf16-rounded) values; the
+    // eight lanes that share a column pair are summed with shuffles, then one atomic per warp
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float s = cs[j][e];
+        s += __shfl_xor_sync(0xffffffffu, s, 4);
+        s += __shfl_xor_sync(0xffffffffu, s, 8);
+        s += __shfl_xor_sync(0xffffffffu, s, 16);
+        cs[j][e] = s;
+      }
+      const int col = n0 + 8 * j + 2 * (lane & 3);
+      if (lane < 4) {
+        if (col < pN) atomicAdd(p.colsum + col, cs[j][0]);
+        if (col + 1 < pN) atomicAdd(p.colsum + col + 1, cs[j][1]);
+      }
     }
   }
 }
 
-static long long* g_gemm_dbg = nullptr;
-long long* gemm_debug_buffer() {
-  static const bool on = [] { const char* e = getenv("BV_GEMM_DBG"); return e && e[0] == '1'; }();
-  if (!on) return nullptr;
-  if (g_gemm_dbg == nullptr && cudaMalloc(&g_gemm_dbg, 32 * 16 * sizeof(long long)) != cudaSuccess) return nullptr;
-  cudaMemset(g_gemm_dbg, 0, 32 * 16 * sizeof(long long));
-  return g_gemm_dbg;
-}
-
-template <int BN, bool OUT_F32, int EF, int CTAS, int AUXM>
+template <int BN, bool OUT_F32, int EF>
 int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
-  using C = Cfg<BN, CTAS, EF == EF_GELU, AUXM == 2>;
-  CUtensorMap tmA, tmB, tmD, tmD2, tmAux;
+  using C = Cfg<BN>;
+  CUtensorMap tmA, tmB;
   int rc;
   const CUtensorMapDataType bf = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   if (g.a_mn) rc = make_tmap_2d(&tmA, bf, g.A, g.M, g.K, g.lda * 2, 64, 64);
   else        rc = make_tmap_2d(&tmA, bf, g.A, g.K, g.M, g.lda * 2, 64, BM);
   if (rc) return rc;
   if (g.b_mn) rc = make_tmap_2d(&tmB, bf, g.B, g.N, g.K, g.ldb * 2, 64, 64);
-  else        rc = make_tmap_2d(&tmB, bf, g.B, g.K, g.N, g.ldb * 2, 64, C::B_ROWS);
+  else        rc = make_tmap_2d(&tmB, bf, g.B, g.K, g.N, g.ldb * 2, 64, BN);
   if (rc) return rc;
-  // epilogue boxes: one warp's 32 rows x one 128-byte row of columns
-  if (OUT_F32) rc = make_tmap_2d(&tmD, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, g.D, g.N, g.M, g.ldd * 4, 32, 32);
-  else         rc = make_tmap_2d(&tmD, bf, g.D, g.N, g.M, g.ldd * 2, 64, 32);
-  if (rc) return rc;
-  tmD2 = tmD;
-  tmAux = tmD;
-  if (AUXM == 2) {
-    rc = make_tmap_2d(&tmAux, bf, g.aux, g.N, g.M, g.ldaux * 2, 64, 32);
-    if (rc) return rc;
-  }
-  if (EF == EF_GELU) {
-    rc = make_tmap_2d(&tmD2, bf, g.D2, g.N, g.M, g.ldd2 * 2, 64, 32);
-    if (rc) return rc;
-  }
 
   GemmDev p;
   p.M = (int)g.M; p.N = (int)g.N; p.K = (int)g.K;
-  p.num_m_tiles = (int)((g.M + BM * CTAS - 1) / (BM * CTAS));
-  p.num_n_tiles = (int)((g.N + BN - 1) / BN);
+  const int num_m = (int)((g.M + BM - 1) / BM);
+  const int num_n = (int)((g.N + BN - 1) / BN);
   p.kblocks_total = (int)((g.K + BK - 1) / BK);
   int splits = g.splits;
-  const int sms = num_sms();
-  const int slots = sms / CTAS;          // concurrently resident tiles
   if (splits <= 0) {
     // auto (reduce-add outputs only, i.e. the weight gradients): the split count whose work units fill
-    // whole waves of the persistent grid best.  27 output tiles (768 x 2304) on 74 CTA-pair slots run
-    // at 73 % with 2 splits (54 units) and at 97 % with 8 (216 units = 2.92 waves); each extra split
-    // costs one more fp32 reduce-add of the output tile, negligible against a K of 10^5.
+    // whole waves of the grid best (one CTA per SM).  Each extra split costs one more fp32 reduce-add
+    // of the output tile, negligible against a K of 10^5.
     splits = 1;
     if (g.reduce_out) {
-      const int tiles = p.num_m_tiles * p.num_n_tiles;
+      const int slots = num_sms();
+      const int tiles = num_m * num_n;
       int smax = p.kblocks_total / 16;
       if (smax > 32) smax = 32;
       double best = -1.0;
@@ -675,17 +321,18 @@ int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
   }
   p.kblocks_per_split = (p.kblocks_total + splits - 1) / splits;
   splits = (p.kblocks_total + p.kblocks_per_split - 1) / p.kblocks_per_split;
-  p.total_tiles = p.num_m_tiles * p.num_n_tiles * splits;
+  if (splits > 65535 || num_m > 65535) { set_error("bv_gemm: grid too large"); return BV_ERR_INVALID; }
   p.a_mn = g.a_mn; p.b_mn = g.b_mn; p.reduce_out = g.reduce_out;
   p.alpha = g.alpha;
   p.bias = g.bias;
   p.colsum = g.colsum;
-  p.dbg = gemm_debug_buffer();
   p.aux = reinterpret_cast<const bf16*>(g.aux);
   p.ldaux = g.ldaux;
   p.aux_row_mod = g.aux_row_mod;
+  p.d = g.D; p.d2 = g.D2;
+  p.ldd = g.ldd; p.ldd2 = g.ldd2;
 
-  auto kern = gemm_kernel<BN, OUT_F32, EF, CTAS, AUXM>;
+  auto kern = gemm_kernel<BN, OUT_F32, EF>;
   // The dynamic-shared-memory opt-in is a per-DEVICE attribute of the kernel: cache it per device
   // (one process may drive several GPUs from several host threads; the flags are atomics and a
   // duplicate set by two racing threads is harmless).
@@ -693,45 +340,30 @@ int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = -1;
   if (dev < 0 || !attr_set[dev].load(std::memory_order_acquire)) {
-    rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         C::SMEM_BYTES), "cudaFuncSetAttribute(gemm)");
+    rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES),
+                    "cudaFuncSetAttribute(gemm)");
     if (rc) return rc;
     if (dev >= 0) attr_set[dev].store(true, std::memory_order_release);
   }
-  const int tiles_resident = p.total_tiles < slots ? p.total_tiles : slots;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>(tiles_resident * CTAS));
-  cfg.blockDim = dim3(NUM_THREADS);
-  cfg.dynamicSmemBytes = C::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CTAS;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return check_cuda(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmD, tmD2, tmAux, p), "gemm_kernel launch");
+  kern<<<dim3(num_n, num_m, splits), NUM_THREADS, C::SMEM_BYTES, stream>>>(tmA, tmB, p);
+  return check_cuda(cudaGetLastError(), "gemm_kernel launch");
 }
 
-template <int BN, int CTAS>
+template <int BN>
 int dispatch_epi(const GemmArgs& g, cudaStream_t s) {
   const bool f32 = (g.out_dtype == DT_F32);
   switch (g.epi) {
     case EPI_NONE:
     case EPI_BIAS:
-      return f32 ? launch_cfg<BN, true, EF_BIAS, CTAS, 0>(g, s) : launch_cfg<BN, false, EF_BIAS, CTAS, 0>(g, s);
+      return f32 ? launch_cfg<BN, true, EF_BIAS>(g, s) : launch_cfg<BN, false, EF_BIAS>(g, s);
     case EPI_BIAS_RESID:
-      if (f32) return launch_cfg<BN, true, EF_RESID, CTAS, 1>(g, s);
-      // plain row-aligned residual: TMA ring; row-modulo (position embedding) operand: per-thread loads
-      return g.aux_row_mod > 0 ? launch_cfg<BN, false, EF_RESID, CTAS, 1>(g, s)
-                               : launch_cfg<BN, false, EF_RESID, CTAS, 2>(g, s);
+      return f32 ? launch_cfg<BN, true, EF_RESID>(g, s) : launch_cfg<BN, false, EF_RESID>(g, s);
     case EPI_BIAS_GELU:
-      return launch_cfg<BN, false, EF_GELU, CTAS, 0>(g, s);
+      return launch_cfg<BN, false, EF_GELU>(g, s);
     case EPI_DGELU:
       if (f32) { set_error("bv_gemm: DGELU epilogue writes bf16"); return BV_ERR_INVALID; }
       if (g.aux_row_mod > 0) { set_error("bv_gemm: DGELU takes a row-aligned aux"); return BV_ERR_INVALID; }
-      return launch_cfg<BN, false, EF_DGELU, CTAS, 2>(g, s);
+      return launch_cfg<BN, false, EF_DGELU>(g, s);
   }
   set_error("bv_gemm: bad epilogue %d", g.epi);
   return BV_ERR_INVALID;
@@ -739,19 +371,16 @@ int dispatch_epi(const GemmArgs& g, cudaStream_t s) {
 
 }  // namespace
 
-int gemm_debug_read(long long* host, int n) {
-  if (g_gemm_dbg == nullptr) return 0;
-  if (n > 32 * 16) n = 32 * 16;
-  cudaDeviceSynchronize();
-  cudaMemcpy(host, g_gemm_dbg, n * sizeof(long long), cudaMemcpyDeviceToHost);
-  return n;
-}
-
 int launch_gemm(const GemmArgs& g, cudaStream_t stream) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) { set_error("bv_gemm: empty problem"); return BV_ERR_INVALID; }
-  // N need not be a multiple of 8 as long as the row strides are (TMA clips the store); bias / aux
-  // must then be readable up to round_up(N, 8) columns (see include/bv_b200.h).
-  if (g.ldd % 8 != 0 && g.out_dtype == DT_BF16) { set_error("bv_gemm: ldd must be a multiple of 8"); return BV_ERR_INVALID; }
+  // N need not be a multiple of 8 as long as the row strides are (TMA clips the loads)
+  // the epilogue stores bf16 pairs / fp32 pairs straight from registers
+  if (g.out_dtype == DT_BF16 && ((reinterpret_cast<uintptr_t>(g.D) & 15) || (g.ldd % 8))) {
+    set_error("bv_gemm: bf16 output must be 16B aligned with ldd %% 8 == 0"); return BV_ERR_INVALID;
+  }
+  if (g.out_dtype == DT_F32 && ((reinterpret_cast<uintptr_t>(g.D) & 7) || (g.ldd % 2))) {
+    set_error("bv_gemm: fp32 output must be 8B aligned with an even ldd"); return BV_ERR_INVALID;
+  }
   if (g.M > 0x7fffffffLL || g.N > 0x7fffffffLL || g.K > 0x7fffffffLL) {
     set_error("bv_gemm: dimension exceeds int32"); return BV_ERR_INVALID;
   }
@@ -768,18 +397,17 @@ int launch_gemm(const GemmArgs& g, cudaStream_t stream) {
   if (g.epi == EPI_BIAS_GELU && (g.out_dtype != DT_BF16 || g.D2 == nullptr || g.reduce_out)) {
     set_error("bv_gemm: BIAS_GELU needs bf16 output, D2 and no reduce"); return BV_ERR_INVALID;
   }
+  if (g.epi == EPI_BIAS_GELU && ((reinterpret_cast<uintptr_t>(g.D2) & 15) || (g.ldd2 % 8))) {
+    set_error("bv_gemm: D2 must be 16B aligned with ldd2 %% 8 == 0"); return BV_ERR_INVALID;
+  }
   if (g.out_dtype != DT_F32 && g.out_dtype != DT_BF16) { set_error("bv_gemm: bad out dtype"); return BV_ERR_INVALID; }
   if (g.colsum != nullptr && (g.out_dtype != DT_BF16 || g.reduce_out)) {
     set_error("bv_gemm: colsum needs a plain bf16 output"); return BV_ERR_INVALID;
   }
   int bn = g.block_n;
   if (bn == 0) bn = (g.N > 128) ? 256 : 128;
-  // BV_GEMM_CTAS=1 selects the single-CTA (cta_group::1) build of the same kernel: a
-  // bring-up / A-B measurement switch, not a fallback (both are sm_100a tcgen05 paths).
-  static const int ctas = [] { const char* e = getenv("BV_GEMM_CTAS"); return (e && e[0] == '1') ? 1 : 2; }();
-  if (ctas == 1) return dispatch_epi<256, 1>(g, stream);
-  if (bn == 256) return dispatch_epi<256, 2>(g, stream);
-  if (bn == 128) return dispatch_epi<128, 2>(g, stream);
+  if (bn == 256) return dispatch_epi<256>(g, stream);
+  if (bn == 128) return dispatch_epi<128>(g, stream);
   set_error("bv_gemm: block_n must be 0, 128 or 256");
   return BV_ERR_INVALID;
 }

@@ -39,20 +39,16 @@ struct AttnArgs {
   float scale;
 };
 int launch_attention_fwd(const AttnArgs& a, cudaStream_t s);
-int launch_attention_fwd_stream(const AttnArgs& a, cudaStream_t s);   // attention_stream.cu
 struct AttnBwdArgs {
   AttnArgs f;
   const void* d_o; int64_t lddo, bsdo;
   void* dq; void* dk; void* dv;                  // bf16, same geometry as q/k/v
   float* dq_colsum; float* dk_colsum; float* dv_colsum;   // optional [H*64] fp32 bias gradients
   int64_t lddq, lddk, lddv, bsdq, bsdk, bsdv;
-  float* delta;                                  // workspace [B, H, Nq] fp32   (streaming kernel)
-  float* dq_accum;                               // workspace [B, Nq, H*64] fp32 (streaming kernel)
+  float* delta;                                  // workspace [B, H, Nq] fp32
+  float* dq_accum;                               // workspace [ceil(Nk/64), B, Nq, H*64] fp32
 };
 int launch_attention_bwd(const AttnBwdArgs& a, cudaStream_t s);
-int launch_attention_bwd_stream(const AttnBwdArgs& a, cudaStream_t s);   // attention_stream.cu
-int gemm_debug_read(long long* host, int n);   // BV_GEMM_DBG=1 timeline of the last GEMM launch
-int attn_debug_read(long long* host, int n);   // BV_ATTN_DBG=1 timeline of the last fwd launch
 
 // ---- integer evaluation paths (eval.cu)
 int launch_top1(const void* logits, int dtype, int64_t rows, int C, int64_t ld, int32_t* idx,

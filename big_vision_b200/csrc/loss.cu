@@ -4,7 +4,7 @@
 //      x_ij   = (zimg_i . ztxt_j) * exp(t') + b
 //      loglik = log_sigmoid(+x_ij) on the positive diagonal, log_sigmoid(-x_ij) elsewhere
 //      loss   = (1/B) sum_i sum_j -loglik_ij            (B = GLOBAL batch, siglip.py:306)
-//    The dot products come from the tcgen05 GEMM; this kernel fuses scale+bias, the
+//    The dot products come from the wgmma GEMM; this kernel fuses scale+bias, the
 //    loss reduction and d loss/d dot (written as the bf16 operand of the two gradient
 //    GEMMs) plus the scalar gradients of t' and b in one pass over the [n, B] slab.
 //  * sigmoid_xent / softmax_xent (K15): utils.py:236-243, 276-281.

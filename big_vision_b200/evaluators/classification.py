@@ -19,7 +19,7 @@ def top1_counts(logits, labels, mask=None):
 
 def zero_shot_best_text(zimg, ztxt):
   """best_txt = (zimg @ ztxt.T).argmax(axis=1)
-  (evaluators/proj/image_text/discriminative_classifier.py:284-288): tcgen05 GEMM + argmax."""
+  (evaluators/proj/image_text/discriminative_classifier.py:284-288): wgmma GEMM + argmax."""
   import torch
   scores = ops.gemm(zimg.to(torch.bfloat16).contiguous(), ztxt.to(torch.bfloat16).contiguous(),
                     out_dtype=torch.float32)

@@ -1,7 +1,7 @@
 """ctypes binding of libbv_b200.so (C ABI declared in include/bv_b200.h).
 
 The product path has no fallback: if the library is missing, or a call is made
-without a compute-capability-10.x device, this module raises.
+without a compute-capability-9.x device, this module raises.
 """
 import ctypes
 import os

@@ -1,11 +1,11 @@
-"""MLP-Mixer on the B200 kernels -- mirror of big_vision/models/mlp_mixer.py:30-124.
+"""MLP-Mixer on the H100 kernels -- mirror of big_vision/models/mlp_mixer.py:30-124.
 
 Same factory / fields / parameter names (`stem`, `MixerBlock_{i}/{LayerNorm_0,LayerNorm_1,
 token_mixing,channel_mixing}/Dense_{0,1}`, `pre_head_layer_norm`, `head`; mlp_mixer.py:145-165).
 The reference is fp32-only; BASELINE.json config 3 asks for bf16 matmuls (fp32 accumulate), which
 is what runs here.  Token mixing applies the MLP along the token axis (mlp_mixer.py:49-51): the
 activations are transposed to [n*d, tokens] (tokens padded to a multiple of 8 for TMA strides), run
-through the same tcgen05 GEMMs, and transposed back fused with the residual add.
+through the same wgmma GEMMs, and transposed back fused with the residual add.
 Stochastic depth (mlp_mixer.py:52,55,76,173-177): block i drops each residual branch per sample with
 probability i/(L-1)*stoch_depth, no 1/(1-p) rescale.  The 0/1 masks are an INPUT of fwd
 (`masks` fp32 [num_blocks, 2, n]; parity tests feed the same masks to the oracle) or, with train=True,

@@ -1,4 +1,4 @@
-"""Text tower on the B200 kernels -- mirror of
+"""Text tower on the H100 kernels -- mirror of
 big_vision/models/proj/image_text/text_transformer.py:29-99.
 
 Embed(vocab, width) + learned posemb -> vit.Encoder (no attention mask: none is passed at

@@ -1,4 +1,4 @@
-"""ViT on the B200 kernels -- host-side mirror of big_vision/models/vit.py.
+"""ViT on the H100 kernels -- host-side mirror of big_vision/models/vit.py.
 
 Same factory (`Model(num_classes, variant=..., **kw)`), same fields, same parameter-tree
 names/shapes as the reference (models/vit.py:186-281, param names SURVEY.md 8b); the

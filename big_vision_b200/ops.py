@@ -5,7 +5,6 @@ no eager/CPU implementation behind these calls.
 """
 import ctypes
 import math
-import os
 
 import torch
 
@@ -157,12 +156,9 @@ def attention_bwd(do, q, k, v, o, lse, heads, scale=None, dq=None, dk=None, dv=N
   if dv is None:
     dv = torch.empty(v.shape, dtype=torch.bfloat16, device=q.device)
   f = _attn_args(q, k, v, o, lse, heads, scale)
-  delta = dq_accum = None
   B, Nq, cols = q.shape
-  if Nq > 256 or k.shape[1] > 256 or os.environ.get("BV_ATTN_BWD", "")[:1] == "s":
-    # workspaces of the key-tile streaming kernel (long sequences)
-    delta = torch.empty((B, heads, Nq), dtype=torch.float32, device=q.device)
-    dq_accum = torch.empty((B, Nq, cols), dtype=torch.float32, device=q.device)
+  delta = torch.empty((B, heads, Nq), dtype=torch.float32, device=q.device)
+  dq_accum = torch.empty(((k.shape[1] + 63) // 64, B, Nq, cols), dtype=torch.float32, device=q.device)
   dop, lddo, bsdo = _attn_view(do)
   dqp, lddq, bsdq = _attn_view(dq)
   dkp, lddk, bsdk = _attn_view(dk)
@@ -172,11 +168,9 @@ def attention_bwd(do, q, k, v, o, lse, heads, scale=None, dq=None, dk=None, dv=N
                        dq_colsum=dq_colsum.data_ptr() if dq_colsum is not None else None,
                        dk_colsum=dk_colsum.data_ptr() if dk_colsum is not None else None,
                        dv_colsum=dv_colsum.data_ptr() if dv_colsum is not None else None,
-                       delta=delta.data_ptr() if delta is not None else None,
-                       dq_accum=dq_accum.data_ptr() if dq_accum is not None else None)
+                       delta=delta.data_ptr(), dq_accum=dq_accum.data_ptr())
   L.call("bv_attention_bwd", ctypes.byref(args), _stream())
-  if delta is not None and (Nq > 256 or k.shape[1] > 256 or os.environ.get("BV_ATTN_BWD", "")[:1] == "s"):
-    L.LAUNCHES[0] += 2          # streaming path = delta pre-kernel + main kernel + dQ conversion
+  L.LAUNCHES[0] += 2            # delta pre-kernel + main kernel + dQ conversion
   return dq, dk, dv
 
 

@@ -140,12 +140,9 @@ def all_reduce_grads(P, d, run_backward):
   """Runs `run_backward()` and all-reduces (SUM) the flat gradient buffer when there are peers.
 
   Default: ONE all-reduce after the backward.  BV_GRAD_ALLREDUCE=overlap selects the bucketed form
-  that runs under the backward (BucketedGradAllReduce).  Measured on 8xB200 (profiles/r02/multi_gpu):
-  single 170.6 ms/step (the all-reduce of the 813 MB buffer takes 5.1 ms), overlapped 174.5 ms/step --
-  every kernel of the backward is a persistent grid of one CTA per SM, so an NCCL kernel that holds a
-  few SMs delays the tail CTAs of the GEMM running beside it by about its own duration, and the
-  "hidden" collective is paid for anyway, plus the extra launches.  Making the overlap pay needs the
-  compute kernels to leave SMs free while a bucket is in flight; not done."""
+  that runs under the backward (BucketedGradAllReduce).  Which of the two is faster on H100 has not
+  been measured: an NCCL kernel that holds a few SMs delays the GEMM tiles running beside it, so the
+  overlapped form pays for part of the collective anyway, plus the extra launches."""
   if d.world == 1:
     run_backward()
     return

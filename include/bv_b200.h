@@ -1,4 +1,4 @@
-/* bv_b200.h -- C ABI of libbv_b200.so: the B200-native (sm_100a) kernels for the
+/* bv_b200.h -- C ABI of libbv_b200.so: the H100-native (sm_90a) kernels for the
  * big_vision ViT / MLP-Mixer / SigLIP training hot path.
  *
  * The reference (google-research/big_vision) has no operator/FFI ABI of its own: the
@@ -46,12 +46,12 @@ extern "C" {
 
 const char* bv_last_error_string(void);
 int bv_version(void);
-/* 1 if the library was compiled for sm_100a and a device of compute capability 10.x is
+/* 1 if the library was compiled for sm_90a and a device of compute capability 9.x is
  * current; the product path refuses to run otherwise (no CPU / other-arch fallback). */
 int bv_device_supported(void);
 
 /* ---------------------------------------------------------------------------------
- * Dense contraction  D[M,N] = epilogue(alpha * sum_k A(m,k) B(n,k))   (tcgen05 + TMA)
+ * Dense contraction  D[M,N] = epilogue(alpha * sum_k A(m,k) B(n,k))   (wgmma + TMA)
  * Replaces flax nn.Dense / nn.DenseGeneral / nn.Conv(patch,stride=patch) forward and both
  * backward contractions: models/vit.py:72,77 (MlpBlock), :93-98 and :176-178
  * (q/k/v/out projections inside MultiHeadDotProductAttention), :212-214 (patch embed as
@@ -63,7 +63,7 @@ int bv_device_supported(void);
  *     forward  Y = X W    : A=X (a_mn=0), B=W[K,N] (b_mn=1)
  *     dgrad    dX = dY W^T: A=dY (a_mn=0), B=W[K,N] read as [N'=K rows, K'=N] (b_mn=0)
  *     wgrad    dW = X^T dY: A=X (a_mn=1), B=dY (b_mn=1), out fp32, reduce_out=1
- *   reduce_out : 1 = accumulate into D with TMA reduce-add (split-K / grad accumulation)
+ *   reduce_out : 1 = accumulate into D with atomic adds (split-K / grad accumulation)
  *   splits     : 0 = auto, >1 only with reduce_out
  *   block_n    : 0 = auto, else 128 or 256
  *   bias (fp32 [N]) and aux (bf16) must be readable up to round_up(N, 8) columns.
@@ -97,9 +97,9 @@ int bv_layernorm_bwd(const void* dy, int dy_dtype, const void* x, int x_dtype, c
 
 /* ---------------------------------------------------------------------------------
  * Scaled-dot-product attention, head dim 64, no mask, any Nq, Nk >= 1
- * (flax MultiHeadDotProductAttention core: models/vit.py:93-98, :176-178).  Sequences up to 256
- * keys run with the whole key range resident on chip; longer ones (config 5: 576) stream 128-key
- * blocks (online combination of per-block softmax statistics; attention_stream.cu).
+ * (flax MultiHeadDotProductAttention core: models/vit.py:93-98, :176-178).  Keys stream through
+ * on-chip memory in 64-key blocks (online combination of per-block softmax statistics), so every
+ * sequence length takes the same path.
  * q/k/v/o are bf16 strided views: element (b, t, h*64 + j) at
  * base + b*bs + t*ld + h*64 + j  (e.g. column slices of the fused QKV GEMM output).
  * lse [B,H,Nq] fp32 = log sum_j exp(scale * q_i.k_j) is saved for the backward.
@@ -120,9 +120,9 @@ typedef struct bv_attn_bwd_args {
   /* optional fp32 [H*64] each: += column sums over the valid rows of dq / dk / dv, i.e. the bias
    * gradients of the projections that produced q / k / v */
   float* dq_colsum; float* dk_colsum; float* dv_colsum;
-  /* workspaces of the key-tile streaming kernel, REQUIRED when Nq > 256 or Nk > 256 (may be NULL
-   * otherwise): delta [B,H,Nq] fp32 = rowsum(O o dO); dq_accum [B,Nq,H*64] fp32, zeroed by the call,
-   * receives the per-key-tile dQ contributions (TMA reduce-add) before the bf16 conversion into dq */
+  /* REQUIRED workspaces: delta [B,H,Nq] fp32 = rowsum(O o dO); dq_accum [ceil(Nk/64),B,Nq,H*64]
+   * fp32 receives the dQ contribution of each 64-key block, summed in block order (reproducible bit
+   * for bit) during the bf16 conversion into dq */
   float* delta; float* dq_accum;
 } bv_attn_bwd_args;
 int bv_attention_bwd(const bv_attn_bwd_args* args, void* stream);

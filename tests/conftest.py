@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-  config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+  config.addinivalue_line("markers", "gpu: needs an H100 (compute capability 9.x)")
 
 
 # GPU files run leaves-first: the kernel-level parity tests, then the models built from them, then
@@ -25,7 +25,7 @@ def _gpu_usable():
     import torch
     if not torch.cuda.is_available():
       return False
-    return torch.cuda.get_device_capability(0)[0] == 10
+    return torch.cuda.get_device_capability(0)[0] == 9
   except Exception:   # pylint: disable=broad-except
     return False
 
@@ -36,7 +36,7 @@ def pytest_collection_modifyitems(config, items):
     return _GPU_ORDER.index(mod) if mod in _GPU_ORDER else len(_GPU_ORDER)
   items.sort(key=key)     # stable: keeps the in-file order
   if not _gpu_usable():
-    skip = pytest.mark.skip(reason="needs a compute-capability 10.x GPU (no CPU fallback exists)")
+    skip = pytest.mark.skip(reason="needs a compute-capability 9.x GPU (no CPU fallback exists)")
     for item in items:
       if "gpu" in item.keywords:
         item.add_marker(skip)

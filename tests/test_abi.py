@@ -73,7 +73,7 @@ def test_bench_workloads_cover_the_five_baseline_configs():
   assert bench.synthetic_batch(wl, 2, seed=0, uint8=True)["image"].dtype.name == "uint8"
   c = bench.synthetic_batch(bench.WORKLOADS["vit_b16_cls"], 4, seed=0)
   assert c["labels"].shape == (4, 1000) and (c["labels"].sum(1) == 1).all()
-  assert bench.WORKLOADS["siglip_l14_336"]["per_gpu_batch"] * 8 == 16384 and wl["per_gpu_batch"] * 8 == 8192
+  assert bench.WORKLOADS["siglip_l14_336"]["per_gpu_batch"] * 8 == 4096 and wl["per_gpu_batch"] * 8 == 6144
   model = bench.build_model(bench.WORKLOADS["siglip_l14_336"])
   assert model.img.scan and model.txt.scan and model.img.width == 1024 and model.img.patch_size == (14, 14)
 

@@ -26,7 +26,7 @@ def _close(got, ref, tol):
 @pytest.fixture(scope="module")
 def ops():
   from big_vision_b200 import lib, ops as _ops
-  assert lib.load().bv_device_supported() == 1, "needs a compute-capability 10.x GPU"
+  assert lib.load().bv_device_supported() == 1, "needs a compute-capability 9.x GPU"
   return _ops
 
 
@@ -142,7 +142,7 @@ def _ref_attention(q, k, v, heads):
 
 @pytest.mark.parametrize("B,H,Nq,Nk", [(3, 2, 64, 64), (2, 12, 196, 196), (5, 3, 197, 197), (4, 2, 1, 196),
                                        (2, 1, 16, 16), (1, 2, 256, 256), (2, 2, 130, 7),
-                                       (4, 3, 64, 64), (6, 12, 64, 64)])   # even batch of 64 tokens: packed tiles
+                                       (4, 3, 64, 64), (6, 12, 64, 64)])   # the text tower's 64 tokens
 def test_attention_forward_backward(ops, B, H, Nq, Nk):
   g = torch.Generator().manual_seed(B * 1000 + Nq)
   d = H * 64
@@ -172,24 +172,25 @@ def test_attention_forward_backward(ops, B, H, Nq, Nk):
     assert (cs[i].double() - ref).abs().max().item() <= 1e-4 * (ref.abs().max().item() + 1)
 
 
-def test_packed_text_tiles_equal_unpacked(ops, monkeypatch):
-  """Two 64-token items per 128-row tile with block-diagonal scores (the text tower at an even batch):
-  same results as one item per tile, forward and backward, including the fused bias gradients."""
+def test_text_tower_attention_is_bitwise_reproducible(ops):
+  """The text tower's shape (64 tokens, 12 heads) run twice, forward and backward with the fused bias
+  gradients: outputs, log-sum-exps and gradients are identical bit for bit; the bias gradients, which are
+  accumulated with fp32 atomics, agree to rounding."""
   g = torch.Generator().manual_seed(11)
   B, H, N = 8, 12, 64
   d = H * 64
   c = _bf(torch.randn(B, N, 3 * d, generator=g)).cuda()
   do = _bf(torch.randn(B, N, d, generator=g)).cuda()
   q, k, v = c[:, :, 0:d], c[:, :, d:2 * d], c[:, :, 2 * d:]
-  res = {}
-  for mode in ("0", "1"):
-    monkeypatch.setenv("BV_ATTN_PACK", mode)
+  runs = []
+  for _ in range(2):
     o, lse = ops.attention_fwd(q, k, v, H)
     cs = torch.zeros(3, d, device="cuda")
     dq, dk, dv = ops.attention_bwd(do, q, k, v, o, lse, H, dq_colsum=cs[0], dk_colsum=cs[1], dv_colsum=cs[2])
-    res[mode] = (o, lse, dq, dk, dv, cs)
-  for a, b, tol in zip(res["1"], res["0"], (2 ** -8, 1e-6, 2 ** -7, 2 ** -7, 2 ** -7, 1e-4)):
-    _close(a, b, tol)
+    runs.append((o, lse, dq, dk, dv, cs))
+  for a, b in zip(runs[0][:5], runs[1][:5]):
+    assert torch.equal(a, b)
+  _close(runs[1][5], runs[0][5], 1e-6)
 
 
 def test_attention_rows_are_convex_combinations(ops):

@@ -1,5 +1,5 @@
 """Times bv_attention_fwd / bwd at the bench shapes with CUDA events (after warm-up):
-  python tools/attn_bench.py [fwd|bwd|both]      env BV_ATTN_FWD / BV_ATTN_BWD select the kernel."""
+  python tools/attn_bench.py [fwd|bwd|both]      env BV_BENCH_SHAPES="B,H,N;..." overrides the shapes."""
 import os
 import sys
 import torch
@@ -38,4 +38,4 @@ if os.environ.get("BV_BENCH_SHAPES"):
 for B, H, N in shapes:
   r = run(B, H, N, what)
   print(f"B={B} H={H} N={N} " + "  ".join(f"{k}: {v[0]:.3f} ms {v[1]:.0f} TFLOP/s" for k, v in r.items()),
-        f"[fwd={os.environ.get('BV_ATTN_FWD','default')} bwd={os.environ.get('BV_ATTN_BWD','default')} sm={os.environ.get('BV_ATTN_SM','-')}]", flush=True)
+        flush=True)

@@ -1,5 +1,6 @@
-"""Launches every kernel of the hot path once or twice at bench-like shapes, for ONE `ncu --set full`
-pass over all of them (tools/ncu_r02.sh).  Not a benchmark: no timing here."""
+"""Launches every kernel of the hot path once or twice at bench-like shapes, so that one profiler pass
+(for example `ncu --set full python tools/kernel_zoo.py`) captures all of them.  Not a benchmark: no
+timing here."""
 import os
 import sys
 
