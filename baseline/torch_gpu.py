@@ -22,7 +22,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 from torch.utils.checkpoint import checkpoint
 
-VIT = {"S": (384, 12, 1536, 6), "B": (768, 12, 3072, 12), "L": (1024, 24, 4096, 16)}
+VIT = {"S": (384, 12, 1536, 6), "B": (768, 12, 3072, 12), "L": (1024, 24, 4096, 16),
+       "So400m": (1152, 27, 4304, 16)}
 MIXER = {"B": (768, 12, 384, 3072)}
 
 

@@ -56,11 +56,13 @@ static AttnArgs to_attn(const bv_attn_args& a) {
   r.scale = a.scale;
   return r;
 }
-int bv_attention_fwd(const bv_attn_args* a, void* stream) {
+int bv_attention_fwd(const bv_attn_args* a, void* stream) { return bv_attention_fwd_hd(a, 64, stream); }
+int bv_attention_fwd_hd(const bv_attn_args* a, int32_t head_dim, void* stream) {
   if (!a) { set_error("bv_attention_fwd: null args"); return BV_ERR_INVALID; }
-  return launch_attention_fwd(to_attn(*a), S(stream));
+  return launch_attention_fwd(to_attn(*a), head_dim, S(stream));
 }
-int bv_attention_bwd(const bv_attn_bwd_args* a, void* stream) {
+int bv_attention_bwd(const bv_attn_bwd_args* a, void* stream) { return bv_attention_bwd_hd(a, 64, stream); }
+int bv_attention_bwd_hd(const bv_attn_bwd_args* a, int32_t head_dim, void* stream) {
   if (!a) { set_error("bv_attention_bwd: null args"); return BV_ERR_INVALID; }
   AttnBwdArgs g;
   g.f = to_attn(a->fwd);
@@ -70,7 +72,7 @@ int bv_attention_bwd(const bv_attn_bwd_args* a, void* stream) {
   g.bsdq = a->bsdq; g.bsdk = a->bsdk; g.bsdv = a->bsdv;
   g.dq_colsum = a->dq_colsum; g.dk_colsum = a->dk_colsum; g.dv_colsum = a->dv_colsum;
   g.delta = a->delta; g.dq_accum = a->dq_accum;
-  return launch_attention_bwd(g, S(stream));
+  return launch_attention_bwd(g, head_dim, S(stream));
 }
 
 int bv_patchify(const float* image, void* patches, int64_t n, int32_t H, int32_t W, int32_t C,

@@ -1,13 +1,20 @@
 // Scaled-dot-product attention forward / backward on sm_90a wgmma (K5, and the MAP head's
 // 1-query attention, K10).  Reference: flax.linen.MultiHeadDotProductAttention as called at
 // models/vit.py:93-98 (self-attention, no mask, no dropout) and models/vit.py:176-178 (MAPHead
-// probe attention): q is scaled by 1/sqrt(dh), softmax over keys, weights times v.  Head dim is
-// fixed at 64 (every ViT variant in models/vit.py:297-300 has width/heads == 64 except "mu" and
-// So400m).
+// probe attention): q is scaled by 1/sqrt(dh), softmax over keys, weights times v.  Head dims 64,
+// 72, 80 and 96 are built (the size table of models/vit.py:284-303: 64 for Ti, S, M, B and L, 72
+// for So400m, 80 for H, 96 for g-opt and G-opt); mu (16), g (88), G (104) and e (112) are not.
+// Every kernel is a template on the head dim DH.
 //
-// q/k/v/o are strided views into the fused QKV GEMM output: element (b, t, h*64+j) at
-// base + b*batch_stride + t*row_stride + h*64 + j; 3-D TMA descriptors read them in place (no head
-// transpose, no padding copies; rows past N are zero-filled).
+// q/k/v/o are strided views into the fused QKV GEMM output: element (b, t, h*DH+j) at
+// base + b*batch_stride + t*row_stride + h*DH + j; TMA descriptors read them in place (no head
+// transpose, no padding copies; rows past N are zero-filled).  At DH = 64 the map is 3-D
+// [cols, tokens, batch] and a tile is one 64-column box.  At DH > 64 the head dim is a dimension of
+// its own, [DH, H, tokens, batch], and a tile is two 128B-swizzled 64-column boxes side by side:
+// columns 0-63 and 64-127, the second zero-filled by TMA past DH.  The contractions over the head
+// dim (S = Q K^T, S^T = K Q^T, dP^T = V dO^T) run in k16 steps up to round_up(DH, 16) and so meet
+// zeros, never the next head's columns.  The products whose N is the head dim (O += P V, dV, dK,
+// dQ) are single n = DH wgmmas across both boxes (MN-major operand, leading byte offset = one box).
 //
 // Both kernels run one warpgroup per CTA on 64-row tiles and stream the other operand in 64-row
 // blocks through a two-slot TMA ring, so any sequence length works with the same code:
@@ -25,16 +32,24 @@ namespace bv {
 
 namespace {
 
-constexpr int DH = 64;
 constexpr int T = 64;                      // rows per tile (queries or keys)
-constexpr int TILE_BYTES = T * DH * 2;     // 8 KB: 64 rows x 128 B, 128B-swizzled
+constexpr int BOX_BYTES = T * 64 * 2;      // 8 KB: 64 rows x 128 B, 128B-swizzled
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float LN2 = 0.6931471805599453f;
 constexpr int THREADS = 128;
-// shared memory: 1024-aligned 8 KB tiles, then three mbarriers (+ alignment slack)
-constexpr int FWD_TILES = 5, BWD_TILES = 7;
-constexpr int FWD_SMEM = FWD_TILES * TILE_BYTES + 1024 + 64;
-constexpr int BWD_SMEM = BWD_TILES * TILE_BYTES + 1024 + 64;
+
+// Per-head-dim geometry.  Shared memory: 1024-aligned tiles, then three mbarriers (+ alignment slack);
+// the forward holds Q and two K / V slots, the backward K, V, two Q / dO slots and the 64 x 64 dS^T tile.
+template <int DH>
+struct Geo {
+  static_assert(DH == 64 || DH == 72 || DH == 80 || DH == 96, "head dims 64, 72, 80, 96");
+  static constexpr int TILE_BYTES = DH > 64 ? 2 * BOX_BYTES : BOX_BYTES;   // a [64 rows x DH] tile
+  static constexpr int KSTEPS = (DH + 15) / 16;                            // k16 steps over the head dim
+  static_assert(KSTEPS >= 4 && KSTEPS <= 8, "one or two 64-column boxes");
+  static constexpr int R = DH / 2;                                         // fp32 registers of a [64 x DH] accumulator
+  static constexpr int FWD_SMEM = 5 * TILE_BYTES + 1024 + 64;
+  static constexpr int BWD_SMEM = 6 * TILE_BYTES + BOX_BYTES + 1024 + 64;
+};
 
 __device__ __forceinline__ float ex2(float x) {
   float y;
@@ -42,30 +57,73 @@ __device__ __forceinline__ float ex2(float x) {
   return y;
 }
 
-int make_tmap_bnd(CUtensorMap* m, const void* ptr, int cols, int64_t N, int64_t B, int64_t ld, int64_t bs) {
-  uint64_t dims[3] = {static_cast<uint64_t>(cols), static_cast<uint64_t>(N), static_cast<uint64_t>(B)};
-  uint64_t strides[2] = {static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(bs) * 2};
-  uint32_t box[3] = {64, T, 1};
-  return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, ptr, dims, strides, box, true);
+int make_tmap_bnd(CUtensorMap* m, const void* ptr, int dh, int H, int64_t N, int64_t B, int64_t ld, int64_t bs) {
+  if (dh == 64) {
+    uint64_t dims[3] = {static_cast<uint64_t>(H) * 64, static_cast<uint64_t>(N), static_cast<uint64_t>(B)};
+    uint64_t strides[2] = {static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(bs) * 2};
+    uint32_t box[3] = {64, T, 1};
+    return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, ptr, dims, strides, box, true);
+  }
+  // [dh, H, N, B] with a head stride of dh * 2 bytes (a multiple of 16 since dh % 8 == 0)
+  uint64_t dims[4] = {static_cast<uint64_t>(dh), static_cast<uint64_t>(H), static_cast<uint64_t>(N),
+                      static_cast<uint64_t>(B)};
+  uint64_t strides[3] = {static_cast<uint64_t>(dh) * 2, static_cast<uint64_t>(ld) * 2, static_cast<uint64_t>(bs) * 2};
+  uint32_t box[4] = {64, 1, T, 1};
+  return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, ptr, dims, strides, box, true);
 }
 
-// Descriptors of a 64 x 64 bf16 tile: K-major (rows = M|N, the 64 columns are the contraction) or
-// MN-major (rows = the contraction, the 64 columns are M|N).  One k step of 16 is 32 B or 16 rows.
+// one [64 rows x DH] tile of head h from row `row` of batch b (TILE_BYTES transaction bytes)
+template <int DH>
+__device__ __forceinline__ void load_tile(uint32_t dst, const CUtensorMap* m, uint32_t bar, int h, int row, int b) {
+  if constexpr (DH == 64) {
+    tma_load_3d(dst, m, bar, h * DH, row, b);
+  } else {
+    tma_load_4d(dst, m, bar, 0, h, row, b);
+    tma_load_4d(dst + BOX_BYTES, m, bar, 64, h, row, b);
+  }
+}
+
+// Descriptors of a 64 x 64 bf16 box: K-major (rows = M|N, the 64 columns are the contraction) or
+// MN-major (rows = the contraction, the 64 columns are M|N; the next 64 columns are the next box,
+// 8 KB on).  One k step of 16 is 32 B or 16 rows.
 __device__ __forceinline__ uint64_t desc_k(uint32_t tile) { return wgmma_desc_sw128(tile, 16u, 1024u); }
 __device__ __forceinline__ uint64_t desc_mn(uint32_t tile) { return wgmma_desc_sw128(tile, 8192u, 1024u); }
 constexpr uint64_t KSTEP_K = 32 >> 4, KSTEP_MN = 2048 >> 4;
 
-// S[64 x 64] = A B^T over the 64-wide head dimension, both tiles K-major
+// D[64 x DH] (+)= A[64 x 16] * B[DH x 16]^T: the wgmma of N = DH
+template <int TA, int TB, int R>
+__device__ __forceinline__ void wgmma_ss_dh(float (&d)[R], uint64_t a, uint64_t b, int scale_d) {
+  if constexpr (R == 32) wgmma_ss_n64<TA, TB>(d, a, b, scale_d);
+  else if constexpr (R == 36) wgmma_ss_n72<TA, TB>(d, a, b, scale_d);
+  else if constexpr (R == 40) wgmma_ss_n80<TA, TB>(d, a, b, scale_d);
+  else wgmma_ss_n96<TA, TB>(d, a, b, scale_d);
+}
+template <int TB, int R>
+__device__ __forceinline__ void wgmma_rs_dh(float (&d)[R], const uint32_t (&a)[4], uint64_t b, int scale_d) {
+  if constexpr (R == 32) wgmma_rs_n64<TB>(d, a, b, scale_d);
+  else if constexpr (R == 36) wgmma_rs_n72<TB>(d, a, b, scale_d);
+  else if constexpr (R == 40) wgmma_rs_n80<TB>(d, a, b, scale_d);
+  else wgmma_rs_n96<TB>(d, a, b, scale_d);
+}
+
+// S[64 x 64] = A B^T over the head dimension (zero-padded to a multiple of 16), both tiles K-major
+template <int DH>
 __device__ __forceinline__ void mma_tile_kk(float (&d)[32], uint32_t a_tile, uint32_t b_tile) {
   const uint64_t a = desc_k(a_tile), b = desc_k(b_tile);
 #pragma unroll
   for (int k = 0; k < 4; ++k) wgmma_ss_n64<0, 0>(d, a + k * KSTEP_K, b + k * KSTEP_K, k > 0 ? 1 : 0);
+  if constexpr (DH > 64) {
+    const uint64_t a1 = desc_k(a_tile + BOX_BYTES), b1 = desc_k(b_tile + BOX_BYTES);
+#pragma unroll
+    for (int k = 0; k < Geo<DH>::KSTEPS - 4; ++k) wgmma_ss_n64<0, 0>(d, a1 + k * KSTEP_K, b1 + k * KSTEP_K, 1);
+  }
 }
-// D[64 x 64] += P[64 x 64] (register fragments) * B, B an MN-major tile (rows = contraction)
-__device__ __forceinline__ void mma_tile_rs(float (&d)[32], const uint32_t (&p)[4][4], uint32_t b_tile) {
+// D[64 x DH] += P[64 x 64] (register fragments) * B, B an MN-major tile (rows = contraction)
+template <int R>
+__device__ __forceinline__ void mma_tile_rs(float (&d)[R], const uint32_t (&p)[4][4], uint32_t b_tile) {
   const uint64_t b = desc_mn(b_tile);
 #pragma unroll
-  for (int k = 0; k < 4; ++k) wgmma_rs_n64<1>(d, p[k], b + k * KSTEP_MN, 1);
+  for (int k = 0; k < 4; ++k) wgmma_rs_dh<1>(d, p[k], b + k * KSTEP_MN, 1);
 }
 
 // accumulator element 4j + e of lane l in warp w: row 16w + l/4 + 8*(e >> 1), column 8j + 2*(l%4) + (e & 1).
@@ -80,9 +138,10 @@ __device__ __forceinline__ void to_frags(const float (&s)[32], uint32_t (&p)[4][
   }
 }
 
-__device__ __forceinline__ void zero(float (&d)[32]) {
+template <int R>
+__device__ __forceinline__ void zero(float (&d)[R]) {
 #pragma unroll
-  for (int i = 0; i < 32; ++i) d[i] = 0.f;
+  for (int i = 0; i < R; ++i) d[i] = 0.f;
 }
 
 // ============================================================================
@@ -96,12 +155,15 @@ struct FwdDev {
   long long ldo, bso;
 };
 
+template <int DH>
 __global__ void __launch_bounds__(THREADS)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FwdDev p) {
+  using G = Geo<DH>;
+  constexpr int TILE_BYTES = G::TILE_BYTES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t q_s = (smem_u32(smem_raw) + 1023u) & ~1023u, k_s = q_s + TILE_BYTES, v_s = q_s + 3 * TILE_BYTES;
-  const uint32_t q_bar = q_s + FWD_TILES * TILE_BYTES;
+  const uint32_t q_bar = q_s + 5 * TILE_BYTES;
   auto kv_bar = [&](int s) { return q_bar + 8u * (1 + s); };
 
   const int qt = static_cast<int>(blockIdx.x % p.QT);
@@ -112,8 +174,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   auto load_kv = [&](int j) {
     const int s = j & 1;
     mbar_expect_tx(kv_bar(s), 2 * TILE_BYTES);
-    tma_load_3d(k_s + s * TILE_BYTES, &tmK, kv_bar(s), h * DH, j * T, b);
-    tma_load_3d(v_s + s * TILE_BYTES, &tmV, kv_bar(s), h * DH, j * T, b);
+    load_tile<DH>(k_s + s * TILE_BYTES, &tmK, kv_bar(s), h, j * T, b);
+    load_tile<DH>(v_s + s * TILE_BYTES, &tmV, kv_bar(s), h, j * T, b);
   };
   if (tid == 0) {
     mbar_init(q_bar, 1);
@@ -121,13 +183,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     mbar_init(kv_bar(1), 1);
     fence_barrier_init();
     mbar_expect_tx(q_bar, TILE_BYTES);
-    tma_load_3d(q_s, &tmQ, q_bar, h * DH, qt * T, b);
+    load_tile<DH>(q_s, &tmQ, q_bar, h, qt * T, b);
     load_kv(0);
     if (p.NB > 1) load_kv(1);
   }
   __syncthreads();
 
-  float o[32], s[32];
+  float o[G::R], s[32];
   zero(o);
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   mbar_wait(q_bar, 0);
@@ -135,7 +197,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const int slot = j & 1;
     mbar_wait(kv_bar(slot), (j >> 1) & 1);
     wgmma_fence();
-    mma_tile_kk(s, q_s, k_s + slot * TILE_BYTES);
+    mma_tile_kk<DH>(s, q_s, k_s + slot * TILE_BYTES);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs(s);
@@ -164,6 +226,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       l[r] += s[i];
       o[i] *= corr[r];
     }
+#pragma unroll
+    for (int i = 32; i < G::R; ++i) o[i] *= corr[(i >> 1) & 1];
     uint32_t pf[4][4];
     to_frags(s, pf);
     wgmma_fence_regs(o);
@@ -188,7 +252,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     if (q >= p.Nq) continue;
     bf16* orow = p.o + b * p.bso + static_cast<long long>(q) * p.ldo + h * DH + 2 * (lane & 3);
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj)
+    for (int jj = 0; jj < DH / 8; ++jj)
       *reinterpret_cast<uint32_t*>(orow + 8 * jj) = pack_bf16(o[4 * jj + 2 * r] * inv[r], o[4 * jj + 2 * r + 1] * inv[r]);
     if ((lane & 3) == 0) p.lse[(static_cast<long long>(b) * p.H + h) * p.Nq + q] = (m[r] + __log2f(l[r])) * LN2;
   }
@@ -203,18 +267,19 @@ struct BwdDev {
   float scale, scale_log2;
   const float* lse;
   const float* delta;
-  float* dq_accum;                        // [KT, B, Nq, H*64] fp32: one dQ slice per key block
+  float* dq_accum;                        // [KT, B, Nq, H*DH] fp32: one dQ slice per key block
   bf16* dk; bf16* dv;
   long long lddk, bsdk, lddv, bsdv;
   float* dk_colsum; float* dv_colsum;
 };
 
-// column sums of a [64 x 64] accumulator tile's stored (bf16-rounded) rows < nvalid: the eight lanes
+// column sums of a [64 x DH] accumulator tile's stored (bf16-rounded) rows < nvalid: the eight lanes
 // that share a column pair are summed with shuffles, then one atomic per warp and column
-__device__ __forceinline__ void tile_colsum(const float (&d)[32], float mul, int row0, int nvalid, float* colsum,
+template <int R>
+__device__ __forceinline__ void tile_colsum(const float (&d)[R], float mul, int row0, int nvalid, float* colsum,
                                             int lane) {
 #pragma unroll
-  for (int jj = 0; jj < 8; ++jj) {
+  for (int jj = 0; jj < R / 4; ++jj) {
     float c[2] = {0.f, 0.f};
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -235,14 +300,17 @@ __device__ __forceinline__ void tile_colsum(const float (&d)[32], float mul, int
   }
 }
 
+template <int DH>
 __global__ void __launch_bounds__(THREADS)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const BwdDev p) {
+  using G = Geo<DH>;
+  constexpr int TILE_BYTES = G::TILE_BYTES;
   // K, V (this CTA's key block), Q / dO ring of two, dS^T staging tile
   extern __shared__ uint8_t smem_raw[];
   const uint32_t k_s = (smem_u32(smem_raw) + 1023u) & ~1023u, v_s = k_s + TILE_BYTES, q_s = k_s + 2 * TILE_BYTES,
                  do_s = k_s + 4 * TILE_BYTES, ds_s = k_s + 6 * TILE_BYTES;
-  const uint32_t kv_bar = k_s + BWD_TILES * TILE_BYTES;
+  const uint32_t kv_bar = ds_s + BOX_BYTES;
   auto q_bar = [&](int s) { return kv_bar + 8u * (1 + s); };
 
   const int kt = static_cast<int>(blockIdx.x % p.KT);
@@ -253,8 +321,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   auto load_q = [&](int i) {
     const int s = i & 1;
     mbar_expect_tx(q_bar(s), 2 * TILE_BYTES);
-    tma_load_3d(q_s + s * TILE_BYTES, &tmQ, q_bar(s), h * DH, i * T, b);
-    tma_load_3d(do_s + s * TILE_BYTES, &tmdO, q_bar(s), h * DH, i * T, b);
+    load_tile<DH>(q_s + s * TILE_BYTES, &tmQ, q_bar(s), h, i * T, b);
+    load_tile<DH>(do_s + s * TILE_BYTES, &tmdO, q_bar(s), h, i * T, b);
   };
   if (tid == 0) {
     mbar_init(kv_bar, 1);
@@ -262,14 +330,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     mbar_init(q_bar(1), 1);
     fence_barrier_init();
     mbar_expect_tx(kv_bar, 2 * TILE_BYTES);
-    tma_load_3d(k_s, &tmK, kv_bar, h * DH, kt * T, b);
-    tma_load_3d(v_s, &tmV, kv_bar, h * DH, kt * T, b);
+    load_tile<DH>(k_s, &tmK, kv_bar, h, kt * T, b);
+    load_tile<DH>(v_s, &tmV, kv_bar, h, kt * T, b);
     load_q(0);
     if (p.QT > 1) load_q(1);
   }
   __syncthreads();
 
-  float dk[32], dv[32];
+  float dk[G::R], dv[G::R];
   zero(dk);
   zero(dv);
   const long long bhq = (static_cast<long long>(b) * p.H + h) * p.Nq;
@@ -282,8 +350,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const uint32_t qi = q_s + slot * TILE_BYTES, doi = do_s + slot * TILE_BYTES;
     float st[32], dpt[32];
     wgmma_fence();
-    mma_tile_kk(st, k_s, qi);            // S^T  = K Q^T
-    mma_tile_kk(dpt, v_s, doi);          // dP^T = V dO^T
+    mma_tile_kk<DH>(st, k_s, qi);        // S^T  = K Q^T
+    mma_tile_kk<DH>(dpt, v_s, doi);      // dP^T = V dO^T
     wgmma_commit();
     // this thread's 16 queries: lse / delta, fetched while the MMAs run
     float lse2[16], dl[16];
@@ -319,7 +387,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     }
     fence_proxy_async();
     __syncthreads();
-    float dq[32];
+    float dq[G::R];
     wgmma_fence_regs(dv);
     wgmma_fence_regs(dk);
     wgmma_fence();
@@ -328,7 +396,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     {
       const uint64_t a = desc_mn(ds_s), bk = desc_mn(k_s);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_ss_n64<1, 1>(dq, a + k * KSTEP_MN, bk + k * KSTEP_MN, k > 0 ? 1 : 0);
+      for (int k = 0; k < 4; ++k) wgmma_ss_dh<1, 1>(dq, a + k * KSTEP_MN, bk + k * KSTEP_MN, k > 0 ? 1 : 0);
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -342,7 +410,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       if (q >= p.Nq) continue;
       float* dst = p.dq_accum + ((static_cast<long long>(kt) * p.B + b) * p.Nq + q) * cols + h * DH + 2 * (lane & 3);
 #pragma unroll
-      for (int jj = 0; jj < 8; ++jj)
+      for (int jj = 0; jj < DH / 8; ++jj)
         *reinterpret_cast<float2*>(dst + 8 * jj) = make_float2(dq[4 * jj + 2 * r] * p.scale,
                                                                dq[4 * jj + 2 * r + 1] * p.scale);
     }
@@ -358,7 +426,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     bf16* kr = p.dk + b * p.bsdk + static_cast<long long>(key) * p.lddk + h * DH + 2 * (lane & 3);
     bf16* vr = p.dv + b * p.bsdv + static_cast<long long>(key) * p.lddv + h * DH + 2 * (lane & 3);
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
+    for (int jj = 0; jj < DH / 8; ++jj) {
       *reinterpret_cast<uint32_t*>(kr + 8 * jj) = pack_bf16(dk[4 * jj + 2 * r] * p.scale, dk[4 * jj + 2 * r + 1] * p.scale);
       *reinterpret_cast<uint32_t*>(vr + 8 * jj) = pack_bf16(dv[4 * jj + 2 * r], dv[4 * jj + 2 * r + 1]);
     }
@@ -367,27 +435,32 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   if (p.dv_colsum != nullptr) tile_colsum(dv, 1.f, k0, p.Nk, p.dv_colsum + h * DH, lane);
 }
 
-// delta[b,h,t] = sum_j O[b,t,h*64+j] * dO[b,t,h*64+j]: eight lanes per (b, t, h) row of 64
+// delta[b,h,t] = sum_j O[b,t,h*DH+j] * dO[b,t,h*DH+j]: LANES lanes per (b, t, h) row, DH/8 of which load
+// eight columns each (8 lanes at DH = 64, 16 above)
+template <int DH>
 __global__ void __launch_bounds__(256)
 attn_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ d_o, float* __restrict__ delta,
                   int64_t B, int H, int N, int64_t ldo, int64_t bso, int64_t lddo, int64_t bsdo) {
+  constexpr int LOG2_LANES = DH == 64 ? 3 : 4, LANES = 1 << LOG2_LANES;
   const int64_t total = B * N * H;                    // head rows
-  const int chunk = threadIdx.x & 7;
-  for (int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 3; r < total;
-       r += (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 3) {
+  const int chunk = threadIdx.x & (LANES - 1);
+  for (int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> LOG2_LANES; r < total;
+       r += (static_cast<int64_t>(gridDim.x) * blockDim.x) >> LOG2_LANES) {
     const int h = static_cast<int>(r % H);
     const int64_t bt = r / H;
     const int t = static_cast<int>(bt % N);
     const int64_t b = bt / N;
-    const uint4 ao = ld_nc_na(reinterpret_cast<const uint4*>(o + b * bso + t * ldo + h * DH + chunk * 8));
-    const uint4 ad = ld_nc_na(reinterpret_cast<const uint4*>(d_o + b * bsdo + t * lddo + h * DH + chunk * 8));
-    float acc = bf16_lo(ao.x) * bf16_lo(ad.x) + bf16_hi(ao.x) * bf16_hi(ad.x);
-    acc += bf16_lo(ao.y) * bf16_lo(ad.y) + bf16_hi(ao.y) * bf16_hi(ad.y);
-    acc += bf16_lo(ao.z) * bf16_lo(ad.z) + bf16_hi(ao.z) * bf16_hi(ad.z);
-    acc += bf16_lo(ao.w) * bf16_lo(ad.w) + bf16_hi(ao.w) * bf16_hi(ad.w);
-    acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-    acc += __shfl_xor_sync(0xffffffffu, acc, 2);
-    acc += __shfl_xor_sync(0xffffffffu, acc, 4);
+    float acc = 0.f;
+    if (chunk < DH / 8) {
+      const uint4 ao = ld_nc_na(reinterpret_cast<const uint4*>(o + b * bso + t * ldo + h * DH + chunk * 8));
+      const uint4 ad = ld_nc_na(reinterpret_cast<const uint4*>(d_o + b * bsdo + t * lddo + h * DH + chunk * 8));
+      acc = bf16_lo(ao.x) * bf16_lo(ad.x) + bf16_hi(ao.x) * bf16_hi(ad.x);
+      acc += bf16_lo(ao.y) * bf16_lo(ad.y) + bf16_hi(ao.y) * bf16_hi(ad.y);
+      acc += bf16_lo(ao.z) * bf16_lo(ad.z) + bf16_hi(ao.z) * bf16_hi(ad.z);
+      acc += bf16_lo(ao.w) * bf16_lo(ad.w) + bf16_hi(ao.w) * bf16_hi(ad.w);
+    }
+#pragma unroll
+    for (int off = 1; off < LANES; off <<= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
     if (chunk == 0) delta[(b * H + h) * N + t] = acc;
   }
 }
@@ -430,6 +503,13 @@ attn_dq_convert_kernel(const float* __restrict__ acc, int KT, bf16* __restrict__
   }
 }
 
+// head dims with kernels; every other one is refused before any CUDA call
+int check_head_dim(int head_dim, const char* who) {
+  if (head_dim == 64 || head_dim == 72 || head_dim == 80 || head_dim == 96) return BV_OK;
+  set_error("%s: head_dim %d is not supported (supported head dims: 64, 72, 80, 96)", who, head_dim);
+  return BV_ERR_UNSUPPORTED;
+}
+
 int check_attn(const AttnArgs& a, const char* who) {
   if (a.B <= 0 || a.H <= 0 || a.Nq <= 0 || a.Nk <= 0 || a.Nq > 65536 || a.Nk > 65536) {
     set_error("%s: need 1 <= Nq,Nk <= 65536 and B,H >= 1 (got B=%lld H=%d Nq=%d Nk=%d)", who,
@@ -448,9 +528,9 @@ int check_attn(const AttnArgs& a, const char* who) {
   return BV_OK;
 }
 
-}  // namespace
-
-int launch_attention_fwd(const AttnArgs& a, cudaStream_t s) {
+template <int DH>
+int attention_fwd(const AttnArgs& a, cudaStream_t s) {
+  using G = Geo<DH>;
   int rc = check_attn(a, "bv_attention_fwd");
   if (rc) return rc;
   FwdDev p;
@@ -461,26 +541,27 @@ int launch_attention_fwd(const AttnArgs& a, cudaStream_t s) {
   p.lse = a.lse;
   p.o = static_cast<bf16*>(a.o);
   p.ldo = a.ldo; p.bso = a.bso;
-  const int cols = a.H * DH;
   CUtensorMap tmQ, tmK, tmV;
-  if ((rc = make_tmap_bnd(&tmQ, a.q, cols, a.Nq, a.B, a.ldq, a.bsq))) return rc;
-  if ((rc = make_tmap_bnd(&tmK, a.k, cols, a.Nk, a.B, a.ldk, a.bsk))) return rc;
-  if ((rc = make_tmap_bnd(&tmV, a.v, cols, a.Nk, a.B, a.ldv, a.bsv))) return rc;
+  if ((rc = make_tmap_bnd(&tmQ, a.q, DH, a.H, a.Nq, a.B, a.ldq, a.bsq))) return rc;
+  if ((rc = make_tmap_bnd(&tmK, a.k, DH, a.H, a.Nk, a.B, a.ldk, a.bsk))) return rc;
+  if ((rc = make_tmap_bnd(&tmV, a.v, DH, a.H, a.Nk, a.B, a.ldv, a.bsv))) return rc;
   const long long grid = a.B * a.H * p.QT;
-  rc = check_cuda(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM),
+  rc = check_cuda(cudaFuncSetAttribute(attn_fwd_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::FWD_SMEM),
                   "cudaFuncSetAttribute(attn_fwd)");
   if (rc) return rc;
-  attn_fwd_kernel<<<static_cast<unsigned>(grid), THREADS, FWD_SMEM, s>>>(tmQ, tmK, tmV, p);
+  attn_fwd_kernel<DH><<<static_cast<unsigned>(grid), THREADS, G::FWD_SMEM, s>>>(tmQ, tmK, tmV, p);
   return check_cuda(cudaGetLastError(), "attn_fwd_kernel launch");
 }
 
-int launch_attention_bwd(const AttnBwdArgs& g, cudaStream_t s) {
+template <int DH>
+int attention_bwd(const AttnBwdArgs& g, cudaStream_t s) {
+  using G = Geo<DH>;
   const AttnArgs& a = g.f;
   int rc = check_attn(a, "bv_attention_bwd");
   if (rc) return rc;
   if (a.lse == nullptr) { set_error("bv_attention_bwd: lse required"); return BV_ERR_INVALID; }
   if (g.dq_accum == nullptr || g.delta == nullptr) {
-    set_error("bv_attention_bwd: needs the dq_accum [ceil(Nk/64),B,Nq,H*64] and delta [B,H,Nq] fp32 workspaces");
+    set_error("bv_attention_bwd: needs the dq_accum [ceil(Nk/64),B,Nq,H*head_dim] and delta [B,H,Nq] fp32 workspaces");
     return BV_ERR_INVALID;
   }
   if ((reinterpret_cast<uintptr_t>(g.d_o) & 15) || (g.lddo % 8) || (g.bsdo % 8)) {
@@ -496,15 +577,16 @@ int launch_attention_bwd(const AttnBwdArgs& g, cudaStream_t s) {
       return BV_ERR_INVALID;
     }
   }
-  if (a.H * DH > 2048) { set_error("bv_attention_bwd: H*64 must be <= 2048"); return BV_ERR_INVALID; }
+  if (a.H * DH > 2048) { set_error("bv_attention_bwd: H*head_dim must be <= 2048"); return BV_ERR_INVALID; }
   const int cols = a.H * DH;
   // delta = rowsum(O o dO)
   {
+    constexpr int lanes = DH == 64 ? 8 : 16;
     const int64_t head_rows = a.B * a.Nq * a.H;
-    int64_t blocks = (head_rows * 8 + 255) / 256;
+    int64_t blocks = (head_rows * lanes + 255) / 256;
     const int64_t cap = static_cast<int64_t>(num_sms()) * 16;
     if (blocks > cap) blocks = cap;
-    attn_delta_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(
+    attn_delta_kernel<DH><<<static_cast<unsigned>(blocks), 256, 0, s>>>(
         reinterpret_cast<const bf16*>(a.o), reinterpret_cast<const bf16*>(g.d_o), g.delta, a.B, a.H, a.Nq,
         a.ldo, a.bso, g.lddo, g.bsdo);
     if ((rc = check_cuda(cudaGetLastError(), "attn_delta_kernel launch"))) return rc;
@@ -522,15 +604,15 @@ int launch_attention_bwd(const AttnBwdArgs& g, cudaStream_t s) {
   p.lddk = g.lddk; p.bsdk = g.bsdk; p.lddv = g.lddv; p.bsdv = g.bsdv;
   p.dk_colsum = g.dk_colsum; p.dv_colsum = g.dv_colsum;
   CUtensorMap tmQ, tmK, tmV, tmdO;
-  if ((rc = make_tmap_bnd(&tmQ, a.q, cols, a.Nq, a.B, a.ldq, a.bsq))) return rc;
-  if ((rc = make_tmap_bnd(&tmK, a.k, cols, a.Nk, a.B, a.ldk, a.bsk))) return rc;
-  if ((rc = make_tmap_bnd(&tmV, a.v, cols, a.Nk, a.B, a.ldv, a.bsv))) return rc;
-  if ((rc = make_tmap_bnd(&tmdO, g.d_o, cols, a.Nq, a.B, g.lddo, g.bsdo))) return rc;
+  if ((rc = make_tmap_bnd(&tmQ, a.q, DH, a.H, a.Nq, a.B, a.ldq, a.bsq))) return rc;
+  if ((rc = make_tmap_bnd(&tmK, a.k, DH, a.H, a.Nk, a.B, a.ldk, a.bsk))) return rc;
+  if ((rc = make_tmap_bnd(&tmV, a.v, DH, a.H, a.Nk, a.B, a.ldv, a.bsv))) return rc;
+  if ((rc = make_tmap_bnd(&tmdO, g.d_o, DH, a.H, a.Nq, a.B, g.lddo, g.bsdo))) return rc;
   const long long grid = a.B * a.H * p.KT;
-  rc = check_cuda(cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM),
+  rc = check_cuda(cudaFuncSetAttribute(attn_bwd_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::BWD_SMEM),
                   "cudaFuncSetAttribute(attn_bwd)");
   if (rc) return rc;
-  attn_bwd_kernel<<<static_cast<unsigned>(grid), THREADS, BWD_SMEM, s>>>(tmQ, tmK, tmV, tmdO, p);
+  attn_bwd_kernel<DH><<<static_cast<unsigned>(grid), THREADS, G::BWD_SMEM, s>>>(tmQ, tmK, tmV, tmdO, p);
   if ((rc = check_cuda(cudaGetLastError(), "attn_bwd_kernel launch"))) return rc;
   {
     const int64_t rows = a.B * a.Nq;
@@ -542,6 +624,30 @@ int launch_attention_bwd(const AttnBwdArgs& g, cudaStream_t s) {
     rc = check_cuda(cudaGetLastError(), "attn_dq_convert_kernel launch");
   }
   return rc;
+}
+
+}  // namespace
+
+int launch_attention_fwd(const AttnArgs& a, int head_dim, cudaStream_t s) {
+  int rc = check_head_dim(head_dim, "bv_attention_fwd");
+  if (rc) return rc;
+  switch (head_dim) {
+    case 72: return attention_fwd<72>(a, s);
+    case 80: return attention_fwd<80>(a, s);
+    case 96: return attention_fwd<96>(a, s);
+    default: return attention_fwd<64>(a, s);
+  }
+}
+
+int launch_attention_bwd(const AttnBwdArgs& g, int head_dim, cudaStream_t s) {
+  int rc = check_head_dim(head_dim, "bv_attention_bwd");
+  if (rc) return rc;
+  switch (head_dim) {
+    case 72: return attention_bwd<72>(g, s);
+    case 80: return attention_bwd<80>(g, s);
+    case 96: return attention_bwd<96>(g, s);
+    default: return attention_bwd<64>(g, s);
+  }
 }
 
 }  // namespace bv

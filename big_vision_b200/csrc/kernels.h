@@ -30,7 +30,7 @@ int launch_layernorm_bwd(const void* dy, int dy_dtype, const void* x, int x_dtyp
 
 // ---- attention (attention.cu)
 struct AttnArgs {
-  const void* q; const void* k; const void* v;   // bf16, [B, N, ld] views with head h at col h*64
+  const void* q; const void* k; const void* v;   // bf16, [B, N, ld] views with head h at col h*head_dim
   void* o;                                       // bf16 [B, Nq, ldo]
   float* lse;                                    // [B, H, Nq] fp32 (log-sum-exp of scaled scores)
   int64_t B; int H; int Nq; int Nk;
@@ -38,17 +38,18 @@ struct AttnArgs {
   int64_t bsq, bsk, bsv, bso;                    // batch strides (elements)
   float scale;
 };
-int launch_attention_fwd(const AttnArgs& a, cudaStream_t s);
+// head_dim: 64, 72, 80 or 96 (anything else: BV_ERR_UNSUPPORTED before any CUDA call)
+int launch_attention_fwd(const AttnArgs& a, int head_dim, cudaStream_t s);
 struct AttnBwdArgs {
   AttnArgs f;
   const void* d_o; int64_t lddo, bsdo;
   void* dq; void* dk; void* dv;                  // bf16, same geometry as q/k/v
-  float* dq_colsum; float* dk_colsum; float* dv_colsum;   // optional [H*64] fp32 bias gradients
+  float* dq_colsum; float* dk_colsum; float* dv_colsum;   // optional [H*head_dim] fp32 bias gradients
   int64_t lddq, lddk, lddv, bsdq, bsdk, bsdv;
   float* delta;                                  // workspace [B, H, Nq] fp32
-  float* dq_accum;                               // workspace [ceil(Nk/64), B, Nq, H*64] fp32
+  float* dq_accum;                               // workspace [ceil(Nk/64), B, Nq, H*head_dim] fp32
 };
-int launch_attention_bwd(const AttnBwdArgs& a, cudaStream_t s);
+int launch_attention_bwd(const AttnBwdArgs& a, int head_dim, cudaStream_t s);
 
 // ---- integer evaluation paths (eval.cu)
 int launch_top1(const void* logits, int dtype, int64_t rows, int C, int64_t ld, int32_t* idx,

@@ -68,6 +68,8 @@ SIGNATURES = {
                          c_vp, c_i64, c_i32, c_vp],
     "bv_attention_fwd": [ctypes.POINTER(AttnArgs), c_vp],
     "bv_attention_bwd": [ctypes.POINTER(AttnBwdArgs), c_vp],
+    "bv_attention_fwd_hd": [ctypes.POINTER(AttnArgs), c_i32, c_vp],
+    "bv_attention_bwd_hd": [ctypes.POINTER(AttnBwdArgs), c_i32, c_vp],
     "bv_patchify": [c_vp, c_vp, c_i64, c_i32, c_i32, c_i32, c_i32, c_vp],
     "bv_patchify_u8": [c_vp, c_vp, c_i64, c_i32, c_i32, c_i32, c_i32, c_f32, c_f32, c_f32, c_f32, c_i32, c_vp],
     "bv_embed_fwd": [c_vp, c_vp, c_vp, c_vp, c_i32, c_i64, c_i32, c_i32, c_i32, c_vp],

@@ -40,6 +40,7 @@ class _Model:
       raise NotImplementedError("dropout > 0 is not on the benchmarked path")
     if self.pool_type not in ("last", "first", "mean", "gap", "max", "gmp", "map"):
       raise NotImplementedError(f"Cannot do pooling '{self.pool_type}'")
+    vit.check_head_dim(self.width, self.num_heads)
     self.prefix = (self.name + "/") if self.name else ""
     self.map_head = (vit.MAPHead(self.prefix + "MAPHead_0/", self.width, self.mlp_dim, self.num_heads)
                      if self.pool_type == "map" else None)

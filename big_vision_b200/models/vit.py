@@ -46,6 +46,14 @@ _VARIANTS = {
 }
 
 
+def check_head_dim(width, num_heads):
+  """Raises NotImplementedError unless width / num_heads is a head dim the attention kernels have."""
+  if width % num_heads or width // num_heads not in ops.ATTN_HEAD_DIMS:
+    raise NotImplementedError(
+        f"width {width} / {num_heads} heads: the attention kernels are built for head dims "
+        f"{', '.join(map(str, ops.ATTN_HEAD_DIMS))}")
+
+
 def decode_variant(variant):
   """"B" / "B/16" -> dict(width, depth, mlp_dim, num_heads[, patch_size]); None -> {}."""
   if variant is None:
@@ -396,8 +404,7 @@ class _Model:
   def __post_init__(self):
     if self.dropout:
       raise NotImplementedError("dropout > 0 is not on the benchmarked path (reference configs use 0)")
-    if self.width % self.num_heads or self.width // self.num_heads != 64:
-      raise NotImplementedError("the attention kernels are built for head dim 64")
+    check_head_dim(self.width, self.num_heads)
     self.mlp = self.mlp_dim or 4 * self.width
     self.prefix = (self.name + "/") if self.name else ""
     self.encoder = Encoder(self.prefix + "Transformer/", self.depth, self.width, self.mlp, self.num_heads,

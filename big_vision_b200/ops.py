@@ -132,23 +132,36 @@ def _attn_args(q, k, v, o, lse, heads, scale):
                     scale=scale)
 
 
+# head dims the attention kernels are built for (bv_attention_fwd_hd / bv_attention_bwd_hd)
+ATTN_HEAD_DIMS = (64, 72, 80, 96)
+
+
+def _head_dim(cols, heads):
+  if cols % heads:
+    raise ValueError(f"attention: {cols} columns do not split into {heads} heads")
+  return cols // heads
+
+
 def attention_fwd(q, k, v, heads, scale=None):
-  """q:[B,Nq,H*64] k,v:[B,Nk,H*64] bf16 (strided views allowed) -> o [B,Nq,H*64], lse [B,H,Nq]."""
+  """q:[B,Nq,H*dh] k,v:[B,Nk,H*dh] bf16 (strided views allowed) -> o [B,Nq,H*dh], lse [B,H,Nq].
+
+  dh is one of ATTN_HEAD_DIMS; the library refuses any other."""
   B, Nq, cols = q.shape
-  assert cols == heads * 64, "head dim must be 64"
+  dh = _head_dim(cols, heads)
   if scale is None:
-    scale = 1.0 / math.sqrt(64)
+    scale = 1.0 / math.sqrt(dh)
   o = torch.empty((B, Nq, cols), dtype=torch.bfloat16, device=q.device)
   lse = torch.empty((B, heads, Nq), dtype=torch.float32, device=q.device)
   args = _attn_args(q, k, v, o, lse, heads, scale)
-  L.call("bv_attention_fwd", ctypes.byref(args), _stream())
+  L.call("bv_attention_fwd_hd", ctypes.byref(args), dh, _stream())
   return o, lse
 
 
 def attention_bwd(do, q, k, v, o, lse, heads, scale=None, dq=None, dk=None, dv=None,
                   dq_colsum=None, dk_colsum=None, dv_colsum=None):
+  dh = _head_dim(q.shape[2], heads)
   if scale is None:
-    scale = 1.0 / math.sqrt(64)
+    scale = 1.0 / math.sqrt(dh)
   if dq is None:
     dq = torch.empty(q.shape, dtype=torch.bfloat16, device=q.device)
   if dk is None:
@@ -169,7 +182,7 @@ def attention_bwd(do, q, k, v, o, lse, heads, scale=None, dq=None, dk=None, dv=N
                        dk_colsum=dk_colsum.data_ptr() if dk_colsum is not None else None,
                        dv_colsum=dv_colsum.data_ptr() if dv_colsum is not None else None,
                        delta=delta.data_ptr(), dq_accum=dq_accum.data_ptr())
-  L.call("bv_attention_bwd", ctypes.byref(args), _stream())
+  L.call("bv_attention_bwd_hd", ctypes.byref(args), dh, _stream())
   L.LAUNCHES[0] += 2            # delta pre-kernel + main kernel + dQ conversion
   return dq, dk, dv
 

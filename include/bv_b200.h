@@ -96,12 +96,15 @@ int bv_layernorm_bwd(const void* dy, int dy_dtype, const void* x, int x_dtype, c
                      int32_t d, void* stream);
 
 /* ---------------------------------------------------------------------------------
- * Scaled-dot-product attention, head dim 64, no mask, any Nq, Nk >= 1
+ * Scaled-dot-product attention, no mask, any Nq, Nk >= 1
  * (flax MultiHeadDotProductAttention core: models/vit.py:93-98, :176-178).  Keys stream through
  * on-chip memory in 64-key blocks (online combination of per-block softmax statistics), so every
  * sequence length takes the same path.
- * q/k/v/o are bf16 strided views: element (b, t, h*64 + j) at
- * base + b*bs + t*ld + h*64 + j  (e.g. column slices of the fused QKV GEMM output).
+ * Head dim dh: 64, 72, 80 or 96 (ViT Ti..L, So400m, H, g-opt / G-opt).  bv_attention_fwd /
+ * bv_attention_bwd are dh = 64; the _hd entry points take dh and refuse any other value with
+ * BV_ERR_UNSUPPORTED before touching the device.
+ * q/k/v/o are bf16 strided views: element (b, t, h*dh + j) at
+ * base + b*bs + t*ld + h*dh + j  (e.g. column slices of the fused QKV GEMM output).
  * lse [B,H,Nq] fp32 = log sum_j exp(scale * q_i.k_j) is saved for the backward.
  * --------------------------------------------------------------------------------- */
 typedef struct bv_attn_args {
@@ -112,20 +115,23 @@ typedef struct bv_attn_args {
   float scale;
 } bv_attn_args;
 int bv_attention_fwd(const bv_attn_args* args, void* stream);
+int bv_attention_fwd_hd(const bv_attn_args* args, int32_t head_dim, void* stream);
 typedef struct bv_attn_bwd_args {
   bv_attn_args fwd;            /* same q,k,v,o,lse as the forward call */
   const void* d_o; int64_t lddo, bsdo;
   void* dq; void* dk; void* dv;
   int64_t lddq, lddk, lddv, bsdq, bsdk, bsdv;
-  /* optional fp32 [H*64] each: += column sums over the valid rows of dq / dk / dv, i.e. the bias
+  /* optional fp32 [H*dh] each: += column sums over the valid rows of dq / dk / dv, i.e. the bias
    * gradients of the projections that produced q / k / v */
   float* dq_colsum; float* dk_colsum; float* dv_colsum;
-  /* REQUIRED workspaces: delta [B,H,Nq] fp32 = rowsum(O o dO); dq_accum [ceil(Nk/64),B,Nq,H*64]
+  /* REQUIRED workspaces: delta [B,H,Nq] fp32 = rowsum(O o dO); dq_accum [ceil(Nk/64),B,Nq,H*dh]
    * fp32 receives the dQ contribution of each 64-key block, summed in block order (reproducible bit
    * for bit) during the bf16 conversion into dq */
   float* delta; float* dq_accum;
 } bv_attn_bwd_args;
 int bv_attention_bwd(const bv_attn_bwd_args* args, void* stream);
+/* H*dh <= 2048 */
+int bv_attention_bwd_hd(const bv_attn_bwd_args* args, int32_t head_dim, void* stream);
 
 /* ---------------------------------------------------------------------------------
  * Data movement / small reductions
