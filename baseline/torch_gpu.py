@@ -23,7 +23,7 @@ import torch.nn.functional as F
 from torch.utils.checkpoint import checkpoint
 
 VIT = {"S": (384, 12, 1536, 6), "B": (768, 12, 3072, 12), "L": (1024, 24, 4096, 16),
-       "So400m": (1152, 27, 4304, 16)}
+       "So400m": (1152, 27, 4304, 16), "G": (1664, 48, 8192, 16)}
 MIXER = {"B": (768, 12, 384, 3072)}
 
 
@@ -204,7 +204,7 @@ def make_step(workload, world, rank, device):
   elif workload["model"] == "vit":
     kw = workload["model_kw"]
     model = ViT(kw["variant"], workload["res"], workload["num_classes"], pool=kw.get("pool_type", "gap"),
-                rep=bool(kw.get("rep_size")))
+                rep=bool(kw.get("rep_size")), remat=workload.get("remat", False))
   else:
     model = Mixer(workload["model_kw"]["variant"], workload["res"], workload["num_classes"])
   model = model.to(device).to(memory_format=torch.channels_last)

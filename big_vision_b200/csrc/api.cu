@@ -173,11 +173,21 @@ int bv_softmax_contrastive_loss(const float* dots, int64_t n, int64_t B, int64_t
 }
 int bv_sigmoid_xent(const float* logits, const float* labels, float* loss, float* dlogits,
                     float* row_loss_ws, int64_t n, int32_t C, void* stream) {
-  return launch_sigmoid_xent(logits, labels, loss, dlogits, row_loss_ws, n, C, S(stream));
+  return bv_sigmoid_xent_ld(logits, C, labels, C, loss, dlogits, C, row_loss_ws, n, C, stream);
+}
+int bv_sigmoid_xent_ld(const float* logits, int64_t ld_logits, const float* labels, int64_t ld_labels, float* loss,
+                       float* dlogits, int64_t ld_dlogits, float* row_loss_ws, int64_t n, int32_t C, void* stream) {
+  return launch_sigmoid_xent(logits, ld_logits, labels, ld_labels, loss, dlogits, ld_dlogits, row_loss_ws, n, C,
+                             S(stream));
 }
 int bv_softmax_xent(const float* logits, const float* labels, float* loss, float* dlogits,
                     float* row_loss_ws, int64_t n, int32_t C, void* stream) {
-  return launch_softmax_xent(logits, labels, loss, dlogits, row_loss_ws, n, C, S(stream));
+  return bv_softmax_xent_ld(logits, C, labels, C, loss, dlogits, C, row_loss_ws, n, C, stream);
+}
+int bv_softmax_xent_ld(const float* logits, int64_t ld_logits, const float* labels, int64_t ld_labels, float* loss,
+                       float* dlogits, int64_t ld_dlogits, float* row_loss_ws, int64_t n, int32_t C, void* stream) {
+  return launch_softmax_xent(logits, ld_logits, labels, ld_labels, loss, dlogits, ld_dlogits, row_loss_ws, n, C,
+                             S(stream));
 }
 
 int bv_adam_step(const bv_adam_args* a, void* stream) {

@@ -2,8 +2,8 @@
 // 1-query attention, K10).  Reference: flax.linen.MultiHeadDotProductAttention as called at
 // models/vit.py:93-98 (self-attention, no mask, no dropout) and models/vit.py:176-178 (MAPHead
 // probe attention): q is scaled by 1/sqrt(dh), softmax over keys, weights times v.  Head dims 64,
-// 72, 80 and 96 are built (the size table of models/vit.py:284-303: 64 for Ti, S, M, B and L, 72
-// for So400m, 80 for H, 96 for g-opt and G-opt); mu (16), g (88), G (104) and e (112) are not.
+// 72, 80, 96 and 104 are built (the size table of models/vit.py:284-303: 64 for Ti, S, M, B and L,
+// 72 for So400m, 80 for H, 96 for g-opt and G-opt, 104 for G); mu (16), g (88) and e (112) are not.
 // Every kernel is a template on the head dim DH.
 //
 // q/k/v/o are strided views into the fused QKV GEMM output: element (b, t, h*DH+j) at
@@ -42,7 +42,7 @@ constexpr int THREADS = 128;
 // the forward holds Q and two K / V slots, the backward K, V, two Q / dO slots and the 64 x 64 dS^T tile.
 template <int DH>
 struct Geo {
-  static_assert(DH == 64 || DH == 72 || DH == 80 || DH == 96, "head dims 64, 72, 80, 96");
+  static_assert(DH == 64 || DH == 72 || DH == 80 || DH == 96 || DH == 104, "head dims 64, 72, 80, 96, 104");
   static constexpr int TILE_BYTES = DH > 64 ? 2 * BOX_BYTES : BOX_BYTES;   // a [64 rows x DH] tile
   static constexpr int KSTEPS = (DH + 15) / 16;                            // k16 steps over the head dim
   static_assert(KSTEPS >= 4 && KSTEPS <= 8, "one or two 64-column boxes");
@@ -96,14 +96,16 @@ __device__ __forceinline__ void wgmma_ss_dh(float (&d)[R], uint64_t a, uint64_t 
   if constexpr (R == 32) wgmma_ss_n64<TA, TB>(d, a, b, scale_d);
   else if constexpr (R == 36) wgmma_ss_n72<TA, TB>(d, a, b, scale_d);
   else if constexpr (R == 40) wgmma_ss_n80<TA, TB>(d, a, b, scale_d);
-  else wgmma_ss_n96<TA, TB>(d, a, b, scale_d);
+  else if constexpr (R == 48) wgmma_ss_n96<TA, TB>(d, a, b, scale_d);
+  else wgmma_ss_n104<TA, TB>(d, a, b, scale_d);
 }
 template <int TB, int R>
 __device__ __forceinline__ void wgmma_rs_dh(float (&d)[R], const uint32_t (&a)[4], uint64_t b, int scale_d) {
   if constexpr (R == 32) wgmma_rs_n64<TB>(d, a, b, scale_d);
   else if constexpr (R == 36) wgmma_rs_n72<TB>(d, a, b, scale_d);
   else if constexpr (R == 40) wgmma_rs_n80<TB>(d, a, b, scale_d);
-  else wgmma_rs_n96<TB>(d, a, b, scale_d);
+  else if constexpr (R == 48) wgmma_rs_n96<TB>(d, a, b, scale_d);
+  else wgmma_rs_n104<TB>(d, a, b, scale_d);
 }
 
 // S[64 x 64] = A B^T over the head dimension (zero-padded to a multiple of 16), both tiles K-major
@@ -505,8 +507,8 @@ attn_dq_convert_kernel(const float* __restrict__ acc, int KT, bf16* __restrict__
 
 // head dims with kernels; every other one is refused before any CUDA call
 int check_head_dim(int head_dim, const char* who) {
-  if (head_dim == 64 || head_dim == 72 || head_dim == 80 || head_dim == 96) return BV_OK;
-  set_error("%s: head_dim %d is not supported (supported head dims: 64, 72, 80, 96)", who, head_dim);
+  if (head_dim == 64 || head_dim == 72 || head_dim == 80 || head_dim == 96 || head_dim == 104) return BV_OK;
+  set_error("%s: head_dim %d is not supported (supported head dims: 64, 72, 80, 96, 104)", who, head_dim);
   return BV_ERR_UNSUPPORTED;
 }
 
@@ -635,6 +637,7 @@ int launch_attention_fwd(const AttnArgs& a, int head_dim, cudaStream_t s) {
     case 72: return attention_fwd<72>(a, s);
     case 80: return attention_fwd<80>(a, s);
     case 96: return attention_fwd<96>(a, s);
+    case 104: return attention_fwd<104>(a, s);
     default: return attention_fwd<64>(a, s);
   }
 }
@@ -646,6 +649,7 @@ int launch_attention_bwd(const AttnBwdArgs& g, int head_dim, cudaStream_t s) {
     case 72: return attention_bwd<72>(g, s);
     case 80: return attention_bwd<80>(g, s);
     case 96: return attention_bwd<96>(g, s);
+    case 104: return attention_bwd<104>(g, s);
     default: return attention_bwd<64>(g, s);
   }
 }

@@ -690,10 +690,15 @@ int launch_drop_cls(const void* x, void* out, int64_t n, int N0, int d, cudaStre
 
 // ---- mixup (K16): utils.py:1146-1158 ---------------------------------------------------------
 //   out[i] = a * x[i] + (1 - a) * x[(i - 1) mod n]      (jnp.roll(x, shift=1, axis=0))
-// One pass, 16-byte vectors; the rolled operand is the row the neighbouring block has just read,
+// One pass, 16-byte vectors when every row is a whole number of them (a scalar pass otherwise, e.g. the
+// [n, 21843] labels of ImageNet-21k); the rolled operand is the row the neighbouring block has just read,
 // so it is served by L2.  Products and the sum are rounded separately (no FMA contraction): the
 // result is bit-identical to the fp32 expression evaluated left to right.
 namespace {
+__device__ __forceinline__ float mix1(float a, float b, float u, float v) {
+  return __fadd_rn(__fmul_rn(a, u), __fmul_rn(b, v));
+}
+
 __global__ void __launch_bounds__(256)
 mixup_kernel(const float4* __restrict__ x, float4* __restrict__ out, int64_t n, int64_t row_vec, float a) {
   const float b = __fsub_rn(1.0f, a);
@@ -704,27 +709,45 @@ mixup_kernel(const float4* __restrict__ x, float4* __restrict__ out, int64_t n, 
     const int64_t ip = (i == 0) ? n - 1 : i - 1;
     const float4 u = x[idx], v = x[ip * row_vec + c];
     float4 o;
-    o.x = __fadd_rn(__fmul_rn(a, u.x), __fmul_rn(b, v.x));
-    o.y = __fadd_rn(__fmul_rn(a, u.y), __fmul_rn(b, v.y));
-    o.z = __fadd_rn(__fmul_rn(a, u.z), __fmul_rn(b, v.z));
-    o.w = __fadd_rn(__fmul_rn(a, u.w), __fmul_rn(b, v.w));
+    o.x = mix1(a, b, u.x, v.x);
+    o.y = mix1(a, b, u.y, v.y);
+    o.z = mix1(a, b, u.z, v.z);
+    o.w = mix1(a, b, u.w, v.w);
     out[idx] = o;
+  }
+}
+
+__global__ void __launch_bounds__(256)
+mixup_scalar_kernel(const float* __restrict__ x, float* __restrict__ out, int64_t n, int64_t row_elems, float a) {
+  const float b = __fsub_rn(1.0f, a);
+  const int64_t total = n * row_elems;
+  for (int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; idx < total;
+       idx += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int64_t i = idx / row_elems, c = idx - i * row_elems;
+    const int64_t ip = (i == 0) ? n - 1 : i - 1;
+    out[idx] = mix1(a, b, x[idx], x[ip * row_elems + c]);
   }
 }
 }  // namespace
 
 int launch_mixup(const float* x, float* out, int64_t n, int64_t row_elems, float a, cudaStream_t s) {
-  if (n <= 0 || row_elems <= 0 || row_elems % 4 != 0 || x == out ||
-      (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(out) & 15)) {
-    set_error("bv_mixup: need n, row_elems >= 1, row_elems %% 4 == 0, 16B-aligned distinct buffers");
+  if (n <= 0 || row_elems <= 0 || x == out ||
+      (reinterpret_cast<uintptr_t>(x) & 3) || (reinterpret_cast<uintptr_t>(out) & 3)) {
+    set_error("bv_mixup: need n, row_elems >= 1, 4B-aligned distinct buffers");
     return BV_ERR_INVALID;
   }
-  const int64_t total = n * (row_elems / 4);
+  const bool vec = row_elems % 4 == 0 && !(reinterpret_cast<uintptr_t>(x) & 15) &&
+                   !(reinterpret_cast<uintptr_t>(out) & 15);
+  const int64_t total = vec ? n * (row_elems / 4) : n * row_elems;
   int64_t blocks = (total + 255) / 256;
   const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
   if (blocks > cap) blocks = cap;
-  mixup_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(
-      reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(out), n, row_elems / 4, a);
+  if (vec) {
+    mixup_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(
+        reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(out), n, row_elems / 4, a);
+  } else {
+    mixup_scalar_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(x, out, n, row_elems, a);
+  }
   return check_cuda(cudaGetLastError(), "mixup_kernel launch");
 }
 

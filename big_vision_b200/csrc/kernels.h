@@ -38,7 +38,7 @@ struct AttnArgs {
   int64_t bsq, bsk, bsv, bso;                    // batch strides (elements)
   float scale;
 };
-// head_dim: 64, 72, 80 or 96 (anything else: BV_ERR_UNSUPPORTED before any CUDA call)
+// head_dim: 64, 72, 80, 96 or 104 (anything else: BV_ERR_UNSUPPORTED before any CUDA call)
 int launch_attention_fwd(const AttnArgs& a, int head_dim, cudaStream_t s);
 struct AttnBwdArgs {
   AttnArgs f;
@@ -106,10 +106,11 @@ int launch_siglip_loss_ew(const float* dots, int64_t n, int64_t B, int64_t ld, i
 int launch_softmax_contrastive(const float* dots, int64_t n, int64_t B, int64_t ld, int64_t row_offset,
                                const float* t_param, int64_t global_B, float weight, void* G, int64_t ldg,
                                float* loss, float* dt, float* ncorrect, float* rows_ws, cudaStream_t s);
-int launch_sigmoid_xent(const float* logits, const float* labels, float* loss, float* dlogits,
-                        float* row_loss, int64_t n, int C, cudaStream_t s);
-int launch_softmax_xent(const float* logits, const float* labels, float* loss, float* dlogits,
-                        float* row_loss, int64_t n, int C, cudaStream_t s);
+// row strides ldx / ldy / ldd >= C (else BV_ERR_INVALID before any CUDA call); dlogits columns C..ldd-1 = 0
+int launch_sigmoid_xent(const float* logits, int64_t ldx, const float* labels, int64_t ldy, float* loss,
+                        float* dlogits, int64_t ldd, float* row_loss, int64_t n, int C, cudaStream_t s);
+int launch_softmax_xent(const float* logits, int64_t ldx, const float* labels, int64_t ldy, float* loss,
+                        float* dlogits, int64_t ldd, float* row_loss, int64_t n, int C, cudaStream_t s);
 
 // ---- optimizer (optim.cu)
 struct AdamArgs {

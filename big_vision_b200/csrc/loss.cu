@@ -157,10 +157,11 @@ softmax_contrastive_kernel(const float* __restrict__ dots, int64_t n, int64_t B,
   }
 }
 
-// one warp per row
+// one warp per row.  Row strides ldx / ldy / ldd; the dlogits columns C..ldd-1 are written as zeros, so
+// a head stored with padded columns can feed the [n, ldd] gradient straight to its GEMMs.
 __global__ void __launch_bounds__(256)
-sigmoid_xent_kernel(const float* __restrict__ logits, const float* __restrict__ labels,
-                    float* __restrict__ loss, float* __restrict__ dlogits,
+sigmoid_xent_kernel(const float* __restrict__ logits, int64_t ldx, const float* __restrict__ labels, int64_t ldy,
+                    float* __restrict__ loss, float* __restrict__ dlogits, int64_t ldd,
                     float* __restrict__ row_loss, int64_t n, int C) {
   const int lane = threadIdx.x & 31;
   const int64_t row = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5);
@@ -168,9 +169,12 @@ sigmoid_xent_kernel(const float* __restrict__ logits, const float* __restrict__ 
   const float inv_n = 1.f / static_cast<float>(n);
   float acc = 0.f;
   for (int c = lane; c < C; c += 32) {
-    const float x = logits[row * C + c], y = labels[row * C + c];
+    const float x = logits[row * ldx + c], y = labels[row * ldy + c];
     acc -= y * log_sigmoid(x) + (1.f - y) * log_sigmoid(-x);
-    if (dlogits) dlogits[row * C + c] = (sigmoid(x) - y) * inv_n;
+    if (dlogits) dlogits[row * ldd + c] = (sigmoid(x) - y) * inv_n;
+  }
+  if (dlogits) {
+    for (int64_t c = C + lane; c < ldd; c += 32) dlogits[row * ldd + c] = 0.f;
   }
   acc = warp_sum(acc);
   if (lane == 0) {
@@ -179,19 +183,19 @@ sigmoid_xent_kernel(const float* __restrict__ logits, const float* __restrict__ 
 }
 
 __global__ void __launch_bounds__(256)
-softmax_xent_kernel(const float* __restrict__ logits, const float* __restrict__ labels,
-                    float* __restrict__ loss, float* __restrict__ dlogits,
+softmax_xent_kernel(const float* __restrict__ logits, int64_t ldx, const float* __restrict__ labels, int64_t ldy,
+                    float* __restrict__ loss, float* __restrict__ dlogits, int64_t ldd,
                     float* __restrict__ row_loss, int64_t n, int C) {
   const int lane = threadIdx.x & 31;
   const int64_t row = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5);
   if (row >= n) return;
   const float inv_n = 1.f / static_cast<float>(n);
   float mx = -INFINITY;
-  for (int c = lane; c < C; c += 32) mx = fmaxf(mx, logits[row * C + c]);
+  for (int c = lane; c < C; c += 32) mx = fmaxf(mx, logits[row * ldx + c]);
   mx = warp_max(mx);
   float se = 0.f, sy = 0.f, sxy = 0.f;
   for (int c = lane; c < C; c += 32) {
-    const float x = logits[row * C + c] - mx, y = labels[row * C + c];
+    const float x = logits[row * ldx + c] - mx, y = labels[row * ldy + c];
     se += __expf(x); sy += y; sxy += y * x;
   }
   se = warp_sum(se); sy = warp_sum(sy); sxy = warp_sum(sxy);
@@ -203,9 +207,10 @@ softmax_xent_kernel(const float* __restrict__ logits, const float* __restrict__ 
   }
   if (dlogits) {
     for (int c = lane; c < C; c += 32) {
-      const float x = logits[row * C + c] - mx, y = labels[row * C + c];
-      dlogits[row * C + c] = (__expf(x - lse) * sy - y) * inv_n;
+      const float x = logits[row * ldx + c] - mx, y = labels[row * ldy + c];
+      dlogits[row * ldd + c] = (__expf(x - lse) * sy - y) * inv_n;
     }
+    for (int64_t c = C + lane; c < ldd; c += 32) dlogits[row * ldd + c] = 0.f;
   }
 }
 
@@ -248,21 +253,31 @@ int launch_softmax_contrastive(const float* dots, int64_t n, int64_t B, int64_t 
   return check_cuda(cudaGetLastError(), "finish_sums_kernel launch");
 }
 
-int launch_sigmoid_xent(const float* logits, const float* labels, float* loss, float* dlogits,
-                        float* row_loss, int64_t n, int C, cudaStream_t s) {
+int launch_sigmoid_xent(const float* logits, int64_t ldx, const float* labels, int64_t ldy, float* loss,
+                        float* dlogits, int64_t ldd, float* row_loss, int64_t n, int C, cudaStream_t s) {
+  if (ldx < C || ldy < C || ldd < C) {
+    set_error("bv_sigmoid_xent_ld: row strides must be >= C (ld_logits %lld, ld_labels %lld, ld_dlogits %lld, C %d)",
+              static_cast<long long>(ldx), static_cast<long long>(ldy), static_cast<long long>(ldd), C);
+    return BV_ERR_INVALID;
+  }
   if (n <= 0) return BV_OK;
-  sigmoid_xent_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(logits, labels, loss, dlogits,
-                                                                        row_loss, n, C);
+  sigmoid_xent_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(logits, ldx, labels, ldy, loss, dlogits,
+                                                                        ldd, row_loss, n, C);
   int rc = check_cuda(cudaGetLastError(), "sigmoid_xent_kernel launch");
   if (rc || row_loss == nullptr) return rc;
   finish_sums_kernel<<<1, 256, 0, s>>>(row_loss, n, loss, nullptr, nullptr);
   return check_cuda(cudaGetLastError(), "finish_sums_kernel launch");
 }
-int launch_softmax_xent(const float* logits, const float* labels, float* loss, float* dlogits,
-                        float* row_loss, int64_t n, int C, cudaStream_t s) {
+int launch_softmax_xent(const float* logits, int64_t ldx, const float* labels, int64_t ldy, float* loss,
+                        float* dlogits, int64_t ldd, float* row_loss, int64_t n, int C, cudaStream_t s) {
+  if (ldx < C || ldy < C || ldd < C) {
+    set_error("bv_softmax_xent_ld: row strides must be >= C (ld_logits %lld, ld_labels %lld, ld_dlogits %lld, C %d)",
+              static_cast<long long>(ldx), static_cast<long long>(ldy), static_cast<long long>(ldd), C);
+    return BV_ERR_INVALID;
+  }
   if (n <= 0) return BV_OK;
-  softmax_xent_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(logits, labels, loss, dlogits,
-                                                                        row_loss, n, C);
+  softmax_xent_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(logits, ldx, labels, ldy, loss, dlogits,
+                                                                        ldd, row_loss, n, C);
   int rc = check_cuda(cudaGetLastError(), "softmax_xent_kernel launch");
   if (rc || row_loss == nullptr) return rc;
   finish_sums_kernel<<<1, 256, 0, s>>>(row_loss, n, loss, nullptr, nullptr);

@@ -98,6 +98,8 @@ SIGNATURES = {
                                     c_vp, c_vp, c_vp],
     "bv_sigmoid_xent": [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp],
     "bv_softmax_xent": [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp],
+    "bv_sigmoid_xent_ld": [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp],
+    "bv_softmax_xent_ld": [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp],
     "bv_adam_step": [ctypes.POINTER(AdamArgs), c_vp],
     "bv_sumsq": [c_vp, c_vp, c_i64, c_vp],
     "bv_adafactor_step": [ctypes.POINTER(AdafactorArgs), c_vp],
@@ -144,7 +146,8 @@ def check(rc, what):
 # kernels launched by this process through the C ABI (bench.py reports it as gpu_launches)
 LAUNCHES = [0]
 _LAUNCHES_PER_CALL = {"bv_embed_bwd": 2, "bv_retrieval_ranks": 2, "bv_siglip_loss": 2,
-                      "bv_sigmoid_xent": 2, "bv_softmax_xent": 2, "bv_softmax_contrastive_loss": 2, "bv_adafactor_step": 4}
+                      "bv_sigmoid_xent": 2, "bv_softmax_xent": 2, "bv_sigmoid_xent_ld": 2, "bv_softmax_xent_ld": 2,
+                      "bv_softmax_contrastive_loss": 2, "bv_adafactor_step": 4}
 LOSS_WS_FLOATS = 8192      # BV_LOSS_WS_FLOATS
 
 

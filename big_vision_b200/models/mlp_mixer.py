@@ -21,6 +21,7 @@ import torch
 from big_vision_b200 import engine as E
 from big_vision_b200 import lib as L
 from big_vision_b200 import ops
+from big_vision_b200.models import common
 from big_vision_b200.models import vit
 
 
@@ -56,6 +57,7 @@ class MlpMixer:
 
   def __post_init__(self):
     self._geom = None
+    self.head = common.ClassifierHead("", self.hidden_dim, self.num_classes, E.zeros) if self.num_classes else None
 
   def drop_p(self, i):
     """mlp_mixer.py:76"""
@@ -92,9 +94,10 @@ class MlpMixer:
         specs += s
         aliases += a
     specs += vit.ln_specs("pre_head_layer_norm/", d)
-    if self.num_classes:
-      specs += [E.ParamSpec("head/kernel", (d, self.num_classes), E.zeros),
-                E.ParamSpec("head/bias", (self.num_classes,), E.zeros)]
+    if self.head is not None:
+      s, a = self.head.specs()
+      specs += s
+      aliases += a
     self._N, self._Np = N, Np
     return specs, aliases
 
@@ -139,21 +142,16 @@ class MlpMixer:
     y, mean, rstd = ops.layernorm_fwd(x, P.f("pre_head_layer_norm/scale"), P.f("pre_head_layer_norm/bias"))
     saved["norm"] = (x, mean, rstd)
     out = ops.pool_fwd(y, n, N, 0, out_dtype=torch.float32)
-    if self.num_classes:
+    if self.head is not None:
       saved["head_in"] = out
-      out = ops.gemm(vit._Model._to16(out), P.h("head/kernel"), b_mn=True, bias=P.f("head/bias"),
-                     out_dtype=torch.float32)
+      out = self.head.fwd(P, out)
     return out, saved
 
   def bwd(self, P, dout, saved):
     n = saved["n"]
     d, N, Np, T = self.hidden_dim, self._N, self._Np, self.tokens_mlp_dim
-    if self.num_classes:
-      d16 = vit._Model._to16(dout)
-      ops.colsum(dout, P.g("head/bias"))
-      ops.gemm(vit._Model._to16(saved["head_in"]), d16, a_mn=True, b_mn=True, out=P.g("head/kernel"),
-               reduce_out=True)
-      dout = ops.gemm(d16, P.h("head/kernel"), out_dtype=torch.float32)
+    if self.head is not None:
+      dout = self.head.bwd(P, dout, saved["head_in"])
     dy = ops.pool_bwd(dout, n, N, 0)
     x, mean, rstd = saved["norm"]
     masks = saved.get("masks")

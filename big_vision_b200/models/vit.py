@@ -20,6 +20,7 @@ import torch
 from big_vision_b200 import engine as E
 from big_vision_b200 import lib as L
 from big_vision_b200 import ops
+from big_vision_b200.models import common
 
 
 def posemb_sincos_2d(h, w, width, temperature=10_000.0):
@@ -411,6 +412,11 @@ class _Model:
                            scan=self.scan, remat_policy=self.remat_policy)
     self.map_head = (MAPHead(self.prefix + "MAPHead_0/", self.width, self.mlp, self.num_heads)
                      if self.pool_type == "map" else None)
+    self.head = None
+    if self.num_classes:
+      rep = (self.width if self.rep_size is True else self.rep_size) if self.rep_size else self.width
+      self.head = common.ClassifierHead(self.prefix, rep, self.num_classes,
+                                        E.zeros if self.head_zeroinit else E.lecun_normal(rep))
     self._geom = None
 
   # ---- parameters ------------------------------------------------------------------------
@@ -451,11 +457,10 @@ class _Model:
       rep = d if self.rep_size is True else self.rep_size
       specs += [E.ParamSpec(p + "pre_logits/kernel", (d, rep), E.lecun_normal(d)),
                 E.ParamSpec(p + "pre_logits/bias", (rep,), E.zeros)]
-    if self.num_classes:
-      rep = (d if self.rep_size is True else self.rep_size) if self.rep_size else d
-      kinit = E.zeros if self.head_zeroinit else E.lecun_normal(rep)
-      specs += [E.ParamSpec(p + "head/kernel", (rep, self.num_classes), kinit),
-                E.ParamSpec(p + "head/bias", (self.num_classes,), E.zeros)]
+    if self.head is not None:
+      s, a = self.head.specs()
+      specs += s
+      aliases += a
     self._in_ch, self._K, self._Kp = in_ch, K, Kp
     return specs, aliases
 
@@ -474,7 +479,8 @@ class _Model:
     return self._sincos
 
   def fwd(self, P, image):
-    """image [n,H,W,C] fp32 in [-1,1] -> (x fp32 [n, out], saved)."""
+    """image [n,H,W,C] fp32 in [-1,1] -> (x fp32 [n, out], saved).  With a class head whose storage is
+    padded (common.ClassifierHead) x is the [n, num_classes] view of the padded logits."""
     if self._geom is None:
       self.setup(image.shape[1:3])
     n = image.shape[0]
@@ -516,34 +522,27 @@ class _Model:
       saved["rep_in"] = out
       out = ops.tanh_fwd(pre)
       saved["rep_out"] = out
-    if self.num_classes:
+    if self.head is not None:
       saved["head_in"] = out
-      out = ops.gemm(self._to16(out), P.h(p + "head/kernel"), b_mn=True, bias=P.f(p + "head/bias"),
-                     out_dtype=torch.float32)
+      out = self.head.fwd(P, out)
     if self.pool_type == "none":
       if out.dtype != torch.float32:
         out = ops.cast(out, torch.empty_like(out, dtype=torch.float32))
       out = out.view(n, N, -1)
     return out, saved
 
-  @staticmethod
-  def _to16(x):
-    if x.dtype == torch.bfloat16:
-      return x
-    return ops.cast(x, torch.empty_like(x, dtype=torch.bfloat16))
+  _to16 = staticmethod(common.to16)
 
   def bwd(self, P, dout, saved):
-    """dout: fp32 [n, out] ([n, N, out] without pooling).  Accumulates parameter gradients into P.grad."""
+    """dout: fp32 [n, out] ([n, N, out] without pooling).  Accumulates parameter gradients into P.grad.
+    With a padded class head, out is the padded class count (ClassifierHead.bwd)."""
     p, d = self.prefix, self.width
     n, N = saved["n"], saved["N"]
     en = self.prefix + "Transformer/encoder_norm/"
     if self.pool_type == "none":
       dout = dout.reshape(n * N, -1)
-    if self.num_classes:
-      d16 = self._to16(dout)
-      ops.colsum(dout, P.g(p + "head/bias"))
-      ops.gemm(self._to16(saved["head_in"]), d16, a_mn=True, b_mn=True, out=P.g(p + "head/kernel"), reduce_out=True)
-      dout = ops.gemm(d16, P.h(p + "head/kernel"), out_dtype=torch.float32)
+    if self.head is not None:
+      dout = self.head.bwd(P, dout, saved["head_in"])
     if self.rep_size:
       dpre = ops.tanh_bwd(dout, saved["rep_out"])
       d16 = self._to16(dpre)

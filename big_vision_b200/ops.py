@@ -133,7 +133,7 @@ def _attn_args(q, k, v, o, lse, heads, scale):
 
 
 # head dims the attention kernels are built for (bv_attention_fwd_hd / bv_attention_bwd_hd)
-ATTN_HEAD_DIMS = (64, 72, 80, 96)
+ATTN_HEAD_DIMS = (64, 72, 80, 96, 104)
 
 
 def _head_dim(cols, heads):
@@ -294,7 +294,7 @@ def gelu_fwd(x):
 
 
 def mixup(x, a):
-  """a * x + (1 - a) * roll(x, 1, axis 0) for an fp32 tensor whose rows have a multiple of 4 elements."""
+  """a * x + (1 - a) * roll(x, 1, axis 0) for an fp32 tensor (rows of any length)."""
   x = x.contiguous()
   assert x.dtype == torch.float32, x.dtype
   out = torch.empty_like(x)
@@ -368,20 +368,26 @@ def softmax_contrastive_loss(dots, row_offset, t_param, global_b, weight, loss, 
   return G
 
 
-def sigmoid_xent(logits, labels, loss, want_grad=True):
+def _xent(name, logits, labels, loss, want_grad, dlogits_cols):
+  logits, ldx = _rowmajor(logits)
+  labels, ldy = _rowmajor(labels)
   n, C = logits.shape
-  dl = torch.empty_like(logits) if want_grad else None
+  dl = torch.empty((n, dlogits_cols or C), dtype=torch.float32, device=logits.device) if want_grad else None
   ws = torch.empty(n, dtype=torch.float32, device=logits.device)
-  L.call("bv_sigmoid_xent", _p(logits), _p(labels), _p(loss), _p(dl), _p(ws), n, C, _stream())
+  L.call(name, _p(logits), ldx, _p(labels), ldy, _p(loss), _p(dl), dl.stride(0) if want_grad else C, _p(ws), n, C,
+         _stream())
   return dl
 
 
-def softmax_xent(logits, labels, loss, want_grad=True):
-  n, C = logits.shape
-  dl = torch.empty_like(logits) if want_grad else None
-  ws = torch.empty(n, dtype=torch.float32, device=logits.device)
-  L.call("bv_softmax_xent", _p(logits), _p(labels), _p(loss), _p(dl), _p(ws), n, C, _stream())
-  return dl
+def sigmoid_xent(logits, labels, loss, want_grad=True, dlogits_cols=None):
+  """Mean sigmoid cross-entropy of logits / labels [n, C] (row-strided views allowed) accumulated into
+  `loss`; returns d loss / d logits [n, dlogits_cols or C], zero in the columns past C."""
+  return _xent("bv_sigmoid_xent_ld", logits, labels, loss, want_grad, dlogits_cols)
+
+
+def softmax_xent(logits, labels, loss, want_grad=True, dlogits_cols=None):
+  """softmax_xent counterpart of sigmoid_xent."""
+  return _xent("bv_softmax_xent_ld", logits, labels, loss, want_grad, dlogits_cols)
 
 
 def sumsq(x, out):

@@ -24,9 +24,13 @@ def loss_and_grads(model, P, images, labels, loss_name="sigmoid_xent", dist_view
   logits, saved = model.fwd(P, images, **fwd_kw)
   loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
   # unpooled models (pool_type="none") give [n, N, classes]: the losses sum over the class axis and
-  # average over all leading axes (utils.py:236-243,276-281), i.e. over the n*N rows
+  # average over all leading axes (utils.py:236-243,276-281), i.e. over the n*N rows.  A head with
+  # padded storage returns a view of [rows, Cp] logits; the gradient is written [rows, Cp] with zero
+  # padding columns, the layout the head's backward GEMMs take.
   flat = logits.reshape(-1, logits.shape[-1])
-  dlogits = _LOSSES[loss_name](flat, labels.reshape(flat.shape), loss).view(logits.shape)
+  ld = flat.stride(0)
+  dlogits = _LOSSES[loss_name](flat, labels.reshape(flat.shape), loss, dlogits_cols=ld)
+  dlogits = dlogits.view(*logits.shape[:-1], ld)
   if dist_view is None:
     model.bwd(P, dlogits, saved)
   else:      # gradient all-reduce (SUM; callers divide by world) overlapped with the backward

@@ -100,7 +100,7 @@ int bv_layernorm_bwd(const void* dy, int dy_dtype, const void* x, int x_dtype, c
  * (flax MultiHeadDotProductAttention core: models/vit.py:93-98, :176-178).  Keys stream through
  * on-chip memory in 64-key blocks (online combination of per-block softmax statistics), so every
  * sequence length takes the same path.
- * Head dim dh: 64, 72, 80 or 96 (ViT Ti..L, So400m, H, g-opt / G-opt).  bv_attention_fwd /
+ * Head dim dh: 64, 72, 80, 96 or 104 (ViT Ti..L, So400m, H, g-opt / G-opt, G).  bv_attention_fwd /
  * bv_attention_bwd are dh = 64; the _hd entry points take dh and refuse any other value with
  * BV_ERR_UNSUPPORTED before touching the device.
  * q/k/v/o are bf16 strided views: element (b, t, h*dh + j) at
@@ -183,7 +183,8 @@ int bv_tanh_fwd(const void* x, void* y, int dtype, int64_t n, void* stream);
 int bv_tanh_bwd(const void* dy, const void* y, void* dx, int dtype, int64_t n, void* stream);
 int bv_gelu_fwd(const void* x, void* y, int dtype, int64_t n, void* stream);
 /* utils.py:1146-1158 (get_mixup): out[i,:] = a * x[i,:] + (1-a) * x[(i-1) mod n,:], fp32, out != x;
- * products and sum rounded separately (bit-identical to the fp32 expression). row_elems % 4 == 0. */
+ * products and sum rounded separately (bit-identical to the fp32 expression).  Any row_elems >= 1 and
+ * 4-byte aligned buffers; 16-byte vectors when row_elems % 4 == 0 and both buffers are 16-byte aligned. */
 int bv_mixup(const float* x, float* out, int64_t n, int64_t row_elems, float a, void* stream);
 int bv_axpby(const void* x, const void* y, void* out, int dtype, float a, float b, int64_t n,
              void* stream);
@@ -238,6 +239,15 @@ int bv_sigmoid_xent(const float* logits, const float* labels, float* loss, float
                     float* row_loss_ws, int64_t n, int32_t C, void* stream);
 int bv_softmax_xent(const float* logits, const float* labels, float* loss, float* dlogits,
                     float* row_loss_ws, int64_t n, int32_t C, void* stream);
+/* The same losses on row-strided logits [n, ld_logits], labels [n, ld_labels] and dlogits
+ * [n, ld_dlogits] (columns 0..C-1 used).  The dlogits columns C..ld_dlogits-1 are written as zeros, so
+ * a classifier head stored with padded columns takes the gradient as its GEMM operand unchanged.
+ * Any ld < C: BV_ERR_INVALID before any CUDA call.  bv_sigmoid_xent / bv_softmax_xent are these calls
+ * with every ld = C. */
+int bv_sigmoid_xent_ld(const float* logits, int64_t ld_logits, const float* labels, int64_t ld_labels, float* loss,
+                       float* dlogits, int64_t ld_dlogits, float* row_loss_ws, int64_t n, int32_t C, void* stream);
+int bv_softmax_xent_ld(const float* logits, int64_t ld_logits, const float* labels, int64_t ld_labels, float* loss,
+                       float* dlogits, int64_t ld_dlogits, float* row_loss_ws, int64_t n, int32_t C, void* stream);
 
 /* ---------------------------------------------------------------------------------
  * Optimizer (optax.py:143-149 chain with scale_by_adam; siglip.py:312-321)
