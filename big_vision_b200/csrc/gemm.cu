@@ -1,4 +1,4 @@
-// Warp-specialised wgmma GEMM for sm_90a.
+// Warp-specialised, persistent wgmma GEMM for sm_90a.
 //
 //   D[M,N] = epilogue( alpha * sum_k A(m,k) * B(n,k) )
 //
@@ -13,44 +13,60 @@
 // (reference call sites: flax Dense/DenseGeneral under models/vit.py:72-77,93-98,
 //  176-178,212-214,261,272; models/mlp_mixer.py:35-37,72,82).
 //
-// One CTA owns one 128 x BN output tile (x one K split).  Roles (384 threads): warpgroup 0 is the
+// The grid is persistent: min(work units, SMs) CTAs, each running a static sequence of work units
+// (one 128 x BN output tile x one K split; gemm_sched.h).  Roles (384 threads): warpgroup 0 is the
 // TMA producer (one thread issues, the rest give their registers back with setmaxnreg), warpgroups
 // 1 and 2 each run m64 x BN x 16 wgmma on their half of the rows from a STAGES-deep ring of shared
-// memory, then apply the epilogue straight from the accumulator registers.
+// memory.  The ring's barriers live for the whole CTA and the producer runs ahead across units, so
+// the next tile's loads overlap this tile's epilogue.  Plain bf16 outputs leave through shared
+// memory and TMA stores; fp32 and bf16 reduce-add outputs store from the registers.
 #include "common.cuh"
+#include "gemm_sched.h"
 #include "host_utils.h"
 #include "kernels.h"
 
 #include <atomic>
 
 #include <stdlib.h>
+#include <string.h>
 
 namespace bv {
 
 namespace {
 
-constexpr int BM = 128;          // rows per CTA (two consumer warpgroups of 64)
+constexpr int BM = 128;          // rows per tile (two consumer warpgroups of 64)
 constexpr int BK = 64;           // 64 bf16 = 128 B = one swizzle row
 constexpr int A_STAGE_BYTES = BM * BK * 2;   // 16 KB
 constexpr int NUM_THREADS = 384;
+constexpr int SUB_BYTES = 64 * 64 * 2;       // one 64 x 64 bf16 output sub-tile, 128B-swizzled
 
 // epilogue families (template parameter)
 enum : int { EF_BIAS = 0, EF_GELU = 1, EF_RESID = 2, EF_DGELU = 3 };
+// output modes (template parameter): fp32 from the registers, bf16 reduce-add from the registers,
+// plain bf16 by TMA store
+enum : int { OM_F32 = 0, OM_BF16_ADD = 1, OM_BF16_TMA = 2 };
 
-template <int BN>
+template <int BN, int OM, int EF>
 struct Cfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
+  // TMA-store staging of bf16 outputs: per consumer warpgroup two buffers (one fills while the
+  // other's store is in flight), each holding one sub-tile of every output (GELU writes two)
+  static constexpr int OUTS = OM != OM_BF16_TMA ? 0 : (EF == EF_GELU ? 2 : 1);
+  static constexpr int BUF_BYTES = OUTS * SUB_BYTES;
+  static constexpr int STAGING_BYTES = 2 * 2 * BUF_BYTES;
   static constexpr int SMEM_LIMIT = 232448 - 2048;         // 227 KB minus barriers / align slack
-  static constexpr int STAGES_FIT = SMEM_LIMIT / STAGE_BYTES;
+  static constexpr int STAGES_FIT = (SMEM_LIMIT - STAGING_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
-  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int STAGING_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int BAR_OFFSET = STAGING_OFFSET + STAGING_BYTES;
   static constexpr int SMEM_BYTES = BAR_OFFSET + 256 + 1024;  // + barriers + align slack
+  static_assert(STAGES >= 3, "shared-memory budget leaves fewer than 3 stages");
 };
 
 struct GemmDev {
-  int M, N, K;
-  int kblocks_total, kblocks_per_split;
+  GemmSched s;
+  int M, N;
   int a_mn, b_mn;        // 1 = MN-major
   int reduce_out;        // 1 = atomic add into D (split-K / grad accumulation)
   float alpha;
@@ -62,22 +78,21 @@ struct GemmDev {
   int aux_row_mod;
 };
 
-// The consumer warpgroup's main loop.  The transpose bits of wgmma are immediates, so each operand
-// layout pair is its own instantiation (a branch between wgmma issues would make ptxas serialise them).
+// The consumer warpgroup's main loop over one unit's k blocks.  `ps` is the running ring position,
+// carried from unit to unit.  The transpose bits of wgmma are immediates, so each operand layout pair
+// is its own instantiation (a branch between wgmma issues would make ptxas serialise them).
 template <int BN, int STAGES, int STAGE_BYTES, int TA, int TB>
-__device__ __forceinline__ void mainloop(float (&acc)[BN / 2], uint32_t base, uint32_t bar_base, int cw, int kb0,
-                                         int kb1) {
+__device__ __forceinline__ void mainloop(float (&acc)[BN / 2], uint32_t base, uint32_t bar_base, int cw,
+                                         PipeState& ps, int kb0, int kb1) {
   // 128B-swizzled operand tiles: K-major rows of 128 B (8-row groups 1024 B apart, K step 32 B);
   // MN-major boxes of 64 (M|N) x 64 (K), 8 KB each (K step 16 rows = 2048 B)
   constexpr uint32_t a_lbo = TA ? 8192u : 16u, b_lbo = TB ? 8192u : 16u;
   constexpr uint32_t a_kstep = TA ? 2048u : 32u, b_kstep = TB ? 2048u : 32u;
-  int stage = 0;
-  uint32_t phase = 0;
   int prev_stage = -1;
   for (int kb = kb0; kb < kb1; ++kb) {
-    mbar_wait(bar_base + 8u * stage, phase);
-    const uint32_t a_s = base + stage * STAGE_BYTES + cw * 8192;
-    const uint32_t b_s = base + stage * STAGE_BYTES + A_STAGE_BYTES;
+    mbar_wait(bar_base + 8u * ps.stage, ps.phase);
+    const uint32_t a_s = base + ps.stage * STAGE_BYTES + cw * 8192;
+    const uint32_t b_s = base + ps.stage * STAGE_BYTES + A_STAGE_BYTES;
     const uint64_t adesc = wgmma_desc_sw128(a_s, a_lbo, 1024u), bdesc = wgmma_desc_sw128(b_s, b_lbo, 1024u);
     wgmma_fence_regs(acc);
     wgmma_fence();
@@ -93,18 +108,195 @@ __device__ __forceinline__ void mainloop(float (&acc)[BN / 2], uint32_t base, ui
     // keep this k block's MMAs in flight; the previous one has retired -> its slot is free
     wgmma_wait<1>();
     if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_base + 8u * (STAGES + prev_stage));
-    prev_stage = stage;
-    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+    prev_stage = ps.stage;
+    ps.advance(STAGES);
   }
+  // every MMA of the unit has retired, so the last slot is free before the epilogue starts
   wgmma_wait<0>();
   wgmma_fence_regs(acc);
   if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_base + 8u * (STAGES + prev_stage));
 }
 
+// alpha, bias and the element-wise op of the epilogue on one column pair (col, col + 1) of one row,
+// both inside the output (col + 1 only if `pair`).  pre0/pre1: GELU's pre-activation (bf16-rounded).
+template <bool OUT_F32, int EF>
+__device__ __forceinline__ void epi_math(const GemmDev& p, float alpha, float c0, float c1, float b0, float b1,
+                                         int row, int col, bool pair, float& v0, float& v1, float& pre0,
+                                         float& pre1) {
+  constexpr bool HAS_AUX = (EF == EF_RESID || EF == EF_DGELU);
+  v0 = c0 * alpha + b0;
+  v1 = c1 * alpha + b1;
+  float a0 = 0.f, a1 = 0.f;
+  if (HAS_AUX) {
+    const long long ar = p.aux_row_mod > 0 ? (row % p.aux_row_mod) : row;
+    const bf16* ap = p.aux + ar * p.ldaux + col;
+    if (pair) {
+      const uint32_t q = *reinterpret_cast<const uint32_t*>(ap);
+      a0 = bf16_lo(q); a1 = bf16_hi(q);
+    } else {
+      a0 = __bfloat162float(*ap);
+    }
+  }
+  pre0 = pre1 = 0.f;
+  if (EF == EF_GELU) {
+    pre0 = round_bf16(v0); pre1 = round_bf16(v1);
+    v0 = gelu_tanh_fast(pre0); v1 = gelu_tanh_fast(pre1);
+  } else if (EF == EF_RESID) {
+    v0 = (OUT_F32 ? v0 : round_bf16(v0)) + a0;
+    v1 = (OUT_F32 ? v1 : round_bf16(v1)) + a1;
+  } else if (EF == EF_DGELU) {
+    v0 *= gelu_tanh_grad_fast(a0);
+    v1 *= gelu_tanh_grad_fast(a1);
+  }
+}
+
+// Accumulator layout (per warp w of the warpgroup, lane l): element 4j + e sits at row
+// 16w + l/4 + 8*(e >> 1), column 8j + 2*(l%4) + (e & 1).
+
+// Bias gradient fused into the producer: s0/s1 are one thread's sums of the stored (bf16-rounded)
+// values in columns col and col + 1; the eight lanes that share a column pair are summed with
+// shuffles, then one atomic per warp and column.
+__device__ __forceinline__ void colsum_add(float* colsum, int N, float s0, float s1, int col, int lane) {
+  s0 += __shfl_xor_sync(0xffffffffu, s0, 4);
+  s0 += __shfl_xor_sync(0xffffffffu, s0, 8);
+  s0 += __shfl_xor_sync(0xffffffffu, s0, 16);
+  s1 += __shfl_xor_sync(0xffffffffu, s1, 4);
+  s1 += __shfl_xor_sync(0xffffffffu, s1, 8);
+  s1 += __shfl_xor_sync(0xffffffffu, s1, 16);
+  if (lane < 4) {
+    if (col < N) atomicAdd(colsum + col, s0);
+    if (col + 1 < N) atomicAdd(colsum + col + 1, s1);
+  }
+}
+
+// Epilogue straight from the registers: fp32 outputs, and bf16 reduce-add outputs (gradient
+// accumulation; never with colsum).
 template <int BN, bool OUT_F32, int EF>
+__device__ __forceinline__ void epilogue_regs(const GemmDev& p, const float (&acc)[BN / 2], int m0, int n0,
+                                              int cw) {
+  const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
+  const int row0 = m0 + cw * 64 + warp * 16 + (lane >> 2);
+  const int pM = p.M, pN = p.N;
+  const float alpha = p.alpha;
+  const bool reduce = p.reduce_out != 0;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = n0 + 8 * j + 2 * (lane & 3);
+    if (col >= pN) continue;
+    const bool pair = col + 1 < pN;
+    float b0 = 0.f, b1 = 0.f;
+    if (p.bias != nullptr) {
+      b0 = __ldg(p.bias + col);
+      if (pair) b1 = __ldg(p.bias + col + 1);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 8 * h;
+      if (row >= pM) continue;
+      float v0, v1, pre0, pre1;
+      epi_math<OUT_F32, EF>(p, alpha, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], b0, b1, row, col, pair, v0, v1,
+                            pre0, pre1);
+      if (OUT_F32) {
+        float* dp = static_cast<float*>(p.d) + row * p.ldd + col;
+        if (reduce) {
+          atomicAdd(dp, v0);
+          if (pair) atomicAdd(dp + 1, v1);
+        } else if (pair) {
+          *reinterpret_cast<float2*>(dp) = make_float2(v0, v1);
+        } else {
+          *dp = v0;
+        }
+      } else {
+        bf16* dp = static_cast<bf16*>(p.d) + row * p.ldd + col;
+        const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
+        if (pair) atomicAdd(reinterpret_cast<__nv_bfloat162*>(dp), o);
+        else atomicAdd(dp, o.x);
+      }
+    }
+  }
+}
+
+// Epilogue through shared memory for plain bf16 outputs: the warpgroup writes each 64-column
+// sub-tile of its 64 rows into a 128B-swizzled staging buffer (the 16-byte chunk index XOR the row
+// mod 8, so the 8 rows of one store instruction hit different banks), and one thread stores it with
+// TMA, which clips rows >= M and columns >= N.  The two buffers alternate; `nstore` counts the
+// warpgroup's sub-tiles across units, and the issuing thread waits until the store that last read a
+// buffer is done reading before the buffer is refilled.
+template <int BN, int EF, int BUF_BYTES>
+__device__ __forceinline__ void epilogue_tma(const GemmDev& p, const CUtensorMap* tmD, const CUtensorMap* tmD2,
+                                             const float (&acc)[BN / 2], int m0, int n0, int cw, uint32_t staging,
+                                             uint32_t& nstore) {
+  const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const int rl0 = warp * 16 + (lane >> 2);       // row within the warpgroup's 64
+  const int row0 = m0 + cw * 64 + rl0;
+  const int pM = p.M, pN = p.N;
+  const float alpha = p.alpha;
+#pragma unroll
+  for (int c = 0; c < BN / 64; ++c) {
+    const uint32_t buf = staging + (nstore & 1u) * BUF_BYTES;
+    if (leader) tma_store_wait_read<1>();
+    named_bar_sync(1 + cw, 128);
+    float cs[8][2];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int j = 8 * c + jj;
+      const int col = n0 + 8 * j + 2 * (lane & 3);
+      cs[jj][0] = cs[jj][1] = 0.f;
+      const bool cin = col < pN, pair = col + 1 < pN;
+      float b0 = 0.f, b1 = 0.f;
+      if (cin && p.bias != nullptr) {
+        b0 = __ldg(p.bias + col);
+        if (pair) b1 = __ldg(p.bias + col + 1);
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int rl = rl0 + 8 * h, row = row0 + 8 * h;
+        float v0 = 0.f, v1 = 0.f, pre0 = 0.f, pre1 = 0.f;
+        const bool in = cin && row < pM;
+        if (in)
+          epi_math<false, EF>(p, alpha, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], b0, b1, row, col, pair, v0, v1,
+                              pre0, pre1);
+        const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
+        if (in) {
+          cs[jj][0] += __low2float(o);
+          cs[jj][1] += pair ? __high2float(o) : 0.f;
+        }
+        const uint32_t off = rl * 128 + ((jj ^ (rl & 7)) << 4) + (lane & 3) * 4;
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(buf + off), "r"(*reinterpret_cast<const uint32_t*>(&o))
+                     : "memory");
+        if (EF == EF_GELU) {
+          const __nv_bfloat162 q = __floats2bfloat162_rn(pre0, pre1);
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(buf + SUB_BYTES + off),
+                       "r"(*reinterpret_cast<const uint32_t*>(&q))
+                       : "memory");
+        }
+      }
+    }
+    // make the generic-proxy writes visible to the TMA engine, then hand the buffer to one thread
+    fence_proxy_async();
+    named_bar_sync(1 + cw, 128);
+    if (leader) {
+      if (n0 + 64 * c < pN && m0 + cw * 64 < pM) {      // sub-tiles wholly past the edge are not stored
+        tma_store_2d(tmD, buf, n0 + 64 * c, m0 + cw * 64);
+        if (EF == EF_GELU) tma_store_2d(tmD2, buf + SUB_BYTES, n0 + 64 * c, m0 + cw * 64);
+      }
+      tma_store_commit();
+    }
+    ++nstore;
+    if (p.colsum != nullptr) {
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+        colsum_add(p.colsum, pN, cs[jj][0], cs[jj][1], n0 + 8 * (8 * c + jj) + 2 * (lane & 3), lane);
+    }
+  }
+}
+
+template <int BN, int OM, int EF>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
-  using C = Cfg<BN>;
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+            const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmD2, const GemmDev p) {
+  using C = Cfg<BN, OM, EF>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t base = (raw_addr + 1023u) & ~1023u;
@@ -113,10 +305,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
 
   const int wg = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 7), 0);
-  const int n0 = static_cast<int>(blockIdx.x) * BN;
-  const int m0 = static_cast<int>(blockIdx.y) * BM;
-  const int kb0 = static_cast<int>(blockIdx.z) * p.kblocks_per_split;
-  const int kb1 = min(kb0 + p.kblocks_per_split, p.kblocks_total);
+  const int units = p.s.units;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
@@ -133,28 +322,30 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     // ========================= TMA producer =========================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (threadIdx.x == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(empty_bar(stage), phase ^ 1u);
-        const uint32_t a_s = base + stage * C::STAGE_BYTES;
-        const uint32_t b_s = a_s + A_STAGE_BYTES;
-        const uint32_t fb = full_bar(stage);
-        mbar_expect_tx(fb, C::STAGE_BYTES);
-        const int k0 = kb * BK;
-        if (p.a_mn) {
+      PipeState ps;
+      for (int u = blockIdx.x; u < units; u += gridDim.x) {
+        const WorkUnit w = gemm_work_unit(p.s, u, BM, BN);
+        for (int kb = w.kb0; kb < w.kb1; ++kb) {
+          mbar_wait(empty_bar(ps.stage), ps.phase ^ 1u);
+          const uint32_t a_s = base + ps.stage * C::STAGE_BYTES;
+          const uint32_t b_s = a_s + A_STAGE_BYTES;
+          const uint32_t fb = full_bar(ps.stage);
+          mbar_expect_tx(fb, C::STAGE_BYTES);
+          const int k0 = kb * BK;
+          if (p.a_mn) {
 #pragma unroll
-          for (int j = 0; j < BM / 64; ++j) tma_load_2d(a_s + j * 8192, &tmA, fb, m0 + 64 * j, k0);
-        } else {
-          tma_load_2d(a_s, &tmA, fb, k0, m0);
-        }
-        if (p.b_mn) {
+            for (int j = 0; j < BM / 64; ++j) tma_load_2d(a_s + j * 8192, &tmA, fb, w.m0 + 64 * j, k0);
+          } else {
+            tma_load_2d(a_s, &tmA, fb, k0, w.m0);
+          }
+          if (p.b_mn) {
 #pragma unroll
-          for (int j = 0; j < BN / 64; ++j) tma_load_2d(b_s + j * 8192, &tmB, fb, n0 + 64 * j, k0);
-        } else {
-          tma_load_2d(b_s, &tmB, fb, k0, n0);
+            for (int j = 0; j < BN / 64; ++j) tma_load_2d(b_s + j * 8192, &tmB, fb, w.n0 + 64 * j, k0);
+          } else {
+            tma_load_2d(b_s, &tmB, fb, k0, w.n0);
+          }
+          ps.advance(C::STAGES);
         }
-        if (++stage == C::STAGES) { stage = 0; phase ^= 1u; }
       }
     }
     return;
@@ -163,122 +354,32 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   // ========================= consumers: warpgroups 1, 2 =========================
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
   const int cw = wg - 1;                        // which 64-row half of the tile
-  float acc[BN / 2];
+  const uint32_t staging = base + C::STAGING_OFFSET + cw * 2 * C::BUF_BYTES;
+  uint32_t nstore = 0;
+  PipeState ps;
   constexpr int S = C::STAGES, SB = C::STAGE_BYTES;
-  if (p.a_mn) {
-    if (p.b_mn) mainloop<BN, S, SB, 1, 1>(acc, base, bar_base, cw, kb0, kb1);
-    else mainloop<BN, S, SB, 1, 0>(acc, base, bar_base, cw, kb0, kb1);
-  } else {
-    if (p.b_mn) mainloop<BN, S, SB, 0, 1>(acc, base, bar_base, cw, kb0, kb1);
-    else mainloop<BN, S, SB, 0, 0>(acc, base, bar_base, cw, kb0, kb1);
-  }
+  for (int u = blockIdx.x; u < units; u += gridDim.x) {
+    const WorkUnit w = gemm_work_unit(p.s, u, BM, BN);
+    float acc[BN / 2];
+    if (p.a_mn) {
+      if (p.b_mn) mainloop<BN, S, SB, 1, 1>(acc, base, bar_base, cw, ps, w.kb0, w.kb1);
+      else mainloop<BN, S, SB, 1, 0>(acc, base, bar_base, cw, ps, w.kb0, w.kb1);
+    } else {
+      if (p.b_mn) mainloop<BN, S, SB, 0, 1>(acc, base, bar_base, cw, ps, w.kb0, w.kb1);
+      else mainloop<BN, S, SB, 0, 0>(acc, base, bar_base, cw, ps, w.kb0, w.kb1);
+    }
 
-  // ========================= epilogue from registers =========================
-  // Accumulator layout (per warp w of the warpgroup, lane l): element 4j + e sits at row
-  // 16w + l/4 + 8*(e >> 1), column 8j + 2*(l%4) + (e & 1).
-  const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
-  const int row0 = m0 + cw * 64 + warp * 16 + (lane >> 2);
-  const int pM = p.M, pN = p.N;
-  const float alpha = p.alpha;
-  const bool reduce = p.reduce_out != 0;
-  constexpr bool HAS_AUX = (EF == EF_RESID || EF == EF_DGELU);
-  float cs[BN / 8][2];
-#pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int col = n0 + 8 * j + 2 * (lane & 3);
-    cs[j][0] = cs[j][1] = 0.f;
-    if (col >= pN) continue;
-    const bool pair = col + 1 < pN;
-    float b0 = 0.f, b1 = 0.f;
-    if (p.bias != nullptr) {
-      b0 = __ldg(p.bias + col);
-      if (pair) b1 = __ldg(p.bias + col + 1);
-    }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = row0 + 8 * h;
-      if (row >= pM) continue;
-      float v0 = acc[4 * j + 2 * h] * alpha + b0, v1 = acc[4 * j + 2 * h + 1] * alpha + b1;
-      float a0 = 0.f, a1 = 0.f;
-      if (HAS_AUX) {
-        const long long ar = p.aux_row_mod > 0 ? (row % p.aux_row_mod) : row;
-        const bf16* ap = p.aux + ar * p.ldaux + col;
-        if (pair) {
-          const uint32_t q = *reinterpret_cast<const uint32_t*>(ap);
-          a0 = bf16_lo(q); a1 = bf16_hi(q);
-        } else {
-          a0 = __bfloat162float(*ap);
-        }
-      }
-      float pre0 = 0.f, pre1 = 0.f;
-      if (EF == EF_GELU) {
-        pre0 = round_bf16(v0); pre1 = round_bf16(v1);
-        v0 = gelu_tanh_fast(pre0); v1 = gelu_tanh_fast(pre1);
-      } else if (EF == EF_RESID) {
-        v0 = (OUT_F32 ? v0 : round_bf16(v0)) + a0;
-        v1 = (OUT_F32 ? v1 : round_bf16(v1)) + a1;
-      } else if (EF == EF_DGELU) {
-        v0 *= gelu_tanh_grad_fast(a0);
-        v1 *= gelu_tanh_grad_fast(a1);
-      }
-      if (OUT_F32) {
-        float* dp = static_cast<float*>(p.d) + row * p.ldd + col;
-        if (reduce) {
-          atomicAdd(dp, v0);
-          if (pair) atomicAdd(dp + 1, v1);
-        } else if (pair) {
-          *reinterpret_cast<float2*>(dp) = make_float2(v0, v1);
-        } else {
-          *dp = v0;
-        }
-      } else {
-        bf16* dp = static_cast<bf16*>(p.d) + row * p.ldd + col;
-        const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
-        if (reduce) {
-          if (pair) atomicAdd(reinterpret_cast<__nv_bfloat162*>(dp), o);
-          else atomicAdd(dp, o.x);
-        } else if (pair) {
-          *reinterpret_cast<__nv_bfloat162*>(dp) = o;
-        } else {
-          *dp = o.x;
-        }
-        cs[j][0] += __low2float(o);
-        cs[j][1] += pair ? __high2float(o) : 0.f;
-        if (EF == EF_GELU) {
-          bf16* d2 = static_cast<bf16*>(p.d2) + row * p.ldd2 + col;
-          const __nv_bfloat162 q = __floats2bfloat162_rn(pre0, pre1);
-          if (pair) *reinterpret_cast<__nv_bfloat162*>(d2) = q;
-          else *d2 = q.x;
-        }
-      }
-    }
+    if constexpr (OM == OM_BF16_TMA) epilogue_tma<BN, EF, C::BUF_BYTES>(p, &tmD, &tmD2, acc, w.m0, w.n0, cw, staging, nstore);
+    else epilogue_regs<BN, OM == OM_F32, EF>(p, acc, w.m0, w.n0, cw);
   }
-  if (!OUT_F32 && p.colsum != nullptr) {
-    // bias gradient fused into the producer: column sums of the stored (bf16-rounded) values; the
-    // eight lanes that share a column pair are summed with shuffles, then one atomic per warp
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        float s = cs[j][e];
-        s += __shfl_xor_sync(0xffffffffu, s, 4);
-        s += __shfl_xor_sync(0xffffffffu, s, 8);
-        s += __shfl_xor_sync(0xffffffffu, s, 16);
-        cs[j][e] = s;
-      }
-      const int col = n0 + 8 * j + 2 * (lane & 3);
-      if (lane < 4) {
-        if (col < pN) atomicAdd(p.colsum + col, cs[j][0]);
-        if (col + 1 < pN) atomicAdd(p.colsum + col + 1, cs[j][1]);
-      }
-    }
-  }
+  // the staging buffers must outlive every bulk store that reads them
+  if (OM == OM_BF16_TMA && (threadIdx.x & 127) == 0) tma_store_wait<0>();
 }
 
-template <int BN, bool OUT_F32, int EF>
+template <int BN, int OM, int EF>
 int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
-  using C = Cfg<BN>;
-  CUtensorMap tmA, tmB;
+  using C = Cfg<BN, OM, EF>;
+  CUtensorMap tmA, tmB, tmD, tmD2;
   int rc;
   const CUtensorMapDataType bf = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   if (g.a_mn) rc = make_tmap_2d(&tmA, bf, g.A, g.M, g.K, g.lda * 2, 64, 64);
@@ -289,39 +390,13 @@ int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
   if (rc) return rc;
 
   GemmDev p;
-  p.M = (int)g.M; p.N = (int)g.N; p.K = (int)g.K;
-  const int num_m = (int)((g.M + BM - 1) / BM);
-  const int num_n = (int)((g.N + BN - 1) / BN);
-  p.kblocks_total = (int)((g.K + BK - 1) / BK);
-  int splits = g.splits;
-  if (splits <= 0) {
-    // auto (reduce-add outputs only, i.e. the weight gradients): the split count whose work units fill
-    // whole waves of the grid best (one CTA per SM).  Each extra split costs one more fp32 reduce-add
-    // of the output tile, negligible against a K of 10^5.
-    splits = 1;
-    if (g.reduce_out) {
-      const int slots = num_sms();
-      const int tiles = num_m * num_n;
-      int smax = p.kblocks_total / 16;
-      if (smax > 32) smax = 32;
-      double best = -1.0;
-      for (int sp = 1; sp <= smax; ++sp) {
-        const int units = tiles * sp;
-        const int waves = (units + slots - 1) / slots;
-        const double eff = static_cast<double>(units) / (static_cast<double>(waves) * slots) - 0.002 * sp;
-        if (eff > best + 1e-9) { best = eff; splits = sp; }
-      }
-    }
-  }
-  if (splits > p.kblocks_total) splits = p.kblocks_total;
-  if (splits < 1) splits = 1;
-  if (splits > 1 && !g.reduce_out) {
+  const long long tiles = ((g.M + BM - 1) / BM) * ((g.N + BN - 1) / BN);
+  if (tiles * ((g.K + BK - 1) / BK) > 0x7fffffffLL) { set_error("bv_gemm: problem too large"); return BV_ERR_INVALID; }
+  if (!gemm_make_sched(g.M, g.N, g.K, BM, BN, BK, g.splits, g.reduce_out != 0, num_sms(), &p.s)) {
     set_error("bv_gemm: split-K requires reduce_out=1");
     return BV_ERR_INVALID;
   }
-  p.kblocks_per_split = (p.kblocks_total + splits - 1) / splits;
-  splits = (p.kblocks_total + p.kblocks_per_split - 1) / p.kblocks_per_split;
-  if (splits > 65535 || num_m > 65535) { set_error("bv_gemm: grid too large"); return BV_ERR_INVALID; }
+  p.M = (int)g.M; p.N = (int)g.N;
   p.a_mn = g.a_mn; p.b_mn = g.b_mn; p.reduce_out = g.reduce_out;
   p.alpha = g.alpha;
   p.bias = g.bias;
@@ -331,8 +406,20 @@ int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
   p.aux_row_mod = g.aux_row_mod;
   p.d = g.D; p.d2 = g.D2;
   p.ldd = g.ldd; p.ldd2 = g.ldd2;
+  // the output maps span exactly M x N, so TMA leaves the rows past M and the columns past N of a
+  // strided output alone
+  memset(&tmD, 0, sizeof(tmD));
+  memset(&tmD2, 0, sizeof(tmD2));
+  if (OM == OM_BF16_TMA) {
+    rc = make_tmap_2d(&tmD, bf, g.D, g.N, g.M, g.ldd * 2, 64, 64);
+    if (rc) return rc;
+    if (EF == EF_GELU) {
+      rc = make_tmap_2d(&tmD2, bf, g.D2, g.N, g.M, g.ldd2 * 2, 64, 64);
+      if (rc) return rc;
+    }
+  }
 
-  auto kern = gemm_kernel<BN, OUT_F32, EF>;
+  auto kern = gemm_kernel<BN, OM, EF>;
   // The dynamic-shared-memory opt-in is a per-DEVICE attribute of the kernel: cache it per device
   // (one process may drive several GPUs from several host threads; the flags are atomics and a
   // duplicate set by two racing threads is harmless).
@@ -345,25 +432,31 @@ int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
     if (rc) return rc;
     if (dev >= 0) attr_set[dev].store(true, std::memory_order_release);
   }
-  kern<<<dim3(num_n, num_m, splits), NUM_THREADS, C::SMEM_BYTES, stream>>>(tmA, tmB, p);
+  const int grid = p.s.units < num_sms() ? p.s.units : num_sms();
+  kern<<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(tmA, tmB, tmD, tmD2, p);
   return check_cuda(cudaGetLastError(), "gemm_kernel launch");
 }
 
+// Plain bf16 outputs leave by TMA store; fp32 outputs and bf16 reduce-add outputs keep the register
+// epilogue.  bf16 reduce-adds (gradient accumulation into bf16, not on the training step's path) run
+// at BN = 128: at 256 their atomics make ptxas spill the accumulators inside the persistent loop.
 template <int BN>
 int dispatch_epi(const GemmArgs& g, cudaStream_t s) {
-  const bool f32 = (g.out_dtype == DT_F32);
+  const bool f32 = (g.out_dtype == DT_F32), add = !f32 && g.reduce_out;
   switch (g.epi) {
     case EPI_NONE:
     case EPI_BIAS:
-      return f32 ? launch_cfg<BN, true, EF_BIAS>(g, s) : launch_cfg<BN, false, EF_BIAS>(g, s);
+      return f32 ? launch_cfg<BN, OM_F32, EF_BIAS>(g, s)
+                 : add ? launch_cfg<128, OM_BF16_ADD, EF_BIAS>(g, s) : launch_cfg<BN, OM_BF16_TMA, EF_BIAS>(g, s);
     case EPI_BIAS_RESID:
-      return f32 ? launch_cfg<BN, true, EF_RESID>(g, s) : launch_cfg<BN, false, EF_RESID>(g, s);
-    case EPI_BIAS_GELU:
-      return launch_cfg<BN, false, EF_GELU>(g, s);
+      return f32 ? launch_cfg<BN, OM_F32, EF_RESID>(g, s)
+                 : add ? launch_cfg<128, OM_BF16_ADD, EF_RESID>(g, s) : launch_cfg<BN, OM_BF16_TMA, EF_RESID>(g, s);
+    case EPI_BIAS_GELU:     // never a reduce-add (refused in launch_gemm)
+      return launch_cfg<BN, OM_BF16_TMA, EF_GELU>(g, s);
     case EPI_DGELU:
       if (f32) { set_error("bv_gemm: DGELU epilogue writes bf16"); return BV_ERR_INVALID; }
       if (g.aux_row_mod > 0) { set_error("bv_gemm: DGELU takes a row-aligned aux"); return BV_ERR_INVALID; }
-      return launch_cfg<BN, false, EF_DGELU>(g, s);
+      return add ? launch_cfg<128, OM_BF16_ADD, EF_DGELU>(g, s) : launch_cfg<BN, OM_BF16_TMA, EF_DGELU>(g, s);
   }
   set_error("bv_gemm: bad epilogue %d", g.epi);
   return BV_ERR_INVALID;
@@ -373,8 +466,7 @@ int dispatch_epi(const GemmArgs& g, cudaStream_t s) {
 
 int launch_gemm(const GemmArgs& g, cudaStream_t stream) {
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) { set_error("bv_gemm: empty problem"); return BV_ERR_INVALID; }
-  // N need not be a multiple of 8 as long as the row strides are (TMA clips the loads)
-  // the epilogue stores bf16 pairs / fp32 pairs straight from registers
+  // N need not be a multiple of 8 as long as the row strides are (TMA clips the loads and stores)
   if (g.out_dtype == DT_BF16 && ((reinterpret_cast<uintptr_t>(g.D) & 15) || (g.ldd % 8))) {
     set_error("bv_gemm: bf16 output must be 16B aligned with ldd %% 8 == 0"); return BV_ERR_INVALID;
   }
