@@ -19,7 +19,9 @@
 // 1 and 2 each run m64 x BN x 16 wgmma on their half of the rows from a STAGES-deep ring of shared
 // memory.  The ring's barriers live for the whole CTA and the producer runs ahead across units, so
 // the next tile's loads overlap this tile's epilogue.  Plain bf16 outputs leave through shared
-// memory and TMA stores; fp32 and bf16 reduce-add outputs store from the registers.
+// memory and TMA stores; a row-aligned aux operand (residual, gelu' pre-activation) arrives by TMA
+// into the same staging buffers during the main loop.  fp32 and bf16 reduce-add outputs store from
+// the registers.
 #include "common.cuh"
 #include "gemm_sched.h"
 #include "host_utils.h"
@@ -40,8 +42,10 @@ constexpr int A_STAGE_BYTES = BM * BK * 2;   // 16 KB
 constexpr int NUM_THREADS = 384;
 constexpr int SUB_BYTES = 64 * 64 * 2;       // one 64 x 64 bf16 output sub-tile, 128B-swizzled
 
-// epilogue families (template parameter)
-enum : int { EF_BIAS = 0, EF_GELU = 1, EF_RESID = 2, EF_DGELU = 3 };
+// epilogue families (template parameter).  EF_RESID_ROWMOD is the residual whose aux rows wrap
+// (aux_row_mod > 0, the position embedding): a tile's row window can wrap around it, so it is not one
+// TMA box and its TMA-store kernel reads aux from global memory in the accumulator layout.
+enum : int { EF_BIAS = 0, EF_GELU = 1, EF_RESID = 2, EF_DGELU = 3, EF_RESID_ROWMOD = 4 };
 // output modes (template parameter): fp32 from the registers, bf16 reduce-add from the registers,
 // plain bf16 by TMA store
 enum : int { OM_F32 = 0, OM_BF16_ADD = 1, OM_BF16_TMA = 2 };
@@ -50,18 +54,25 @@ template <int BN, int OM, int EF>
 struct Cfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  // TMA-store staging of bf16 outputs: per consumer warpgroup two buffers (one fills while the
-  // other's store is in flight), each holding one sub-tile of every output (GELU writes two)
+  // TMA-store staging of bf16 outputs, each buffer holding one sub-tile of every output (GELU writes
+  // two).  Per consumer warpgroup either two buffers (one fills while the other's store is in
+  // flight), or, when aux is loaded by TMA, one buffer per sub-tile of the unit, so that the whole
+  // unit's aux is prefetched during its main loop.
+  static constexpr bool AUX_TMA = OM == OM_BF16_TMA && (EF == EF_RESID || EF == EF_DGELU);
   static constexpr int OUTS = OM != OM_BF16_TMA ? 0 : (EF == EF_GELU ? 2 : 1);
   static constexpr int BUF_BYTES = OUTS * SUB_BYTES;
-  static constexpr int STAGING_BYTES = 2 * 2 * BUF_BYTES;
+  static constexpr int BUFS = AUX_TMA ? BN / 64 : 2;
+  static constexpr int STAGING_BYTES = 2 * BUFS * BUF_BYTES;
   static constexpr int SMEM_LIMIT = 232448 - 2048;         // 227 KB minus barriers / align slack
   static constexpr int STAGES_FIT = (SMEM_LIMIT - STAGING_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
   static constexpr int STAGING_OFFSET = STAGES * STAGE_BYTES;
   static constexpr int BAR_OFFSET = STAGING_OFFSET + STAGING_BYTES;
+  // barriers: full and empty per stage, then (AUX_TMA) one per staging buffer of each warpgroup
+  static constexpr int AUX_BAR = 2 * STAGES;
   static constexpr int SMEM_BYTES = BAR_OFFSET + 256 + 1024;  // + barriers + align slack
   static_assert(STAGES >= 3, "shared-memory budget leaves fewer than 3 stages");
+  static_assert(8 * (AUX_BAR + (AUX_TMA ? 2 * BUFS : 0)) <= 256, "barriers overflow their 256 bytes");
 };
 
 struct GemmDev {
@@ -81,9 +92,11 @@ struct GemmDev {
 // The consumer warpgroup's main loop over one unit's k blocks.  `ps` is the running ring position,
 // carried from unit to unit.  The transpose bits of wgmma are immediates, so each operand layout pair
 // is its own instantiation (a branch between wgmma issues would make ptxas serialise them).
-template <int BN, int STAGES, int STAGE_BYTES, int TA, int TB>
+// `after_first` runs once, after the first k block's MMAs are committed, so that whatever it waits
+// for overlaps them.
+template <int BN, int STAGES, int STAGE_BYTES, int TA, int TB, typename F>
 __device__ __forceinline__ void mainloop(float (&acc)[BN / 2], uint32_t base, uint32_t bar_base, int cw,
-                                         PipeState& ps, int kb0, int kb1) {
+                                         PipeState& ps, int kb0, int kb1, F&& after_first) {
   // 128B-swizzled operand tiles: K-major rows of 128 B (8-row groups 1024 B apart, K step 32 B);
   // MN-major boxes of 64 (M|N) x 64 (K), 8 KB each (K step 16 rows = 2048 B)
   constexpr uint32_t a_lbo = TA ? 8192u : 16u, b_lbo = TB ? 8192u : 16u;
@@ -105,6 +118,7 @@ __device__ __forceinline__ void mainloop(float (&acc)[BN / 2], uint32_t base, ui
     }
     wgmma_commit();
     wgmma_fence_regs(acc);
+    if (kb == kb0) after_first();
     // keep this k block's MMAs in flight; the previous one has retired -> its slot is free
     wgmma_wait<1>();
     if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_base + 8u * (STAGES + prev_stage));
@@ -117,31 +131,33 @@ __device__ __forceinline__ void mainloop(float (&acc)[BN / 2], uint32_t base, ui
   if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_base + 8u * (STAGES + prev_stage));
 }
 
-// alpha, bias and the element-wise op of the epilogue on one column pair (col, col + 1) of one row,
-// both inside the output (col + 1 only if `pair`).  pre0/pre1: GELU's pre-activation (bf16-rounded).
+// The aux pair (col, col + 1) of one row, read from global memory in the accumulator layout (col + 1
+// only if `pair`); aux_row_mod > 0 wraps the row.  The register epilogues and EF_RESID_ROWMOD use it.
+__device__ __forceinline__ void aux_global(const GemmDev& p, int row, int col, bool pair, float& a0, float& a1) {
+  const long long ar = p.aux_row_mod > 0 ? (row % p.aux_row_mod) : row;
+  const bf16* ap = p.aux + ar * p.ldaux + col;
+  if (pair) {
+    const uint32_t q = *reinterpret_cast<const uint32_t*>(ap);
+    a0 = bf16_lo(q); a1 = bf16_hi(q);
+  } else {
+    a0 = __bfloat162float(*ap);
+    a1 = 0.f;
+  }
+}
+
+// alpha, bias and the element-wise op of the epilogue on one column pair (col, col + 1) of one row.
+// a0/a1: the aux pair (residual or gelu' pre-activation).  pre0/pre1: GELU's pre-activation
+// (bf16-rounded).
 template <bool OUT_F32, int EF>
-__device__ __forceinline__ void epi_math(const GemmDev& p, float alpha, float c0, float c1, float b0, float b1,
-                                         int row, int col, bool pair, float& v0, float& v1, float& pre0,
-                                         float& pre1) {
-  constexpr bool HAS_AUX = (EF == EF_RESID || EF == EF_DGELU);
+__device__ __forceinline__ void epi_math(float alpha, float c0, float c1, float b0, float b1, float a0, float a1,
+                                         float& v0, float& v1, float& pre0, float& pre1) {
   v0 = c0 * alpha + b0;
   v1 = c1 * alpha + b1;
-  float a0 = 0.f, a1 = 0.f;
-  if (HAS_AUX) {
-    const long long ar = p.aux_row_mod > 0 ? (row % p.aux_row_mod) : row;
-    const bf16* ap = p.aux + ar * p.ldaux + col;
-    if (pair) {
-      const uint32_t q = *reinterpret_cast<const uint32_t*>(ap);
-      a0 = bf16_lo(q); a1 = bf16_hi(q);
-    } else {
-      a0 = __bfloat162float(*ap);
-    }
-  }
   pre0 = pre1 = 0.f;
   if (EF == EF_GELU) {
     pre0 = round_bf16(v0); pre1 = round_bf16(v1);
     v0 = gelu_tanh_fast(pre0); v1 = gelu_tanh_fast(pre1);
-  } else if (EF == EF_RESID) {
+  } else if (EF == EF_RESID || EF == EF_RESID_ROWMOD) {
     v0 = (OUT_F32 ? v0 : round_bf16(v0)) + a0;
     v1 = (OUT_F32 ? v1 : round_bf16(v1)) + a1;
   } else if (EF == EF_DGELU) {
@@ -193,9 +209,9 @@ __device__ __forceinline__ void epilogue_regs(const GemmDev& p, const float (&ac
     for (int h = 0; h < 2; ++h) {
       const int row = row0 + 8 * h;
       if (row >= pM) continue;
-      float v0, v1, pre0, pre1;
-      epi_math<OUT_F32, EF>(p, alpha, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], b0, b1, row, col, pair, v0, v1,
-                            pre0, pre1);
+      float v0, v1, pre0, pre1, a0 = 0.f, a1 = 0.f;
+      if (EF == EF_RESID || EF == EF_DGELU) aux_global(p, row, col, pair, a0, a1);
+      epi_math<OUT_F32, EF>(alpha, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], b0, b1, a0, a1, v0, v1, pre0, pre1);
       if (OUT_F32) {
         float* dp = static_cast<float*>(p.d) + row * p.ldd + col;
         if (reduce) {
@@ -219,13 +235,19 @@ __device__ __forceinline__ void epilogue_regs(const GemmDev& p, const float (&ac
 // Epilogue through shared memory for plain bf16 outputs: the warpgroup writes each 64-column
 // sub-tile of its 64 rows into a 128B-swizzled staging buffer (the 16-byte chunk index XOR the row
 // mod 8, so the 8 rows of one store instruction hit different banks), and one thread stores it with
-// TMA, which clips rows >= M and columns >= N.  The two buffers alternate; `nstore` counts the
-// warpgroup's sub-tiles across units, and the issuing thread waits until the store that last read a
-// buffer is done reading before the buffer is refilled.
+// TMA, which clips rows >= M and columns >= N.
+//
+// Without a TMA-loaded aux the two buffers alternate; `nstore` counts the warpgroup's sub-tiles across
+// units, and the issuing thread waits until the store that last read a buffer is done reading before
+// the buffer is refilled.  With one (EF_RESID, EF_DGELU), sub-tile c uses buffer c, which already
+// holds the aux sub-tile (issue_aux_loads, same swizzle): each thread waits on the buffer's barrier
+// (phase `aux_parity`), reads its aux pair at the offset where it then writes its output pair, and the
+// output overwrites the aux in place.
 template <int BN, int EF, int BUF_BYTES>
 __device__ __forceinline__ void epilogue_tma(const GemmDev& p, const CUtensorMap* tmD, const CUtensorMap* tmD2,
                                              const float (&acc)[BN / 2], int m0, int n0, int cw, uint32_t staging,
-                                             uint32_t& nstore) {
+                                             uint32_t& nstore, uint32_t aux_bar, uint32_t aux_parity) {
+  constexpr bool AUX_TMA = (EF == EF_RESID || EF == EF_DGELU);
   const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
   const bool leader = (threadIdx.x & 127) == 0;
   const int rl0 = warp * 16 + (lane >> 2);       // row within the warpgroup's 64
@@ -234,9 +256,15 @@ __device__ __forceinline__ void epilogue_tma(const GemmDev& p, const CUtensorMap
   const float alpha = p.alpha;
 #pragma unroll
   for (int c = 0; c < BN / 64; ++c) {
-    const uint32_t buf = staging + (nstore & 1u) * BUF_BYTES;
-    if (leader) tma_store_wait_read<1>();
-    named_bar_sync(1 + cw, 128);
+    uint32_t buf;
+    if constexpr (AUX_TMA) {
+      buf = staging + c * BUF_BYTES;
+      mbar_wait(aux_bar + 8u * c, aux_parity);
+    } else {
+      buf = staging + (nstore & 1u) * BUF_BYTES;
+      if (leader) tma_store_wait_read<1>();
+      named_bar_sync(1 + cw, 128);
+    }
     float cs[8][2];
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj) {
@@ -252,17 +280,26 @@ __device__ __forceinline__ void epilogue_tma(const GemmDev& p, const CUtensorMap
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int rl = rl0 + 8 * h, row = row0 + 8 * h;
+        const uint32_t off = rl * 128 + ((jj ^ (rl & 7)) << 4) + (lane & 3) * 4;
         float v0 = 0.f, v1 = 0.f, pre0 = 0.f, pre1 = 0.f;
         const bool in = cin && row < pM;
-        if (in)
-          epi_math<false, EF>(p, alpha, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], b0, b1, row, col, pair, v0, v1,
-                              pre0, pre1);
+        if (in) {
+          float a0 = 0.f, a1 = 0.f;
+          if constexpr (AUX_TMA) {
+            // without `pair`, a1 is the box's zero fill past column N and is never stored
+            uint32_t q;
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(q) : "r"(buf + off));
+            a0 = bf16_lo(q); a1 = bf16_hi(q);
+          } else if constexpr (EF == EF_RESID_ROWMOD) {
+            aux_global(p, row, col, pair, a0, a1);
+          }
+          epi_math<false, EF>(alpha, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], b0, b1, a0, a1, v0, v1, pre0, pre1);
+        }
         const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
         if (in) {
           cs[jj][0] += __low2float(o);
           cs[jj][1] += pair ? __high2float(o) : 0.f;
         }
-        const uint32_t off = rl * 128 + ((jj ^ (rl & 7)) << 4) + (lane & 3) * 4;
         asm volatile("st.shared.b32 [%0], %1;" ::"r"(buf + off), "r"(*reinterpret_cast<const uint32_t*>(&o))
                      : "memory");
         if (EF == EF_GELU) {
@@ -283,7 +320,7 @@ __device__ __forceinline__ void epilogue_tma(const GemmDev& p, const CUtensorMap
       }
       tma_store_commit();
     }
-    ++nstore;
+    if (!AUX_TMA) ++nstore;
     if (p.colsum != nullptr) {
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj)
@@ -292,10 +329,33 @@ __device__ __forceinline__ void epilogue_tma(const GemmDev& p, const CUtensorMap
   }
 }
 
+// Run by the warpgroup's leader thread, which owns the warpgroup's bulk-store groups: once every store
+// of the previous unit has finished reading its staging buffer, TMA-load this unit's aux sub-tiles
+// (64 rows x 64 columns, 128B-swizzled like the outputs) into buffers 0 .. BN/64 - 1.  A sub-tile
+// wholly past N, or a warpgroup whose 64 rows are all past M, is never stored, so its aux is not
+// loaded; a plain arrival completes the barrier's phase instead, which keeps every barrier's phase
+// equal to the unit count and the consumers' wait unconditional.
+template <int BN>
+__device__ __forceinline__ void issue_aux_loads(const CUtensorMap* tmAux, int M, int N, int m0, int n0, int cw,
+                                                uint32_t staging, uint32_t aux_bar) {
+  tma_store_wait_read<0>();
+#pragma unroll
+  for (int c = 0; c < BN / 64; ++c) {
+    const uint32_t bar = aux_bar + 8u * c;
+    if (n0 + 64 * c < N && m0 + cw * 64 < M) {
+      mbar_expect_tx(bar, SUB_BYTES);        // the full box, zero fill included
+      tma_load_2d(staging + c * SUB_BYTES, tmAux, bar, n0 + 64 * c, m0 + cw * 64);
+    } else {
+      mbar_arrive(bar);
+    }
+  }
+}
+
 template <int BN, int OM, int EF>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmD2, const GemmDev p) {
+            const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmD2,
+            const __grid_constant__ CUtensorMap tmAux, const GemmDev p) {
   using C = Cfg<BN, OM, EF>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -310,9 +370,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (C::AUX_TMA) tma_prefetch_desc(&tmAux);
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 2);     // one arrival per consumer warpgroup
+    }
+    if (C::AUX_TMA) {
+      for (int b = 0; b < 2 * C::BUFS; ++b) mbar_init(bar_base + 8u * (C::AUX_BAR + b), 1);
     }
     fence_barrier_init();
   }
@@ -354,22 +418,31 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   // ========================= consumers: warpgroups 1, 2 =========================
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
   const int cw = wg - 1;                        // which 64-row half of the tile
-  const uint32_t staging = base + C::STAGING_OFFSET + cw * 2 * C::BUF_BYTES;
-  uint32_t nstore = 0;
+  const uint32_t staging = base + C::STAGING_OFFSET + cw * C::BUFS * C::BUF_BYTES;
+  const uint32_t aux_bar = bar_base + 8u * (C::AUX_BAR + cw * C::BUFS);
+  const bool leader = (threadIdx.x & 127) == 0;
+  uint32_t nstore = 0, nunit = 0;
   PipeState ps;
   constexpr int S = C::STAGES, SB = C::STAGE_BYTES;
-  for (int u = blockIdx.x; u < units; u += gridDim.x) {
+  for (int u = blockIdx.x; u < units; u += gridDim.x, ++nunit) {
     const WorkUnit w = gemm_work_unit(p.s, u, BM, BN);
+    // the leader's wait for the previous unit's stores overlaps the first k block's MMAs
+    auto after_first = [&]() {
+      if constexpr (C::AUX_TMA) {
+        if (leader) issue_aux_loads<BN>(&tmAux, p.M, p.N, w.m0, w.n0, cw, staging, aux_bar);
+      }
+    };
     float acc[BN / 2];
     if (p.a_mn) {
-      if (p.b_mn) mainloop<BN, S, SB, 1, 1>(acc, base, bar_base, cw, ps, w.kb0, w.kb1);
-      else mainloop<BN, S, SB, 1, 0>(acc, base, bar_base, cw, ps, w.kb0, w.kb1);
+      if (p.b_mn) mainloop<BN, S, SB, 1, 1>(acc, base, bar_base, cw, ps, w.kb0, w.kb1, after_first);
+      else mainloop<BN, S, SB, 1, 0>(acc, base, bar_base, cw, ps, w.kb0, w.kb1, after_first);
     } else {
-      if (p.b_mn) mainloop<BN, S, SB, 0, 1>(acc, base, bar_base, cw, ps, w.kb0, w.kb1);
-      else mainloop<BN, S, SB, 0, 0>(acc, base, bar_base, cw, ps, w.kb0, w.kb1);
+      if (p.b_mn) mainloop<BN, S, SB, 0, 1>(acc, base, bar_base, cw, ps, w.kb0, w.kb1, after_first);
+      else mainloop<BN, S, SB, 0, 0>(acc, base, bar_base, cw, ps, w.kb0, w.kb1, after_first);
     }
 
-    if constexpr (OM == OM_BF16_TMA) epilogue_tma<BN, EF, C::BUF_BYTES>(p, &tmD, &tmD2, acc, w.m0, w.n0, cw, staging, nstore);
+    if constexpr (OM == OM_BF16_TMA)
+      epilogue_tma<BN, EF, C::BUF_BYTES>(p, &tmD, &tmD2, acc, w.m0, w.n0, cw, staging, nstore, aux_bar, nunit & 1u);
     else epilogue_regs<BN, OM == OM_F32, EF>(p, acc, w.m0, w.n0, cw);
   }
   // the staging buffers must outlive every bulk store that reads them
@@ -379,7 +452,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 template <int BN, int OM, int EF>
 int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
   using C = Cfg<BN, OM, EF>;
-  CUtensorMap tmA, tmB, tmD, tmD2;
+  CUtensorMap tmA, tmB, tmD, tmD2, tmAux;
   int rc;
   const CUtensorMapDataType bf = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   if (g.a_mn) rc = make_tmap_2d(&tmA, bf, g.A, g.M, g.K, g.lda * 2, 64, 64);
@@ -410,6 +483,7 @@ int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
   // strided output alone
   memset(&tmD, 0, sizeof(tmD));
   memset(&tmD2, 0, sizeof(tmD2));
+  memset(&tmAux, 0, sizeof(tmAux));
   if (OM == OM_BF16_TMA) {
     rc = make_tmap_2d(&tmD, bf, g.D, g.N, g.M, g.ldd * 2, 64, 64);
     if (rc) return rc;
@@ -417,6 +491,12 @@ int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
       rc = make_tmap_2d(&tmD2, bf, g.D2, g.N, g.M, g.ldd2 * 2, 64, 64);
       if (rc) return rc;
     }
+  }
+  // aux is read through the same M x N window and box as the output it is staged with (the checks in
+  // launch_gemm give TMA's 16-byte base and row-stride alignment)
+  if (C::AUX_TMA) {
+    rc = make_tmap_2d(&tmAux, bf, g.aux, g.N, g.M, g.ldaux * 2, 64, 64);
+    if (rc) return rc;
   }
 
   auto kern = gemm_kernel<BN, OM, EF>;
@@ -433,7 +513,7 @@ int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
     if (dev >= 0) attr_set[dev].store(true, std::memory_order_release);
   }
   const int grid = p.s.units < num_sms() ? p.s.units : num_sms();
-  kern<<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(tmA, tmB, tmD, tmD2, p);
+  kern<<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(tmA, tmB, tmD, tmD2, tmAux, p);
   return check_cuda(cudaGetLastError(), "gemm_kernel launch");
 }
 
@@ -449,8 +529,10 @@ int dispatch_epi(const GemmArgs& g, cudaStream_t s) {
       return f32 ? launch_cfg<BN, OM_F32, EF_BIAS>(g, s)
                  : add ? launch_cfg<128, OM_BF16_ADD, EF_BIAS>(g, s) : launch_cfg<BN, OM_BF16_TMA, EF_BIAS>(g, s);
     case EPI_BIAS_RESID:
-      return f32 ? launch_cfg<BN, OM_F32, EF_RESID>(g, s)
-                 : add ? launch_cfg<128, OM_BF16_ADD, EF_RESID>(g, s) : launch_cfg<BN, OM_BF16_TMA, EF_RESID>(g, s);
+      if (f32) return launch_cfg<BN, OM_F32, EF_RESID>(g, s);
+      if (add) return launch_cfg<128, OM_BF16_ADD, EF_RESID>(g, s);
+      return g.aux_row_mod > 0 ? launch_cfg<BN, OM_BF16_TMA, EF_RESID_ROWMOD>(g, s)
+                               : launch_cfg<BN, OM_BF16_TMA, EF_RESID>(g, s);
     case EPI_BIAS_GELU:     // never a reduce-add (refused in launch_gemm)
       return launch_cfg<BN, OM_BF16_TMA, EF_GELU>(g, s);
     case EPI_DGELU:

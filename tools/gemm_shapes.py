@@ -6,11 +6,13 @@ algorithmic HBM bytes (operands read once, outputs written once) at its HBM3 ban
   python tools/gemm_shapes.py                    # table (CUDA events)
   python tools/gemm_shapes.py --dump DIR         # also write every output of one call per shape as .npy
   python tools/gemm_shapes.py --pairs 256        # a smaller batch
+  python tools/gemm_shapes.py --block-n 128      # every GEMM at 128-column tiles
 
 bf16 outputs are dumped as their uint16 bit patterns, fp32 outputs as float32, so two builds
 (BV_LIB_PATH) can be compared bit for bit.  Inputs come from a seeded generator on the device.
 """
 import argparse
+import functools
 import os
 import sys
 
@@ -58,10 +60,11 @@ class Bufs:
     return self.cache[key]
 
 
-def cases(pairs, bufs):
+def cases(pairs, bufs, block_n=0):
   """(name, M, N, K, out tensors, fn, algorithmic bytes) for every GEMM of the step.  Output tensors
   are allocated by the caller-visible closures so that a dump sees exactly what one call wrote."""
   out = []
+  gemm = functools.partial(ops.gemm, block_n=block_n)
 
   def add(name, M, N, K, make, nbytes):
     out.append((name, M, N, K, make, nbytes))
@@ -81,64 +84,64 @@ def cases(pairs, bufs):
 
     def fwd_qkv(x=x, wq=wq, b3=b3, M=M):
       o = torch.empty(M, 3 * D, device="cuda", dtype=torch.bfloat16)
-      return [o], lambda: ops.gemm(x, wq, b_mn=True, bias=b3, out=o)
+      return [o], lambda: gemm(x, wq, b_mn=True, bias=b3, out=o)
     add(f"{tower} fwd qkv       bias", M, 3 * D, D, fwd_qkv, bf * (M * D + D * 3 * D + M * 3 * D))
 
     def fwd_out(x=x, wo=wo, bd=bd, M=M):
       o = torch.empty(M, D, device="cuda", dtype=torch.bfloat16)
-      return [o], lambda: ops.gemm(x, wo, b_mn=True, bias=bd, aux=x, out=o, epilogue=L.EPI_BIAS_RESID)
+      return [o], lambda: gemm(x, wo, b_mn=True, bias=bd, aux=x, out=o, epilogue=L.EPI_BIAS_RESID)
     add(f"{tower} fwd out_proj  +resid", M, D, D, fwd_out, bf * (M * D + D * D + M * D + M * D))
 
     def fwd_d0(x=x, w0=w0, bm=bm, M=M):
       o = torch.empty(M, MLP, device="cuda", dtype=torch.bfloat16)
       o2 = torch.empty(M, MLP, device="cuda", dtype=torch.bfloat16)
-      return [o, o2], lambda: ops.gemm(x, w0, b_mn=True, bias=bm, out=o, out2=o2, epilogue=L.EPI_BIAS_GELU)
+      return [o, o2], lambda: gemm(x, w0, b_mn=True, bias=bm, out=o, out2=o2, epilogue=L.EPI_BIAS_GELU)
     add(f"{tower} fwd Dense_0   gelu", M, MLP, D, fwd_d0, bf * (M * D + D * MLP + 2 * M * MLP))
 
     def fwd_d1(h=h, w1=w1, bd=bd, x=x, M=M):
       o = torch.empty(M, D, device="cuda", dtype=torch.bfloat16)
-      return [o], lambda: ops.gemm(h, w1, b_mn=True, bias=bd, aux=x, out=o, epilogue=L.EPI_BIAS_RESID)
+      return [o], lambda: gemm(h, w1, b_mn=True, bias=bd, aux=x, out=o, epilogue=L.EPI_BIAS_RESID)
     add(f"{tower} fwd Dense_1   +resid", M, D, MLP, fwd_d1, bf * (M * MLP + MLP * D + 2 * M * D))
 
     def wg_d1(h=h, x=x):
       o = torch.zeros(MLP, D, device="cuda", dtype=torch.float32)
-      return [o], lambda: ops.gemm(h, x, a_mn=True, b_mn=True, out=o, reduce_out=True)
+      return [o], lambda: gemm(h, x, a_mn=True, b_mn=True, out=o, reduce_out=True)
     add(f"{tower} wgrad Dense_1 f32+=", MLP, D, M, wg_d1, bf * (M * MLP + M * D) + 4 * 2 * MLP * D)
 
     def dg_d1(x=x, w1=w1, h=h, M=M):
       o = torch.empty(M, MLP, device="cuda", dtype=torch.bfloat16)
       cs = torch.zeros(MLP, device="cuda", dtype=torch.float32)
-      return [o, cs], lambda: ops.gemm(x, w1, aux=h, out=o, epilogue=L.EPI_DGELU, colsum=cs)
+      return [o, cs], lambda: gemm(x, w1, aux=h, out=o, epilogue=L.EPI_DGELU, colsum=cs)
     add(f"{tower} dgrad Dense_1 gelu'+colsum", M, MLP, D, dg_d1, bf * (M * D + MLP * D + 2 * M * MLP))
 
     def wg_d0(x=x, h=h):
       o = torch.zeros(D, MLP, device="cuda", dtype=torch.float32)
-      return [o], lambda: ops.gemm(x, h, a_mn=True, b_mn=True, out=o, reduce_out=True)
+      return [o], lambda: gemm(x, h, a_mn=True, b_mn=True, out=o, reduce_out=True)
     add(f"{tower} wgrad Dense_0 f32+=", D, MLP, M, wg_d0, bf * (M * D + M * MLP) + 4 * 2 * MLP * D)
 
     def dg_d0(h=h, w0=w0, M=M):
       o = torch.empty(M, D, device="cuda", dtype=torch.bfloat16)
-      return [o], lambda: ops.gemm(h, w0, out=o)
+      return [o], lambda: gemm(h, w0, out=o)
     add(f"{tower} dgrad Dense_0", M, D, MLP, dg_d0, bf * (M * MLP + MLP * D + M * D))
 
     def wg_out(x=x):
       o = torch.zeros(D, D, device="cuda", dtype=torch.float32)
-      return [o], lambda: ops.gemm(x, x, a_mn=True, b_mn=True, out=o, reduce_out=True)
+      return [o], lambda: gemm(x, x, a_mn=True, b_mn=True, out=o, reduce_out=True)
     add(f"{tower} wgrad out_proj f32+=", D, D, M, wg_out, bf * 2 * M * D + 4 * 2 * D * D)
 
     def dg_out(x=x, wo=wo, M=M):
       o = torch.empty(M, D, device="cuda", dtype=torch.bfloat16)
-      return [o], lambda: ops.gemm(x, wo, out=o)
+      return [o], lambda: gemm(x, wo, out=o)
     add(f"{tower} dgrad out_proj", M, D, D, dg_out, bf * (2 * M * D + D * D))
 
     def wg_qkv(x=x, dq=dq):
       o = torch.zeros(D, 3 * D, device="cuda", dtype=torch.float32)
-      return [o], lambda: ops.gemm(x, dq, a_mn=True, b_mn=True, out=o, reduce_out=True)
+      return [o], lambda: gemm(x, dq, a_mn=True, b_mn=True, out=o, reduce_out=True)
     add(f"{tower} wgrad qkv     f32+=", D, 3 * D, M, wg_qkv, bf * (M * D + M * 3 * D) + 4 * 2 * 3 * D * D)
 
     def dg_qkv(dq=dq, wq=wq, M=M):
       o = torch.empty(M, D, device="cuda", dtype=torch.bfloat16)
-      return [o], lambda: ops.gemm(dq, wq, out=o)
+      return [o], lambda: gemm(dq, wq, out=o)
     add(f"{tower} dgrad qkv", M, D, 3 * D, dg_qkv, bf * (M * 3 * D + 3 * D * D + M * D))
 
   # image tower only: the patch embedding (position embedding added row-modulo) and the MAP head's
@@ -155,29 +158,38 @@ def cases(pairs, bufs):
 
   def emb():
     o = torch.empty(M, D, device="cuda", dtype=torch.bfloat16)
-    return [o], lambda: ops.gemm(pt, we, b_mn=True, bias=bd, aux=pos, aux_row_mod=IMG_TOKENS, out=o,
+    return [o], lambda: gemm(pt, we, b_mn=True, bias=bd, aux=pos, aux_row_mod=IMG_TOKENS, out=o,
                                  epilogue=L.EPI_BIAS_RESID)
   add("img fwd patch emb  +posemb", M, D, PATCH, emb, 2 * (M * PATCH + PATCH * D + M * D))
 
   def wg_emb():
     o = torch.zeros(PATCH, D, device="cuda", dtype=torch.float32)
-    return [o], lambda: ops.gemm(pt, x, a_mn=True, b_mn=True, out=o, reduce_out=True)
+    return [o], lambda: gemm(pt, x, a_mn=True, b_mn=True, out=o, reduce_out=True)
   add("img wgrad patch emb f32+=", PATCH, D, M, wg_emb, 2 * (M * PATCH + M * D) + 8 * PATCH * D)
 
   def kv():
     o = torch.empty(M, 2 * D, device="cuda", dtype=torch.bfloat16)
-    return [o], lambda: ops.gemm(x, wkv, b_mn=True, bias=bkv, out=o)
+    return [o], lambda: gemm(x, wkv, b_mn=True, bias=bkv, out=o)
   add("img fwd MAP kv     bias", M, 2 * D, D, kv, 2 * (M * D + 2 * D * D + 2 * M * D))
 
   def wg_kv():
     o = torch.zeros(D, 2 * D, device="cuda", dtype=torch.float32)
-    return [o], lambda: ops.gemm(x, dkv, a_mn=True, b_mn=True, out=o, reduce_out=True)
+    return [o], lambda: gemm(x, dkv, a_mn=True, b_mn=True, out=o, reduce_out=True)
   add("img wgrad MAP kv   f32+=", D, 2 * D, M, wg_kv, 2 * (M * D + 2 * M * D) + 8 * 2 * D * D)
 
   def dg_kv():
     o = torch.empty(M, D, device="cuda", dtype=torch.bfloat16)
-    return [o], lambda: ops.gemm(dkv, wkv, out=o)
+    return [o], lambda: gemm(dkv, wkv, out=o)
   add("img dgrad MAP kv", M, D, 2 * D, dg_kv, 2 * (2 * M * D + 2 * D * D + M * D))
+
+  # appended (earlier cases keep their --dump indices): gelu' without the bias-gradient colsum, so the
+  # table separates the colsum's atomics from the rest of that GEMM
+  x, w1, h = bufs.get("img.x", (M, D)), bufs.get("w1", (MLP, D), 0.03), bufs.get("img.h", (M, MLP))
+
+  def dg_d1_nocs():
+    o = torch.empty(M, MLP, device="cuda", dtype=torch.bfloat16)
+    return [o], lambda: gemm(x, w1, aux=h, out=o, epilogue=L.EPI_DGELU)
+  add("img dgrad Dense_1 gelu'", M, MLP, D, dg_d1_nocs, 2 * (M * D + MLP * D + 2 * M * MLP))
   return out
 
 
@@ -186,6 +198,8 @@ def main():
   ap.add_argument("--pairs", type=int, default=768, help="image-text pairs per step (bench.py: 768)")
   ap.add_argument("--reps", type=int, default=10)
   ap.add_argument("--dump", metavar="DIR", default=None)
+  ap.add_argument("--block-n", type=int, default=0, choices=[0, 128, 256],
+                  help="tile width of every GEMM (0: the library's choice)")
   args = ap.parse_args()
   if not torch.cuda.is_available():
     raise SystemExit("gemm_shapes.py needs a GPU")
@@ -194,7 +208,7 @@ def main():
   total_ms = total_flop = 0.0
   print(f"{'case':34s} {'M':>7s} {'N':>5s} {'K':>7s} {'us':>9s} {'TFLOP/s':>8s} {'flop-lb us':>10s} "
         f"{'byte-lb us':>10s}")
-  for i, (name, M, N, K, make, nbytes) in enumerate(cases(args.pairs, bufs)):
+  for i, (name, M, N, K, make, nbytes) in enumerate(cases(args.pairs, bufs, args.block_n)):
     outs, fn = make()
     if args.dump:
       fn()
