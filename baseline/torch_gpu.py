@@ -140,15 +140,24 @@ class TextTower(nn.Module):
 
 
 class TwoTowers(nn.Module):
-  def __init__(self, img_variant, txt_size, res, out, remat=False):
+  def __init__(self, img_variant, txt_size, res, out, remat=False, freeze_img=False):
     super().__init__()
     self.img = ViT(img_variant, res, None, pool="map", remat=remat)
     self.txt = TextTower(txt_size, 32_000, 64, out, remat)
     self.t = nn.Parameter(torch.tensor([math.log(10.0)]))
     self.b = nn.Parameter(torch.tensor([-10.0]))
+    # locked-image tuning (SigLiT): the image tower gets no gradient and its forward records no graph
+    self.freeze_img = freeze_img
+    if freeze_img:
+      self.img.requires_grad_(False)
 
   def forward(self, image, text):
-    zi, zt = self.img(image).float(), self.txt(text).float()
+    if self.freeze_img:
+      with torch.no_grad():
+        zi = self.img(image).float()
+    else:
+      zi = self.img(image).float()
+    zt = self.txt(text).float()
     zi = zi / (zi.norm(dim=-1, keepdim=True) + 1e-8)
     zt = zt / (zt.norm(dim=-1, keepdim=True) + 1e-8)
     return zi, zt
@@ -200,7 +209,7 @@ def make_step(workload, world, rank, device):
   if kind == "siglip":
     kw = workload["model_kw"]
     model = TwoTowers(kw["image"]["variant"], kw["text"]["variant"], workload["res"], kw["out_dim"][1],
-                      remat=workload.get("remat", False))
+                      remat=workload.get("remat", False), freeze_img=workload.get("freeze_img", False))
   elif workload["model"] == "vit":
     kw = workload["model_kw"]
     model = ViT(kw["variant"], workload["res"], workload["num_classes"], pool=kw.get("pool_type", "gap"),
@@ -209,15 +218,15 @@ def make_step(workload, world, rank, device):
     model = Mixer(workload["model_kw"]["variant"], workload["res"], workload["num_classes"])
   model = model.to(device).to(memory_format=torch.channels_last)
   # decoupled weight decay on the matmul / conv kernels only (optax.py:133 mask `.*/kernel$`)
-  decay = [m.weight for m in model.modules() if isinstance(m, (nn.Linear, nn.Conv2d))]
+  decay = [m.weight for m in model.modules() if isinstance(m, (nn.Linear, nn.Conv2d)) and m.weight.requires_grad]
   ids = {id(p) for p in decay}
-  rest = [p for p in model.parameters() if id(p) not in ids]
+  rest = [p for p in model.parameters() if id(p) not in ids and p.requires_grad]
   opt = torch.optim.AdamW([{"params": decay, "weight_decay": 1e-4}, {"params": rest, "weight_decay": 0.0}],
                           lr=1e-3, betas=(0.9, 0.95), fused=True)
   net = model
   if world > 1:
     net = torch.nn.parallel.DistributedDataParallel(model, device_ids=[device.index], gradient_as_bucket_view=True)
-  params = list(model.parameters())
+  params = [p for p in model.parameters() if p.requires_grad]
 
   def step(batch):
     opt.zero_grad(set_to_none=True)

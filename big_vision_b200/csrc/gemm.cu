@@ -45,7 +45,9 @@ constexpr int SUB_BYTES = 64 * 64 * 2;       // one 64 x 64 bf16 output sub-tile
 // epilogue families (template parameter).  EF_RESID_ROWMOD is the residual whose aux rows wrap
 // (aux_row_mod > 0, the position embedding): a tile's row window can wrap around it, so it is not one
 // TMA box and its TMA-store kernel reads aux from global memory in the accumulator layout.
-enum : int { EF_BIAS = 0, EF_GELU = 1, EF_RESID = 2, EF_DGELU = 3, EF_RESID_ROWMOD = 4 };
+// EF_GELU_ACT is EF_GELU without the pre-activation output (forward-only MLPs): one staging buffer
+// per sub-tile, so it keeps the stage count of EF_BIAS.
+enum : int { EF_BIAS = 0, EF_GELU = 1, EF_RESID = 2, EF_DGELU = 3, EF_RESID_ROWMOD = 4, EF_GELU_ACT = 5 };
 // output modes (template parameter): fp32 from the registers, bf16 reduce-add from the registers,
 // plain bf16 by TMA store
 enum : int { OM_F32 = 0, OM_BF16_ADD = 1, OM_BF16_TMA = 2 };
@@ -154,7 +156,7 @@ __device__ __forceinline__ void epi_math(float alpha, float c0, float c1, float 
   v0 = c0 * alpha + b0;
   v1 = c1 * alpha + b1;
   pre0 = pre1 = 0.f;
-  if (EF == EF_GELU) {
+  if (EF == EF_GELU || EF == EF_GELU_ACT) {
     pre0 = round_bf16(v0); pre1 = round_bf16(v1);
     v0 = gelu_tanh_fast(pre0); v1 = gelu_tanh_fast(pre1);
   } else if (EF == EF_RESID || EF == EF_RESID_ROWMOD) {
@@ -535,6 +537,8 @@ int dispatch_epi(const GemmArgs& g, cudaStream_t s) {
                                : launch_cfg<BN, OM_BF16_TMA, EF_RESID>(g, s);
     case EPI_BIAS_GELU:     // never a reduce-add (refused in launch_gemm)
       return launch_cfg<BN, OM_BF16_TMA, EF_GELU>(g, s);
+    case EPI_BIAS_GELU_ACT:
+      return launch_cfg<BN, OM_BF16_TMA, EF_GELU_ACT>(g, s);
     case EPI_DGELU:
       if (f32) { set_error("bv_gemm: DGELU epilogue writes bf16"); return BV_ERR_INVALID; }
       if (g.aux_row_mod > 0) { set_error("bv_gemm: DGELU takes a row-aligned aux"); return BV_ERR_INVALID; }
@@ -558,7 +562,9 @@ int launch_gemm(const GemmArgs& g, cudaStream_t stream) {
   if (g.M > 0x7fffffffLL || g.N > 0x7fffffffLL || g.K > 0x7fffffffLL) {
     set_error("bv_gemm: dimension exceeds int32"); return BV_ERR_INVALID;
   }
-  if (g.epi < EPI_NONE || g.epi > EPI_DGELU) { set_error("bv_gemm: bad epilogue %d", g.epi); return BV_ERR_INVALID; }
+  if (g.epi < EPI_NONE || g.epi > EPI_BIAS_GELU_ACT) {
+    set_error("bv_gemm: bad epilogue %d", g.epi); return BV_ERR_INVALID;
+  }
   if ((g.epi == EPI_BIAS_RESID || g.epi == EPI_DGELU) && g.aux == nullptr) {
     set_error("bv_gemm: epilogue %d needs aux", g.epi); return BV_ERR_INVALID;
   }
@@ -573,6 +579,9 @@ int launch_gemm(const GemmArgs& g, cudaStream_t stream) {
   }
   if (g.epi == EPI_BIAS_GELU && ((reinterpret_cast<uintptr_t>(g.D2) & 15) || (g.ldd2 % 8))) {
     set_error("bv_gemm: D2 must be 16B aligned with ldd2 %% 8 == 0"); return BV_ERR_INVALID;
+  }
+  if (g.epi == EPI_BIAS_GELU_ACT && (g.out_dtype != DT_BF16 || g.reduce_out)) {
+    set_error("bv_gemm: BIAS_GELU_ACT needs bf16 output and no reduce"); return BV_ERR_INVALID;
   }
   if (g.out_dtype != DT_F32 && g.out_dtype != DT_BF16) { set_error("bv_gemm: bad out dtype"); return BV_ERR_INVALID; }
   if (g.colsum != nullptr && (g.out_dtype != DT_BF16 || g.reduce_out)) {

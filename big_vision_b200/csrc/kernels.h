@@ -5,7 +5,8 @@
 
 namespace bv {
 
-enum : int { EPI_NONE = 0, EPI_BIAS = 1, EPI_BIAS_GELU = 2, EPI_BIAS_RESID = 3, EPI_DGELU = 4 };
+enum : int { EPI_NONE = 0, EPI_BIAS = 1, EPI_BIAS_GELU = 2, EPI_BIAS_RESID = 3, EPI_DGELU = 4,
+             EPI_BIAS_GELU_ACT = 5 };
 
 struct GemmArgs {
   const void* A; const void* B; void* D; void* D2;

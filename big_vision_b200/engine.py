@@ -146,6 +146,35 @@ class FlatParams:
   def zero_grad(self):
     self.grad.zero_()
 
+  def trained_ranges(self, frozen):
+    """[(lo, hi), ...]: the flat-buffer slices of every stored parameter NOT in `frozen` (storage
+    names), each with its alignment padding, neighbours merged, in layout order."""
+    out = []
+    for name, (off, shape) in sorted(self.offsets.items(), key=lambda kv: kv[1][0]):
+      if name in frozen:
+        continue
+      hi = off + (int(np.prod(shape)) + ALIGN - 1) // ALIGN * ALIGN
+      if out and out[-1][1] == off:
+        out[-1][1] = hi
+      else:
+        out.append([off, hi])
+    return [tuple(r) for r in out]
+
+
+def stage_cut(storages, stages, frozen):
+  """Index of the lowest of `stages` (bottom-up; each a tuple of storage-name prefixes) that holds a
+  storage not in `frozen`: a backward that stops there still reaches every trained parameter.
+  len(stages) when everything is frozen; 0 when nothing is (`frozen` empty or None).  `frozen=True`
+  means every storage."""
+  if frozen is True:
+    return len(stages)
+  if not frozen:
+    return 0
+  for i, prefixes in enumerate(stages):
+    if any(s.startswith(prefixes) and s not in frozen for s in storages):
+      return i
+  return len(stages)
+
 
 # ---- initialisers (numpy; same distributions as the reference's, see SURVEY.md 3.4) -------
 def xavier_uniform(fan_in, fan_out):

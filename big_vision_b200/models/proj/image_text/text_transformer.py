@@ -74,33 +74,64 @@ class _Model:
   def _tok(self, Ln):
     return {"last": Ln - 1, "first": 0}.get(self.pool_type)
 
-  def fwd(self, P, text):
-    """text int32 [n, L] -> (fp32 [n, out], saved)."""
+  def stages(self):
+    """Backward stages bottom-up (storage-name prefixes): Embed_0 with pos_embedding, every encoder
+    block (the scan-stacked encoder is one), encoder_norm, the MAP head, head."""
+    p = self.prefix
+    out = [(p + "Embed_0/", p + "pos_embedding")] + self.encoder.stages()
+    out.append((p + "Encoder_0/encoder_norm/",))
+    if self.map_head is not None:
+      out.append((self.map_head.p,))
+    if self.num_classes:
+      out.append((p + "head/",))
+    return out
+
+  def _stage_indices(self):
+    """Indices into stages() of encoder_norm, the MAP head and head."""
+    i_norm = 1 + (1 if self.scan else self.depth)
+    i_map = i_norm + 1
+    return i_norm, i_map, i_map + (self.map_head is not None)
+
+  def cut(self, P, frozen):
+    """Index into stages() of the lowest stage with a trained parameter (see vit._Model.cut)."""
+    cache = self.__dict__.setdefault("_cuts", {})
+    key = frozen if frozen is True or frozen is None else frozenset(frozen)
+    if key not in cache:
+      cache[key] = E.stage_cut(P.offsets, self.stages(), frozen)
+    return cache[key]
+
+  def fwd(self, P, text, frozen=None):
+    """text int32 [n, L] -> (fp32 [n, out], saved).  `frozen` as in vit._Model.fwd: the stages below
+    the cut run forward-only and save nothing."""
     n, Ln = text.shape
     d, p = self.width, self.prefix
+    cut = self.cut(P, frozen)
+    i_norm, i_map, i_head = self._stage_indices()
     x = ops.embed_fwd(text, P.f(p + "Embed_0/embedding"), P.f(p + "pos_embedding").view(Ln, d))
-    x, enc_saved = self.encoder.fwd(P, x, n, Ln)
+    train_from = 0 if cut <= 1 else (self.depth if self.scan else min(cut - 1, self.depth))
+    x, enc_saved = self.encoder.fwd(P, x, n, Ln, train_from=train_from)
     en = p + "Encoder_0/encoder_norm/"
-    saved = {"text": text, "enc": enc_saved, "n": n, "L": Ln}
+    saved = {"text": text, "enc": enc_saved, "n": n, "L": Ln, "cut": cut, "train_from": train_from}
+    keep_norm = cut <= i_norm
     tok = self._tok(Ln)
     if tok is not None:
       # LayerNorm is per token: LN(x)[:, tok] == LN(x[:, tok]) -- normalise only the pooled row
       xt = ops.pool_fwd(x, n, Ln, 1, tok=tok)
       out, mean, rstd = ops.layernorm_fwd(xt, P.f(en + "scale"), P.f(en + "bias"))
-      saved["norm"] = (xt, mean, rstd)
+      saved["norm"] = (xt, mean, rstd) if keep_norm else None
     else:
       encd, mean, rstd = ops.layernorm_fwd(x, P.f(en + "scale"), P.f(en + "bias"))
-      saved["norm"] = (x, mean, rstd)
+      saved["norm"] = (x, mean, rstd) if keep_norm else None
       if self.map_head is not None:
-        out, saved["map"] = self.map_head.fwd(P, encd, n, Ln)
+        out, saved["map"] = self.map_head.fwd(P, encd, n, Ln, save=cut <= i_map)
         out = vit._Model._to16(out)
       elif self.pool_type in ("max", "gmp"):
         out = ops.pool_fwd(encd, n, Ln, 2)
-        saved["encd"] = encd
+        saved["encd"] = encd if keep_norm else None
       else:
         out = ops.pool_fwd(encd, n, Ln, 0)
     if self.num_classes:
-      saved["head_in"] = out
+      saved["head_in"] = out if cut <= i_head else None
       out = ops.gemm(out, P.h(p + "head/kernel"), b_mn=True, bias=P.f(p + "head/bias"),
                      out_dtype=torch.float32)
     return out, saved
@@ -108,18 +139,25 @@ class _Model:
   def bwd(self, P, dout, saved):
     p, d = self.prefix, self.width
     n, Ln = saved["n"], saved["L"]
+    cut, train_from = saved["cut"], saved["train_from"]
+    if cut == len(self.stages()):        # wholly frozen: nothing to do
+      return
+    i_norm, i_map, i_head = self._stage_indices()
     en = p + "Encoder_0/encoder_norm/"
     if self.num_classes:
       d16 = vit._Model._to16(dout)
       ops.colsum(dout, P.g(p + "head/bias"))
       ops.gemm(saved["head_in"], d16, a_mn=True, b_mn=True, out=P.g(p + "head/kernel"), reduce_out=True)
+      if cut == i_head:
+        return
       dout = ops.gemm(d16, P.h(p + "head/kernel"))          # bf16 [n, d]
     else:
       dout = vit._Model._to16(dout)
-    last_b = self.encoder.last_bias_grad(P)
+    # below the cut the last block is frozen: its Dense_1 bias gradient stays zero
+    last_b = self.encoder.last_bias_grad(P) if cut < i_norm else None
     tok = self._tok(Ln)
-    xs, mean, rstd = saved["norm"]
     if tok is not None:
+      xs, mean, rstd = saved["norm"]
       dxt = ops.layernorm_bwd(dout, xs, P.f(en + "scale"), mean, rstd, dscale=P.g(en + "scale"),
                               dbias=P.g(en + "bias"), dx_colsum=last_b)
       dx = ops.pool_bwd(dxt, n, Ln, 1, tok=tok)
@@ -127,17 +165,24 @@ class _Model:
       if self.map_head is not None:
         denc = self.map_head.bwd(P, ops.cast(dout, torch.empty_like(dout, dtype=torch.float32)),
                                  saved["map"], n, Ln)
+        if cut == i_map:
+          return
       elif self.pool_type in ("max", "gmp"):
         denc = ops.pool_max_bwd(dout, saved["encd"], n, Ln)
       else:
         denc = ops.pool_bwd(dout, n, Ln, 0)
+      xs, mean, rstd = saved["norm"]
       dx = ops.layernorm_bwd(denc, xs, P.f(en + "scale"), mean, rstd, dscale=P.g(en + "scale"),
                              dbias=P.g(en + "bias"), dx_colsum=last_b)
-    dx = self.encoder.bwd(P, dx, saved["enc"], n, Ln, None)
+    if cut == i_norm:
+      return
+    dx = self.encoder.bwd(P, dx, saved["enc"], n, Ln, None, train_from=train_from)
+    if cut > 0:          # Embed_0 and pos_embedding are frozen
+      return
     ops.embed_bwd(saved["text"], dx, P.g(p + "Embed_0/embedding"), P.g(p + "pos_embedding").view(Ln, d))
 
   def apply(self, variables, text, *, train=False):
-    x, _ = self.fwd(variables["params"], text)
+    x, _ = self.fwd(variables["params"], text, frozen=True)     # forward-only, same bits
     return x, {"logits" if self.num_classes else "pre_logits": x}
 
 

@@ -52,35 +52,46 @@ class Model:
     specs, aliases = self.specs(image_shape, text_shape)
     return E.FlatParams(specs, aliases, device).init(seed)
 
-  def fwd(self, P, image, text):
-    """-> (zimg fp32 [n,D], ztxt fp32 [n,D], saved)."""
+  def tower_frozen(self, P, frozen):
+    """(image tower wholly frozen, text tower wholly frozen) under `frozen` (optax.Chain.frozen()):
+    such a tower runs forward-only, and neither the loss nor the backward computes its gradient."""
+    return (self.img.cut(P, frozen) == len(self.img.stages()),
+            self.txt.cut(P, frozen) == len(self.txt.stages()))
+
+  def fwd(self, P, image, text, frozen=None):
+    """-> (zimg fp32 [n,D], ztxt fp32 [n,D], saved).  `frozen` as in vit._Model.fwd; a wholly frozen
+    tower keeps nothing for the backward (its saved entries are None)."""
     saved = {}
     ztxt = zimg = None
     if text is not None:
-      e, saved["txt"] = self.txt.fwd(P, text)
+      e, s = self.txt.fwd(P, text, frozen=frozen)
       ztxt, nrm = ops.l2norm_fwd(e, eps=1e-8)
-      saved["txt_norm"] = (ztxt, nrm)
+      live = self.txt.cut(P, frozen) < len(self.txt.stages())
+      saved["txt"], saved["txt_norm"] = (s, (ztxt, nrm)) if live else (None, None)
     if image is not None:
-      e, saved["img"] = self.img.fwd(P, image)
+      e, s = self.img.fwd(P, image, frozen=frozen)
       zimg, nrm = ops.l2norm_fwd(e, eps=1e-8)
-      saved["img_norm"] = (zimg, nrm)
+      live = self.img.cut(P, frozen) < len(self.img.stages())
+      saved["img"], saved["img_norm"] = (s, (zimg, nrm)) if live else (None, None)
     return zimg, ztxt, saved
 
   def bwd(self, P, dzimg, dztxt, saved):
-    """dzimg/dztxt: fp32 [n,D] gradients w.r.t. the normalised embeddings."""
-    if dztxt is not None:
+    """dzimg/dztxt: fp32 [n,D] gradients w.r.t. the normalised embeddings.  A tower is skipped, its
+    L2-norm backward included, when its gradient is None or it was wholly frozen in the forward."""
+    if dztxt is not None and saved.get("txt_norm") is not None:
       z, nrm = saved["txt_norm"]
       self.txt.bwd(P, ops.l2norm_bwd(dztxt, z, nrm, eps=1e-8), saved["txt"])
       saved["txt"] = None
-    if dzimg is not None:
+    if dzimg is not None and saved.get("img_norm") is not None:
       z, nrm = saved["img_norm"]
       self.img.bwd(P, ops.l2norm_bwd(dzimg, z, nrm, eps=1e-8), saved["img"])
       saved["img"] = None
 
   def apply(self, variables, image, text=None, **kw):
-    """(zimg, ztxt, out) like the flax apply (two_towers.py:39-90)."""
+    """(zimg, ztxt, out) like the flax apply (two_towers.py:39-90); forward-only (same bits as the
+    training forward, nothing kept for a backward)."""
     P = variables["params"]
-    zimg, ztxt, _ = self.fwd(P, image, text)
+    zimg, ztxt, _ = self.fwd(P, image, text, frozen=True)
     out = {"t": P.f("t").exp(), "t/parameter": P.f("t")}
     if self.bias_init is not None:
       out["b"] = P.f("b")

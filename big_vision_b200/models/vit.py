@@ -129,14 +129,19 @@ class Scope:
     return Scope(self.P, self.prefix + rel, self.index)
 
 
-def mlp_fwd(S, y, resid, out_dtype=torch.bfloat16):
-  """resid + Dense_1(gelu(Dense_0(y))) with S the MlpBlock's Scope.  Returns (out, saved)."""
-  act, pre = ops.gemm(y, S.h("Dense_0/kernel"), b_mn=True, bias=S.f("Dense_0/bias"),
-                      epilogue=L.EPI_BIAS_GELU)
+def mlp_fwd(S, y, resid, out_dtype=torch.bfloat16, save=True):
+  """resid + Dense_1(gelu(Dense_0(y))) with S the MlpBlock's Scope.  Returns (out, saved).
+  save=False (forward only): GELU's pre-activation is not written at all, saved is None."""
+  if save:
+    act, pre = ops.gemm(y, S.h("Dense_0/kernel"), b_mn=True, bias=S.f("Dense_0/bias"),
+                        epilogue=L.EPI_BIAS_GELU)
+  else:
+    act = ops.gemm(y, S.h("Dense_0/kernel"), b_mn=True, bias=S.f("Dense_0/bias"),
+                   epilogue=L.EPI_BIAS_GELU_ACT)
   out = ops.gemm(act, S.h("Dense_1/kernel"), b_mn=True, bias=S.f("Dense_1/bias"),
                  aux=resid, epilogue=L.EPI_BIAS_RESID if resid is not None else L.EPI_BIAS,
                  out_dtype=out_dtype)
-  return out, (y, act, pre)
+  return out, ((y, act, pre) if save else None)
 
 
 def mlp_bwd(S, dout, saved, want_bias2_grad=True):
@@ -210,7 +215,9 @@ class EncoderBlock:
   def scope(self, P):
     return Scope(P, self.p, self.index)
 
-  def fwd(self, P, x, n, N):
+  def fwd(self, P, x, n, N, save=True):
+    """save=False (forward only): same output bits; every intermediate is released as soon as the
+    next op has consumed it and saved is None."""
     d = self.d
     S = self.scope(P)
     A = S.sub("MultiHeadDotProductAttention_0/")
@@ -218,9 +225,17 @@ class EncoderBlock:
     qkv = ops.gemm(ln1, A.h("qkv/kernel"), b_mn=True, bias=A.f("qkv/bias"))
     qkv3 = qkv.view(n, N, 3 * d)
     o, lse = ops.attention_fwd(qkv3[:, :, 0:d], qkv3[:, :, d:2 * d], qkv3[:, :, 2 * d:], self.heads)
+    if not save:
+      del ln1, mean1, rstd1, qkv, qkv3, lse
     x1 = ops.gemm(o.view(n * N, d), A.h("out_proj/kernel"), b_mn=True,
                   bias=A.f("out/bias"), aux=x, epilogue=L.EPI_BIAS_RESID)
+    if not save:
+      del o
     ln2, mean2, rstd2 = ops.layernorm_fwd(x1, S.f("LayerNorm_1/scale"), S.f("LayerNorm_1/bias"))
+    if not save:
+      del mean2, rstd2
+      x2, _ = mlp_fwd(S.sub("MlpBlock_0/"), ln2, x1, save=False)
+      return x2, None
     x2, mlp_saved = mlp_fwd(S.sub("MlpBlock_0/"), ln2, x1)
     return x2, (x, ln1, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, mlp_saved)
 
@@ -293,9 +308,23 @@ class Encoder:
     specs = specs + ln_specs(self.prefix + "encoder_norm/", self.d)
     return specs, aliases
 
-  def fwd(self, P, x, n, N):
+  def stages(self):
+    """Storage-name prefixes of the blocks as backward stages, bottom-up: one per block, or ONE for
+    the scan-stacked encoder (a single storage holds every block)."""
+    if self.scan:
+      return [(self.blocks[0].p,)]
+    return [(b.p,) for b in self.blocks]
+
+  def fwd(self, P, x, n, N, train_from=0):
+    """Blocks below `train_from` run forward-only: they keep nothing (not even a scan block's
+    input) and each block's intermediates are freed once the next block has consumed them.
+    saved[i] is None for those blocks."""
     saved = []
-    for b in self.blocks:
+    for i, b in enumerate(self.blocks):
+      if i < train_from:
+        x, _ = b.fwd(P, x, n, N, save=False)
+        saved.append(None)
+        continue
       x_in = x
       x, s = b.fwd(P, x, n, N)
       saved.append(x_in if self.scan else s)      # remat: keep the block input only
@@ -305,9 +334,14 @@ class Encoder:
     """Gradient buffer that must receive colsum(d x_out): the last block's Dense_1 bias."""
     return self.blocks[-1].dense1_bias_grad(P)
 
-  def bwd(self, P, dx, saved, n, N, dx_colsum_out):
-    for i in reversed(range(self.depth)):
-      cs = self.blocks[i - 1].dense1_bias_grad(P) if i > 0 else dx_colsum_out
+  def bwd(self, P, dx, saved, n, N, dx_colsum_out, train_from=0):
+    """Runs the blocks from the top down to `train_from` (the lowest with a saved forward); with
+    train_from > 0 the block below is frozen, so nothing is accumulated into its gradient."""
+    for i in reversed(range(train_from, self.depth)):
+      if i > train_from:
+        cs = self.blocks[i - 1].dense1_bias_grad(P)
+      else:
+        cs = dx_colsum_out if i == 0 else None
       s = saved[i]
       if self.scan:                               # recompute the block from its input
         x_out, s = self.blocks[i].fwd(P, s, n, N)
@@ -336,7 +370,7 @@ class MAPHead:
     return ([probe] + s + ln_specs(self.p + "LayerNorm_0/", d)
             + mlp_specs(self.p + "MlpBlock_0/", d, self.m)), a
 
-  def fwd(self, P, enc, n, N):
+  def fwd(self, P, enc, n, N, save=True):
     d = self.d
     q1 = ops.gemm(P.h(self.p + "probe").view(1, d), P.h(self.att + "q/kernel"), b_mn=True,
                   bias=P.f(self.att + "q/bias"))
@@ -344,9 +378,13 @@ class MAPHead:
     kv = ops.gemm(enc, P.h(self.att + "kv/kernel"), b_mn=True, bias=P.f(self.att + "kv/bias"))
     kv3 = kv.view(n, N, 2 * d)
     o, lse = ops.attention_fwd(qn.view(n, 1, d), kv3[:, :, 0:d], kv3[:, :, d:], self.heads)
+    if not save:
+      del kv, kv3, lse
     a = ops.gemm(o.view(n, d), P.h(self.att + "out_proj/kernel"), b_mn=True, bias=P.f(self.att + "out/bias"))
     y, mean, rstd = ops.layernorm_fwd(a, P.f(self.p + "LayerNorm_0/scale"), P.f(self.p + "LayerNorm_0/bias"))
-    out, mlp_saved = mlp_fwd(Scope(P, self.p + "MlpBlock_0/"), y, a, out_dtype=torch.float32)
+    out, mlp_saved = mlp_fwd(Scope(P, self.p + "MlpBlock_0/"), y, a, out_dtype=torch.float32, save=save)
+    if not save:
+      return out, None
     return out, (enc, qn, kv, o, lse, a, mean, rstd, mlp_saved)
 
   def bwd(self, P, dout, saved, n, N):
@@ -478,52 +516,97 @@ class _Model:
       self._sincos = torch.from_numpy(posemb_sincos_2d(gh, gw, self.width)).to(P.device).bfloat16()
     return self._sincos
 
-  def fwd(self, P, image):
+  def stages(self):
+    """The model as backward stages, bottom-up, each a tuple of storage-name prefixes: embedding
+    (patch kernel, posemb, cls), every encoder block (the scan-stacked encoder is one), encoder_norm,
+    the MAP head, pre_logits, head.  Parameterless pools belong to no stage."""
+    p = self.prefix
+    out = [(p + "embedding/", p + "pos_embedding", p + "cls")] + self.encoder.stages()
+    out.append((p + "Transformer/encoder_norm/",))
+    if self.map_head is not None:
+      out.append((self.map_head.p,))
+    if self.rep_size:
+      out.append((p + "pre_logits/",))
+    if self.head is not None:
+      out.append((self.head.p,))
+    return out
+
+  def _stage_indices(self):
+    """Indices into stages() of encoder_norm, the MAP head, pre_logits and head (an absent one shares
+    the index of the next)."""
+    i_norm = 1 + (1 if self.scan else self.depth)
+    i_map = i_norm + 1
+    i_pre = i_map + (self.map_head is not None)
+    return i_norm, i_map, i_pre, i_pre + bool(self.rep_size)
+
+  def cut(self, P, frozen):
+    """Index into stages() of the lowest stage with a trained parameter (engine.stage_cut): the
+    backward stops there and everything below runs forward-only.  len(stages()) = wholly frozen."""
+    cache = self.__dict__.setdefault("_cuts", {})
+    key = frozen if frozen is True or frozen is None else frozenset(frozen)
+    if key not in cache:
+      cache[key] = E.stage_cut(P.offsets, self.stages(), frozen)
+    return cache[key]
+
+  def fwd(self, P, image, frozen=None):
     """image [n,H,W,C] fp32 in [-1,1] -> (x fp32 [n, out], saved).  With a class head whose storage is
-    padded (common.ClassifierHead) x is the [n, num_classes] view of the padded logits."""
+    padded (common.ClassifierHead) x is the [n, num_classes] view of the padded logits.
+
+    `frozen`: storage names that receive no gradient (optax.Chain.frozen()), or True for all of them
+    (inference).  Stages below the cut (see cut()) run forward-only and save nothing; the output is
+    bit-identical either way."""
     if self._geom is None:
       self.setup(image.shape[1:3])
     n = image.shape[0]
     gh, gw = self._geom
     N0, d, p = gh * gw, self.width, self.prefix
+    cut = self.cut(P, frozen)
+    i_norm, i_map, i_pre, i_head = self._stage_indices()
     patches = ops.patchify(image, self.patch_size[0])
     x = ops.gemm(patches, P.h(p + "embedding/kernel_flat"), b_mn=True, bias=P.f(p + "embedding/bias"),
                  aux=self._posemb16(P), aux_row_mod=N0, epilogue=L.EPI_BIAS_RESID)
+    if cut > 0:
+      del patches
+      patches = None
     N = N0
     if self.pool_type == "tok":
       # cls token is prepended AFTER the position embedding was added (models/vit.py:223-225)
       x = ops.concat_cls(x, P.f(p + "cls").view(d), n, N0)
       N = N0 + 1
-    x, enc_saved = self.encoder.fwd(P, x, n, N)
+    train_from = 0 if cut <= 1 else (self.depth if self.scan else min(cut - 1, self.depth))
+    x, enc_saved = self.encoder.fwd(P, x, n, N, train_from=train_from)
     en = self.prefix + "Transformer/encoder_norm/"
-    saved = {"patches": patches, "enc": enc_saved, "n": n, "N": N}
+    saved = {"patches": patches, "enc": enc_saved, "n": n, "N": N, "cut": cut, "train_from": train_from}
+    keep_norm = cut <= i_norm
     if self.pool_type == "map":
       encd, mean, rstd = ops.layernorm_fwd(x, P.f(en + "scale"), P.f(en + "bias"))
-      saved["norm"] = (x, mean, rstd)
-      out, saved["map"] = self.map_head.fwd(P, encd, n, N)
+      saved["norm"] = (x, mean, rstd) if keep_norm else None
+      del x
+      out, saved["map"] = self.map_head.fwd(P, encd, n, N, save=cut <= i_map)
     elif self.pool_type == "gap":
       encd, mean, rstd = ops.layernorm_fwd(x, P.f(en + "scale"), P.f(en + "bias"))
-      saved["norm"] = (x, mean, rstd)
+      saved["norm"] = (x, mean, rstd) if keep_norm else None
       out = ops.pool_fwd(encd, n, N, 0, out_dtype=torch.float32)
     elif self.pool_type in ("0", "tok"):
       # LayerNorm is per token, so LN(x)[:, 0] == LN(x[:, 0]): select first, normalise one row
       x0 = ops.pool_fwd(x, n, N, 1, tok=0)
       out, mean, rstd = ops.layernorm_fwd(x0, P.f(en + "scale"), P.f(en + "bias"), out_dtype=torch.float32)
-      saved["norm"] = (x0, mean, rstd)
+      saved["norm"] = (x0, mean, rstd) if keep_norm else None
     elif self.pool_type == "none":
       # no pooling (models/vit.py:252-253): pre_logits / head run on every token, out is [n, N, .]
       out, mean, rstd = ops.layernorm_fwd(x, P.f(en + "scale"), P.f(en + "bias"))
-      saved["norm"] = (x, mean, rstd)
+      saved["norm"] = (x, mean, rstd) if keep_norm else None
     else:
       raise ValueError(f"Unknown pool type: '{self.pool_type}'")
     if self.rep_size:
       pre = ops.gemm(self._to16(out), P.h(p + "pre_logits/kernel"), b_mn=True,
                      bias=P.f(p + "pre_logits/bias"), out_dtype=torch.float32)
-      saved["rep_in"] = out
+      keep = cut <= i_pre
+      saved["rep_in"] = out if keep else None
       out = ops.tanh_fwd(pre)
-      saved["rep_out"] = out
+      saved["rep_out"] = out if keep else None
     if self.head is not None:
-      saved["head_in"] = out
+      saved["head_in"] = out if cut <= i_head else None
       out = self.head.fwd(P, out)
     if self.pool_type == "none":
       if out.dtype != torch.float32:
@@ -538,20 +621,31 @@ class _Model:
     With a padded class head, out is the padded class count (ClassifierHead.bwd)."""
     p, d = self.prefix, self.width
     n, N = saved["n"], saved["N"]
+    cut, train_from = saved["cut"], saved["train_from"]
+    if cut == len(self.stages()):        # wholly frozen: nothing to do
+      return
+    i_norm, i_map, i_pre, i_head = self._stage_indices()
     en = self.prefix + "Transformer/encoder_norm/"
     if self.pool_type == "none":
       dout = dout.reshape(n * N, -1)
     if self.head is not None:
       dout = self.head.bwd(P, dout, saved["head_in"])
+      if cut == i_head:
+        return
     if self.rep_size:
       dpre = ops.tanh_bwd(dout, saved["rep_out"])
       d16 = self._to16(dpre)
       ops.colsum(dpre, P.g(p + "pre_logits/bias"))
       ops.gemm(self._to16(saved["rep_in"]), d16, a_mn=True, b_mn=True, out=P.g(p + "pre_logits/kernel"), reduce_out=True)
+      if cut == i_pre:
+        return
       dout = ops.gemm(d16, P.h(p + "pre_logits/kernel"), out_dtype=torch.float32)
-    last_b = self.encoder.last_bias_grad(P)
+    # below the cut the last block is frozen: its Dense_1 bias gradient stays zero
+    last_b = self.encoder.last_bias_grad(P) if cut < i_norm else None
     if self.pool_type == "map":
       denc = self.map_head.bwd(P, dout, saved["map"], n, N)
+      if cut == i_map:
+        return
       x, mean, rstd = saved["norm"]
       dx = ops.layernorm_bwd(denc, x, P.f(en + "scale"), mean, rstd, dscale=P.g(en + "scale"),
                              dbias=P.g(en + "bias"), dx_colsum=last_b)
@@ -565,6 +659,11 @@ class _Model:
       dx0 = ops.layernorm_bwd(dout, x0, P.f(en + "scale"), mean, rstd, dscale=P.g(en + "scale"),
                               dbias=P.g(en + "bias"), dx_colsum=last_b)
       dx = ops.pool_bwd(dx0, n, N, 1, tok=0)
+    if cut == i_norm:
+      return
+    if cut > 0:          # the embedding is frozen: the encoder's backward is the last one
+      self.encoder.bwd(P, dx, saved["enc"], n, N, None, train_from=train_from)
+      return
     # encoder: the column sum of the gradient reaching the embedding output is the patch-embed
     # bias gradient (models/vit.py:212-214)
     if self.pool_type == "tok":
@@ -591,7 +690,7 @@ class _Model:
   def apply(self, variables, image, *, train=False):
     """(x, out) like flax apply (models/vit.py:206-276); `out` holds what this path keeps."""
     P = variables["params"]
-    x, saved = self.fwd(P, image)
+    x, _ = self.fwd(P, image, frozen=True)     # no backward follows: forward-only, same bits
     out = {"head_input": x} if not (self.rep_size or self.num_classes) else {}
     out["pre_logits" if not self.num_classes else "logits"] = x
     return x, out

@@ -191,6 +191,12 @@ class Chain:
                          else [(storage, base)]):
           self.tensors.append((_AdafactorTensor(nm, view, self.af["min_dim_size_to_factor"]), slot, lr_mult, wd))
 
+  def frozen(self):
+    """frozenset of the storage names whose schedule is None.  The models' forward takes it
+    (`frozen=`) to run the stages that hold no trained parameter forward-only, and the gradient
+    all-reduce skips their ranges."""
+    return frozenset(storage for storage, slot, *_ in self.per_storage if slot is None)
+
   def init(self, P):
     dev = P.flat.device
     state = {"count": 0, "scalars": torch.zeros(4, dtype=torch.float32, device=dev)}   # [gnorm_sq, upd_sq, param_sq]

@@ -15,11 +15,20 @@ from big_vision_b200.trainers.proj.image_text.siglip import Dist
 _LOSSES = {"sigmoid_xent": ops.sigmoid_xent, "softmax_xent": ops.softmax_xent}
 
 
-def loss_and_grads(model, P, images, labels, loss_name="sigmoid_xent", dist_view=None, **fwd_kw):
+def loss_and_grads(model, P, images, labels, loss_name="sigmoid_xent", dist_view=None, frozen=None, **fwd_kw):
   """value_and_grad(loss_fn)(params) of train.py:295-303 on this rank's shard; P.grad holds the
-  LOCAL gradient of the LOCAL-mean loss (callers average across ranks)."""
+  LOCAL gradient of the LOCAL-mean loss (callers average across ranks).
+
+  `frozen` (storage names, optax.Chain.frozen()): parameters that get no gradient.  Models with
+  backward stages (ViT) run the stages below the lowest trained one forward-only -- a linear probe
+  (`head/.*` trained, the rest None) runs the backbone without a backward -- and the all-reduce
+  covers the trained ranges only.  Other models (MLP-Mixer) ignore it and run the full path."""
   if loss_name not in _LOSSES:
     raise NotImplementedError(f"loss {loss_name}")
+  ranges = None
+  if frozen and hasattr(model, "stages"):
+    fwd_kw["frozen"] = frozen
+    ranges = P.trained_ranges(frozen)
   P.zero_grad()
   logits, saved = model.fwd(P, images, **fwd_kw)
   loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
@@ -35,7 +44,7 @@ def loss_and_grads(model, P, images, labels, loss_name="sigmoid_xent", dist_view
     model.bwd(P, dlogits, saved)
   else:      # gradient all-reduce (SUM; callers divide by world) overlapped with the backward
     from big_vision_b200.trainers.proj.image_text.siglip import all_reduce_grads
-    all_reduce_grads(P, dist_view, lambda: model.bwd(P, dlogits, saved))
+    all_reduce_grads(P, dist_view, lambda: model.bwd(P, dlogits, saved), ranges=ranges)
   return loss, logits
 
 
@@ -43,6 +52,7 @@ def make_update_fn(model, tx, config):
   mixup_p = (config.get("mixup") or {}).get("p")
   loss_name = config.get("loss", "sigmoid_xent")
   d = Dist()
+  frozen = tx.frozen() if hasattr(tx, "frozen") else frozenset()
 
   def update_fn(train_state, rng, batch):
     P, opt = train_state["params"], train_state["opt"]
@@ -55,7 +65,7 @@ def make_update_fn(model, tx, config):
     # stochastic depth (Mixer, mlp_mixer.py:173-177) draws its masks from the step's rng like the
     # reference's `rngs={"dropout": rng}` (train.py:296-299)
     kw = dict(train=True, rng=rng) if getattr(model, "stoch_depth", 0.0) else {}
-    loss, _ = loss_and_grads(model, P, images, labels, loss_name, dist_view=d, **kw)
+    loss, _ = loss_and_grads(model, P, images, labels, loss_name, dist_view=d, frozen=frozen, **kw)
     # the loss is the mean over the GLOBAL batch: sum the per-rank means and divide by world
     d.all_reduce_sum(loss)
     sc = tx.update(P, opt, grad_mult=1.0 / d.world)

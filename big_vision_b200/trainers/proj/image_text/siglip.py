@@ -94,8 +94,9 @@ class BucketedGradAllReduce:
   stream carries on with the next block -- and `finish()` reduces what is left and joins.
   Elementwise SUM over the same values as one big all-reduce: results are identical."""
 
-  def __init__(self, P, d, bucket_elems=8 << 20):
+  def __init__(self, P, d, bucket_elems=8 << 20, ranges=None):
     self.P, self.d, self.bucket = P, d, bucket_elems
+    self.ranges = ranges                   # trained [lo, hi) slices (None: the whole buffer)
     idx = {s.name: i for i, s in enumerate(P.specs)}
     self.idx = idx
     self.groups = []                       # (lo, hi, [spec index ...], [offset ...]) in layout order
@@ -110,9 +111,11 @@ class BucketedGradAllReduce:
     self.P.on_ready = self.ready
 
   def _launch(self, lo, hi):
-    if hi > lo:
-      h = dist.all_reduce(self.P.grad[lo:hi], op=dist.ReduceOp.SUM, async_op=True)
-      self.handles.append(h)
+    for a, b in ([(lo, hi)] if self.ranges is None else
+                 [(max(lo, r0), min(hi, r1)) for r0, r1 in self.ranges]):
+      if b > a:
+        h = dist.all_reduce(self.P.grad[a:b], op=dist.ReduceOp.SUM, async_op=True)
+        self.handles.append(h)
 
   def ready(self, name):
     """Everything at or after storage parameter `name` in spec order has its final gradient."""
@@ -136,10 +139,12 @@ class BucketedGradAllReduce:
     self.handles = []
 
 
-def all_reduce_grads(P, d, run_backward):
+def all_reduce_grads(P, d, run_backward, ranges=None):
   """Runs `run_backward()` and all-reduces (SUM) the flat gradient buffer when there are peers.
+  `ranges` (FlatParams.trained_ranges) restricts the reduction to those [lo, hi) slices: frozen
+  parameters have no gradient to reduce, and their slices stay as the backward left them.
 
-  Default: ONE all-reduce after the backward.  BV_GRAD_ALLREDUCE=overlap selects the bucketed form
+  Default: ONE all-reduce after the backward (one per range).  BV_GRAD_ALLREDUCE=overlap selects the bucketed form
   that runs under the backward (BucketedGradAllReduce).  Which of the two is faster on H100 has not
   been measured: an NCCL kernel that holds a few SMs delays the GEMM tiles running beside it, so the
   overlapped form pays for part of the collective anyway, plus the extra launches."""
@@ -148,9 +153,13 @@ def all_reduce_grads(P, d, run_backward):
     return
   if os.environ.get("BV_GRAD_ALLREDUCE") != "overlap":
     run_backward()
-    d.all_reduce_sum(P.grad)
+    if ranges is None:
+      d.all_reduce_sum(P.grad)
+    else:
+      for lo, hi in ranges:
+        d.all_reduce_sum(P.grad[lo:hi])
     return
-  red = BucketedGradAllReduce(P, d)
+  red = BucketedGradAllReduce(P, d, ranges=ranges)
   red.begin()
   try:
     run_backward()
@@ -158,12 +167,13 @@ def all_reduce_grads(P, d, run_backward):
     red.finish()
 
 
-def sigmoid_loss_fwd_bwd(P, zimg, ztxt, d, scal):
+def sigmoid_loss_fwd_bwd(P, zimg, ztxt, d, scal, img_grad=True, txt_grad=True):
   """Pairwise sigmoid loss + gradients for the local image rows against ALL text rows.
 
   scal: fp32 device tensor [>=1]; scal[0] += this rank's share of the loss.
   dt/db are accumulated straight into the gradient slots of `t` and `b`.
-  Returns (dzimg [n,D] fp32, dztxt_local [n,D] fp32).
+  Returns (dzimg [n,D] fp32, dztxt_local [n,D] fp32); img_grad / txt_grad = False (a wholly frozen
+  tower) skips that embedding's gradient, its GEMM and its collective, and returns None for it.
   """
   n, D = zimg.shape
   ztxt_all = d.all_gather_rows(ztxt)                       # C1
@@ -174,13 +184,16 @@ def sigmoid_loss_fwd_bwd(P, zimg, ztxt, d, scal):
   has_b = "b" in P.offsets
   G = ops.siglip_loss(dots, d.rank * n, P.f("t"), P.f("b") if has_b else None, B,
                       scal[0:1], P.g("t"), P.g("b") if has_b else None)
-  dzimg = ops.gemm(G, zt16, b_mn=True, out_dtype=torch.float32)                  # G . ztxt_all
-  dztxt_all = ops.gemm(G, zi16, a_mn=True, b_mn=True, out_dtype=torch.float32)   # G^T . zimg
-  dztxt = d.reduce_scatter_rows(dztxt_all)                 # C2
+  dzimg = dztxt = None
+  if img_grad:
+    dzimg = ops.gemm(G, zt16, b_mn=True, out_dtype=torch.float32)                  # G . ztxt_all
+  if txt_grad:
+    dztxt_all = ops.gemm(G, zi16, a_mn=True, b_mn=True, out_dtype=torch.float32)   # G^T . zimg
+    dztxt = d.reduce_scatter_rows(dztxt_all)               # C2
   return dzimg, dztxt
 
 
-def chunked_sigmoid_loss_fwd_bwd(P, zimg, ztxt, d, scal):
+def chunked_sigmoid_loss_fwd_bwd(P, zimg, ztxt, d, scal, img_grad=True, txt_grad=True):
   """The memory-lean variant of the same loss: section 3.1 of arxiv.org/abs/2303.15343,
   `chunked_sigmoid_loss` in _deprecated_contrastive.py:168-200.  G rounds; round r scores the local
   images against rank r's texts only, so the live slab is [n, n] instead of [n, B].  Positives sit
@@ -192,7 +205,7 @@ def chunked_sigmoid_loss_fwd_bwd(P, zimg, ztxt, d, scal):
   B = n * d.world
   zi16 = ops.cast(zimg, torch.empty_like(zimg, dtype=torch.bfloat16))
   has_b = "b" in P.offsets
-  dzimg = torch.zeros((n, D), dtype=torch.float32, device=zimg.device)
+  dzimg = torch.zeros((n, D), dtype=torch.float32, device=zimg.device) if img_grad else None
   dztxt = None
   for r in range(d.world):
     chunk = d.broadcast_rows(ztxt, src=r)                          # C1, one peer per round
@@ -200,15 +213,17 @@ def chunked_sigmoid_loss_fwd_bwd(P, zimg, ztxt, d, scal):
     dots = ops.gemm(zi16, zc16, out_dtype=torch.float32)           # [n, n]
     G = ops.siglip_loss(dots, 0 if r == d.rank else -n, P.f("t"), P.f("b") if has_b else None, B,
                         scal[0:1], P.g("t"), P.g("b") if has_b else None)
-    ops.gemm(G, zc16, b_mn=True, out=dzimg, reduce_out=True)       # dzimg += G . chunk
-    dzc = ops.gemm(G, zi16, a_mn=True, b_mn=True, out_dtype=torch.float32)   # G^T . zimg  [n, D]
-    dzc = d.reduce_rows(dzc, dst=r)                                # C2, delivered to the owner
-    if r == d.rank:
-      dztxt = dzc
+    if img_grad:
+      ops.gemm(G, zc16, b_mn=True, out=dzimg, reduce_out=True)     # dzimg += G . chunk
+    if txt_grad:
+      dzc = ops.gemm(G, zi16, a_mn=True, b_mn=True, out_dtype=torch.float32)   # G^T . zimg  [n, D]
+      dzc = d.reduce_rows(dzc, dst=r)                              # C2, delivered to the owner
+      if r == d.rank:
+        dztxt = dzc
   return dzimg, dztxt
 
 
-def softmax_loss_fwd_bwd(P, zimg, ztxt, d, scal):
+def softmax_loss_fwd_bwd(P, zimg, ztxt, d, scal, img_grad=True, txt_grad=True):
   """The CLIP softmax loss, `softmax_loss` of _deprecated_contrastive.py:80-101 (config.loss_fn="softmax"):
   0.5 * (image->text + text->image) InfoNCE, each direction a softmax of the local rows against ALL
   gathered columns with the positive on this rank's diagonal block; temperature only (no bias).
@@ -229,15 +244,18 @@ def softmax_loss_fwd_bwd(P, zimg, ztxt, d, scal):
   # text -> image: local texts against all images
   dots = ops.gemm(zt16, zia16, out_dtype=torch.float32)                          # [n, B]
   G2 = ops.softmax_contrastive_loss(dots, off, P.f("t"), B, 0.5, scal[0:1], P.g("t"), scal[2:3])
-  dzimg = ops.gemm(G1, zta16, b_mn=True, out_dtype=torch.float32)                # G1 . ztxt_all
-  dztxt = ops.gemm(G2, zia16, b_mn=True, out_dtype=torch.float32)                # G2 . zimg_all
   # contributions to the OTHER ranks' rows (the gathered operand of each direction), summed back
-  dztxt_all = ops.gemm(G1, zi16, a_mn=True, b_mn=True, out_dtype=torch.float32)  # G1^T . zimg   [B, D]
-  dzimg_all = ops.gemm(G2, zt16, a_mn=True, b_mn=True, out_dtype=torch.float32)  # G2^T . ztxt   [B, D]
-  dztxt = ops.axpby(dztxt, d.reduce_scatter_rows(dztxt_all), 1.0, 1.0) if d.world > 1 else \
-      ops.axpby(dztxt, dztxt_all, 1.0, 1.0)
-  dzimg = ops.axpby(dzimg, d.reduce_scatter_rows(dzimg_all), 1.0, 1.0) if d.world > 1 else \
-      ops.axpby(dzimg, dzimg_all, 1.0, 1.0)
+  dzimg = dztxt = None
+  if txt_grad:
+    dztxt = ops.gemm(G2, zia16, b_mn=True, out_dtype=torch.float32)              # G2 . zimg_all
+    dztxt_all = ops.gemm(G1, zi16, a_mn=True, b_mn=True, out_dtype=torch.float32)  # G1^T . zimg [B, D]
+    dztxt = ops.axpby(dztxt, d.reduce_scatter_rows(dztxt_all), 1.0, 1.0) if d.world > 1 else \
+        ops.axpby(dztxt, dztxt_all, 1.0, 1.0)
+  if img_grad:
+    dzimg = ops.gemm(G1, zta16, b_mn=True, out_dtype=torch.float32)              # G1 . ztxt_all
+    dzimg_all = ops.gemm(G2, zt16, a_mn=True, b_mn=True, out_dtype=torch.float32)  # G2^T . ztxt [B, D]
+    dzimg = ops.axpby(dzimg, d.reduce_scatter_rows(dzimg_all), 1.0, 1.0) if d.world > 1 else \
+        ops.axpby(dzimg, dzimg_all, 1.0, 1.0)
   return dzimg, dztxt
 
 
@@ -256,20 +274,31 @@ def _loss_fn(config):
 def make_update_fn(model, tx, config=None):
   """Returns update_fn(train_state, rng, batch) -> (train_state, measurements), the
   signature of siglip.py:275.  train_state = {"params": FlatParams, "opt": opt_state};
-  it is updated IN PLACE (the reference donates it, siglip.py:273)."""
+  it is updated IN PLACE (the reference donates it, siglip.py:273).
+
+  Parameters whose schedule is None (tx.frozen(), e.g. the image tower under SigLiT's
+  `schedule=[("img/.*", None), (".*", ...)]`) get no gradient: the stages that hold only frozen
+  parameters run forward-only, a wholly frozen tower gets no embedding gradient from the loss, and
+  the gradient all-reduce covers the trained ranges only."""
   d = Dist()
   loss_fwd_bwd = _loss_fn(config)
+  frozen = tx.frozen() if hasattr(tx, "frozen") else frozenset()
+  plan = {}
 
   def update_fn(train_state, rng, batch):
     del rng  # dropout is 0 on this path; nothing stochastic in the step
     P, opt = train_state["params"], train_state["opt"]
     images, labels = batch["image"], batch["labels"]
+    if id(P) not in plan:
+      plan.clear()
+      plan[id(P)] = _frozen_plan(model, P, frozen)
+    fz, ranges, (img_frozen, txt_frozen) = plan[id(P)]
     P.zero_grad()
     scal = torch.zeros(4, dtype=torch.float32, device=P.flat.device)
-    zimg, ztxt, saved = model.fwd(P, images, labels)
-    dzimg, dztxt = loss_fwd_bwd(P, zimg, ztxt, d, scal)
+    zimg, ztxt, saved = model.fwd(P, images, labels, frozen=fz)
+    dzimg, dztxt = loss_fwd_bwd(P, zimg, ztxt, d, scal, img_grad=not img_frozen, txt_grad=not txt_frozen)
     # C3 (+ dt, db inside the flat buffer), bucketed and overlapped with the backward
-    all_reduce_grads(P, d, lambda: model.bwd(P, dzimg, dztxt, saved))
+    all_reduce_grads(P, d, lambda: model.bwd(P, dzimg, dztxt, saved), ranges=ranges)
     d.all_reduce_sum(scal)                                 # C4: loss
     sc = tx.update(P, opt, grad_mult=1.0)
     measurements = {
@@ -283,15 +312,26 @@ def make_update_fn(model, tx, config=None):
   return update_fn
 
 
-def loss_and_grads(model, P, images, labels, loss_fn="sigmoid"):
+def _frozen_plan(model, P, frozen):
+  """(frozen for the forward or None, trained ranges for the all-reduce or None, (image tower wholly
+  frozen, text tower wholly frozen)); all None / False when nothing is frozen: today's path."""
+  if not frozen:
+    return None, None, (False, False)
+  return frozen, P.trained_ranges(frozen), model.tower_frozen(P, frozen)
+
+
+def loss_and_grads(model, P, images, labels, loss_fn="sigmoid", frozen=None):
   """value_and_grad(loss_fn)(params) of siglip.py:287-311 without the optimizer: returns the
-  global loss (device scalar) with P.grad holding d loss / d params (summed over ranks)."""
+  global loss (device scalar) with P.grad holding d loss / d params (summed over ranks).  `frozen`
+  (storage names, optax.Chain.frozen()) as in make_update_fn: their gradients are not computed."""
   d = Dist()
   sigmoid_loss_fwd_bwd = _loss_fn({"loss_fn": loss_fn})   # pylint: disable=redefined-outer-name
+  fz, ranges, (img_frozen, txt_frozen) = _frozen_plan(model, P, frozen)
   P.zero_grad()
   scal = torch.zeros(4, dtype=torch.float32, device=P.flat.device)
-  zimg, ztxt, saved = model.fwd(P, images, labels)
-  dzimg, dztxt = sigmoid_loss_fwd_bwd(P, zimg, ztxt, d, scal)
-  all_reduce_grads(P, d, lambda: model.bwd(P, dzimg, dztxt, saved))
+  zimg, ztxt, saved = model.fwd(P, images, labels, frozen=fz)
+  dzimg, dztxt = sigmoid_loss_fwd_bwd(P, zimg, ztxt, d, scal, img_grad=not img_frozen,
+                                      txt_grad=not txt_frozen)
+  all_reduce_grads(P, d, lambda: model.bwd(P, dzimg, dztxt, saved), ranges=ranges)
   d.all_reduce_sum(scal)
   return scal[0], {"zimg": zimg, "ztxt": ztxt, "dzimg": dzimg, "dztxt": dztxt}

@@ -43,6 +43,8 @@ extern "C" {
 #define BV_EPI_BIAS_GELU 2   /* D2 = bf16(alpha*acc + bias); D = gelu_tanh(D2)       */
 #define BV_EPI_BIAS_RESID 3  /* D = bf16(alpha*acc + bias) + aux[m (% aux_row_mod), n] */
 #define BV_EPI_DGELU 4       /* D = alpha*acc * gelu_tanh'(aux[m, n])                */
+#define BV_EPI_BIAS_GELU_ACT 5 /* D = gelu_tanh(bf16(alpha*acc + bias)); no D2: the
+                                  forward-only BIAS_GELU (same bits as its D)          */
 
 const char* bv_last_error_string(void);
 int bv_version(void);

@@ -190,6 +190,17 @@ def cases(pairs, bufs, block_n=0):
     o = torch.empty(M, MLP, device="cuda", dtype=torch.bfloat16)
     return [o], lambda: gemm(x, w1, aux=h, out=o, epilogue=L.EPI_DGELU)
   add("img dgrad Dense_1 gelu'", M, MLP, D, dg_d1_nocs, 2 * (M * D + MLP * D + 2 * M * MLP))
+
+  # appended: the forward-only Dense_0 (a frozen tower, apply()) writes the activation only, no
+  # pre-activation; compare with the "fwd Dense_0 gelu" rows of the same tower
+  w0, bm = bufs.get("w0", (D, MLP), 0.03), bufs.get("b3072", (MLP,), 1.0, torch.float32)
+  for tower, Mt in (("img", pairs * IMG_TOKENS), ("txt", pairs * TXT_TOKENS)):
+    xt = bufs.get(f"{tower}.x", (Mt, D))
+
+    def fwd_d0_act(xt=xt, Mt=Mt):
+      o = torch.empty(Mt, MLP, device="cuda", dtype=torch.bfloat16)
+      return [o], lambda: gemm(xt, w0, b_mn=True, bias=bm, out=o, epilogue=L.EPI_BIAS_GELU_ACT)
+    add(f"{tower} fwd Dense_0   gelu act only", Mt, MLP, D, fwd_d0_act, 2 * (Mt * D + D * MLP + Mt * MLP))
   return out
 
 
