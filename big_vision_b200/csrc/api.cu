@@ -71,7 +71,7 @@ int bv_attention_bwd_hd(const bv_attn_bwd_args* a, int32_t head_dim, void* strea
   g.lddq = a->lddq; g.lddk = a->lddk; g.lddv = a->lddv;
   g.bsdq = a->bsdq; g.bsdk = a->bsdk; g.bsdv = a->bsdv;
   g.dq_colsum = a->dq_colsum; g.dk_colsum = a->dk_colsum; g.dv_colsum = a->dv_colsum;
-  g.delta = a->delta; g.dq_accum = a->dq_accum;
+  g.delta = a->delta;                  // a->dq_accum is ignored (kept for the struct layout)
   return launch_attention_bwd(g, head_dim, S(stream));
 }
 

@@ -16,14 +16,19 @@
 // zeros, never the next head's columns.  The products whose N is the head dim (O += P V, dV, dK,
 // dQ) are single n = DH wgmmas across both boxes (MN-major operand, leading byte offset = one box).
 //
-// Both kernels run one warpgroup per CTA on 64-row tiles and stream the other operand in 64-row
+// Every kernel runs one warpgroup per CTA on 64-row tiles and streams the other operand in 64-row
 // blocks through a two-slot TMA ring, so any sequence length works with the same code:
 //   forward   (b, h, 64 queries):  S = Q K^T (smem x smem), online softmax in registers,
 //             O += P V with P as the register A operand of wgmma.
-//   backward  (b, h, 64 keys):     S^T = K Q^T, dP^T = V dO^T, P^T and dS^T in registers,
-//             dV += P^T dO, dK += dS^T Q (register A operands), dQ_kt = dS K through a swizzled
-//             shared-memory copy of dS^T, stored per key block in fp32; a second kernel sums the
-//             key blocks in a fixed order (bit-reproducible) and converts to bf16.
+//   backward, after delta = rowsum(O o dO), two kernels that each own their outputs and sum over
+//   the streamed blocks in a fixed order inside one wgmma accumulator (bit-reproducible, no
+//   cross-CTA reduction, no workspace):
+//     dQ      (b, h, 64 queries):  S = Q K^T, dP = dO V^T, P = exp(scale S - lse),
+//             dS = P o (dP - delta), dQ += dS K with dS as the register A operand.
+//     dK, dV  (b, h, 64 keys):     S^T = K Q^T, dP^T = V dO^T, P^T and dS^T in registers,
+//             dV += P^T dO, dK += dS^T Q (register A operands).
+//   S and dP are computed twice, once per kernel: 7 instead of 5 64 x 64 x DH products per tile
+//   pair, which is cheaper than the HBM traffic of summing per-key-block dQ partials across CTAs.
 #include "common.cuh"
 #include "host_utils.h"
 #include "kernels.h"
@@ -39,7 +44,8 @@ constexpr float LN2 = 0.6931471805599453f;
 constexpr int THREADS = 128;
 
 // Per-head-dim geometry.  Shared memory: 1024-aligned tiles, then three mbarriers (+ alignment slack);
-// the forward holds Q and two K / V slots, the backward K, V, two Q / dO slots and the 64 x 64 dS^T tile.
+// the forward holds Q and two K / V slots, the dQ kernel Q, dO and two K / V slots, the dK / dV
+// kernel K, V and two Q / dO slots.
 template <int DH>
 struct Geo {
   static_assert(DH == 64 || DH == 72 || DH == 80 || DH == 96 || DH == 104, "head dims 64, 72, 80, 96, 104");
@@ -48,7 +54,7 @@ struct Geo {
   static_assert(KSTEPS >= 4 && KSTEPS <= 8, "one or two 64-column boxes");
   static constexpr int R = DH / 2;                                         // fp32 registers of a [64 x DH] accumulator
   static constexpr int FWD_SMEM = 5 * TILE_BYTES + 1024 + 64;
-  static constexpr int BWD_SMEM = 6 * TILE_BYTES + BOX_BYTES + 1024 + 64;
+  static constexpr int BWD_SMEM = 6 * TILE_BYTES + 1024 + 64;
 };
 
 __device__ __forceinline__ float ex2(float x) {
@@ -90,15 +96,7 @@ __device__ __forceinline__ uint64_t desc_k(uint32_t tile) { return wgmma_desc_sw
 __device__ __forceinline__ uint64_t desc_mn(uint32_t tile) { return wgmma_desc_sw128(tile, 8192u, 1024u); }
 constexpr uint64_t KSTEP_K = 32 >> 4, KSTEP_MN = 2048 >> 4;
 
-// D[64 x DH] (+)= A[64 x 16] * B[DH x 16]^T: the wgmma of N = DH
-template <int TA, int TB, int R>
-__device__ __forceinline__ void wgmma_ss_dh(float (&d)[R], uint64_t a, uint64_t b, int scale_d) {
-  if constexpr (R == 32) wgmma_ss_n64<TA, TB>(d, a, b, scale_d);
-  else if constexpr (R == 36) wgmma_ss_n72<TA, TB>(d, a, b, scale_d);
-  else if constexpr (R == 40) wgmma_ss_n80<TA, TB>(d, a, b, scale_d);
-  else if constexpr (R == 48) wgmma_ss_n96<TA, TB>(d, a, b, scale_d);
-  else wgmma_ss_n104<TA, TB>(d, a, b, scale_d);
-}
+// D[64 x DH] += A[64 x 16] (register fragment) * B[DH x 16]^T: the wgmma of N = DH
 template <int TB, int R>
 __device__ __forceinline__ void wgmma_rs_dh(float (&d)[R], const uint32_t (&a)[4], uint64_t b, int scale_d) {
   if constexpr (R == 32) wgmma_rs_n64<TB>(d, a, b, scale_d);
@@ -265,14 +263,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 // ============================================================================
 struct BwdDev {
   int H, Nq, Nk, QT, KT;
-  long long B;
   float scale, scale_log2;
   const float* lse;
   const float* delta;
-  float* dq_accum;                        // [KT, B, Nq, H*DH] fp32: one dQ slice per key block
-  bf16* dk; bf16* dv;
-  long long lddk, bsdk, lddv, bsdv;
-  float* dk_colsum; float* dv_colsum;
+  bf16* dq; bf16* dk; bf16* dv;
+  long long lddq, bsdq, lddk, bsdk, lddv, bsdv;
+  float* dq_colsum; float* dk_colsum; float* dv_colsum;
 };
 
 // column sums of a [64 x DH] accumulator tile's stored (bf16-rounded) rows < nvalid: the eight lanes
@@ -302,17 +298,115 @@ __device__ __forceinline__ void tile_colsum(const float (&d)[R], float mul, int 
   }
 }
 
+// dQ of one (b, h, 64-query) block: the key blocks stream through the K / V ring and their dS K
+// products accumulate in order in one register tile
 template <int DH>
 __global__ void __launch_bounds__(THREADS)
-attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const BwdDev p) {
+attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                   const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const BwdDev p) {
   using G = Geo<DH>;
   constexpr int TILE_BYTES = G::TILE_BYTES;
-  // K, V (this CTA's key block), Q / dO ring of two, dS^T staging tile
+  // Q, dO (this CTA's query block), K / V ring of two
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t q_s = (smem_u32(smem_raw) + 1023u) & ~1023u, do_s = q_s + TILE_BYTES, k_s = q_s + 2 * TILE_BYTES,
+                 v_s = q_s + 4 * TILE_BYTES;
+  const uint32_t q_bar = q_s + 6 * TILE_BYTES;
+  auto kv_bar = [&](int s) { return q_bar + 8u * (1 + s); };
+
+  const int qt = static_cast<int>(blockIdx.x % p.QT);
+  const int bh = static_cast<int>(blockIdx.x / p.QT);
+  const int h = bh % p.H, b = bh / p.H;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+
+  auto load_kv = [&](int j) {
+    const int s = j & 1;
+    mbar_expect_tx(kv_bar(s), 2 * TILE_BYTES);
+    load_tile<DH>(k_s + s * TILE_BYTES, &tmK, kv_bar(s), h, j * T, b);
+    load_tile<DH>(v_s + s * TILE_BYTES, &tmV, kv_bar(s), h, j * T, b);
+  };
+  if (tid == 0) {
+    mbar_init(q_bar, 1);
+    mbar_init(kv_bar(0), 1);
+    mbar_init(kv_bar(1), 1);
+    fence_barrier_init();
+    mbar_expect_tx(q_bar, 2 * TILE_BYTES);
+    load_tile<DH>(q_s, &tmQ, q_bar, h, qt * T, b);
+    load_tile<DH>(do_s, &tmdO, q_bar, h, qt * T, b);
+    load_kv(0);
+    if (p.KT > 1) load_kv(1);
+  }
+  __syncthreads();
+
+  float dq[G::R];
+  zero(dq);
+  // this thread's two queries (rows r = 0, 1): lse in base 2 and delta; +inf -> P = 0 past Nq
+  const long long bhq = (static_cast<long long>(b) * p.H + h) * p.Nq;
+  const int q0 = qt * T + 16 * warp + (lane >> 2);
+  float lse2[2], dl[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int q = q0 + 8 * r;
+    lse2[r] = q < p.Nq ? p.lse[bhq + q] * LOG2E : INFINITY;
+    dl[r] = q < p.Nq ? p.delta[bhq + q] : 0.f;
+  }
+  mbar_wait(q_bar, 0);
+  for (int j = 0; j < p.KT; ++j) {
+    const int slot = j & 1;
+    mbar_wait(kv_bar(slot), (j >> 1) & 1);
+    const uint32_t kj = k_s + slot * TILE_BYTES, vj = v_s + slot * TILE_BYTES;
+    float s[32], dp[32];
+    wgmma_fence();
+    mma_tile_kk<DH>(s, q_s, kj);          // S  = Q K^T
+    mma_tile_kk<DH>(dp, do_s, vj);        // dP = dO V^T
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    wgmma_fence_regs(dp);
+    // P = exp(scale S - lse), dS = P o (dP - delta); keys past Nk (zero-filled K rows) get P = 0
+    const int kbase = j * T + 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const int r = (i >> 1) & 1;
+      const int key = kbase + 8 * (i >> 2) + (i & 1);
+      const float pr = key < p.Nk ? ex2(s[i] * p.scale_log2 - lse2[r]) : 0.f;
+      dp[i] = pr * (dp[i] - dl[r]);
+    }
+    uint32_t sf[4][4];
+    to_frags(dp, sf);
+    wgmma_fence_regs(dq);
+    wgmma_fence();
+    mma_tile_rs(dq, sf, kj);              // dQ += dS K
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(dq);
+    __syncthreads();                      // every warp is done with this slot
+    if (tid == 0 && j + 2 < p.KT) load_kv(j + 2);
+  }
+  // dQ (scaled) for the queries of this block, and its fused column sum
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int q = q0 + 8 * r;
+    if (q >= p.Nq) continue;
+    bf16* qr = p.dq + b * p.bsdq + static_cast<long long>(q) * p.lddq + h * DH + 2 * (lane & 3);
+#pragma unroll
+    for (int jj = 0; jj < DH / 8; ++jj)
+      *reinterpret_cast<uint32_t*>(qr + 8 * jj) = pack_bf16(dq[4 * jj + 2 * r] * p.scale, dq[4 * jj + 2 * r + 1] * p.scale);
+  }
+  if (p.dq_colsum != nullptr) tile_colsum(dq, p.scale, q0, p.Nq, p.dq_colsum + h * DH, lane);
+}
+
+// dK, dV of one (b, h, 64-key) block: the query blocks stream through the Q / dO ring
+template <int DH>
+__global__ void __launch_bounds__(THREADS)
+attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const BwdDev p) {
+  using G = Geo<DH>;
+  constexpr int TILE_BYTES = G::TILE_BYTES;
+  // K, V (this CTA's key block), Q / dO ring of two
   extern __shared__ uint8_t smem_raw[];
   const uint32_t k_s = (smem_u32(smem_raw) + 1023u) & ~1023u, v_s = k_s + TILE_BYTES, q_s = k_s + 2 * TILE_BYTES,
-                 do_s = k_s + 4 * TILE_BYTES, ds_s = k_s + 6 * TILE_BYTES;
-  const uint32_t kv_bar = ds_s + BOX_BYTES;
+                 do_s = k_s + 4 * TILE_BYTES;
+  const uint32_t kv_bar = k_s + 6 * TILE_BYTES;
   auto q_bar = [&](int s) { return kv_bar + 8u * (1 + s); };
 
   const int kt = static_cast<int>(blockIdx.x % p.KT);
@@ -343,7 +437,6 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   zero(dk);
   zero(dv);
   const long long bhq = (static_cast<long long>(b) * p.H + h) * p.Nq;
-  const int cols = p.H * DH;
   const int key_row = 16 * warp + (lane >> 2);      // + 8r: this thread's rows of the key block
   mbar_wait(kv_bar, 0);
   for (int i = 0; i < p.QT; ++i) {
@@ -376,47 +469,16 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     uint32_t pf[4][4], sf[4][4];
     to_frags(st, pf);
     to_frags(dpt, sf);
-    // dS^T -> shared memory (rows = keys, 128B swizzle), the MN-major A operand of dQ = dS K
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-      for (int f = 0; f < 4; ++f) {
-        const int r = key_row + 8 * (f & 1);
-        const int chunk = 2 * kk + (f >> 1);
-        const uint32_t addr = ds_s + r * 128 + ((chunk ^ (r & 7)) << 4) + 4 * (lane & 3);
-        asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(sf[kk][f]) : "memory");
-      }
-    }
-    fence_proxy_async();
-    __syncthreads();
-    float dq[G::R];
     wgmma_fence_regs(dv);
     wgmma_fence_regs(dk);
     wgmma_fence();
     mma_tile_rs(dv, pf, doi);            // dV += P^T dO
     mma_tile_rs(dk, sf, qi);             // dK += dS^T Q
-    {
-      const uint64_t a = desc_mn(ds_s), bk = desc_mn(k_s);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_ss_dh<1, 1>(dq, a + k * KSTEP_MN, bk + k * KSTEP_MN, k > 0 ? 1 : 0);
-    }
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs(dv);
     wgmma_fence_regs(dk);
-    wgmma_fence_regs(dq);
-    // dQ rows of this query block (rows = queries here) from this key block: this CTA's slice
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      const int q = i * T + 16 * warp + (lane >> 2) + 8 * r;
-      if (q >= p.Nq) continue;
-      float* dst = p.dq_accum + ((static_cast<long long>(kt) * p.B + b) * p.Nq + q) * cols + h * DH + 2 * (lane & 3);
-#pragma unroll
-      for (int jj = 0; jj < DH / 8; ++jj)
-        *reinterpret_cast<float2*>(dst + 8 * jj) = make_float2(dq[4 * jj + 2 * r] * p.scale,
-                                                               dq[4 * jj + 2 * r + 1] * p.scale);
-    }
-    __syncthreads();                     // the Q / dO slot and the dS^T tile are free again
+    __syncthreads();                     // every warp is done with this Q / dO slot
     if (tid == 0 && i + 2 < p.QT) load_q(i + 2);
   }
   // dK (scaled), dV for the keys of this block, and their fused column sums
@@ -464,44 +526,6 @@ attn_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ d_o, floa
 #pragma unroll
     for (int off = 1; off < LANES; off <<= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
     if (chunk == 0) delta[(b * H + h) * N + t] = acc;
-  }
-}
-
-// dq[b,t,c] = bf16(sum_kt acc[kt,b,t,c]) summed in kt order; optional colsum[c] += sum over (b,t) of the
-// ROUNDED values (the bias gradient of the query projection, same definition as the fused column sums
-// of dk / dv).
-// Block = 256 threads: thread (rl, cg) walks rows rl, rl+R, ... of its row chunk for column group cg.
-__global__ void __launch_bounds__(256)
-attn_dq_convert_kernel(const float* __restrict__ acc, int KT, bf16* __restrict__ dq, float* __restrict__ colsum,
-                       int64_t rows_total, int N, int cols, int64_t lddq, int64_t bsdq, int rows_per_block) {
-  const int groups = cols / 8;                        // 8-column groups
-  const int rlanes = 256 / groups > 0 ? 256 / groups : 1;
-  const int cg = threadIdx.x % groups, rl = threadIdx.x / groups;
-  const int64_t r0 = static_cast<int64_t>(blockIdx.x) * rows_per_block;
-  float cs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-  if (rl < rlanes) {
-    for (int64_t r = r0 + rl; r < r0 + rows_per_block && r < rows_total; r += rlanes) {
-      float4 a = *reinterpret_cast<const float4*>(acc + r * cols + cg * 8);
-      float4 c = *reinterpret_cast<const float4*>(acc + r * cols + cg * 8 + 4);
-      for (int kt = 1; kt < KT; ++kt) {
-        const float* src = acc + (kt * rows_total + r) * cols + cg * 8;
-        const float4 a2 = *reinterpret_cast<const float4*>(src), c2 = *reinterpret_cast<const float4*>(src + 4);
-        a.x += a2.x; a.y += a2.y; a.z += a2.z; a.w += a2.w;
-        c.x += c2.x; c.y += c2.y; c.z += c2.z; c.w += c2.w;
-      }
-      uint4 q;
-      q.x = pack_bf16(a.x, a.y); q.y = pack_bf16(a.z, a.w);
-      q.z = pack_bf16(c.x, c.y); q.w = pack_bf16(c.z, c.w);
-      const int64_t b = r / N;
-      const int t = static_cast<int>(r % N);
-      *reinterpret_cast<uint4*>(dq + b * bsdq + t * lddq + cg * 8) = q;
-      cs[0] += bf16_lo(q.x); cs[1] += bf16_hi(q.x); cs[2] += bf16_lo(q.y); cs[3] += bf16_hi(q.y);
-      cs[4] += bf16_lo(q.z); cs[5] += bf16_hi(q.z); cs[6] += bf16_lo(q.w); cs[7] += bf16_hi(q.w);
-    }
-    if (colsum != nullptr) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) atomicAdd(colsum + cg * 8 + k, cs[k]);
-    }
   }
 }
 
@@ -562,15 +586,14 @@ int attention_bwd(const AttnBwdArgs& g, cudaStream_t s) {
   int rc = check_attn(a, "bv_attention_bwd");
   if (rc) return rc;
   if (a.lse == nullptr) { set_error("bv_attention_bwd: lse required"); return BV_ERR_INVALID; }
-  if (g.dq_accum == nullptr || g.delta == nullptr) {
-    set_error("bv_attention_bwd: needs the dq_accum [ceil(Nk/64),B,Nq,H*head_dim] and delta [B,H,Nq] fp32 workspaces");
+  if (g.delta == nullptr) {
+    set_error("bv_attention_bwd: needs the delta [B,H,Nq] fp32 workspace");
     return BV_ERR_INVALID;
   }
   if ((reinterpret_cast<uintptr_t>(g.d_o) & 15) || (g.lddo % 8) || (g.bsdo % 8)) {
     set_error("bv_attention_bwd: d_o must be 16B aligned with strides that are multiples of 8");
     return BV_ERR_INVALID;
   }
-  // dq / dk / dv are written with 16-byte / 4-byte vector stores
   const void* grads[3] = {g.dq, g.dk, g.dv};
   const int64_t lds[3] = {g.lddq, g.lddk, g.lddv}, bss[3] = {g.bsdq, g.bsdk, g.bsdv};
   for (int i = 0; i < 3; ++i) {
@@ -579,8 +602,6 @@ int attention_bwd(const AttnBwdArgs& g, cudaStream_t s) {
       return BV_ERR_INVALID;
     }
   }
-  if (a.H * DH > 2048) { set_error("bv_attention_bwd: H*head_dim must be <= 2048"); return BV_ERR_INVALID; }
-  const int cols = a.H * DH;
   // delta = rowsum(O o dO)
   {
     constexpr int lanes = DH == 64 ? 8 : 16;
@@ -594,37 +615,33 @@ int attention_bwd(const AttnBwdArgs& g, cudaStream_t s) {
     if ((rc = check_cuda(cudaGetLastError(), "attn_delta_kernel launch"))) return rc;
   }
   BwdDev p;
-  p.H = a.H; p.Nq = a.Nq; p.Nk = a.Nk; p.B = a.B;
+  p.H = a.H; p.Nq = a.Nq; p.Nk = a.Nk;
   p.QT = (a.Nq + T - 1) / T;
   p.KT = (a.Nk + T - 1) / T;
   p.scale = a.scale;
   p.scale_log2 = a.scale * LOG2E;
   p.lse = a.lse;
   p.delta = g.delta;
-  p.dq_accum = g.dq_accum;
-  p.dk = static_cast<bf16*>(g.dk); p.dv = static_cast<bf16*>(g.dv);
-  p.lddk = g.lddk; p.bsdk = g.bsdk; p.lddv = g.lddv; p.bsdv = g.bsdv;
-  p.dk_colsum = g.dk_colsum; p.dv_colsum = g.dv_colsum;
+  p.dq = static_cast<bf16*>(g.dq); p.dk = static_cast<bf16*>(g.dk); p.dv = static_cast<bf16*>(g.dv);
+  p.lddq = g.lddq; p.bsdq = g.bsdq; p.lddk = g.lddk; p.bsdk = g.bsdk; p.lddv = g.lddv; p.bsdv = g.bsdv;
+  p.dq_colsum = g.dq_colsum; p.dk_colsum = g.dk_colsum; p.dv_colsum = g.dv_colsum;
   CUtensorMap tmQ, tmK, tmV, tmdO;
   if ((rc = make_tmap_bnd(&tmQ, a.q, DH, a.H, a.Nq, a.B, a.ldq, a.bsq))) return rc;
   if ((rc = make_tmap_bnd(&tmK, a.k, DH, a.H, a.Nk, a.B, a.ldk, a.bsk))) return rc;
   if ((rc = make_tmap_bnd(&tmV, a.v, DH, a.H, a.Nk, a.B, a.ldv, a.bsv))) return rc;
   if ((rc = make_tmap_bnd(&tmdO, g.d_o, DH, a.H, a.Nq, a.B, g.lddo, g.bsdo))) return rc;
-  const long long grid = a.B * a.H * p.KT;
-  rc = check_cuda(cudaFuncSetAttribute(attn_bwd_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::BWD_SMEM),
-                  "cudaFuncSetAttribute(attn_bwd)");
+  // query blocks of one (b, h) are adjacent in the dQ grid (and key blocks in the dK / dV grid), so the
+  // streamed K / V (Q / dO) tiles they share are served from L2
+  rc = check_cuda(cudaFuncSetAttribute(attn_bwd_dq_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::BWD_SMEM),
+                  "cudaFuncSetAttribute(attn_bwd_dq)");
   if (rc) return rc;
-  attn_bwd_kernel<DH><<<static_cast<unsigned>(grid), THREADS, G::BWD_SMEM, s>>>(tmQ, tmK, tmV, tmdO, p);
-  if ((rc = check_cuda(cudaGetLastError(), "attn_bwd_kernel launch"))) return rc;
-  {
-    const int64_t rows = a.B * a.Nq;
-    const int rows_per_block = 256;
-    const int64_t blocks = (rows + rows_per_block - 1) / rows_per_block;
-    attn_dq_convert_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(
-        g.dq_accum, p.KT, reinterpret_cast<bf16*>(g.dq), g.dq_colsum, rows, a.Nq, cols, g.lddq, g.bsdq,
-        rows_per_block);
-    rc = check_cuda(cudaGetLastError(), "attn_dq_convert_kernel launch");
-  }
+  attn_bwd_dq_kernel<DH><<<static_cast<unsigned>(a.B * a.H * p.QT), THREADS, G::BWD_SMEM, s>>>(tmQ, tmK, tmV, tmdO, p);
+  if ((rc = check_cuda(cudaGetLastError(), "attn_bwd_dq_kernel launch"))) return rc;
+  rc = check_cuda(cudaFuncSetAttribute(attn_bwd_dkdv_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::BWD_SMEM),
+                  "cudaFuncSetAttribute(attn_bwd_dkdv)");
+  if (rc) return rc;
+  attn_bwd_dkdv_kernel<DH><<<static_cast<unsigned>(a.B * a.H * p.KT), THREADS, G::BWD_SMEM, s>>>(tmQ, tmK, tmV, tmdO, p);
+  rc = check_cuda(cudaGetLastError(), "attn_bwd_dkdv_kernel launch");
   return rc;
 }
 

@@ -48,7 +48,6 @@ struct AttnBwdArgs {
   float* dq_colsum; float* dk_colsum; float* dv_colsum;   // optional [H*head_dim] fp32 bias gradients
   int64_t lddq, lddk, lddv, bsdq, bsdk, bsdv;
   float* delta;                                  // workspace [B, H, Nq] fp32
-  float* dq_accum;                               // workspace [ceil(Nk/64), B, Nq, H*head_dim] fp32
 };
 int launch_attention_bwd(const AttnBwdArgs& a, int head_dim, cudaStream_t s);
 

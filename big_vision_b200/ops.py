@@ -169,9 +169,8 @@ def attention_bwd(do, q, k, v, o, lse, heads, scale=None, dq=None, dk=None, dv=N
   if dv is None:
     dv = torch.empty(v.shape, dtype=torch.bfloat16, device=q.device)
   f = _attn_args(q, k, v, o, lse, heads, scale)
-  B, Nq, cols = q.shape
+  B, Nq, _ = q.shape
   delta = torch.empty((B, heads, Nq), dtype=torch.float32, device=q.device)
-  dq_accum = torch.empty(((k.shape[1] + 63) // 64, B, Nq, cols), dtype=torch.float32, device=q.device)
   dop, lddo, bsdo = _attn_view(do)
   dqp, lddq, bsdq = _attn_view(dq)
   dkp, lddk, bsdk = _attn_view(dk)
@@ -181,9 +180,9 @@ def attention_bwd(do, q, k, v, o, lse, heads, scale=None, dq=None, dk=None, dv=N
                        dq_colsum=dq_colsum.data_ptr() if dq_colsum is not None else None,
                        dk_colsum=dk_colsum.data_ptr() if dk_colsum is not None else None,
                        dv_colsum=dv_colsum.data_ptr() if dv_colsum is not None else None,
-                       delta=delta.data_ptr(), dq_accum=dq_accum.data_ptr())
+                       delta=delta.data_ptr())
   L.call("bv_attention_bwd_hd", ctypes.byref(args), dh, _stream())
-  L.LAUNCHES[0] += 2            # delta pre-kernel + main kernel + dQ conversion
+  L.LAUNCHES[0] += 2            # delta pre-kernel + dQ kernel + dK / dV kernel
   return dq, dk, dv
 
 

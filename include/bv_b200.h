@@ -126,13 +126,12 @@ typedef struct bv_attn_bwd_args {
   /* optional fp32 [H*dh] each: += column sums over the valid rows of dq / dk / dv, i.e. the bias
    * gradients of the projections that produced q / k / v */
   float* dq_colsum; float* dk_colsum; float* dv_colsum;
-  /* REQUIRED workspaces: delta [B,H,Nq] fp32 = rowsum(O o dO); dq_accum [ceil(Nk/64),B,Nq,H*dh]
-   * fp32 receives the dQ contribution of each 64-key block, summed in block order (reproducible bit
-   * for bit) during the bf16 conversion into dq */
+  /* REQUIRED workspace: delta [B,H,Nq] fp32 = rowsum(O o dO).  dq, dk and dv are each summed in a
+   * fixed order inside one kernel (reproducible bit for bit), with no other workspace.
+   * dq_accum is IGNORED and may be NULL; it is kept so that the struct layout stays the same. */
   float* delta; float* dq_accum;
 } bv_attn_bwd_args;
 int bv_attention_bwd(const bv_attn_bwd_args* args, void* stream);
-/* H*dh <= 2048 */
 int bv_attention_bwd_hd(const bv_attn_bwd_args* args, int32_t head_dim, void* stream);
 
 /* ---------------------------------------------------------------------------------
