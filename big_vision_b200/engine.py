@@ -176,6 +176,60 @@ def stage_cut(storages, stages, frozen):
   return len(stages)
 
 
+class Stage:
+  """Defaults of a backward stage (see Staged)."""
+  ready = None
+
+  def sink(self, P):
+    return None
+
+
+class Staged:
+  """A model built as `self._stages`, a bottom-up list of backward stages (Stage).  Each stage has
+    `prefixes`: the storage-name prefixes of its parameters;
+    `fwd(P, x, geom, save) -> (y, saved)`: with save=False it keeps nothing (saved is None) and frees
+        each intermediate once it has been consumed;
+    `bwd(P, dy, saved, geom, sink, need_dx) -> dx`: accumulates its parameter gradients; `sink` (or
+        None) receives colsum(dx), and with need_dx=False dx is not computed and None is returned;
+    `sink(P)`: the gradient buffer that equals the column sum of the stage's output gradient, or None;
+    `ready`: None, or the storage name from which on (in spec order) every gradient is final once the
+        stage's backward has run (P.on_ready, the bucketed gradient all-reduce)."""
+
+  def stages(self):
+    """The stages' storage-name prefixes, bottom-up."""
+    return [s.prefixes for s in self._stages]
+
+  def cut(self, P, frozen):
+    """Index into stages() of the lowest stage with a trained parameter (stage_cut): the backward stops
+    there and everything below runs forward-only.  len(stages()) = wholly frozen."""
+    cache = self.__dict__.setdefault("_cuts", {})
+    key = frozen if frozen is True or frozen is None else frozenset(frozen)
+    if key not in cache:
+      cache[key] = stage_cut(P.offsets, self.stages(), frozen)
+    return cache[key]
+
+  def _stages_fwd(self, P, x, geom, frozen):
+    """Runs every stage; those below the cut save nothing.  -> (output, saved for _stages_bwd)."""
+    cut = self.cut(P, frozen)
+    saved = []
+    for i, stage in enumerate(self._stages):
+      x, s = stage.fwd(P, x, geom, i >= cut)
+      saved.append(s)
+    return x, {"stages": saved, "geom": geom, "cut": cut}
+
+  def _stages_bwd(self, P, dy, saved):
+    """Runs the backward from the top stage down to the cut, dropping each stage's saved tensors once
+    its backward is done."""
+    stages, kept, geom, cut = self._stages, saved["stages"], saved["geom"], saved["cut"]
+    on_ready = getattr(P, "on_ready", None)
+    for i in reversed(range(cut, len(stages))):
+      sink = stages[i - 1].sink(P) if i - 1 >= cut else None
+      dy = stages[i].bwd(P, dy, kept[i], geom, sink, i > cut)
+      kept[i] = None
+      if on_ready is not None and stages[i].ready is not None:
+        on_ready(stages[i].ready)
+
+
 # ---- initialisers (numpy; same distributions as the reference's, see SURVEY.md 3.4) -------
 def xavier_uniform(fan_in, fan_out):
   def init(rng, shape):

@@ -23,8 +23,9 @@ def to16(x):
   return ops.cast(x, torch.empty_like(x, dtype=torch.bfloat16))
 
 
-class ClassifierHead:
-  """The `head` Dense (kernel [rep, C], bias [C]) of a classifier, logits in fp32.
+class ClassifierHead(E.Stage):
+  """The `head` Dense (kernel [rep, C], bias [C]) of a classifier, logits in fp32; a backward stage
+  (engine.Staged) of the ViT.
 
   The kernel is the MN-major B operand of the head GEMM, and TMA needs its row stride to be a multiple
   of 16 bytes.  So with C % 8 != 0 (21843 classes for ImageNet-21k, 37 for Oxford pets, ...) it is
@@ -40,6 +41,7 @@ class ClassifierHead:
     self.Cp = (num_classes + 7) // 8 * 8
     pad = "_pad" if self.Cp != self.C else ""
     self.p, self.kernel, self.bias = prefix + "head/", prefix + "head/kernel" + pad, prefix + "head/bias" + pad
+    self.prefixes = (self.p,)
 
   def specs(self):
     rep, C, Cp, init = self.rep, self.C, self.Cp, self.kernel_init
@@ -52,21 +54,22 @@ class ClassifierHead:
                E.Alias(self.p + "bias", self.bias, lambda t: t[:C])]
     return specs, aliases
 
-  def fwd(self, P, x):
-    """x [rows, rep] -> logits fp32 [rows, C]: a view of the [rows, Cp] GEMM output when padded."""
+  def fwd(self, P, x, geom=None, save=True):
+    """x [rows, rep] -> (logits fp32 [rows, C], x if save): a view of the [rows, Cp] GEMM output when
+    padded."""
     out = ops.gemm(to16(x), P.h(self.kernel), b_mn=True, bias=P.f(self.bias), out_dtype=torch.float32)
-    return out if self.Cp == self.C else out[:, :self.C]
+    return (out if self.Cp == self.C else out[:, :self.C]), (x if save else None)
 
-  def bwd(self, P, dlogits, x):
+  def bwd(self, P, dlogits, x, geom=None, sink=None, need_dx=True):
     """dlogits fp32 [rows, Cp], zero in the columns past C; x the forward's input.  Accumulates the
-    head's gradients and returns d x (fp32 [rows, rep])."""
+    head's gradients and returns d x (fp32 [rows, rep]), or None with need_dx=False."""
     if tuple(dlogits.shape[1:]) != (self.Cp,):
       raise ValueError(f"head backward: the logit gradient must be [rows, {self.Cp}] (padded to "
                        f"{self.Cp} zero-filled columns), got {tuple(dlogits.shape)}")
     d16 = to16(dlogits)
     ops.colsum(dlogits, P.g(self.bias))
     ops.gemm(to16(x), d16, a_mn=True, b_mn=True, out=P.g(self.kernel), reduce_out=True)
-    return ops.gemm(d16, P.h(self.kernel), out_dtype=torch.float32)
+    return ops.gemm(d16, P.h(self.kernel), out_dtype=torch.float32) if need_dx else None
 
 
 def _report(ckpt_names, model_names, only_model, only_ckpt):

@@ -143,8 +143,7 @@ class MlpMixer:
     saved["norm"] = (x, mean, rstd)
     out = ops.pool_fwd(y, n, N, 0, out_dtype=torch.float32)
     if self.head is not None:
-      saved["head_in"] = out
-      out = self.head.fwd(P, out)
+      out, saved["head_in"] = self.head.fwd(P, out)
     return out, saved
 
   def bwd(self, P, dout, saved):

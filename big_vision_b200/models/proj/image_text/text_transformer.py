@@ -1,7 +1,7 @@
 """Text tower on the H100 kernels -- mirror of
 big_vision/models/proj/image_text/text_transformer.py:29-99.
 
-Embed(vocab, width) + learned posemb -> vit.Encoder (no attention mask: none is passed at
+Embed(vocab, width) + learned posemb -> the vit encoder blocks (no attention mask: none is passed at
 text_transformer.py:72-75) -> pool ("last" by default; "first", "mean"/"gap", "max"/"gmp", "map",
 :82-93) -> Dense head (:97-98).
 `out["vocab_logits"]` (:80) is dead in training and is never computed here.
@@ -17,11 +17,65 @@ import torch
 
 from big_vision_b200 import engine as E
 from big_vision_b200 import ops
-from big_vision_b200.models import vit
+from big_vision_b200.models import common, vit
+
+
+class _Embed(E.Stage):
+  """Embed_0 plus the learned position embedding (text_transformer.py:62-70)."""
+
+  def __init__(self, prefix, d):
+    self.p, self.d = prefix, d
+    self.prefixes = (prefix + "Embed_0/", prefix + "pos_embedding")
+
+  def fwd(self, P, text, geom, save=True):
+    _, Ln = geom
+    x = ops.embed_fwd(text, P.f(self.p + "Embed_0/embedding"), P.f(self.p + "pos_embedding").view(Ln, self.d))
+    return x, (text if save else None)
+
+  def bwd(self, P, dx, text, geom, sink=None, need_dx=False):
+    _, Ln = geom
+    ops.embed_bwd(text, dx, P.g(self.p + "Embed_0/embedding"), P.g(self.p + "pos_embedding").view(Ln, self.d))
+
+
+class _MAPHead(vit.MAPHead):
+  """The MAP head with a bf16 output, the dtype of the tower's other pools."""
+
+  def fwd(self, P, enc, geom, save=True):
+    out, saved = super().fwd(P, enc, geom, save)
+    return common.to16(out), saved
+
+  def bwd(self, P, dout, saved, geom, sink=None, need_dx=True):
+    return super().bwd(P, ops.cast(dout, torch.empty_like(dout, dtype=torch.float32)), saved, geom, sink, need_dx)
+
+
+class _Head(E.Stage):
+  """The `head` Dense (text_transformer.py:97-98): bf16 input, fp32 output, bf16 input gradient."""
+
+  def __init__(self, prefix, d, out):
+    self.p, self.d, self.out = prefix + "head/", d, out
+    self.prefixes = (self.p,)
+
+  def specs(self):
+    return [E.ParamSpec(self.p + "kernel", (self.d, self.out), E.lecun_normal(self.d)),
+            E.ParamSpec(self.p + "bias", (self.out,), E.zeros)], []
+
+  def fwd(self, P, x, geom, save=True):
+    out = ops.gemm(x, P.h(self.p + "kernel"), b_mn=True, bias=P.f(self.p + "bias"), out_dtype=torch.float32)
+    return out, (x if save else None)
+
+  def bwd(self, P, dout, x, geom, sink=None, need_dx=True):
+    d16 = common.to16(dout)
+    ops.colsum(dout, P.g(self.p + "bias"))
+    ops.gemm(x, d16, a_mn=True, b_mn=True, out=P.g(self.p + "kernel"), reduce_out=True)
+    return ops.gemm(d16, P.h(self.p + "kernel")) if need_dx else None
+
+
+# pool_type -> vit.NormPool's pool ("map": encoder_norm alone, then the MAP head stage)
+_POOLS = {"last": "last", "first": "first", "mean": "mean", "gap": "mean", "max": "max", "gmp": "max", "map": None}
 
 
 @dataclass
-class _Model:
+class _Model(E.Staged):
   """Fields as text_transformer._Model (text_transformer.py:43-52)."""
   num_classes: Optional[int] = None
   width: int = 512
@@ -38,14 +92,19 @@ class _Model:
   def __post_init__(self):
     if self.dropout:
       raise NotImplementedError("dropout > 0 is not on the benchmarked path")
-    if self.pool_type not in ("last", "first", "mean", "gap", "max", "gmp", "map"):
+    if self.pool_type not in _POOLS:
       raise NotImplementedError(f"Cannot do pooling '{self.pool_type}'")
     vit.check_head_dim(self.width, self.num_heads)
-    self.prefix = (self.name + "/") if self.name else ""
-    self.map_head = (vit.MAPHead(self.prefix + "MAPHead_0/", self.width, self.mlp_dim, self.num_heads)
-                     if self.pool_type == "map" else None)
-    self.encoder = vit.Encoder(self.prefix + "Encoder_0/", self.depth, self.width,
-                               self.mlp_dim, self.num_heads, scan=self.scan, remat_policy=self.remat_policy)
+    self.prefix = p = (self.name + "/") if self.name else ""
+    d, enc = self.width, p + "Encoder_0/"
+    # the backward stages, bottom-up (engine.Staged)
+    self._stages = ([_Embed(p, d)]
+                    + vit.encoder_stages(enc, self.depth, d, self.mlp_dim, self.num_heads, self.scan, self.remat_policy)
+                    + [vit.NormPool(enc + "encoder_norm/", d, _POOLS[self.pool_type], torch.bfloat16)])
+    if self.pool_type == "map":
+      self._stages.append(_MAPHead(p + "MAPHead_0/", d, self.mlp_dim, self.num_heads))
+    if self.num_classes:
+      self._stages.append(_Head(p, d, self.num_classes))
     self._len = None
 
   def specs(self, text_len):
@@ -56,130 +115,26 @@ class _Model:
         E.ParamSpec(p + "Embed_0/embedding", (self.vocab_size, d), E.normal(1 / math.sqrt(d))),
         E.ParamSpec(p + "pos_embedding", (1, text_len, d), E.normal(1 / math.sqrt(d))),
     ]
-    s, aliases = self.encoder.specs()
-    specs += s
-    if self.map_head is not None:
-      s, a = self.map_head.specs()
+    aliases = []
+    for stage in self._stages[1:]:
+      s, a = stage.specs()
       specs += s
       aliases += a
-    if self.num_classes:
-      specs += [E.ParamSpec(p + "head/kernel", (d, self.num_classes), E.lecun_normal(d)),
-                E.ParamSpec(p + "head/bias", (self.num_classes,), E.zeros)]
     return specs, aliases
 
   def init(self, seed, text_shape, device="cuda"):
     specs, aliases = self.specs(text_shape[1])
     return E.FlatParams(specs, aliases, device).init(seed)
 
-  def _tok(self, Ln):
-    return {"last": Ln - 1, "first": 0}.get(self.pool_type)
-
-  def stages(self):
-    """Backward stages bottom-up (storage-name prefixes): Embed_0 with pos_embedding, every encoder
-    block (the scan-stacked encoder is one), encoder_norm, the MAP head, head."""
-    p = self.prefix
-    out = [(p + "Embed_0/", p + "pos_embedding")] + self.encoder.stages()
-    out.append((p + "Encoder_0/encoder_norm/",))
-    if self.map_head is not None:
-      out.append((self.map_head.p,))
-    if self.num_classes:
-      out.append((p + "head/",))
-    return out
-
-  def _stage_indices(self):
-    """Indices into stages() of encoder_norm, the MAP head and head."""
-    i_norm = 1 + (1 if self.scan else self.depth)
-    i_map = i_norm + 1
-    return i_norm, i_map, i_map + (self.map_head is not None)
-
-  def cut(self, P, frozen):
-    """Index into stages() of the lowest stage with a trained parameter (see vit._Model.cut)."""
-    cache = self.__dict__.setdefault("_cuts", {})
-    key = frozen if frozen is True or frozen is None else frozenset(frozen)
-    if key not in cache:
-      cache[key] = E.stage_cut(P.offsets, self.stages(), frozen)
-    return cache[key]
-
   def fwd(self, P, text, frozen=None):
-    """text int32 [n, L] -> (fp32 [n, out], saved).  `frozen` as in vit._Model.fwd: the stages below
-    the cut run forward-only and save nothing."""
-    n, Ln = text.shape
-    d, p = self.width, self.prefix
-    cut = self.cut(P, frozen)
-    i_norm, i_map, i_head = self._stage_indices()
-    x = ops.embed_fwd(text, P.f(p + "Embed_0/embedding"), P.f(p + "pos_embedding").view(Ln, d))
-    train_from = 0 if cut <= 1 else (self.depth if self.scan else min(cut - 1, self.depth))
-    x, enc_saved = self.encoder.fwd(P, x, n, Ln, train_from=train_from)
-    en = p + "Encoder_0/encoder_norm/"
-    saved = {"text": text, "enc": enc_saved, "n": n, "L": Ln, "cut": cut, "train_from": train_from}
-    keep_norm = cut <= i_norm
-    tok = self._tok(Ln)
-    if tok is not None:
-      # LayerNorm is per token: LN(x)[:, tok] == LN(x[:, tok]) -- normalise only the pooled row
-      xt = ops.pool_fwd(x, n, Ln, 1, tok=tok)
-      out, mean, rstd = ops.layernorm_fwd(xt, P.f(en + "scale"), P.f(en + "bias"))
-      saved["norm"] = (xt, mean, rstd) if keep_norm else None
-    else:
-      encd, mean, rstd = ops.layernorm_fwd(x, P.f(en + "scale"), P.f(en + "bias"))
-      saved["norm"] = (x, mean, rstd) if keep_norm else None
-      if self.map_head is not None:
-        out, saved["map"] = self.map_head.fwd(P, encd, n, Ln, save=cut <= i_map)
-        out = vit._Model._to16(out)
-      elif self.pool_type in ("max", "gmp"):
-        out = ops.pool_fwd(encd, n, Ln, 2)
-        saved["encd"] = encd if keep_norm else None
-      else:
-        out = ops.pool_fwd(encd, n, Ln, 0)
-    if self.num_classes:
-      saved["head_in"] = out if cut <= i_head else None
-      out = ops.gemm(out, P.h(p + "head/kernel"), b_mn=True, bias=P.f(p + "head/bias"),
-                     out_dtype=torch.float32)
-    return out, saved
+    """text int32 [n, L] -> (fp32 [n, out], saved); bf16 [n, width] without a head.  `frozen` as in
+    vit._Model.fwd: the stages below the cut run forward-only and save nothing."""
+    return self._stages_fwd(P, text, tuple(text.shape), frozen)
 
   def bwd(self, P, dout, saved):
-    p, d = self.prefix, self.width
-    n, Ln = saved["n"], saved["L"]
-    cut, train_from = saved["cut"], saved["train_from"]
-    if cut == len(self.stages()):        # wholly frozen: nothing to do
-      return
-    i_norm, i_map, i_head = self._stage_indices()
-    en = p + "Encoder_0/encoder_norm/"
-    if self.num_classes:
-      d16 = vit._Model._to16(dout)
-      ops.colsum(dout, P.g(p + "head/bias"))
-      ops.gemm(saved["head_in"], d16, a_mn=True, b_mn=True, out=P.g(p + "head/kernel"), reduce_out=True)
-      if cut == i_head:
-        return
-      dout = ops.gemm(d16, P.h(p + "head/kernel"))          # bf16 [n, d]
-    else:
-      dout = vit._Model._to16(dout)
-    # below the cut the last block is frozen: its Dense_1 bias gradient stays zero
-    last_b = self.encoder.last_bias_grad(P) if cut < i_norm else None
-    tok = self._tok(Ln)
-    if tok is not None:
-      xs, mean, rstd = saved["norm"]
-      dxt = ops.layernorm_bwd(dout, xs, P.f(en + "scale"), mean, rstd, dscale=P.g(en + "scale"),
-                              dbias=P.g(en + "bias"), dx_colsum=last_b)
-      dx = ops.pool_bwd(dxt, n, Ln, 1, tok=tok)
-    else:
-      if self.map_head is not None:
-        denc = self.map_head.bwd(P, ops.cast(dout, torch.empty_like(dout, dtype=torch.float32)),
-                                 saved["map"], n, Ln)
-        if cut == i_map:
-          return
-      elif self.pool_type in ("max", "gmp"):
-        denc = ops.pool_max_bwd(dout, saved["encd"], n, Ln)
-      else:
-        denc = ops.pool_bwd(dout, n, Ln, 0)
-      xs, mean, rstd = saved["norm"]
-      dx = ops.layernorm_bwd(denc, xs, P.f(en + "scale"), mean, rstd, dscale=P.g(en + "scale"),
-                             dbias=P.g(en + "bias"), dx_colsum=last_b)
-    if cut == i_norm:
-      return
-    dx = self.encoder.bwd(P, dx, saved["enc"], n, Ln, None, train_from=train_from)
-    if cut > 0:          # Embed_0 and pos_embedding are frozen
-      return
-    ops.embed_bwd(saved["text"], dx, P.g(p + "Embed_0/embedding"), P.g(p + "pos_embedding").view(Ln, d))
+    if not self.num_classes:       # the tower's output is bf16
+      dout = common.to16(dout)
+    self._stages_bwd(P, dout, saved)
 
   def apply(self, variables, text, *, train=False):
     x, _ = self.fwd(variables["params"], text, frozen=True)     # forward-only, same bits

@@ -199,12 +199,16 @@ def mha_specs(p, d, heads, fuse_qkv=True, stack=0):
   return specs, aliases
 
 
-class EncoderBlock:
+class EncoderBlock(E.Stage):
   """Encoder1DBlock (models/vit.py:81-112): x + MHSA(LN(x)); x + MLP(LN(x)).
   `index` = position in the scan-stacked `encoderblock` sub-tree (None: own `encoderblock_{i}`)."""
 
   def __init__(self, prefix, d, m, heads, index=None):
     self.p, self.d, self.m, self.heads, self.index = prefix, d, m, heads, index
+    self.prefixes = (prefix,)
+    # every parameter from this block on (in spec order) has its final gradient after its backward: a
+    # data-parallel trainer can start reducing them while the earlier blocks are still running
+    self.ready = prefix + "LayerNorm_0/scale" if index is None else None
 
   def specs(self, stack=0):
     att = self.p + "MultiHeadDotProductAttention_0/"
@@ -215,9 +219,10 @@ class EncoderBlock:
   def scope(self, P):
     return Scope(P, self.p, self.index)
 
-  def fwd(self, P, x, n, N, save=True):
+  def fwd(self, P, x, geom, save=True):
     """save=False (forward only): same output bits; every intermediate is released as soon as the
     next op has consumed it and saved is None."""
+    n, N = geom
     d = self.d
     S = self.scope(P)
     A = S.sub("MultiHeadDotProductAttention_0/")
@@ -239,14 +244,15 @@ class EncoderBlock:
     x2, mlp_saved = mlp_fwd(S.sub("MlpBlock_0/"), ln2, x1)
     return x2, (x, ln1, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, mlp_saved)
 
-  def dense1_bias_grad(self, P):
-    """Receives colsum(d block-output): the gradient of this block's MlpBlock Dense_1 bias."""
+  def sink(self, P):
+    """colsum(d block-output) is the gradient of this block's MlpBlock Dense_1 bias."""
     return self.scope(P).g("MlpBlock_0/Dense_1/bias")
 
-  def bwd(self, P, dx2, saved, n, N, dx_colsum_out):
+  def bwd(self, P, dx2, saved, geom, sink, need_dx=True):
     """dx2: bf16 [M,d] grad of block output; colsum(dx2) has ALREADY been accumulated into
     this block's Dense_1 bias grad by whoever produced dx2.  Returns dx (grad of block input);
-    colsum(dx) is accumulated into `dx_colsum_out` (the upstream bias/posemb gradient)."""
+    colsum(dx) is accumulated into `sink` (the bias gradient of the stage below)."""
+    n, N = geom
     d = self.d
     S = self.scope(P)
     A = S.sub("MultiHeadDotProductAttention_0/")
@@ -273,95 +279,110 @@ class EncoderBlock:
     del dqkv
     dx = ops.layernorm_bwd(dln1, x, S.f("LayerNorm_0/scale"), mean1, rstd1, dres=dx1,
                            dscale=S.g("LayerNorm_0/scale"), dbias=S.g("LayerNorm_0/bias"),
-                           dx_colsum=dx_colsum_out)
+                           dx_colsum=sink)
     return dx
 
 
-class Encoder:
-  """vit.Encoder (models/vit.py:115-160): depth blocks + LayerNorm("encoder_norm").
+class ScanEncoder(E.Stage):
+  """The encoder blocks as the reference's nn.scan over ONE `encoderblock` whose parameters carry a
+  leading depth axis, each iteration wrapped in nn.remat with policy `nothing_saveable`
+  (models/vit.py:129-148): only the block INPUT survives the forward and the block is recomputed in
+  the backward, which is what makes L/14@336 at 2048 pairs per GPU fit in HBM.  One backward stage:
+  a single storage holds every block."""
 
-  scan=False: a Python loop over `encoderblock_{i}` (models/vit.py:151-158); everything the backward
-  needs is kept.  scan=True: the reference's nn.scan over ONE `encoderblock` whose parameters carry
-  a leading depth axis, each iteration wrapped in nn.remat with policy `nothing_saveable`
-  (models/vit.py:129-148): only the block INPUT survives the forward and the block is recomputed
-  in the backward, which is what makes L/14@336 at 2048 pairs per GPU fit in HBM."""
-
-  def __init__(self, prefix, depth, d, m, heads, scan=False, remat_policy="nothing_saveable"):
-    self.prefix, self.depth, self.d, self.scan = prefix, depth, d, scan
-    if scan and remat_policy not in ("nothing_saveable", None):
+  def __init__(self, prefix, depth, d, m, heads, remat_policy="nothing_saveable"):
+    if remat_policy not in ("nothing_saveable", None):
       raise NotImplementedError(f"remat_policy={remat_policy!r}: only nothing_saveable (recompute the "
                                 "whole block) is built")
-    if scan:
-      self.blocks = [EncoderBlock(f"{prefix}encoderblock/", d, m, heads, index=i) for i in range(depth)]
-    else:
-      self.blocks = [EncoderBlock(f"{prefix}encoderblock_{i}/", d, m, heads) for i in range(depth)]
+    self.blocks = [EncoderBlock(f"{prefix}encoderblock/", d, m, heads, index=i) for i in range(depth)]
+    self.prefixes = (self.blocks[0].p,)
 
   def specs(self):
-    specs, aliases = [], []
-    if self.scan:
-      specs, aliases = self.blocks[0].specs(stack=self.depth)
-    else:
-      for b in self.blocks:
-        s, a = b.specs()
-        specs += s
-        aliases += a
-    specs = specs + ln_specs(self.prefix + "encoder_norm/", self.d)
-    return specs, aliases
+    return self.blocks[0].specs(stack=len(self.blocks))
 
-  def stages(self):
-    """Storage-name prefixes of the blocks as backward stages, bottom-up: one per block, or ONE for
-    the scan-stacked encoder (a single storage holds every block)."""
-    if self.scan:
-      return [(self.blocks[0].p,)]
-    return [(b.p,) for b in self.blocks]
+  def fwd(self, P, x, geom, save=True):
+    saved = [] if save else None
+    for b in self.blocks:
+      if save:
+        saved.append(x)                           # remat: keep the block input only
+      x, _ = b.fwd(P, x, geom, save)
+    return x, saved
 
-  def fwd(self, P, x, n, N, train_from=0):
-    """Blocks below `train_from` run forward-only: they keep nothing (not even a scan block's
-    input) and each block's intermediates are freed once the next block has consumed them.
-    saved[i] is None for those blocks."""
-    saved = []
-    for i, b in enumerate(self.blocks):
-      if i < train_from:
-        x, _ = b.fwd(P, x, n, N, save=False)
-        saved.append(None)
-        continue
-      x_in = x
-      x, s = b.fwd(P, x, n, N)
-      saved.append(x_in if self.scan else s)      # remat: keep the block input only
-    return x, saved   # pre-encoder_norm activations; the caller applies encoder_norm
+  def sink(self, P):
+    return self.blocks[-1].sink(P)
 
-  def last_bias_grad(self, P):
-    """Gradient buffer that must receive colsum(d x_out): the last block's Dense_1 bias."""
-    return self.blocks[-1].dense1_bias_grad(P)
-
-  def bwd(self, P, dx, saved, n, N, dx_colsum_out, train_from=0):
-    """Runs the blocks from the top down to `train_from` (the lowest with a saved forward); with
-    train_from > 0 the block below is frozen, so nothing is accumulated into its gradient."""
-    for i in reversed(range(train_from, self.depth)):
-      if i > train_from:
-        cs = self.blocks[i - 1].dense1_bias_grad(P)
-      else:
-        cs = dx_colsum_out if i == 0 else None
-      s = saved[i]
-      if self.scan:                               # recompute the block from its input
-        x_out, s = self.blocks[i].fwd(P, s, n, N)
-        del x_out
-      dx = self.blocks[i].bwd(P, dx, s, n, N, cs)
+  def bwd(self, P, dx, saved, geom, sink, need_dx=True):
+    for i in reversed(range(len(self.blocks))):
+      x_out, s = self.blocks[i].fwd(P, saved[i], geom)    # recompute the block from its input
+      del x_out
+      dx = self.blocks[i].bwd(P, dx, s, geom, self.blocks[i - 1].sink(P) if i else sink)
       saved[i] = s = None
-      # every parameter from this block on (in spec order) now has its final gradient: lets a
-      # data-parallel trainer start reducing them while the earlier blocks are still running
-      hook = getattr(P, "on_ready", None)
-      if hook is not None and not self.scan:
-        hook(self.blocks[i].p + "LayerNorm_0/scale")
     return dx
 
 
-class MAPHead:
+def encoder_stages(prefix, depth, d, m, heads, scan=False, remat_policy="nothing_saveable"):
+  """The blocks of vit.Encoder (models/vit.py:115-160) as backward stages: one per `encoderblock_{i}`
+  (models/vit.py:151-158), or one ScanEncoder with scan=True."""
+  if scan:
+    return [ScanEncoder(prefix, depth, d, m, heads, remat_policy)]
+  return [EncoderBlock(f"{prefix}encoderblock_{i}/", d, m, heads) for i in range(depth)]
+
+
+class NormPool(E.Stage):
+  """encoder_norm (models/vit.py:160) and the pooling that follows it.  `pool`: "mean"; "first" or
+  "last" (one token); "max"; None (no pooling: LN only, for the MAP head and pool_type "none").  A
+  pooled output has dtype `out_dtype`; an unpooled one is bf16."""
+
+  def __init__(self, prefix, d, pool, out_dtype):
+    self.p, self.d, self.pool = prefix, d, pool
+    self.out_dtype = out_dtype if pool else torch.bfloat16
+    self.prefixes = (prefix,)
+
+  def specs(self):
+    return ln_specs(self.p, self.d), []
+
+  def _tok(self, N):
+    return 0 if self.pool == "first" else N - 1
+
+  def fwd(self, P, x, geom, save=True):
+    n, N = geom
+    scale, bias = P.f(self.p + "scale"), P.f(self.p + "bias")
+    if self.pool in ("first", "last"):
+      # LayerNorm is per token: LN(x)[:, t] == LN(x[:, t]) -- select first, normalise one row
+      x = ops.pool_fwd(x, n, N, 1, tok=self._tok(N))
+      y, mean, rstd = ops.layernorm_fwd(x, scale, bias, out_dtype=self.out_dtype)
+      return y, ((x, mean, rstd, None) if save else None)
+    encd, mean, rstd = ops.layernorm_fwd(x, scale, bias)
+    saved = (x, mean, rstd, encd if self.pool == "max" else None) if save else None
+    if self.pool == "mean":
+      return ops.pool_fwd(encd, n, N, 0, out_dtype=self.out_dtype), saved
+    if self.pool == "max":
+      return ops.pool_fwd(encd, n, N, 2, out_dtype=self.out_dtype), saved
+    return encd, saved
+
+  def bwd(self, P, dy, saved, geom, sink, need_dx=True):
+    n, N = geom
+    x, mean, rstd, encd = saved
+    if dy.dtype != self.out_dtype:
+      dy = ops.cast(dy, torch.empty_like(dy, dtype=self.out_dtype))
+    grads = dict(dscale=P.g(self.p + "scale"), dbias=P.g(self.p + "bias"), dx_colsum=sink)
+    if self.pool in ("first", "last"):
+      dx = ops.layernorm_bwd(dy, x, P.f(self.p + "scale"), mean, rstd, **grads)
+      return ops.pool_bwd(dx, n, N, 1, tok=self._tok(N)) if need_dx else None
+    if self.pool == "mean":
+      dy = ops.pool_bwd(dy, n, N, 0)
+    elif self.pool == "max":
+      dy = ops.pool_max_bwd(dy, encd, n, N)
+    return ops.layernorm_bwd(dy, x, P.f(self.p + "scale"), mean, rstd, **grads)
+
+
+class MAPHead(E.Stage):
   """Multihead attention pooling (models/vit.py:163-183)."""
 
   def __init__(self, prefix, d, m, heads):
     self.p, self.d, self.m, self.heads = prefix, d, m, heads
     self.att = prefix + "MultiHeadDotProductAttention_0/"
+    self.prefixes = (prefix,)
 
   def specs(self):
     d = self.d
@@ -370,7 +391,8 @@ class MAPHead:
     return ([probe] + s + ln_specs(self.p + "LayerNorm_0/", d)
             + mlp_specs(self.p + "MlpBlock_0/", d, self.m)), a
 
-  def fwd(self, P, enc, n, N, save=True):
+  def fwd(self, P, enc, geom, save=True):
+    n, N = geom
     d = self.d
     q1 = ops.gemm(P.h(self.p + "probe").view(1, d), P.h(self.att + "q/kernel"), b_mn=True,
                   bias=P.f(self.att + "q/bias"))
@@ -387,8 +409,9 @@ class MAPHead:
       return out, None
     return out, (enc, qn, kv, o, lse, a, mean, rstd, mlp_saved)
 
-  def bwd(self, P, dout, saved, n, N):
-    """dout fp32 [n,d] -> d(enc) bf16 [n*N, d]."""
+  def bwd(self, P, dout, saved, geom, sink=None, need_dx=True):
+    """dout fp32 [n,d] -> d(enc) bf16 [n*N, d] (None with need_dx=False)."""
+    n, N = geom
     d = self.d
     enc, qn, kv, o, lse, a, mean, rstd, mlp_saved = saved
     dout16 = ops.cast(dout, torch.empty_like(dout, dtype=torch.bfloat16))
@@ -406,7 +429,7 @@ class MAPHead:
                       self.heads, dq=dq.view(n, 1, d), dk=dkv3[:, :, 0:d], dv=dkv3[:, :, d:])
     ops.colsum(dkv, P.g(self.att + "kv/bias"))
     ops.gemm(enc, dkv, a_mn=True, b_mn=True, out=P.g(self.att + "kv/kernel"), reduce_out=True)
-    denc = ops.gemm(dkv, P.h(self.att + "kv/kernel"))
+    denc = ops.gemm(dkv, P.h(self.att + "kv/kernel")) if need_dx else None
     # the single probe query is shared by the batch: its gradient is the batch sum of dq
     dq1 = torch.zeros(d, dtype=torch.float32, device=dq.device)
     ops.colsum(dq, dq1)
@@ -418,11 +441,96 @@ class MAPHead:
     return denc
 
 
+class PatchEmbedding(E.Stage):
+  """The patch embedding (models/vit.py:212-225): a Dense over flattened patches with the position
+  embedding added in its epilogue, then [cls] prepended when `cls`."""
+
+  def __init__(self, prefix, patch_size, d, posemb, cls):
+    self.p, self.patch_size, self.d, self.posemb, self.cls = prefix, patch_size, d, posemb, cls
+    self.prefixes = (prefix + "embedding/", prefix + "pos_embedding", prefix + "cls")
+    self._sincos = None
+
+  def _posemb16(self, P, image):
+    if self.posemb == "learn":
+      return P.h(self.p + "pos_embedding").view(-1, self.d)
+    if self._sincos is None or self._sincos.device != P.device:
+      (ph, pw), (H, W) = self.patch_size, image.shape[1:3]
+      self._sincos = torch.from_numpy(posemb_sincos_2d(H // ph, W // pw, self.d)).to(P.device).bfloat16()
+    return self._sincos
+
+  def fwd(self, P, image, geom, save=True):
+    n, N = geom
+    N0, p = N - self.cls, self.p
+    patches = ops.patchify(image, self.patch_size[0])
+    x = ops.gemm(patches, P.h(p + "embedding/kernel_flat"), b_mn=True, bias=P.f(p + "embedding/bias"),
+                 aux=self._posemb16(P, image), aux_row_mod=N0, epilogue=L.EPI_BIAS_RESID)
+    saved = patches if save else None
+    del patches
+    if self.cls:
+      # cls token is prepended AFTER the position embedding was added (models/vit.py:223-225)
+      x = ops.concat_cls(x, P.f(p + "cls").view(self.d), n, N0)
+    return x, saved
+
+  def sink(self, P):
+    # the column sum of the gradient reaching the embedding output is the patch-embed bias gradient
+    # (models/vit.py:212-214); with [cls] it is summed over the patch tokens only (bwd)
+    return None if self.cls else P.g(self.p + "embedding/bias")
+
+  def bwd(self, P, dx, patches, geom, sink=None, need_dx=False):
+    n, N = geom
+    d, p = self.d, self.p
+    if self.cls:
+      # batch-sum of the gradient at every token position: row 0 is d cls, the rest d pos_embedding;
+      # the patch-embed bias gradient is the sum of the latter over positions
+      N0 = N - 1
+      tmp = torch.zeros(N * d, dtype=torch.float32, device=dx.device)
+      ops.colsum(dx.view(n, N * d), tmp)
+      gcls = P.g(p + "cls").view(d)
+      ops.axpby(gcls, tmp[:d], 1.0, 1.0, out=gcls)
+      if self.posemb == "learn":
+        gpos = P.g(p + "pos_embedding").view(N0 * d)
+        ops.axpby(gpos, tmp[d:], 1.0, 1.0, out=gpos)
+      ops.colsum(tmp[d:].view(N0, d), P.g(p + "embedding/bias"))
+      dx = ops.drop_cls(dx, n, N0)
+    elif self.posemb == "learn":
+      ops.colsum(dx.view(n, N * d), P.g(p + "pos_embedding").view(N * d))
+    ops.gemm(patches, dx, a_mn=True, b_mn=True, out=P.g(p + "embedding/kernel_flat"), reduce_out=True)
+
+
+class PreLogits(E.Stage):
+  """pre_logits: tanh(Dense(x)) (models/vit.py:258-265), fp32 output."""
+
+  def __init__(self, prefix, d, rep):
+    self.p, self.d, self.rep = prefix + "pre_logits/", d, rep
+    self.prefixes = (self.p,)
+
+  def specs(self):
+    return [E.ParamSpec(self.p + "kernel", (self.d, self.rep), E.lecun_normal(self.d)),
+            E.ParamSpec(self.p + "bias", (self.rep,), E.zeros)], []
+
+  def fwd(self, P, x, geom, save=True):
+    pre = ops.gemm(common.to16(x), P.h(self.p + "kernel"), b_mn=True, bias=P.f(self.p + "bias"),
+                   out_dtype=torch.float32)
+    y = ops.tanh_fwd(pre)
+    return y, ((x, y) if save else None)
+
+  def bwd(self, P, dy, saved, geom, sink=None, need_dx=True):
+    x, y = saved
+    dpre = ops.tanh_bwd(dy, y)
+    d16 = common.to16(dpre)
+    ops.colsum(dpre, P.g(self.p + "bias"))
+    ops.gemm(common.to16(x), d16, a_mn=True, b_mn=True, out=P.g(self.p + "kernel"), reduce_out=True)
+    return ops.gemm(d16, P.h(self.p + "kernel"), out_dtype=torch.float32) if need_dx else None
+
+
 # ------------------------------------------------------------------------------------------
 # the model
 # ------------------------------------------------------------------------------------------
+_POOLS = {"gap": "mean", "0": "first", "tok": "first", "map": None, "none": None}   # -> NormPool's pool
+
+
 @dataclass
-class _Model:
+class _Model(E.Staged):
   """ViT model; fields as in models/vit.py:186-204."""
   num_classes: Optional[int] = None
   patch_size: Sequence[int] = (16, 16)
@@ -443,18 +551,26 @@ class _Model:
   def __post_init__(self):
     if self.dropout:
       raise NotImplementedError("dropout > 0 is not on the benchmarked path (reference configs use 0)")
+    if self.pool_type not in _POOLS:
+      raise ValueError(f"Unknown pool type: '{self.pool_type}'")
     check_head_dim(self.width, self.num_heads)
     self.mlp = self.mlp_dim or 4 * self.width
-    self.prefix = (self.name + "/") if self.name else ""
-    self.encoder = Encoder(self.prefix + "Transformer/", self.depth, self.width, self.mlp, self.num_heads,
-                           scan=self.scan, remat_policy=self.remat_policy)
-    self.map_head = (MAPHead(self.prefix + "MAPHead_0/", self.width, self.mlp, self.num_heads)
-                     if self.pool_type == "map" else None)
+    self.prefix = p = (self.name + "/") if self.name else ""
+    d, enc = self.width, p + "Transformer/"
+    rep = (d if self.rep_size is True else self.rep_size) if self.rep_size else d
     self.head = None
     if self.num_classes:
-      rep = (self.width if self.rep_size is True else self.rep_size) if self.rep_size else self.width
-      self.head = common.ClassifierHead(self.prefix, rep, self.num_classes,
-                                        E.zeros if self.head_zeroinit else E.lecun_normal(rep))
+      self.head = common.ClassifierHead(p, rep, self.num_classes, E.zeros if self.head_zeroinit else E.lecun_normal(rep))
+    # the backward stages, bottom-up (engine.Staged); parameterless pools belong to no stage of their own
+    self._stages = ([PatchEmbedding(p, self.patch_size, d, self.posemb, self.pool_type == "tok")]
+                    + encoder_stages(enc, self.depth, d, self.mlp, self.num_heads, self.scan, self.remat_policy)
+                    + [NormPool(enc + "encoder_norm/", d, _POOLS[self.pool_type], torch.float32)])
+    if self.pool_type == "map":
+      self._stages.append(MAPHead(p + "MAPHead_0/", d, self.mlp, self.num_heads))
+    if self.rep_size:
+      self._stages.append(PreLogits(p, d, rep))
+    if self.head is not None:
+      self._stages.append(self.head)
     self._geom = None
 
   # ---- parameters ------------------------------------------------------------------------
@@ -484,19 +600,8 @@ class _Model:
       specs.append(E.ParamSpec(p + "pos_embedding", (1, gh * gw, d), E.normal(1 / math.sqrt(d))))
     if self.pool_type == "tok":
       specs.append(E.ParamSpec(p + "cls", (1, 1, d), E.zeros))
-    s, a = self.encoder.specs()
-    specs += s
-    aliases += a
-    if self.map_head is not None:
-      s, a = self.map_head.specs()
-      specs += s
-      aliases += a
-    if self.rep_size:
-      rep = d if self.rep_size is True else self.rep_size
-      specs += [E.ParamSpec(p + "pre_logits/kernel", (d, rep), E.lecun_normal(d)),
-                E.ParamSpec(p + "pre_logits/bias", (rep,), E.zeros)]
-    if self.head is not None:
-      s, a = self.head.specs()
+    for stage in self._stages[1:]:
+      s, a = stage.specs()
       specs += s
       aliases += a
     self._in_ch, self._K, self._Kp = in_ch, K, Kp
@@ -508,46 +613,6 @@ class _Model:
     return E.FlatParams(specs, aliases, device).init(seed)
 
   # ---- forward / backward ----------------------------------------------------------------
-  def _posemb16(self, P):
-    if self.posemb == "learn":
-      return P.h(self.prefix + "pos_embedding").view(-1, self.width)
-    if getattr(self, "_sincos", None) is None or self._sincos.device != P.device:
-      gh, gw = self._geom
-      self._sincos = torch.from_numpy(posemb_sincos_2d(gh, gw, self.width)).to(P.device).bfloat16()
-    return self._sincos
-
-  def stages(self):
-    """The model as backward stages, bottom-up, each a tuple of storage-name prefixes: embedding
-    (patch kernel, posemb, cls), every encoder block (the scan-stacked encoder is one), encoder_norm,
-    the MAP head, pre_logits, head.  Parameterless pools belong to no stage."""
-    p = self.prefix
-    out = [(p + "embedding/", p + "pos_embedding", p + "cls")] + self.encoder.stages()
-    out.append((p + "Transformer/encoder_norm/",))
-    if self.map_head is not None:
-      out.append((self.map_head.p,))
-    if self.rep_size:
-      out.append((p + "pre_logits/",))
-    if self.head is not None:
-      out.append((self.head.p,))
-    return out
-
-  def _stage_indices(self):
-    """Indices into stages() of encoder_norm, the MAP head, pre_logits and head (an absent one shares
-    the index of the next)."""
-    i_norm = 1 + (1 if self.scan else self.depth)
-    i_map = i_norm + 1
-    i_pre = i_map + (self.map_head is not None)
-    return i_norm, i_map, i_pre, i_pre + bool(self.rep_size)
-
-  def cut(self, P, frozen):
-    """Index into stages() of the lowest stage with a trained parameter (engine.stage_cut): the
-    backward stops there and everything below runs forward-only.  len(stages()) = wholly frozen."""
-    cache = self.__dict__.setdefault("_cuts", {})
-    key = frozen if frozen is True or frozen is None else frozenset(frozen)
-    if key not in cache:
-      cache[key] = E.stage_cut(P.offsets, self.stages(), frozen)
-    return cache[key]
-
   def fwd(self, P, image, frozen=None):
     """image [n,H,W,C] fp32 in [-1,1] -> (x fp32 [n, out], saved).  With a class head whose storage is
     padded (common.ClassifierHead) x is the [n, num_classes] view of the padded logits.
@@ -559,132 +624,22 @@ class _Model:
       self.setup(image.shape[1:3])
     n = image.shape[0]
     gh, gw = self._geom
-    N0, d, p = gh * gw, self.width, self.prefix
-    cut = self.cut(P, frozen)
-    i_norm, i_map, i_pre, i_head = self._stage_indices()
-    patches = ops.patchify(image, self.patch_size[0])
-    x = ops.gemm(patches, P.h(p + "embedding/kernel_flat"), b_mn=True, bias=P.f(p + "embedding/bias"),
-                 aux=self._posemb16(P), aux_row_mod=N0, epilogue=L.EPI_BIAS_RESID)
-    if cut > 0:
-      del patches
-      patches = None
-    N = N0
-    if self.pool_type == "tok":
-      # cls token is prepended AFTER the position embedding was added (models/vit.py:223-225)
-      x = ops.concat_cls(x, P.f(p + "cls").view(d), n, N0)
-      N = N0 + 1
-    train_from = 0 if cut <= 1 else (self.depth if self.scan else min(cut - 1, self.depth))
-    x, enc_saved = self.encoder.fwd(P, x, n, N, train_from=train_from)
-    en = self.prefix + "Transformer/encoder_norm/"
-    saved = {"patches": patches, "enc": enc_saved, "n": n, "N": N, "cut": cut, "train_from": train_from}
-    keep_norm = cut <= i_norm
-    if self.pool_type == "map":
-      encd, mean, rstd = ops.layernorm_fwd(x, P.f(en + "scale"), P.f(en + "bias"))
-      saved["norm"] = (x, mean, rstd) if keep_norm else None
-      del x
-      out, saved["map"] = self.map_head.fwd(P, encd, n, N, save=cut <= i_map)
-    elif self.pool_type == "gap":
-      encd, mean, rstd = ops.layernorm_fwd(x, P.f(en + "scale"), P.f(en + "bias"))
-      saved["norm"] = (x, mean, rstd) if keep_norm else None
-      out = ops.pool_fwd(encd, n, N, 0, out_dtype=torch.float32)
-    elif self.pool_type in ("0", "tok"):
-      # LayerNorm is per token, so LN(x)[:, 0] == LN(x[:, 0]): select first, normalise one row
-      x0 = ops.pool_fwd(x, n, N, 1, tok=0)
-      out, mean, rstd = ops.layernorm_fwd(x0, P.f(en + "scale"), P.f(en + "bias"), out_dtype=torch.float32)
-      saved["norm"] = (x0, mean, rstd) if keep_norm else None
-    elif self.pool_type == "none":
-      # no pooling (models/vit.py:252-253): pre_logits / head run on every token, out is [n, N, .]
-      out, mean, rstd = ops.layernorm_fwd(x, P.f(en + "scale"), P.f(en + "bias"))
-      saved["norm"] = (x, mean, rstd) if keep_norm else None
-    else:
-      raise ValueError(f"Unknown pool type: '{self.pool_type}'")
-    if self.rep_size:
-      pre = ops.gemm(self._to16(out), P.h(p + "pre_logits/kernel"), b_mn=True,
-                     bias=P.f(p + "pre_logits/bias"), out_dtype=torch.float32)
-      keep = cut <= i_pre
-      saved["rep_in"] = out if keep else None
-      out = ops.tanh_fwd(pre)
-      saved["rep_out"] = out if keep else None
-    if self.head is not None:
-      saved["head_in"] = out if cut <= i_head else None
-      out = self.head.fwd(P, out)
+    N = gh * gw + (self.pool_type == "tok")
+    out, saved = self._stages_fwd(P, image, (n, N), frozen)
     if self.pool_type == "none":
+      # no pooling (models/vit.py:252-253): pre_logits / head run on every token, out is [n, N, .]
       if out.dtype != torch.float32:
         out = ops.cast(out, torch.empty_like(out, dtype=torch.float32))
       out = out.view(n, N, -1)
     return out, saved
 
-  _to16 = staticmethod(common.to16)
-
   def bwd(self, P, dout, saved):
     """dout: fp32 [n, out] ([n, N, out] without pooling).  Accumulates parameter gradients into P.grad.
     With a padded class head, out is the padded class count (ClassifierHead.bwd)."""
-    p, d = self.prefix, self.width
-    n, N = saved["n"], saved["N"]
-    cut, train_from = saved["cut"], saved["train_from"]
-    if cut == len(self.stages()):        # wholly frozen: nothing to do
-      return
-    i_norm, i_map, i_pre, i_head = self._stage_indices()
-    en = self.prefix + "Transformer/encoder_norm/"
     if self.pool_type == "none":
+      n, N = saved["geom"]
       dout = dout.reshape(n * N, -1)
-    if self.head is not None:
-      dout = self.head.bwd(P, dout, saved["head_in"])
-      if cut == i_head:
-        return
-    if self.rep_size:
-      dpre = ops.tanh_bwd(dout, saved["rep_out"])
-      d16 = self._to16(dpre)
-      ops.colsum(dpre, P.g(p + "pre_logits/bias"))
-      ops.gemm(self._to16(saved["rep_in"]), d16, a_mn=True, b_mn=True, out=P.g(p + "pre_logits/kernel"), reduce_out=True)
-      if cut == i_pre:
-        return
-      dout = ops.gemm(d16, P.h(p + "pre_logits/kernel"), out_dtype=torch.float32)
-    # below the cut the last block is frozen: its Dense_1 bias gradient stays zero
-    last_b = self.encoder.last_bias_grad(P) if cut < i_norm else None
-    if self.pool_type == "map":
-      denc = self.map_head.bwd(P, dout, saved["map"], n, N)
-      if cut == i_map:
-        return
-      x, mean, rstd = saved["norm"]
-      dx = ops.layernorm_bwd(denc, x, P.f(en + "scale"), mean, rstd, dscale=P.g(en + "scale"),
-                             dbias=P.g(en + "bias"), dx_colsum=last_b)
-    elif self.pool_type in ("gap", "none"):
-      denc = ops.pool_bwd(dout, n, N, 0) if self.pool_type == "gap" else self._to16(dout)
-      x, mean, rstd = saved["norm"]
-      dx = ops.layernorm_bwd(denc, x, P.f(en + "scale"), mean, rstd, dscale=P.g(en + "scale"),
-                             dbias=P.g(en + "bias"), dx_colsum=last_b)
-    else:
-      x0, mean, rstd = saved["norm"]
-      dx0 = ops.layernorm_bwd(dout, x0, P.f(en + "scale"), mean, rstd, dscale=P.g(en + "scale"),
-                              dbias=P.g(en + "bias"), dx_colsum=last_b)
-      dx = ops.pool_bwd(dx0, n, N, 1, tok=0)
-    if cut == i_norm:
-      return
-    if cut > 0:          # the embedding is frozen: the encoder's backward is the last one
-      self.encoder.bwd(P, dx, saved["enc"], n, N, None, train_from=train_from)
-      return
-    # encoder: the column sum of the gradient reaching the embedding output is the patch-embed
-    # bias gradient (models/vit.py:212-214)
-    if self.pool_type == "tok":
-      dx = self.encoder.bwd(P, dx, saved["enc"], n, N, None)
-      # batch-sum of the gradient at every token position: row 0 is d cls, the rest d pos_embedding;
-      # the patch-embed bias gradient is the sum of the latter over positions
-      N0 = N - 1
-      tmp = torch.zeros(N * d, dtype=torch.float32, device=dx.device)
-      ops.colsum(dx.view(n, N * d), tmp)
-      gcls = P.g(p + "cls").view(d)
-      ops.axpby(gcls, tmp[:d], 1.0, 1.0, out=gcls)
-      if self.posemb == "learn":
-        gpos = P.g(p + "pos_embedding").view(N0 * d)
-        ops.axpby(gpos, tmp[d:], 1.0, 1.0, out=gpos)
-      ops.colsum(tmp[d:].view(N0, d), P.g(p + "embedding/bias"))
-      dx = ops.drop_cls(dx, n, N0)
-    else:
-      dx = self.encoder.bwd(P, dx, saved["enc"], n, N, P.g(p + "embedding/bias"))
-      if self.posemb == "learn":
-        ops.colsum(dx.view(n, N * d), P.g(p + "pos_embedding").view(N * d))
-    ops.gemm(saved["patches"], dx, a_mn=True, b_mn=True, out=P.g(p + "embedding/kernel_flat"), reduce_out=True)
+    self._stages_bwd(P, dout, saved)
 
   # ---- reference-style entry points --------------------------------------------------------
   def apply(self, variables, image, *, train=False):

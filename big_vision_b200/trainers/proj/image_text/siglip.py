@@ -88,8 +88,8 @@ class BucketedGradAllReduce:
   text tower from its head down to its embedding, then the image tower likewise), and the flat
   gradient buffer is laid out in spec order inside each of its two groups (decayed kernels | the
   rest).  So the finished part of each group grows from the group's end towards its start: whenever
-  the backward reports "everything from spec `name` on is done" (`P.on_ready`, called by
-  vit.Encoder.bwd after every block) and at least `bucket_elems` new elements are final, that slice
+  the backward reports "everything from spec `name` on is done" (`P.on_ready`, called by the stage
+  runner engine.Staged after every unstacked encoder block) and at least `bucket_elems` new elements are final, that slice
   is all-reduced asynchronously -- NCCL's stream waits for the kernels enqueued so far, the main
   stream carries on with the next block -- and `finish()` reduces what is left and joins.
   Elementwise SUM over the same values as one big all-reduce: results are identical."""
