@@ -10,7 +10,7 @@ reference names and shapes still resolve.
 """
 import re
 from dataclasses import dataclass
-from typing import Callable, Dict, List, Optional, Tuple
+from typing import Callable, Dict, List, NamedTuple, Optional, Tuple
 
 import numpy as np
 import torch
@@ -176,22 +176,31 @@ def stage_cut(storages, stages, frozen):
   return len(stages)
 
 
+class Geom(NamedTuple):
+  """What every stage of one forward sees besides its input: n samples of N tokens each, and the
+  MLP-Mixer's stochastic-depth masks of that forward (None: no residual branch is dropped)."""
+  n: int
+  N: int
+  masks: Optional[torch.Tensor] = None
+
+
 class Stage:
   """Defaults of a backward stage (see Staged)."""
   ready = None
 
-  def sink(self, P):
+  def sink(self, P, geom):
     return None
 
 
 class Staged:
   """A model built as `self._stages`, a bottom-up list of backward stages (Stage).  Each stage has
     `prefixes`: the storage-name prefixes of its parameters;
-    `fwd(P, x, geom, save) -> (y, saved)`: with save=False it keeps nothing (saved is None) and frees
-        each intermediate once it has been consumed;
+    `fwd(P, x, geom, save) -> (y, saved)`: `geom` is the forward's Geom; with save=False it keeps
+        nothing (saved is None) and frees each intermediate once it has been consumed;
     `bwd(P, dy, saved, geom, sink, need_dx) -> dx`: accumulates its parameter gradients; `sink` (or
         None) receives colsum(dx), and with need_dx=False dx is not computed and None is returned;
-    `sink(P)`: the gradient buffer that equals the column sum of the stage's output gradient, or None;
+    `sink(P, geom)`: the gradient buffer that equals the column sum of the stage's output gradient, or
+        None;
     `ready`: None, or the storage name from which on (in spec order) every gradient is final once the
         stage's backward has run (P.on_ready, the bucketed gradient all-reduce)."""
 
@@ -223,7 +232,7 @@ class Staged:
     stages, kept, geom, cut = self._stages, saved["stages"], saved["geom"], saved["cut"]
     on_ready = getattr(P, "on_ready", None)
     for i in reversed(range(cut, len(stages))):
-      sink = stages[i - 1].sink(P) if i - 1 >= cut else None
+      sink = stages[i - 1].sink(P, geom) if i - 1 >= cut else None
       dy = stages[i].bwd(P, dy, kept[i], geom, sink, i > cut)
       kept[i] = None
       if on_ready is not None and stages[i].ready is not None:

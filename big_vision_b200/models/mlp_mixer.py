@@ -11,6 +11,8 @@ probability i/(L-1)*stoch_depth, no 1/(1-p) rescale.  The 0/1 masks are an INPUT
 (`masks` fp32 [num_blocks, 2, n]; parity tests feed the same masks to the oracle) or, with train=True,
 are drawn from the numpy Generator passed as `rng` (the reference draws them from JAX's threefry
 stream, which cannot be reproduced without JAX).
+The model is a list of backward stages (engine.Staged): the stem (vit.PatchEmbedding without a position
+embedding), one MixerBlock per block, pre_head_layer_norm with the mean pool (vit.NormPool) and the head.
 """
 from dataclasses import dataclass
 from typing import Optional, Tuple
@@ -43,8 +45,104 @@ def _dense_specs(p, fan_in, fan_out, store_cols=None):
   return specs, aliases
 
 
+class MixerBlock(E.Stage):
+  """MixerBlock_{i} (mlp_mixer.py:40-55): x + token-mixing MLP over the tokens of LayerNorm_0(x), then
+  x + channel-mixing MLP over LayerNorm_1(x).  With the forward's stochastic-depth masks (geom.masks)
+  each residual branch is dropped per sample."""
+
+  def __init__(self, i, N, d, tokens_mlp_dim, channels_mlp_dim):
+    self.i, self.N, self.Np = i, N, (N + 7) // 8 * 8
+    self.d, self.T, self.C = d, tokens_mlp_dim, channels_mlp_dim
+    self.p = p = f"MixerBlock_{i}/"
+    self.tm, self.cm = p + "token_mixing/", p + "channel_mixing/"
+    self.prefixes = (p,)
+    self.ready = p + "LayerNorm_0/scale"
+    # token-mixing Dense_1 writes [n*d, N] in rows of Np elements: its storage is padded (specs)
+    pad = "_pad" if self.Np != N else ""
+    self.k1, self.b1 = self.tm + "Dense_1/kernel" + pad, self.tm + "Dense_1/bias" + pad
+
+  def specs(self):
+    p, tm, cm, N, d = self.p, self.tm, self.cm, self.N, self.d
+    specs, aliases = vit.ln_specs(p + "LayerNorm_0/", d) + vit.ln_specs(p + "LayerNorm_1/", d), []
+    for nm, fi, fo, sc in ((tm + "Dense_0/", N, self.T, None),
+                           (tm + "Dense_1/", self.T, N, self.Np),
+                           (cm + "Dense_0/", d, self.C, None),
+                           (cm + "Dense_1/", self.C, d, None)):
+      s, a = _dense_specs(nm, fi, fo, sc)
+      specs += s
+      aliases += a
+    return specs, aliases
+
+  def fwd(self, P, x, geom, save=True):
+    """save=False (forward only): same output bits; every intermediate is released as soon as the
+    next op has consumed it, GELU's pre-activations are not written and saved is None."""
+    n, N, masks = geom
+    d, p, tm = self.d, self.p, self.tm
+    y, mean1, rstd1 = ops.layernorm_fwd(x, P.f(p + "LayerNorm_0/scale"), P.f(p + "LayerNorm_0/bias"))
+    yt = ops.transpose_tokens(y, n, N, d)                                   # [n*d, Np]
+    del y
+    if save:
+      hact, hpre = ops.gemm(yt, P.h(tm + "Dense_0/kernel"), b_mn=True, bias=P.f(tm + "Dense_0/bias"),
+                            epilogue=L.EPI_BIAS_GELU, K=N)
+    else:
+      del mean1, rstd1
+      hact = ops.gemm(yt, P.h(tm + "Dense_0/kernel"), b_mn=True, bias=P.f(tm + "Dense_0/bias"),
+                      epilogue=L.EPI_BIAS_GELU_ACT, K=N)
+      del yt
+    ot = torch.empty((n * d, self.Np), dtype=torch.bfloat16, device=x.device)
+    ops.gemm(hact, P.h(self.k1), b_mn=True, bias=P.f(self.b1), out=ot, N=N)
+    if not save:
+      del hact
+    x1 = ops.untranspose_add(ot, x, n, N, d)
+    del ot
+    if masks is not None:
+      x1 = ops.row_select(x1, x, masks[self.i, 0], n, N)                    # x + mask * branch
+    y2, mean2, rstd2 = ops.layernorm_fwd(x1, P.f(p + "LayerNorm_1/scale"), P.f(p + "LayerNorm_1/bias"))
+    if not save:
+      del mean2, rstd2
+    x2, mlp_saved = vit.mlp_fwd(vit.Scope(P, self.cm), y2, x1, save=save)
+    if masks is not None:
+      x2 = ops.row_select(x2, x1, masks[self.i, 1], n, N)
+    if not save:
+      return x2, None
+    return x2, (x, mean1, rstd1, yt, hact, hpre, x1, mean2, rstd2, mlp_saved)
+
+  def sink(self, P, geom):
+    """colsum(d block-output) is the gradient of channel_mixing/Dense_1/bias -- but not with stochastic
+    depth: the gradient entering the branch is then mask * d block-output, and bwd sums it itself."""
+    return P.g(self.cm + "Dense_1/bias") if geom.masks is None else None
+
+  def bwd(self, P, dx, saved, geom, sink, need_dx=True):
+    """dx: bf16 [n*N, d] grad of the block output.  Returns the grad of the block input; colsum of it is
+    accumulated into `sink`.  need_dx changes nothing: LayerNorm_0's gradients need the full chain."""
+    n, N, masks = geom
+    d, p, tm = self.d, self.p, self.tm
+    x, mean1, rstd1, yt, hact, hpre, x1, mean2, rstd2, mlp_saved = saved
+    # channel mixing
+    dbr = dx if masks is None else ops.row_select(dx, None, masks[self.i, 1], n, N)
+    dy2 = vit.mlp_bwd(vit.Scope(P, self.cm), dbr, mlp_saved, want_bias2_grad=self.sink(P, geom) is None)
+    dx1 = ops.layernorm_bwd(dy2, x1, P.f(p + "LayerNorm_1/scale"), mean2, rstd2, dres=dx,
+                            dscale=P.g(p + "LayerNorm_1/scale"), dbias=P.g(p + "LayerNorm_1/bias"))
+    # token mixing
+    dbr = dx1 if masks is None else ops.row_select(dx1, None, masks[self.i, 0], n, N)
+    dot = ops.transpose_tokens(dbr, n, N, d)                                # [n*d, Np], pad = 0
+    ops.colsum(dot, P.g(self.b1))
+    ops.gemm(hact, dot, a_mn=True, b_mn=True, out=P.g(self.k1), reduce_out=True, N=N)
+    dhpre = ops.gemm(dot, P.h(self.k1), aux=hpre, epilogue=L.EPI_DGELU, K=N)    # [n*d, T]
+    # separate column-sum pass: with n*d rows over only T columns the GEMM epilogue's fused bias
+    # gradient is all atomic contention (measured 2.62 vs 1.26 + 0.07 ms per call)
+    ops.colsum(dhpre, P.g(tm + "Dense_0/bias"))
+    ops.gemm(yt, dhpre, a_mn=True, b_mn=True, out=P.g(tm + "Dense_0/kernel"), reduce_out=True, M=N)
+    dyt = torch.empty((n * d, self.Np), dtype=torch.bfloat16, device=dx.device)
+    ops.gemm(dhpre, P.h(tm + "Dense_0/kernel"), out=dyt, N=N)
+    dyl = ops.untranspose_add(dyt, None, n, N, d)
+    return ops.layernorm_bwd(dyl, x, P.f(p + "LayerNorm_0/scale"), mean1, rstd1, dres=dx1,
+                             dscale=P.g(p + "LayerNorm_0/scale"), dbias=P.g(p + "LayerNorm_0/bias"),
+                             dx_colsum=sink)
+
+
 @dataclass
-class MlpMixer:
+class MlpMixer(E.Staged):
   """Fields as mlp_mixer.MlpMixer (mlp_mixer.py:58-68)."""
   patch_size: Tuple[int, int] = (16, 16)
   num_classes: Optional[int] = None
@@ -56,8 +154,8 @@ class MlpMixer:
   stoch_depth: float = 0.0
 
   def __post_init__(self):
-    self._geom = None
     self.head = common.ClassifierHead("", self.hidden_dim, self.num_classes, E.zeros) if self.num_classes else None
+    self._stages = self._N = None
 
   def drop_p(self, i):
     """mlp_mixer.py:76"""
@@ -72,128 +170,42 @@ class MlpMixer:
 
   def specs(self, image_hw, in_ch=3):
     ph, pw = self.patch_size
-    self._geom = (image_hw[0] // ph, image_hw[1] // pw)
-    N = self._geom[0] * self._geom[1]
-    Np = (N + 7) // 8 * 8
+    N = (image_hw[0] // ph) * (image_hw[1] // pw)
     d = self.hidden_dim
-    K = ph * pw * in_ch
-    Kp = (K + 7) // 8 * 8
-    lec = E.lecun_normal(K)
-    specs = [E.ParamSpec("stem/kernel_flat", (Kp, d),
-                         lambda rng, shape: np.concatenate([lec(rng, (K, d)), np.zeros((Kp - K, d))], 0)),
-             E.ParamSpec("stem/bias", (d,), E.zeros)]
-    aliases = [E.Alias("stem/kernel", "stem/kernel_flat", lambda t: t[:K].unflatten(0, (ph, pw, in_ch)))]
-    for i in range(self.num_blocks):
-      p = f"MixerBlock_{i}/"
-      specs += vit.ln_specs(p + "LayerNorm_0/", d) + vit.ln_specs(p + "LayerNorm_1/", d)
-      for nm, fi, fo, sc in ((p + "token_mixing/Dense_0/", N, self.tokens_mlp_dim, None),
-                             (p + "token_mixing/Dense_1/", self.tokens_mlp_dim, N, Np),
-                             (p + "channel_mixing/Dense_0/", d, self.channels_mlp_dim, None),
-                             (p + "channel_mixing/Dense_1/", self.channels_mlp_dim, d, None)):
-        s, a = _dense_specs(nm, fi, fo, sc)
-        specs += s
-        aliases += a
-    specs += vit.ln_specs("pre_head_layer_norm/", d)
+    # the backward stages, bottom-up (engine.Staged); the blocks' token-mixing MLPs are as wide as N
+    self._stages = ([vit.PatchEmbedding("", "stem", self.patch_size, d, None, False)]
+                    + [MixerBlock(i, N, d, self.tokens_mlp_dim, self.channels_mlp_dim) for i in range(self.num_blocks)]
+                    + [vit.NormPool("pre_head_layer_norm/", d, "mean", torch.float32)])
     if self.head is not None:
-      s, a = self.head.specs()
+      self._stages.append(self.head)
+    specs, aliases = self._stages[0].specs(N, in_ch)
+    for stage in self._stages[1:]:
+      s, a = stage.specs()
       specs += s
       aliases += a
-    self._N, self._Np = N, Np
+    self._N = N
     return specs, aliases
 
   def init(self, seed, image_shape, device="cuda"):
     specs, aliases = self.specs(image_shape[1:3], image_shape[3])
     return E.FlatParams(specs, aliases, device).init(seed)
 
-  @staticmethod
-  def _store(P, p, what):
-    """Name of the stored kernel/bias (padded storage if it exists)."""
-    return p + what + ("_pad" if (p + what + "_pad") in P.offsets else "")
-
-  def fwd(self, P, image, *, train=False, rng=None, masks=None):
+  def fwd(self, P, image, *, train=False, rng=None, masks=None, frozen=None):
+    """image [n,H,W,C] fp32 -> (x fp32 [n, out], saved).  `masks` fp32 [num_blocks, 2, n], or drawn from
+    `rng` with train=True.  `frozen` as in vit._Model.fwd: the stages below the cut run forward-only and
+    save nothing."""
     n = image.shape[0]
-    d, N, Np, T = self.hidden_dim, self._N, self._Np, self.tokens_mlp_dim
     if masks is None and train and self.stoch_depth:
       if rng is None:
         raise ValueError("stoch_depth > 0 in training needs an rng (numpy Generator) or explicit masks")
       masks = self.draw_masks(rng, n, image.device)
-    patches = ops.patchify(image, self.patch_size[0])
-    x = ops.gemm(patches, P.h("stem/kernel_flat"), b_mn=True, bias=P.f("stem/bias"))
-    saved = {"patches": patches, "n": n, "blocks": [], "masks": masks}
-    for i in range(self.num_blocks):
-      p = f"MixerBlock_{i}/"
-      tm, cm = p + "token_mixing/", p + "channel_mixing/"
-      y, mean1, rstd1 = ops.layernorm_fwd(x, P.f(p + "LayerNorm_0/scale"), P.f(p + "LayerNorm_0/bias"))
-      yt = ops.transpose_tokens(y, n, N, d)                                   # [n*d, Np]
-      hact, hpre = ops.gemm(yt, P.h(tm + "Dense_0/kernel"), b_mn=True, bias=P.f(tm + "Dense_0/bias"),
-                            epilogue=L.EPI_BIAS_GELU, K=N)
-      ot = torch.empty((n * d, Np), dtype=torch.bfloat16, device=x.device)
-      ops.gemm(hact, P.h(self._store(P, tm + "Dense_1/", "kernel")), b_mn=True,
-               bias=P.f(self._store(P, tm + "Dense_1/", "bias")), out=ot, N=N)
-      x1 = ops.untranspose_add(ot, x, n, N, d)
-      if masks is not None:
-        x1 = ops.row_select(x1, x, masks[i, 0], n, N)                         # x + mask * branch
-      y2, mean2, rstd2 = ops.layernorm_fwd(x1, P.f(p + "LayerNorm_1/scale"), P.f(p + "LayerNorm_1/bias"))
-      x2, mlp_saved = vit.mlp_fwd(vit.Scope(P, cm), y2, x1)
-      if masks is not None:
-        x2 = ops.row_select(x2, x1, masks[i, 1], n, N)
-      saved["blocks"].append((x, mean1, rstd1, yt, hact, hpre, x1, mean2, rstd2, mlp_saved))
-      x = x2
-    y, mean, rstd = ops.layernorm_fwd(x, P.f("pre_head_layer_norm/scale"), P.f("pre_head_layer_norm/bias"))
-    saved["norm"] = (x, mean, rstd)
-    out = ops.pool_fwd(y, n, N, 0, out_dtype=torch.float32)
-    if self.head is not None:
-      out, saved["head_in"] = self.head.fwd(P, out)
-    return out, saved
+    return self._stages_fwd(P, image, E.Geom(n, self._N, masks), frozen)
 
   def bwd(self, P, dout, saved):
-    n = saved["n"]
-    d, N, Np, T = self.hidden_dim, self._N, self._Np, self.tokens_mlp_dim
-    if self.head is not None:
-      dout = self.head.bwd(P, dout, saved["head_in"])
-    dy = ops.pool_bwd(dout, n, N, 0)
-    x, mean, rstd = saved["norm"]
-    masks = saved.get("masks")
-    # with stochastic depth the gradient entering a branch is mask * dx, so the fused
-    # "colsum(dx) -> the previous block's Dense_1 bias gradient" shortcut does not apply
-    last = f"MixerBlock_{self.num_blocks - 1}/channel_mixing/Dense_1/bias"
-    dx = ops.layernorm_bwd(dy, x, P.f("pre_head_layer_norm/scale"), mean, rstd,
-                           dscale=P.g("pre_head_layer_norm/scale"), dbias=P.g("pre_head_layer_norm/bias"),
-                           dx_colsum=P.g(last) if masks is None else None)
-    for i in reversed(range(self.num_blocks)):
-      p = f"MixerBlock_{i}/"
-      tm, cm = p + "token_mixing/", p + "channel_mixing/"
-      x, mean1, rstd1, yt, hact, hpre, x1, mean2, rstd2, mlp_saved = saved["blocks"][i]
-      saved["blocks"][i] = None
-      # channel mixing (colsum(dx) already went into this block's channel_mixing/Dense_1/bias)
-      dbr = dx if masks is None else ops.row_select(dx, None, masks[i, 1], n, N)
-      dy2 = vit.mlp_bwd(vit.Scope(P, cm), dbr, mlp_saved, want_bias2_grad=masks is not None)
-      dx1 = ops.layernorm_bwd(dy2, x1, P.f(p + "LayerNorm_1/scale"), mean2, rstd2, dres=dx,
-                              dscale=P.g(p + "LayerNorm_1/scale"), dbias=P.g(p + "LayerNorm_1/bias"))
-      # token mixing
-      k1, b1 = self._store(P, tm + "Dense_1/", "kernel"), self._store(P, tm + "Dense_1/", "bias")
-      dbr = dx1 if masks is None else ops.row_select(dx1, None, masks[i, 0], n, N)
-      dot = ops.transpose_tokens(dbr, n, N, d)                                # [n*d, Np], pad = 0
-      ops.colsum(dot, P.g(b1))
-      ops.gemm(hact, dot, a_mn=True, b_mn=True, out=P.g(k1), reduce_out=True, N=N)
-      dhpre = ops.gemm(dot, P.h(k1), aux=hpre, epilogue=L.EPI_DGELU, K=N)    # [n*d, T]
-      # separate column-sum pass: with n*d rows over only T columns the GEMM epilogue's fused bias
-      # gradient is all atomic contention (measured 2.62 vs 1.26 + 0.07 ms per call)
-      ops.colsum(dhpre, P.g(tm + "Dense_0/bias"))
-      ops.gemm(yt, dhpre, a_mn=True, b_mn=True, out=P.g(tm + "Dense_0/kernel"), reduce_out=True, M=N)
-      dyt = torch.empty((n * d, Np), dtype=torch.bfloat16, device=dx.device)
-      ops.gemm(dhpre, P.h(tm + "Dense_0/kernel"), out=dyt, N=N)
-      dyl = ops.untranspose_add(dyt, None, n, N, d)
-      prev = (P.g(f"MixerBlock_{i - 1}/channel_mixing/Dense_1/bias") if i > 0 else P.g("stem/bias"))
-      if masks is not None and i > 0:
-        prev = None
-      dx = ops.layernorm_bwd(dyl, x, P.f(p + "LayerNorm_0/scale"), mean1, rstd1, dres=dx1,
-                             dscale=P.g(p + "LayerNorm_0/scale"), dbias=P.g(p + "LayerNorm_0/bias"),
-                             dx_colsum=prev)
-    ops.gemm(saved["patches"], dx, a_mn=True, b_mn=True, out=P.g("stem/kernel_flat"), reduce_out=True)
+    self._stages_bwd(P, dout, saved)
 
   def apply(self, variables, image, *, train=False):
-    x, _ = self.fwd(variables["params"], image)
+    x, _ = self.fwd(variables["params"], image, frozen=True)     # no backward follows: forward-only, same bits
     return x, {"logits" if self.num_classes else "pre_logits": x}
 
 

@@ -28,12 +28,12 @@ class _Embed(E.Stage):
     self.prefixes = (prefix + "Embed_0/", prefix + "pos_embedding")
 
   def fwd(self, P, text, geom, save=True):
-    _, Ln = geom
+    Ln = geom.N
     x = ops.embed_fwd(text, P.f(self.p + "Embed_0/embedding"), P.f(self.p + "pos_embedding").view(Ln, self.d))
     return x, (text if save else None)
 
   def bwd(self, P, dx, text, geom, sink=None, need_dx=False):
-    _, Ln = geom
+    Ln = geom.N
     ops.embed_bwd(text, dx, P.g(self.p + "Embed_0/embedding"), P.g(self.p + "pos_embedding").view(Ln, self.d))
 
 
@@ -129,7 +129,7 @@ class _Model(E.Staged):
   def fwd(self, P, text, frozen=None):
     """text int32 [n, L] -> (fp32 [n, out], saved); bf16 [n, width] without a head.  `frozen` as in
     vit._Model.fwd: the stages below the cut run forward-only and save nothing."""
-    return self._stages_fwd(P, text, tuple(text.shape), frozen)
+    return self._stages_fwd(P, text, E.Geom(*text.shape), frozen)
 
   def bwd(self, P, dout, saved):
     if not self.num_classes:       # the tower's output is bf16

@@ -222,7 +222,7 @@ class EncoderBlock(E.Stage):
   def fwd(self, P, x, geom, save=True):
     """save=False (forward only): same output bits; every intermediate is released as soon as the
     next op has consumed it and saved is None."""
-    n, N = geom
+    n, N = geom.n, geom.N
     d = self.d
     S = self.scope(P)
     A = S.sub("MultiHeadDotProductAttention_0/")
@@ -244,7 +244,7 @@ class EncoderBlock(E.Stage):
     x2, mlp_saved = mlp_fwd(S.sub("MlpBlock_0/"), ln2, x1)
     return x2, (x, ln1, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, mlp_saved)
 
-  def sink(self, P):
+  def sink(self, P, geom):
     """colsum(d block-output) is the gradient of this block's MlpBlock Dense_1 bias."""
     return self.scope(P).g("MlpBlock_0/Dense_1/bias")
 
@@ -252,7 +252,7 @@ class EncoderBlock(E.Stage):
     """dx2: bf16 [M,d] grad of block output; colsum(dx2) has ALREADY been accumulated into
     this block's Dense_1 bias grad by whoever produced dx2.  Returns dx (grad of block input);
     colsum(dx) is accumulated into `sink` (the bias gradient of the stage below)."""
-    n, N = geom
+    n, N = geom.n, geom.N
     d = self.d
     S = self.scope(P)
     A = S.sub("MultiHeadDotProductAttention_0/")
@@ -308,14 +308,14 @@ class ScanEncoder(E.Stage):
       x, _ = b.fwd(P, x, geom, save)
     return x, saved
 
-  def sink(self, P):
-    return self.blocks[-1].sink(P)
+  def sink(self, P, geom):
+    return self.blocks[-1].sink(P, geom)
 
   def bwd(self, P, dx, saved, geom, sink, need_dx=True):
     for i in reversed(range(len(self.blocks))):
       x_out, s = self.blocks[i].fwd(P, saved[i], geom)    # recompute the block from its input
       del x_out
-      dx = self.blocks[i].bwd(P, dx, s, geom, self.blocks[i - 1].sink(P) if i else sink)
+      dx = self.blocks[i].bwd(P, dx, s, geom, self.blocks[i - 1].sink(P, geom) if i else sink)
       saved[i] = s = None
     return dx
 
@@ -345,7 +345,7 @@ class NormPool(E.Stage):
     return 0 if self.pool == "first" else N - 1
 
   def fwd(self, P, x, geom, save=True):
-    n, N = geom
+    n, N = geom.n, geom.N
     scale, bias = P.f(self.p + "scale"), P.f(self.p + "bias")
     if self.pool in ("first", "last"):
       # LayerNorm is per token: LN(x)[:, t] == LN(x[:, t]) -- select first, normalise one row
@@ -361,7 +361,7 @@ class NormPool(E.Stage):
     return encd, saved
 
   def bwd(self, P, dy, saved, geom, sink, need_dx=True):
-    n, N = geom
+    n, N = geom.n, geom.N
     x, mean, rstd, encd = saved
     if dy.dtype != self.out_dtype:
       dy = ops.cast(dy, torch.empty_like(dy, dtype=self.out_dtype))
@@ -392,7 +392,7 @@ class MAPHead(E.Stage):
             + mlp_specs(self.p + "MlpBlock_0/", d, self.m)), a
 
   def fwd(self, P, enc, geom, save=True):
-    n, N = geom
+    n, N = geom.n, geom.N
     d = self.d
     q1 = ops.gemm(P.h(self.p + "probe").view(1, d), P.h(self.att + "q/kernel"), b_mn=True,
                   bias=P.f(self.att + "q/bias"))
@@ -411,7 +411,7 @@ class MAPHead(E.Stage):
 
   def bwd(self, P, dout, saved, geom, sink=None, need_dx=True):
     """dout fp32 [n,d] -> d(enc) bf16 [n*N, d] (None with need_dx=False)."""
-    n, N = geom
+    n, N = geom.n, geom.N
     d = self.d
     enc, qn, kv, o, lse, a, mean, rstd, mlp_saved = saved
     dout16 = ops.cast(dout, torch.empty_like(dout, dtype=torch.bfloat16))
@@ -442,13 +442,33 @@ class MAPHead(E.Stage):
 
 
 class PatchEmbedding(E.Stage):
-  """The patch embedding (models/vit.py:212-225): a Dense over flattened patches with the position
-  embedding added in its epilogue, then [cls] prepended when `cls`."""
+  """The patch embedding (models/vit.py:212-225): a Dense over flattened patches, stored under
+  `prefix + name`, with the position embedding added in its epilogue, then [cls] prepended when `cls`.
+  posemb=None adds no position embedding: the MLP-Mixer's stem (models/mlp_mixer.py:72)."""
 
-  def __init__(self, prefix, patch_size, d, posemb, cls):
+  def __init__(self, prefix, name, patch_size, d, posemb, cls):
     self.p, self.patch_size, self.d, self.posemb, self.cls = prefix, patch_size, d, posemb, cls
-    self.prefixes = (prefix + "embedding/", prefix + "pos_embedding", prefix + "cls")
+    self.w = prefix + name + "/"
+    self.prefixes = ((self.w,) + ((prefix + "pos_embedding",) if posemb == "learn" else ())
+                     + ((prefix + "cls",) if cls else ()))
     self._sincos = None
+
+  def specs(self, tokens, in_ch):
+    """The kernel is stored flattened [ph*pw*in_ch, d] (the im2col column order), padded to a multiple
+    of 8 rows, and exposed under `kernel` as [ph, pw, in_ch, d]."""
+    (ph, pw), d, w = self.patch_size, self.d, self.w
+    K = ph * pw * in_ch
+    Kp = (K + 7) // 8 * 8
+    lec = E.lecun_normal(K)   # flax Conv default kernel_init, fan_in = ph*pw*C
+    specs = [E.ParamSpec(w + "kernel_flat", (Kp, d),
+                         lambda rng, shape: np.concatenate([lec(rng, (K, d)), np.zeros((Kp - K, d))], 0)),
+             E.ParamSpec(w + "bias", (d,), E.zeros)]
+    aliases = [E.Alias(w + "kernel", w + "kernel_flat", lambda t: t[:K].unflatten(0, (ph, pw, in_ch)))]
+    if self.posemb == "learn":
+      specs.append(E.ParamSpec(self.p + "pos_embedding", (1, tokens, d), E.normal(1 / math.sqrt(d))))
+    if self.cls:
+      specs.append(E.ParamSpec(self.p + "cls", (1, 1, d), E.zeros))
+    return specs, aliases
 
   def _posemb16(self, P, image):
     if self.posemb == "learn":
@@ -459,25 +479,28 @@ class PatchEmbedding(E.Stage):
     return self._sincos
 
   def fwd(self, P, image, geom, save=True):
-    n, N = geom
-    N0, p = N - self.cls, self.p
+    n, N = geom.n, geom.N
+    N0, w = N - self.cls, self.w
     patches = ops.patchify(image, self.patch_size[0])
-    x = ops.gemm(patches, P.h(p + "embedding/kernel_flat"), b_mn=True, bias=P.f(p + "embedding/bias"),
-                 aux=self._posemb16(P, image), aux_row_mod=N0, epilogue=L.EPI_BIAS_RESID)
+    if self.posemb:
+      x = ops.gemm(patches, P.h(w + "kernel_flat"), b_mn=True, bias=P.f(w + "bias"),
+                   aux=self._posemb16(P, image), aux_row_mod=N0, epilogue=L.EPI_BIAS_RESID)
+    else:
+      x = ops.gemm(patches, P.h(w + "kernel_flat"), b_mn=True, bias=P.f(w + "bias"))
     saved = patches if save else None
     del patches
     if self.cls:
       # cls token is prepended AFTER the position embedding was added (models/vit.py:223-225)
-      x = ops.concat_cls(x, P.f(p + "cls").view(self.d), n, N0)
+      x = ops.concat_cls(x, P.f(self.p + "cls").view(self.d), n, N0)
     return x, saved
 
-  def sink(self, P):
+  def sink(self, P, geom):
     # the column sum of the gradient reaching the embedding output is the patch-embed bias gradient
     # (models/vit.py:212-214); with [cls] it is summed over the patch tokens only (bwd)
-    return None if self.cls else P.g(self.p + "embedding/bias")
+    return None if self.cls else P.g(self.w + "bias")
 
   def bwd(self, P, dx, patches, geom, sink=None, need_dx=False):
-    n, N = geom
+    n, N = geom.n, geom.N
     d, p = self.d, self.p
     if self.cls:
       # batch-sum of the gradient at every token position: row 0 is d cls, the rest d pos_embedding;
@@ -490,11 +513,11 @@ class PatchEmbedding(E.Stage):
       if self.posemb == "learn":
         gpos = P.g(p + "pos_embedding").view(N0 * d)
         ops.axpby(gpos, tmp[d:], 1.0, 1.0, out=gpos)
-      ops.colsum(tmp[d:].view(N0, d), P.g(p + "embedding/bias"))
+      ops.colsum(tmp[d:].view(N0, d), P.g(self.w + "bias"))
       dx = ops.drop_cls(dx, n, N0)
     elif self.posemb == "learn":
       ops.colsum(dx.view(n, N * d), P.g(p + "pos_embedding").view(N * d))
-    ops.gemm(patches, dx, a_mn=True, b_mn=True, out=P.g(p + "embedding/kernel_flat"), reduce_out=True)
+    ops.gemm(patches, dx, a_mn=True, b_mn=True, out=P.g(self.w + "kernel_flat"), reduce_out=True)
 
 
 class PreLogits(E.Stage):
@@ -562,7 +585,7 @@ class _Model(E.Staged):
     if self.num_classes:
       self.head = common.ClassifierHead(p, rep, self.num_classes, E.zeros if self.head_zeroinit else E.lecun_normal(rep))
     # the backward stages, bottom-up (engine.Staged); parameterless pools belong to no stage of their own
-    self._stages = ([PatchEmbedding(p, self.patch_size, d, self.posemb, self.pool_type == "tok")]
+    self._stages = ([PatchEmbedding(p, "embedding", self.patch_size, d, self.posemb, self.pool_type == "tok")]
                     + encoder_stages(enc, self.depth, d, self.mlp, self.num_heads, self.scan, self.remat_policy)
                     + [NormPool(enc + "encoder_norm/", d, _POOLS[self.pool_type], torch.float32)])
     if self.pool_type == "map":
@@ -584,27 +607,11 @@ class _Model(E.Staged):
     if image_hw is not None:
       self.setup(image_hw)
     gh, gw = self._geom
-    d, p = self.width, self.prefix
-    ph, pw = self.patch_size
-    K = ph * pw * in_ch
-    Kp = (K + 7) // 8 * 8
-    lec = E.lecun_normal(K)   # flax Conv default kernel_init, fan_in = ph*pw*C
-    specs = [
-        E.ParamSpec(p + "embedding/kernel_flat", (Kp, d),
-                    lambda rng, shape: np.concatenate([lec(rng, (K, d)), np.zeros((Kp - K, d))], 0)),
-        E.ParamSpec(p + "embedding/bias", (d,), E.zeros),
-    ]
-    aliases = [E.Alias(p + "embedding/kernel", p + "embedding/kernel_flat",
-                       lambda t: t[:K].unflatten(0, (ph, pw, in_ch)))]
-    if self.posemb == "learn":
-      specs.append(E.ParamSpec(p + "pos_embedding", (1, gh * gw, d), E.normal(1 / math.sqrt(d))))
-    if self.pool_type == "tok":
-      specs.append(E.ParamSpec(p + "cls", (1, 1, d), E.zeros))
+    specs, aliases = self._stages[0].specs(gh * gw, in_ch)
     for stage in self._stages[1:]:
       s, a = stage.specs()
       specs += s
       aliases += a
-    self._in_ch, self._K, self._Kp = in_ch, K, Kp
     return specs, aliases
 
   def init(self, seed, image_shape, device="cuda"):
@@ -625,7 +632,7 @@ class _Model(E.Staged):
     n = image.shape[0]
     gh, gw = self._geom
     N = gh * gw + (self.pool_type == "tok")
-    out, saved = self._stages_fwd(P, image, (n, N), frozen)
+    out, saved = self._stages_fwd(P, image, E.Geom(n, N), frozen)
     if self.pool_type == "none":
       # no pooling (models/vit.py:252-253): pre_logits / head run on every token, out is [n, N, .]
       if out.dtype != torch.float32:
@@ -637,8 +644,8 @@ class _Model(E.Staged):
     """dout: fp32 [n, out] ([n, N, out] without pooling).  Accumulates parameter gradients into P.grad.
     With a padded class head, out is the padded class count (ClassifierHead.bwd)."""
     if self.pool_type == "none":
-      n, N = saved["geom"]
-      dout = dout.reshape(n * N, -1)
+      geom = saved["geom"]
+      dout = dout.reshape(geom.n * geom.N, -1)
     self._stages_bwd(P, dout, saved)
 
   # ---- reference-style entry points --------------------------------------------------------

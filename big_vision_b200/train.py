@@ -19,14 +19,13 @@ def loss_and_grads(model, P, images, labels, loss_name="sigmoid_xent", dist_view
   """value_and_grad(loss_fn)(params) of train.py:295-303 on this rank's shard; P.grad holds the
   LOCAL gradient of the LOCAL-mean loss (callers average across ranks).
 
-  `frozen` (storage names, optax.Chain.frozen()): parameters that get no gradient.  Models with
-  backward stages (ViT) run the stages below the lowest trained one forward-only -- a linear probe
-  (`head/.*` trained, the rest None) runs the backbone without a backward -- and the all-reduce
-  covers the trained ranges only.  Other models (MLP-Mixer) ignore it and run the full path."""
+  `frozen` (storage names, optax.Chain.frozen()): parameters that get no gradient.  The model's backward
+  stages below the lowest trained one run forward-only -- a linear probe (`head/.*` trained, the
+  rest None) runs the backbone without a backward -- and the all-reduce covers the trained ranges only."""
   if loss_name not in _LOSSES:
     raise NotImplementedError(f"loss {loss_name}")
   ranges = None
-  if frozen and hasattr(model, "stages"):
+  if frozen:
     fwd_kw["frozen"] = frozen
     ranges = P.trained_ranges(frozen)
   P.zero_grad()

@@ -34,6 +34,15 @@ def _vit(pool="map", scan=False, rep=False, classes=10):
   return model, E.FlatParams(specs, aliases, "cpu")
 
 
+def _mixer():
+  from big_vision_b200 import engine as E
+  from big_vision_b200.models import mlp_mixer
+  model = mlp_mixer.Model(10, patch_size=(16, 16), num_blocks=3, hidden_dim=64, tokens_mlp_dim=32,
+                          channels_mlp_dim=128)
+  specs, aliases = model.specs((32, 48), 3)
+  return model, E.FlatParams(specs, aliases, "cpu")
+
+
 def _two_towers(scan=False):
   from big_vision_b200 import engine as E
   from big_vision_b200.models.proj.image_text import two_towers
@@ -81,6 +90,16 @@ def test_blocks_are_stages_and_the_cut_falls_on_the_lowest_trained_block():
   assert len(stages) == 1 + 3 + 1 + 1          # embedding, 3 blocks, encoder_norm, head
   frozen = _tx(P, [("embedding/.*|pos_embedding|Transformer/encoderblock_0/.*", None), (".*", SCHED)]).frozen()
   assert stages[model.cut(P, frozen)] == ("Transformer/encoderblock_1/",)
+
+
+def test_mixer_stages_are_stem_blocks_pre_head_and_head():
+  model, P = _mixer()
+  assert model.stages() == [("stem/",), ("MixerBlock_0/",), ("MixerBlock_1/",), ("MixerBlock_2/",),
+                            ("pre_head_layer_norm/",), ("head/",)]
+  assert model.cut(P, _tx(P, [("head/.*", SCHED), (".*", None)]).frozen()) == 5
+  frozen = _tx(P, [("stem/.*|MixerBlock_0/.*", None), (".*", SCHED)]).frozen()
+  assert model.stages()[model.cut(P, frozen)] == ("MixerBlock_1/",)
+  assert model.cut(P, _tx(P, [("MixerBlock_1/.*", None), (".*", SCHED)]).frozen()) == 0
 
 
 def test_scan_stacked_encoder_is_one_stage():

@@ -1,11 +1,12 @@
 """GPU: frozen parameters cost only a forward pass.
 
-A SigLiT step (image tower frozen) and a ViT linear probe (head only) against the same step run the
-full way: the forward is bit-identical, every trained gradient matches, every frozen gradient is
-exactly zero, the frozen parameters do not move in 3 optimizer steps and the trained ones follow the
-full path.  The SigLiT step's peak memory drops by the image tower's saved activations; apply() is
-the forward-only path and returns the training forward's bits.  The single-output bias + GELU
-epilogue (EPI_BIAS_GELU_ACT) writes the dual-output epilogue's first output bit for bit."""
+A SigLiT step (image tower frozen) and a ViT or MLP-Mixer linear probe (head only) against the same
+step run the full way: the forward is bit-identical, every trained gradient matches, every frozen
+gradient is exactly zero, the frozen parameters do not move in 3 optimizer steps and the trained ones
+follow the full path.  The SigLiT step's peak memory drops by the image tower's saved activations;
+apply() is the forward-only path and returns the training forward's bits, and so does a forward-only
+Mixer run under stochastic-depth masks.  The single-output bias + GELU epilogue (EPI_BIAS_GELU_ACT)
+writes the dual-output epilogue's first output bit for bit."""
 import os
 import sys
 
@@ -154,10 +155,14 @@ def test_apply_is_the_forward_bit_for_bit():
   assert torch.equal(out["t"], P.f("t").exp())
 
 
-# ---- ViT linear probe through train.make_update_fn --------------------------------------------
-def _probe_model(pool):
-  from big_vision_b200.models import vit
-  model = vit.Model(16, width=64, depth=2, mlp_dim=128, num_heads=1, patch_size=(16, 16), pool_type=pool)
+# ---- ViT and MLP-Mixer linear probes through train.make_update_fn ----------------------------
+def _probe_model(kind):
+  from big_vision_b200.models import mlp_mixer, vit
+  if kind == "mixer":        # 12 tokens: the token-mixing storage is padded to 16
+    model = mlp_mixer.Model(16, patch_size=(16, 16), num_blocks=2, hidden_dim=64, tokens_mlp_dim=32,
+                            channels_mlp_dim=128)
+  else:
+    model = vit.Model(16, width=64, depth=2, mlp_dim=128, num_heads=1, patch_size=(16, 16), pool_type=kind)
   shape = (4, 64, 48, 3)
   P = model.init(0, shape, device="cuda")
   rng = np.random.default_rng(1)
@@ -169,10 +174,10 @@ def _probe_model(pool):
   return model, P, tree, shape, image, labels
 
 
-@pytest.mark.parametrize("pool", ["map", "tok", "gap"])
-def test_linear_probe_step(pool):
+@pytest.mark.parametrize("kind", ["map", "tok", "gap", "mixer"])
+def test_linear_probe_step(kind):
   from big_vision_b200 import train
-  model, P, tree, shape, image, labels = _probe_model(pool)
+  model, P, tree, shape, image, labels = _probe_model(kind)
   schedule = [("head/.*", SCHED), (".*", None)]
   frozen = _tx(P, schedule).frozen()
   assert model.cut(P, frozen) == len(model.stages()) - 1
@@ -198,6 +203,11 @@ def test_linear_probe_step(pool):
   _check_steps(P0, finals[0], finals[1], frozen, lr)
   x, _ = model.apply({"params": P}, image)
   assert torch.equal(x, logits_f)
+  if kind == "mixer":        # the stochastic-depth masks reach the forward-only blocks as well
+    masks = torch.tensor([[[1, 1, 1, 1], [1, 1, 1, 1]], [[1, 0, 1, 0], [0, 1, 1, 0]]], dtype=torch.float32).cuda()
+    x_saved, _ = model.fwd(P, image, masks=masks)
+    x_fwd, _ = model.fwd(P, image, masks=masks, frozen=True)
+    assert torch.equal(x_fwd, x_saved) and not torch.equal(x_fwd, x)
 
 
 # ---- the single-output GELU epilogue ------------------------------------------------------------
