@@ -193,8 +193,10 @@ class Stage:
 
 
 class Staged:
-  """A model built as `self._stages`, a bottom-up list of backward stages (Stage).  Each stage has
+  """A model built as `self._stages`, a bottom-up list of backward stages (Stage), which the model's
+  specs() builds once the input geometry is known (_build).  Each stage has
     `prefixes`: the storage-name prefixes of its parameters;
+    `specs() -> (specs, aliases)`: its parameters;
     `fwd(P, x, geom, save) -> (y, saved)`: `geom` is the forward's Geom; with save=False it keeps
         nothing (saved is None) and frees each intermediate once it has been consumed;
     `bwd(P, dy, saved, geom, sink, need_dx) -> dx`: accumulates its parameter gradients; `sink` (or
@@ -203,6 +205,16 @@ class Staged:
         None;
     `ready`: None, or the storage name from which on (in spec order) every gradient is final once the
         stage's backward has run (P.on_ready, the bucketed gradient all-reduce)."""
+
+  def _build(self, stages):
+    """Makes `stages` the model's stage list -> (specs, aliases) of all their parameters, in stage order."""
+    self._stages = stages
+    specs, aliases = [], []
+    for stage in stages:
+      s, a = stage.specs()
+      specs += s
+      aliases += a
+    return specs, aliases
 
   def stages(self):
     """The stages' storage-name prefixes, bottom-up."""

@@ -5,8 +5,8 @@ of the freshly initialised tree and the checkpoint's values, except for names ma
 `dont_load` regex (those keep their init value and may be absent on either side); any other
 structural difference is an error that lists both sides.
 
-`ClassifierHead` is the `head` Dense of the ViT and MLP-Mixer classifiers, the one place that knows
-how its parameters are stored.
+`Dense` is the Dense stage of every model's heads (pre_logits, the class heads), and `dense_specs` the
+one place that knows how a Dense with padded columns is stored.
 """
 import numpy as np
 import torch
@@ -23,53 +23,71 @@ def to16(x):
   return ops.cast(x, torch.empty_like(x, dtype=torch.bfloat16))
 
 
-class ClassifierHead(E.Stage):
-  """The `head` Dense (kernel [rep, C], bias [C]) of a classifier, logits in fp32; a backward stage
-  (engine.Staged) of the ViT.
+def dense_specs(prefix, fan_in, fan_out, init, store_cols=None):
+  """(specs, aliases) of a Dense: kernel [fan_in, fan_out] from `init`, zero bias [fan_out].
 
-  The kernel is the MN-major B operand of the head GEMM, and TMA needs its row stride to be a multiple
-  of 16 bytes.  So with C % 8 != 0 (21843 classes for ImageNet-21k, 37 for Oxford pets, ...) it is
-  stored as `head/kernel_pad` [rep, Cp] and `head/bias_pad` [Cp], Cp = round_up(C, 8), and exposed
-  under the reference names as the views [:, :C] and [:C].  The padding starts at zero and stays
-  exactly zero: the logit gradient is zero in its padding columns (the xent kernels write it so), so
-  the padding's gradient is zero, and an Adam / scale update and the weight decay of zero are zero;
-  Adafactor updates the reference-shaped views only.  With C % 8 == 0 nothing is padded or aliased.
-  """
+  A kernel that is the MN-major B operand of a GEMM needs a row stride of a multiple of 16 bytes (TMA).
+  With `store_cols` > fan_out the kernel and bias are stored as `kernel_pad` [fan_in, store_cols] and
+  `bias_pad` [store_cols], zero past column fan_out, and exposed under the reference names as the views
+  [:, :fan_out] and [:fan_out].  The first spec is always the kernel, the second the bias."""
+  sc = store_cols or fan_out
+  if sc == fan_out:
+    return [E.ParamSpec(prefix + "kernel", (fan_in, fan_out), init),
+            E.ParamSpec(prefix + "bias", (fan_out,), E.zeros)], []
+  pad = np.zeros((fan_in, sc - fan_out))
+  specs = [E.ParamSpec(prefix + "kernel_pad", (fan_in, sc),
+                       lambda rng, shape: np.concatenate([init(rng, (fan_in, fan_out)), pad], 1)),
+           E.ParamSpec(prefix + "bias_pad", (sc,), E.zeros)]
+  aliases = [E.Alias(prefix + "kernel", prefix + "kernel_pad", lambda t: t[:, :fan_out]),
+             E.Alias(prefix + "bias", prefix + "bias_pad", lambda t: t[:fan_out])]
+  return specs, aliases
 
-  def __init__(self, prefix, rep, num_classes, kernel_init):
-    self.rep, self.C, self.kernel_init = rep, num_classes, kernel_init
-    self.Cp = (num_classes + 7) // 8 * 8
-    pad = "_pad" if self.Cp != self.C else ""
-    self.p, self.kernel, self.bias = prefix + "head/", prefix + "head/kernel" + pad, prefix + "head/bias" + pad
-    self.prefixes = (self.p,)
+
+class Dense(E.Stage):
+  """A Dense stored under `prefix` (kernel [fan_in, fan_out], bias [fan_out]) as a backward stage
+  (engine.Staged): bf16 GEMM operands, fp32 output, tanh(x W + b) with `tanh` (the ViT's pre_logits),
+  the input gradient in `dx_dtype`.  `rep` is the input width (a head's representation size), `C` the
+  output width.
+
+  pad=True is for class heads: when the class count C = fan_out is not a multiple of 8 (21843 for
+  ImageNet-21k, 37 for Oxford pets, ...) the kernel and bias are stored with Cp = round_up(C, 8)
+  columns (dense_specs), the output is the [rows, C] view of the [rows, Cp] GEMM output, and the
+  backward takes the output gradient as [rows, Cp].  The padding starts at zero and stays exactly zero:
+  the logit gradient is zero in its padding columns (the xent kernels write it so), so the padding's
+  gradient is zero, and an Adam / scale update and the weight decay of zero are zero; Adafactor
+  updates the reference-shaped views only."""
+
+  def __init__(self, prefix, fan_in, fan_out, kernel_init, *, tanh=False, dx_dtype=torch.float32, pad=False):
+    self.p, self.rep, self.C, self.tanh, self.dx_dtype = prefix, fan_in, fan_out, tanh, dx_dtype
+    self.Cp = (fan_out + 7) // 8 * 8 if pad else fan_out
+    self._specs = dense_specs(prefix, fan_in, fan_out, kernel_init, self.Cp)
+    self.kernel, self.bias = (s.name for s in self._specs[0])
+    self.prefixes = (prefix,)
 
   def specs(self):
-    rep, C, Cp, init = self.rep, self.C, self.Cp, self.kernel_init
-    if Cp == C:
-      return [E.ParamSpec(self.kernel, (rep, C), init), E.ParamSpec(self.bias, (C,), E.zeros)], []
-    specs = [E.ParamSpec(self.kernel, (rep, Cp),
-                         lambda rng, shape: np.concatenate([init(rng, (rep, C)), np.zeros((rep, Cp - C))], 1)),
-             E.ParamSpec(self.bias, (Cp,), E.zeros)]
-    aliases = [E.Alias(self.p + "kernel", self.kernel, lambda t: t[:, :C]),
-               E.Alias(self.p + "bias", self.bias, lambda t: t[:C])]
-    return specs, aliases
+    return self._specs
 
   def fwd(self, P, x, geom=None, save=True):
-    """x [rows, rep] -> (logits fp32 [rows, C], x if save): a view of the [rows, Cp] GEMM output when
-    padded."""
-    out = ops.gemm(to16(x), P.h(self.kernel), b_mn=True, bias=P.f(self.bias), out_dtype=torch.float32)
-    return (out if self.Cp == self.C else out[:, :self.C]), (x if save else None)
+    """x [rows, fan_in] -> (y fp32 [rows, C], saved)."""
+    y = ops.gemm(to16(x), P.h(self.kernel), b_mn=True, bias=P.f(self.bias), out_dtype=torch.float32)
+    if self.tanh:
+      y = ops.tanh_fwd(y)
+    saved = (x, y if self.tanh else None) if save else None
+    return (y if self.Cp == self.C else y[:, :self.C]), saved
 
-  def bwd(self, P, dlogits, x, geom=None, sink=None, need_dx=True):
-    """dlogits fp32 [rows, Cp], zero in the columns past C; x the forward's input.  Accumulates the
-    head's gradients and returns d x (fp32 [rows, rep]), or None with need_dx=False."""
-    if tuple(dlogits.shape[1:]) != (self.Cp,):
-      raise ValueError(f"head backward: the logit gradient must be [rows, {self.Cp}] (padded to "
-                       f"{self.Cp} zero-filled columns), got {tuple(dlogits.shape)}")
-    d16 = to16(dlogits)
-    ops.colsum(dlogits, P.g(self.bias))
+  def bwd(self, P, dy, saved, geom=None, sink=None, need_dx=True):
+    """dy fp32 [rows, Cp], zero in the columns past C.  Accumulates the Dense's gradients and returns
+    d x ([rows, fan_in] in dx_dtype), or None with need_dx=False."""
+    if tuple(dy.shape[1:]) != (self.Cp,):
+      raise ValueError(f"{self.p} backward: the output gradient must be [rows, {self.Cp}] (the stored "
+                       f"columns, zero past column {self.C}), got {tuple(dy.shape)}")
+    x, y = saved
+    if self.tanh:
+      dy = ops.tanh_bwd(dy, y)
+    d16 = to16(dy)
+    ops.colsum(dy, P.g(self.bias))
     ops.gemm(to16(x), d16, a_mn=True, b_mn=True, out=P.g(self.kernel), reduce_out=True)
-    return ops.gemm(d16, P.h(self.kernel), out_dtype=torch.float32) if need_dx else None
+    return ops.gemm(d16, P.h(self.kernel), out_dtype=self.dx_dtype) if need_dx else None
 
 
 def _report(ckpt_names, model_names, only_model, only_ckpt):

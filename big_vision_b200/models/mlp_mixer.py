@@ -27,24 +27,6 @@ from big_vision_b200.models import common
 from big_vision_b200.models import vit
 
 
-def _dense_specs(p, fan_in, fan_out, store_cols=None):
-  """flax nn.Dense defaults: lecun_normal kernel, zeros bias.  `store_cols` pads the stored
-  kernel/bias columns (TMA row strides must be multiples of 16 bytes)."""
-  lec = E.lecun_normal(fan_in)
-  sc = store_cols or fan_out
-  if sc == fan_out:
-    return [E.ParamSpec(p + "kernel", (fan_in, fan_out), lec),
-            E.ParamSpec(p + "bias", (fan_out,), E.zeros)], []
-  pad = sc - fan_out
-  specs = [E.ParamSpec(p + "kernel_pad", (fan_in, sc),
-                       lambda rng, shape: np.concatenate([lec(rng, (fan_in, fan_out)),
-                                                          np.zeros((fan_in, pad))], 1)),
-           E.ParamSpec(p + "bias_pad", (sc,), E.zeros)]
-  aliases = [E.Alias(p + "kernel", p + "kernel_pad", lambda t: t[:, :fan_out]),
-             E.Alias(p + "bias", p + "bias_pad", lambda t: t[:fan_out])]
-  return specs, aliases
-
-
 class MixerBlock(E.Stage):
   """MixerBlock_{i} (mlp_mixer.py:40-55): x + token-mixing MLP over the tokens of LayerNorm_0(x), then
   x + channel-mixing MLP over LayerNorm_1(x).  With the forward's stochastic-depth masks (geom.masks)
@@ -54,24 +36,24 @@ class MixerBlock(E.Stage):
     self.i, self.N, self.Np = i, N, (N + 7) // 8 * 8
     self.d, self.T, self.C = d, tokens_mlp_dim, channels_mlp_dim
     self.p = p = f"MixerBlock_{i}/"
-    self.tm, self.cm = p + "token_mixing/", p + "channel_mixing/"
+    self.tm, self.cm = tm, cm = p + "token_mixing/", p + "channel_mixing/"
     self.prefixes = (p,)
     self.ready = p + "LayerNorm_0/scale"
-    # token-mixing Dense_1 writes [n*d, N] in rows of Np elements: its storage is padded (specs)
-    pad = "_pad" if self.Np != N else ""
-    self.k1, self.b1 = self.tm + "Dense_1/kernel" + pad, self.tm + "Dense_1/bias" + pad
-
-  def specs(self):
-    p, tm, cm, N, d = self.p, self.tm, self.cm, self.N, self.d
     specs, aliases = vit.ln_specs(p + "LayerNorm_0/", d) + vit.ln_specs(p + "LayerNorm_1/", d), []
+    # flax nn.Dense defaults: lecun_normal kernel, zero bias.  Token-mixing Dense_1 writes [n*d, N] in
+    # rows of Np elements: its storage is padded.
     for nm, fi, fo, sc in ((tm + "Dense_0/", N, self.T, None),
                            (tm + "Dense_1/", self.T, N, self.Np),
                            (cm + "Dense_0/", d, self.C, None),
                            (cm + "Dense_1/", self.C, d, None)):
-      s, a = _dense_specs(nm, fi, fo, sc)
+      s, a = common.dense_specs(nm, fi, fo, E.lecun_normal(fi), sc)
       specs += s
       aliases += a
-    return specs, aliases
+    self._specs = specs, aliases
+    self.k1, self.b1 = (s.name for s in specs if s.name.startswith(tm + "Dense_1/"))
+
+  def specs(self):
+    return self._specs
 
   def fwd(self, P, x, geom, save=True):
     """save=False (forward only): same output bits; every intermediate is released as soon as the
@@ -153,10 +135,6 @@ class MlpMixer(E.Staged):
   model_name: Optional[str] = None
   stoch_depth: float = 0.0
 
-  def __post_init__(self):
-    self.head = common.ClassifierHead("", self.hidden_dim, self.num_classes, E.zeros) if self.num_classes else None
-    self._stages = self._N = None
-
   def drop_p(self, i):
     """mlp_mixer.py:76"""
     return (i / max(self.num_blocks - 1, 1)) * self.stoch_depth
@@ -169,22 +147,17 @@ class MlpMixer(E.Staged):
     return torch.from_numpy(keep).to(device)
 
   def specs(self, image_hw, in_ch=3):
-    ph, pw = self.patch_size
-    N = (image_hw[0] // ph) * (image_hw[1] // pw)
+    """Builds the backward stages for [n, *image_hw, in_ch] images -> (specs, aliases)."""
     d = self.hidden_dim
-    # the backward stages, bottom-up (engine.Staged); the blocks' token-mixing MLPs are as wide as N
-    self._stages = ([vit.PatchEmbedding("", "stem", self.patch_size, d, None, False)]
-                    + [MixerBlock(i, N, d, self.tokens_mlp_dim, self.channels_mlp_dim) for i in range(self.num_blocks)]
-                    + [vit.NormPool("pre_head_layer_norm/", d, "mean", torch.float32)])
+    self.head = common.Dense("head/", d, self.num_classes, E.zeros, pad=True) if self.num_classes else None
+    # bottom-up; the blocks' token-mixing MLPs are as wide as the stem's token count
+    stem = vit.PatchEmbedding("", "stem", image_hw, self.patch_size, in_ch, d, None, False)
+    stages = ([stem] + [MixerBlock(i, stem.tokens, d, self.tokens_mlp_dim, self.channels_mlp_dim)
+                        for i in range(self.num_blocks)]
+              + [vit.NormPool("pre_head_layer_norm/", d, "mean", torch.float32)])
     if self.head is not None:
-      self._stages.append(self.head)
-    specs, aliases = self._stages[0].specs(N, in_ch)
-    for stage in self._stages[1:]:
-      s, a = stage.specs()
-      specs += s
-      aliases += a
-    self._N = N
-    return specs, aliases
+      stages.append(self.head)
+    return self._build(stages)
 
   def init(self, seed, image_shape, device="cuda"):
     specs, aliases = self.specs(image_shape[1:3], image_shape[3])
@@ -199,7 +172,7 @@ class MlpMixer(E.Staged):
       if rng is None:
         raise ValueError("stoch_depth > 0 in training needs an rng (numpy Generator) or explicit masks")
       masks = self.draw_masks(rng, n, image.device)
-    return self._stages_fwd(P, image, E.Geom(n, self._N, masks), frozen)
+    return self._stages_fwd(P, image, E.Geom(n, self._stages[0].tokens, masks), frozen)
 
   def bwd(self, P, dout, saved):
     self._stages_bwd(P, dout, saved)

@@ -21,11 +21,17 @@ from big_vision_b200.models import common, vit
 
 
 class _Embed(E.Stage):
-  """Embed_0 plus the learned position embedding (text_transformer.py:62-70)."""
+  """Embed_0 plus the learned position embedding (text_transformer.py:62-70) of `text_len` tokens."""
 
-  def __init__(self, prefix, d):
-    self.p, self.d = prefix, d
+  def __init__(self, prefix, vocab_size, text_len, d):
+    self.p, self.vocab_size, self.text_len, self.d = prefix, vocab_size, text_len, d
     self.prefixes = (prefix + "Embed_0/", prefix + "pos_embedding")
+
+  def specs(self):
+    # flax nn.Embed default init: variance_scaling(1.0, "fan_in", "normal", out_axis=0)
+    d, init = self.d, E.normal(1 / math.sqrt(self.d))
+    return [E.ParamSpec(self.p + "Embed_0/embedding", (self.vocab_size, d), init),
+            E.ParamSpec(self.p + "pos_embedding", (1, self.text_len, d), init)], []
 
   def fwd(self, P, text, geom, save=True):
     Ln = geom.N
@@ -35,39 +41,6 @@ class _Embed(E.Stage):
   def bwd(self, P, dx, text, geom, sink=None, need_dx=False):
     Ln = geom.N
     ops.embed_bwd(text, dx, P.g(self.p + "Embed_0/embedding"), P.g(self.p + "pos_embedding").view(Ln, self.d))
-
-
-class _MAPHead(vit.MAPHead):
-  """The MAP head with a bf16 output, the dtype of the tower's other pools."""
-
-  def fwd(self, P, enc, geom, save=True):
-    out, saved = super().fwd(P, enc, geom, save)
-    return common.to16(out), saved
-
-  def bwd(self, P, dout, saved, geom, sink=None, need_dx=True):
-    return super().bwd(P, ops.cast(dout, torch.empty_like(dout, dtype=torch.float32)), saved, geom, sink, need_dx)
-
-
-class _Head(E.Stage):
-  """The `head` Dense (text_transformer.py:97-98): bf16 input, fp32 output, bf16 input gradient."""
-
-  def __init__(self, prefix, d, out):
-    self.p, self.d, self.out = prefix + "head/", d, out
-    self.prefixes = (self.p,)
-
-  def specs(self):
-    return [E.ParamSpec(self.p + "kernel", (self.d, self.out), E.lecun_normal(self.d)),
-            E.ParamSpec(self.p + "bias", (self.out,), E.zeros)], []
-
-  def fwd(self, P, x, geom, save=True):
-    out = ops.gemm(x, P.h(self.p + "kernel"), b_mn=True, bias=P.f(self.p + "bias"), out_dtype=torch.float32)
-    return out, (x if save else None)
-
-  def bwd(self, P, dout, x, geom, sink=None, need_dx=True):
-    d16 = common.to16(dout)
-    ops.colsum(dout, P.g(self.p + "bias"))
-    ops.gemm(x, d16, a_mn=True, b_mn=True, out=P.g(self.p + "kernel"), reduce_out=True)
-    return ops.gemm(d16, P.h(self.p + "kernel")) if need_dx else None
 
 
 # pool_type -> vit.NormPool's pool ("map": encoder_norm alone, then the MAP head stage)
@@ -95,32 +68,20 @@ class _Model(E.Staged):
     if self.pool_type not in _POOLS:
       raise NotImplementedError(f"Cannot do pooling '{self.pool_type}'")
     vit.check_head_dim(self.width, self.num_heads)
-    self.prefix = p = (self.name + "/") if self.name else ""
-    d, enc = self.width, p + "Encoder_0/"
-    # the backward stages, bottom-up (engine.Staged)
-    self._stages = ([_Embed(p, d)]
-                    + vit.encoder_stages(enc, self.depth, d, self.mlp_dim, self.num_heads, self.scan, self.remat_policy)
-                    + [vit.NormPool(enc + "encoder_norm/", d, _POOLS[self.pool_type], torch.bfloat16)])
-    if self.pool_type == "map":
-      self._stages.append(_MAPHead(p + "MAPHead_0/", d, self.mlp_dim, self.num_heads))
-    if self.num_classes:
-      self._stages.append(_Head(p, d, self.num_classes))
-    self._len = None
+    self.prefix = (self.name + "/") if self.name else ""
 
   def specs(self, text_len):
-    self._len = text_len
-    d, p = self.width, self.prefix
-    specs = [
-        # flax nn.Embed default init: variance_scaling(1.0, "fan_in", "normal", out_axis=0)
-        E.ParamSpec(p + "Embed_0/embedding", (self.vocab_size, d), E.normal(1 / math.sqrt(d))),
-        E.ParamSpec(p + "pos_embedding", (1, text_len, d), E.normal(1 / math.sqrt(d))),
-    ]
-    aliases = []
-    for stage in self._stages[1:]:
-      s, a = stage.specs()
-      specs += s
-      aliases += a
-    return specs, aliases
+    """Builds the backward stages for [n, text_len] token ids -> (specs, aliases)."""
+    p, d, enc = self.prefix, self.width, self.prefix + "Encoder_0/"
+    # bottom-up; the pools and the MAP head output bf16
+    stages = ([_Embed(p, self.vocab_size, text_len, d)]
+              + vit.encoder_stages(enc, self.depth, d, self.mlp_dim, self.num_heads, self.scan, self.remat_policy)
+              + [vit.NormPool(enc + "encoder_norm/", d, _POOLS[self.pool_type], torch.bfloat16)])
+    if self.pool_type == "map":
+      stages.append(vit.MAPHead(p + "MAPHead_0/", d, self.mlp_dim, self.num_heads, torch.bfloat16))
+    if self.num_classes:    # text_transformer.py:97-98
+      stages.append(common.Dense(p + "head/", d, self.num_classes, E.lecun_normal(d), dx_dtype=torch.bfloat16))
+    return self._build(stages)
 
   def init(self, seed, text_shape, device="cuda"):
     specs, aliases = self.specs(text_shape[1])

@@ -377,10 +377,12 @@ class NormPool(E.Stage):
 
 
 class MAPHead(E.Stage):
-  """Multihead attention pooling (models/vit.py:163-183)."""
+  """Multihead attention pooling (models/vit.py:163-183).  Its MLP writes fp32; with out_dtype bf16 (the
+  text tower's) the output is cast to bf16, and the backward casts the bf16 output gradient to fp32
+  before it proceeds as for an fp32 output."""
 
-  def __init__(self, prefix, d, m, heads):
-    self.p, self.d, self.m, self.heads = prefix, d, m, heads
+  def __init__(self, prefix, d, m, heads, out_dtype=torch.float32):
+    self.p, self.d, self.m, self.heads, self.out_dtype = prefix, d, m, heads, out_dtype
     self.att = prefix + "MultiHeadDotProductAttention_0/"
     self.prefixes = (prefix,)
 
@@ -405,15 +407,19 @@ class MAPHead(E.Stage):
     a = ops.gemm(o.view(n, d), P.h(self.att + "out_proj/kernel"), b_mn=True, bias=P.f(self.att + "out/bias"))
     y, mean, rstd = ops.layernorm_fwd(a, P.f(self.p + "LayerNorm_0/scale"), P.f(self.p + "LayerNorm_0/bias"))
     out, mlp_saved = mlp_fwd(Scope(P, self.p + "MlpBlock_0/"), y, a, out_dtype=torch.float32, save=save)
+    if self.out_dtype != torch.float32:
+      out = ops.cast(out, torch.empty_like(out, dtype=self.out_dtype))
     if not save:
       return out, None
     return out, (enc, qn, kv, o, lse, a, mean, rstd, mlp_saved)
 
   def bwd(self, P, dout, saved, geom, sink=None, need_dx=True):
-    """dout fp32 [n,d] -> d(enc) bf16 [n*N, d] (None with need_dx=False)."""
+    """dout [n,d] in out_dtype -> d(enc) bf16 [n*N, d] (None with need_dx=False)."""
     n, N = geom.n, geom.N
     d = self.d
     enc, qn, kv, o, lse, a, mean, rstd, mlp_saved = saved
+    if self.out_dtype != torch.float32:
+      dout = ops.cast(dout, torch.empty_like(dout, dtype=torch.float32))
     dout16 = ops.cast(dout, torch.empty_like(dout, dtype=torch.bfloat16))
     dy = mlp_bwd(Scope(P, self.p + "MlpBlock_0/"), dout16, mlp_saved, want_bias2_grad=True)
     da = ops.layernorm_bwd(dy, a, P.f(self.p + "LayerNorm_0/scale"), mean, rstd, dres=dout16,
@@ -442,21 +448,24 @@ class MAPHead(E.Stage):
 
 
 class PatchEmbedding(E.Stage):
-  """The patch embedding (models/vit.py:212-225): a Dense over flattened patches, stored under
-  `prefix + name`, with the position embedding added in its epilogue, then [cls] prepended when `cls`.
-  posemb=None adds no position embedding: the MLP-Mixer's stem (models/mlp_mixer.py:72)."""
+  """The patch embedding (models/vit.py:212-225) of [n, *image_hw, in_ch] images: a Dense over flattened
+  patches, stored under `prefix + name`, with the position embedding added in its epilogue, then [cls]
+  prepended when `cls`.  posemb=None adds no position embedding: the MLP-Mixer's stem
+  (models/mlp_mixer.py:72).  `tokens`: the output's tokens per image."""
 
-  def __init__(self, prefix, name, patch_size, d, posemb, cls):
-    self.p, self.patch_size, self.d, self.posemb, self.cls = prefix, patch_size, d, posemb, cls
+  def __init__(self, prefix, name, image_hw, patch_size, in_ch, d, posemb, cls):
+    self.p, self.patch_size, self.in_ch, self.d, self.posemb, self.cls = prefix, patch_size, in_ch, d, posemb, cls
+    self.grid = (image_hw[0] // patch_size[0], image_hw[1] // patch_size[1])
+    self.tokens = self.grid[0] * self.grid[1] + cls
     self.w = prefix + name + "/"
     self.prefixes = ((self.w,) + ((prefix + "pos_embedding",) if posemb == "learn" else ())
                      + ((prefix + "cls",) if cls else ()))
     self._sincos = None
 
-  def specs(self, tokens, in_ch):
+  def specs(self):
     """The kernel is stored flattened [ph*pw*in_ch, d] (the im2col column order), padded to a multiple
     of 8 rows, and exposed under `kernel` as [ph, pw, in_ch, d]."""
-    (ph, pw), d, w = self.patch_size, self.d, self.w
+    (ph, pw), (gh, gw), d, w, in_ch = self.patch_size, self.grid, self.d, self.w, self.in_ch
     K = ph * pw * in_ch
     Kp = (K + 7) // 8 * 8
     lec = E.lecun_normal(K)   # flax Conv default kernel_init, fan_in = ph*pw*C
@@ -465,17 +474,16 @@ class PatchEmbedding(E.Stage):
              E.ParamSpec(w + "bias", (d,), E.zeros)]
     aliases = [E.Alias(w + "kernel", w + "kernel_flat", lambda t: t[:K].unflatten(0, (ph, pw, in_ch)))]
     if self.posemb == "learn":
-      specs.append(E.ParamSpec(self.p + "pos_embedding", (1, tokens, d), E.normal(1 / math.sqrt(d))))
+      specs.append(E.ParamSpec(self.p + "pos_embedding", (1, gh * gw, d), E.normal(1 / math.sqrt(d))))
     if self.cls:
       specs.append(E.ParamSpec(self.p + "cls", (1, 1, d), E.zeros))
     return specs, aliases
 
-  def _posemb16(self, P, image):
+  def _posemb16(self, P):
     if self.posemb == "learn":
       return P.h(self.p + "pos_embedding").view(-1, self.d)
     if self._sincos is None or self._sincos.device != P.device:
-      (ph, pw), (H, W) = self.patch_size, image.shape[1:3]
-      self._sincos = torch.from_numpy(posemb_sincos_2d(H // ph, W // pw, self.d)).to(P.device).bfloat16()
+      self._sincos = torch.from_numpy(posemb_sincos_2d(*self.grid, self.d)).to(P.device).bfloat16()
     return self._sincos
 
   def fwd(self, P, image, geom, save=True):
@@ -484,7 +492,7 @@ class PatchEmbedding(E.Stage):
     patches = ops.patchify(image, self.patch_size[0])
     if self.posemb:
       x = ops.gemm(patches, P.h(w + "kernel_flat"), b_mn=True, bias=P.f(w + "bias"),
-                   aux=self._posemb16(P, image), aux_row_mod=N0, epilogue=L.EPI_BIAS_RESID)
+                   aux=self._posemb16(P), aux_row_mod=N0, epilogue=L.EPI_BIAS_RESID)
     else:
       x = ops.gemm(patches, P.h(w + "kernel_flat"), b_mn=True, bias=P.f(w + "bias"))
     saved = patches if save else None
@@ -520,32 +528,6 @@ class PatchEmbedding(E.Stage):
     ops.gemm(patches, dx, a_mn=True, b_mn=True, out=P.g(self.w + "kernel_flat"), reduce_out=True)
 
 
-class PreLogits(E.Stage):
-  """pre_logits: tanh(Dense(x)) (models/vit.py:258-265), fp32 output."""
-
-  def __init__(self, prefix, d, rep):
-    self.p, self.d, self.rep = prefix + "pre_logits/", d, rep
-    self.prefixes = (self.p,)
-
-  def specs(self):
-    return [E.ParamSpec(self.p + "kernel", (self.d, self.rep), E.lecun_normal(self.d)),
-            E.ParamSpec(self.p + "bias", (self.rep,), E.zeros)], []
-
-  def fwd(self, P, x, geom, save=True):
-    pre = ops.gemm(common.to16(x), P.h(self.p + "kernel"), b_mn=True, bias=P.f(self.p + "bias"),
-                   out_dtype=torch.float32)
-    y = ops.tanh_fwd(pre)
-    return y, ((x, y) if save else None)
-
-  def bwd(self, P, dy, saved, geom, sink=None, need_dx=True):
-    x, y = saved
-    dpre = ops.tanh_bwd(dy, y)
-    d16 = common.to16(dpre)
-    ops.colsum(dpre, P.g(self.p + "bias"))
-    ops.gemm(common.to16(x), d16, a_mn=True, b_mn=True, out=P.g(self.p + "kernel"), reduce_out=True)
-    return ops.gemm(d16, P.h(self.p + "kernel"), out_dtype=torch.float32) if need_dx else None
-
-
 # ------------------------------------------------------------------------------------------
 # the model
 # ------------------------------------------------------------------------------------------
@@ -578,41 +560,26 @@ class _Model(E.Staged):
       raise ValueError(f"Unknown pool type: '{self.pool_type}'")
     check_head_dim(self.width, self.num_heads)
     self.mlp = self.mlp_dim or 4 * self.width
-    self.prefix = p = (self.name + "/") if self.name else ""
-    d, enc = self.width, p + "Transformer/"
-    rep = (d if self.rep_size is True else self.rep_size) if self.rep_size else d
-    self.head = None
-    if self.num_classes:
-      self.head = common.ClassifierHead(p, rep, self.num_classes, E.zeros if self.head_zeroinit else E.lecun_normal(rep))
-    # the backward stages, bottom-up (engine.Staged); parameterless pools belong to no stage of their own
-    self._stages = ([PatchEmbedding(p, "embedding", self.patch_size, d, self.posemb, self.pool_type == "tok")]
-                    + encoder_stages(enc, self.depth, d, self.mlp, self.num_heads, self.scan, self.remat_policy)
-                    + [NormPool(enc + "encoder_norm/", d, _POOLS[self.pool_type], torch.float32)])
-    if self.pool_type == "map":
-      self._stages.append(MAPHead(p + "MAPHead_0/", d, self.mlp, self.num_heads))
-    if self.rep_size:
-      self._stages.append(PreLogits(p, d, rep))
-    if self.head is not None:
-      self._stages.append(self.head)
-    self._geom = None
+    self.prefix = (self.name + "/") if self.name else ""
 
   # ---- parameters ------------------------------------------------------------------------
-  def setup(self, image_hw):
-    ph, pw = self.patch_size
-    H, W = image_hw
-    self._geom = (H // ph, W // pw)
-    return self
-
-  def specs(self, image_hw=None, in_ch=3):
-    if image_hw is not None:
-      self.setup(image_hw)
-    gh, gw = self._geom
-    specs, aliases = self._stages[0].specs(gh * gw, in_ch)
-    for stage in self._stages[1:]:
-      s, a = stage.specs()
-      specs += s
-      aliases += a
-    return specs, aliases
+  def specs(self, image_hw, in_ch=3):
+    """Builds the backward stages for [n, *image_hw, in_ch] images -> (specs, aliases)."""
+    p, d, enc = self.prefix, self.width, self.prefix + "Transformer/"
+    rep = (d if self.rep_size is True else self.rep_size) if self.rep_size else d
+    head_init = E.zeros if self.head_zeroinit else E.lecun_normal(rep)
+    self.head = common.Dense(p + "head/", rep, self.num_classes, head_init, pad=True) if self.num_classes else None
+    # bottom-up; parameterless pools belong to no stage of their own
+    embed = PatchEmbedding(p, "embedding", image_hw, self.patch_size, in_ch, d, self.posemb, self.pool_type == "tok")
+    stages = ([embed] + encoder_stages(enc, self.depth, d, self.mlp, self.num_heads, self.scan, self.remat_policy)
+              + [NormPool(enc + "encoder_norm/", d, _POOLS[self.pool_type], torch.float32)])
+    if self.pool_type == "map":
+      stages.append(MAPHead(p + "MAPHead_0/", d, self.mlp, self.num_heads))
+    if self.rep_size:   # models/vit.py:258-265
+      stages.append(common.Dense(p + "pre_logits/", d, rep, E.lecun_normal(d), tanh=True))
+    if self.head is not None:
+      stages.append(self.head)
+    return self._build(stages)
 
   def init(self, seed, image_shape, device="cuda"):
     """Counterpart of model.init(rng, zeros_image)["params"] (train.py:195-205)."""
@@ -621,17 +588,13 @@ class _Model(E.Staged):
 
   # ---- forward / backward ----------------------------------------------------------------
   def fwd(self, P, image, frozen=None):
-    """image [n,H,W,C] fp32 in [-1,1] -> (x fp32 [n, out], saved).  With a class head whose storage is
-    padded (common.ClassifierHead) x is the [n, num_classes] view of the padded logits.
+    """image [n,H,W,C] fp32 in [-1,1] (the shape given to specs()) -> (x fp32 [n, out], saved).  With a
+    class head whose storage is padded (common.Dense) x is the [n, num_classes] view of the padded logits.
 
     `frozen`: storage names that receive no gradient (optax.Chain.frozen()), or True for all of them
     (inference).  Stages below the cut (see cut()) run forward-only and save nothing; the output is
     bit-identical either way."""
-    if self._geom is None:
-      self.setup(image.shape[1:3])
-    n = image.shape[0]
-    gh, gw = self._geom
-    N = gh * gw + (self.pool_type == "tok")
+    n, N = image.shape[0], self._stages[0].tokens
     out, saved = self._stages_fwd(P, image, E.Geom(n, N), frozen)
     if self.pool_type == "none":
       # no pooling (models/vit.py:252-253): pre_logits / head run on every token, out is [n, N, .]
@@ -642,7 +605,7 @@ class _Model(E.Staged):
 
   def bwd(self, P, dout, saved):
     """dout: fp32 [n, out] ([n, N, out] without pooling).  Accumulates parameter gradients into P.grad.
-    With a padded class head, out is the padded class count (ClassifierHead.bwd)."""
+    With a padded class head, out is the padded class count (common.Dense.bwd)."""
     if self.pool_type == "none":
       geom = saved["geom"]
       dout = dout.reshape(geom.n * geom.N, -1)

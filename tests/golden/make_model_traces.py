@@ -29,9 +29,12 @@ GOLDEN = os.path.join(HERE, "model_traces.json.gz")
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 sys.path.insert(0, os.path.dirname(HERE))
 
-# ViT: every pool, with and without scan and pre_logits, a padded 37-class head; sin-cos posemb with scan
-VIT_MODELS = [dict(pool_type=pool, scan=scan, rep_size=rep, posemb="sincos2d" if scan else "learn")
-              for pool in ("gap", "map", "tok", "0", "none") for scan in (False, True) for rep in (False, 32)]
+# ViT: every pool, with and without scan and pre_logits, a padded 37-class head; sin-cos posemb with scan.
+# Then every pool without a class head: pre_logits or the pooled encoder output is the model's output.
+VIT_MODELS = ([dict(pool_type=pool, scan=scan, rep_size=rep, posemb="sincos2d" if scan else "learn")
+               for pool in ("gap", "map", "tok", "0", "none") for scan in (False, True) for rep in (False, 32)]
+              + [dict(pool_type=pool, rep_size=rep, num_classes=None)
+                 for pool in ("gap", "map", "tok", "0", "none") for rep in (False, 32)])
 # name -> regex of the TRAINED storage names (everything else is frozen); None: nothing frozen
 VIT_SCHEDULES = {
     "all": None,
@@ -147,7 +150,8 @@ def vit_models():
   from big_vision_b200 import engine as E
   from big_vision_b200.models import vit
   for kw in VIT_MODELS:
-    model = vit.Model(37, width=64, depth=3, mlp_dim=128, num_heads=1, patch_size=(16, 16), **kw)
+    model = vit.Model(**{"num_classes": 37, "width": 64, "depth": 3, "mlp_dim": 128, "num_heads": 1,
+                         "patch_size": (16, 16), **kw})
     P = E.FlatParams(*model.specs((32, 32), 3), "cpu")
     yield "vit " + " ".join(f"{k}={v}" for k, v in kw.items()), model, P
 
@@ -195,8 +199,8 @@ def vit_traces(patch):
       def step():
         y, saved = model.fwd(P, image, frozen=frozen)
         nbytes = saved_bytes(saved, P, image)
-        rows = y.shape[:-1]
-        model.bwd(P, torch.zeros(rows + (model.head.Cp,)), saved)
+        cols = y.shape[-1] if model.head is None else model.head.Cp
+        model.bwd(P, torch.zeros(y.shape[:-1] + (cols,)), saved)
         return nbytes
       lines, nbytes = _run(P, patch, step)
       out[f"{tag} / {sched}"] = {"calls": lines, "saved_bytes": nbytes}

@@ -1,9 +1,9 @@
 """CPU: what the ViT, two-tower and MLP-Mixer models launch, where they accumulate and what they keep.
 
 The models run on CPU tensors with the C-ABI call replaced by a recorder (tests/golden/make_model_traces.py)
-over every pool, with and without scan, the Mixer with and without token padding and stochastic-depth
-masks, under the freezing schedules that place the backward's cut on each kind of stage, and under
-apply().  The traces must equal the committed ones call for call: every entry point, scalar argument and
+over every pool, with and without scan, the ViT with and without a class head, the Mixer with and without
+token padding and stochastic-depth masks, under the freezing schedules that place the backward's cut on
+each kind of stage, and under apply().  The traces must equal the committed ones call for call: every entry point, scalar argument and
 argument-struct field, every parameter pointer, the P.on_ready calls and the bytes kept for the backward.
 So must each configuration's parameter layout and the checksum of its seed-0 init."""
 import difflib

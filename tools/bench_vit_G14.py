@@ -1,7 +1,7 @@
 """ViT-G/14 classification pre-training step (configs/proj/scaling_laws/train_vit_g.py with its one-line
 switch to `G/14`): 224x224, MAP pool, the 29,593-class JFT head, sigmoid_xent, BV-Adafactor, per-block
 recompute.  Head dim 104 (1664 / 16) and a class count that is not a multiple of 8, so the head is
-stored padded (models/common.py ClassifierHead).  1,930.4 M parameters: the flat fp32 parameter and
+stored padded (models/common.py Dense, pad=True).  1,930.4 M parameters: the flat fp32 parameter and
 gradient buffers are 7.2 GiB each.
 
 Registers `scaling_laws_vit_G14` into bench.WORKLOADS and sets bench.OPT_CONFIG to the config's
