@@ -1,0 +1,115 @@
+"""CPU: every entry point of include/bv_b200.h is named here with the GPU test(s) that check it directly
+against a reference of the same operation (not only through a whole-model test, whose tolerances are far
+too loose to pin one kernel).  A new ABI function without such a test, or a table row that names a test
+that does not exist, fails this file on a machine without a GPU."""
+import ast
+import os
+import re
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+TESTS = os.path.join(ROOT, "tests")
+
+# entry points with nothing to compute on the device
+EXEMPT = {"bv_version", "bv_device_supported", "bv_last_error_string"}
+
+KE = "test_kernel_edges_gpu"
+KG = "test_kernels_gpu"
+COVERAGE = {
+    "bv_gemm": [f"{KG}::test_dense_forward_epilogues", f"{KG}::test_dense_backward_contractions",
+                "test_gemm_aux_tma_gpu::test_resid_matches_fp32_oracle",
+                f"{KE}::test_gemm_gelu_epilogues_over_every_bf16_input",
+                f"{KE}::test_resid_epilogue_position_embedding_periods"],
+    "bv_layernorm_fwd": [f"{KG}::test_layernorm", f"{KG}::test_layernorm_constant_rows_hit_the_variance_clamp"],
+    "bv_layernorm_bwd": [f"{KG}::test_layernorm"],
+    "bv_attention_fwd": ["test_head_dim_gpu::test_head_dim_64_through_hd_entry_points_is_bitwise_the_old_path"],
+    "bv_attention_fwd_hd": [f"{KG}::test_attention_forward_backward", "test_head_dim_gpu::test_forward_matches_fp64"],
+    "bv_attention_bwd": ["test_head_dim_gpu::test_head_dim_64_through_hd_entry_points_is_bitwise_the_old_path"],
+    "bv_attention_bwd_hd": [f"{KG}::test_attention_forward_backward",
+                            "test_attention_bwd_split_gpu::test_backward_matches_fp64"],
+    "bv_patchify": [f"{KG}::test_patchify_embed_pool_l2norm", f"{KE}::test_patchify_layout_and_zero_pad"],
+    "bv_patchify_u8": [f"{KG}::test_patchify_u8_fuses_value_range_bit_exactly",
+                       f"{KE}::test_patchify_layout_and_zero_pad"],
+    "bv_embed_fwd": [f"{KE}::test_embed_fwd_and_bwd"],
+    "bv_embed_bwd": [f"{KE}::test_embed_fwd_and_bwd"],
+    "bv_colsum": [f"{KE}::test_colsum", f"{KE}::test_colsum_of_the_patch_embedding_view"],
+    "bv_cast": [f"{KE}::test_cast_both_directions_bit_exact"],
+    "bv_l2norm_fwd": [f"{KE}::test_l2norm"],
+    "bv_l2norm_bwd": [f"{KE}::test_l2norm"],
+    "bv_pool_fwd": [f"{KE}::test_pool_fwd_mean", f"{KE}::test_pool_token_mode_and_pool_bwd"],
+    "bv_pool_bwd": [f"{KE}::test_pool_token_mode_and_pool_bwd"],
+    "bv_pool_max_bwd": [f"{KG}::test_patchify_embed_pool_l2norm"],
+    "bv_broadcast_row": [f"{KE}::test_broadcast_row"],
+    "bv_tanh_fwd": [f"{KE}::test_standalone_gelu_and_tanh_over_every_bf16_input"],
+    "bv_tanh_bwd": [f"{KE}::test_standalone_gelu_and_tanh_over_every_bf16_input"],
+    "bv_gelu_fwd": [f"{KE}::test_standalone_gelu_and_tanh_over_every_bf16_input"],
+    "bv_mixup": ["test_classifier_gpu::test_mixup_kernel_is_bit_exact",
+                 "test_class_count_gpu::test_mixup_scalar_path_is_bit_exact"],
+    "bv_axpby": [f"{KE}::test_axpby"],
+    "bv_concat_cls": [f"{KE}::test_concat_and_drop_cls_bit_exact"],
+    "bv_drop_cls": [f"{KE}::test_concat_and_drop_cls_bit_exact"],
+    "bv_transpose_tokens": [f"{KG}::test_token_transposes_are_exact"],
+    "bv_untranspose_add": [f"{KG}::test_token_transposes_are_exact"],
+    "bv_row_select": [f"{KE}::test_row_select_bit_exact"],
+    "bv_siglip_loss": [f"{KG}::test_siglip_loss_slab", f"{KE}::test_siglip_loss_elementwise"],
+    "bv_softmax_contrastive_loss": [f"{KG}::test_softmax_contrastive_slab",
+                                    f"{KE}::test_softmax_contrastive_at_batch_6144"],
+    "bv_sigmoid_xent": ["test_class_count_gpu::test_xent_ld_with_ld_C_gives_the_bits_of_the_plain_entry_point"],
+    "bv_softmax_xent": ["test_class_count_gpu::test_xent_ld_with_ld_C_gives_the_bits_of_the_plain_entry_point"],
+    "bv_sigmoid_xent_ld": [f"{KG}::test_classification_losses", f"{KE}::test_classification_losses_wide_logits"],
+    "bv_softmax_xent_ld": [f"{KG}::test_classification_losses", f"{KE}::test_classification_losses_wide_logits"],
+    "bv_adam_step": [f"{KG}::test_adam_matches_optax_chain", f"{KE}::test_adam_step_state_and_norms"],
+    "bv_sumsq": [f"{KE}::test_sumsq"],
+    "bv_scale_step": [f"{KE}::test_scale_step_state_and_norms"],
+    "bv_adafactor_step": ["test_optax_gpu::test_adafactor_matches_oracle"],
+    "bv_top1": ["test_eval_paths::test_top1_matches_oracle", "test_eval_paths::test_top1_nan_and_zero_shot"],
+    "bv_retrieval_ranks": ["test_eval_paths::test_retrieval_ranks_match_stable_argsort",
+                           "test_eval_paths::test_retrieval_golden_on_device"],
+}
+
+
+def _header_functions():
+  """The same parse as test_abi.py: every `bv_name(` outside comments."""
+  src = open(os.path.join(ROOT, "include", "bv_b200.h")).read()
+  src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
+  return sorted(set(re.findall(r"\b(bv_[a-z0-9_]+)\s*\(", src)))
+
+
+def _is_gpu_mark(dec):
+  """`pytest.mark.gpu` (bare or called)."""
+  if isinstance(dec, ast.Call):
+    dec = dec.func
+  return isinstance(dec, ast.Attribute) and dec.attr == "gpu"
+
+
+def _gpu_tests():
+  """module::name of every top-level test function in tests/*_gpu.py, and of those marked gpu in
+  tests/test_eval_paths.py."""
+  out = set()
+  for fn in sorted(os.listdir(TESTS)):
+    mod, ext = os.path.splitext(fn)
+    if ext != ".py" or not (mod.endswith("_gpu") or mod == "test_eval_paths"):
+      continue
+    tree = ast.parse(open(os.path.join(TESTS, fn)).read())
+    for node in tree.body:
+      if isinstance(node, ast.FunctionDef) and node.name.startswith("test_"):
+        if mod == "test_eval_paths" and not any(_is_gpu_mark(d) for d in node.decorator_list):
+          continue
+        out.add(f"{mod}::{node.name}")
+  return out
+
+
+def test_table_keys_are_exactly_the_header_entry_points():
+  declared = set(_header_functions()) - EXEMPT
+  assert len(declared) >= 40
+  missing, extra = declared - set(COVERAGE), set(COVERAGE) - declared
+  assert not missing, f"entry points without a direct GPU test in COVERAGE: {sorted(missing)}"
+  assert not extra, f"COVERAGE rows for functions the header does not declare: {sorted(extra)}"
+
+
+def test_every_named_test_exists_as_a_gpu_test():
+  known = _gpu_tests()
+  assert len(known) > 50
+  for fn, tests in COVERAGE.items():
+    assert tests, fn
+    for t in tests:
+      assert t in known, f"{fn}: {t} is not a GPU test function in tests/"

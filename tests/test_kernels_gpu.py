@@ -95,32 +95,125 @@ def test_gemm_is_linear_at_full_size(ops):
   assert torch.equal(s1[rows], a1[rows].float() @ w.float())
 
 
-@pytest.mark.parametrize("rows,d", [(1000, 768), (77, 384), (513, 1024), (9, 64),
-                                    (5000, 768), (4099, 320), (4500, 1024)])   # >= 4096 rows: streaming kernels
+U32 = 2.0 ** -24
+
+
+def _ulp(ref, dtype):
+  """Spacing of `dtype` at |ref| (fp64), floored at the spacing of the smallest normal number."""
+  e = torch.floor(torch.log2(ref.abs().clamp_min(2.0 ** -126)))
+  return torch.exp2(e - (7 if dtype == torch.bfloat16 else 23))
+
+
+def _check(got, ref, bound, what):
+  """Element-wise |got - ref| <= bound (the bound of each element, not a fraction of the tensor max)."""
+  got, ref = got.detach().double(), ref.detach().double().to(got.device)
+  bound = torch.as_tensor(bound, dtype=F64, device=got.device).expand_as(ref)
+  assert not torch.isnan(got).any(), what
+  err = (got - ref).abs()
+  ok = err <= bound
+  if not bool(ok.all()):
+    i = tuple((~ok).nonzero()[0].tolist())
+    raise AssertionError(f"{what}: {int((~ok).sum())} of {ok.numel()} elements out of bound; first at {i}: "
+                         f"got {got[i].item()!r} ref {ref[i].item()!r} bound {bound[i].item():.3e}")
+
+
+# widths of every model (Ti 192, mu 32, So400m 1152, H 1280, g 1408, g-opt / G-opt 1536, G 1664, e 1792,
+# the 2048 limit; 264 and 1032 leave one chunk in the last register slot) on both sides of the 4096 rows
+# where the bf16 streaming kernels take over (nch = d / 256 <= 4; the generic kernels at every nch)
+_LN_CASES = ([(1000, 768), (77, 384), (513, 1024), (9, 64), (5000, 768), (4099, 320), (4500, 1024)] +
+             [(r, d) for d in (32, 192, 264, 1032, 1152, 1280, 1408, 1536, 1664, 1792, 2048) for r in (777, 4100)])
+
+
+@pytest.mark.parametrize("rows,d", _LN_CASES)
 def test_layernorm(ops, rows, d):
-  g = torch.Generator().manual_seed(rows)
-  x = _bf(torch.randn(rows, d, generator=g) * 2 + 0.5)
-  sc = torch.randn(d, generator=g) * 0.2 + 1
-  bi = torch.randn(d, generator=g) * 0.1
-  dy = _bf(torch.randn(rows, d, generator=g))
-  dres = _bf(torch.randn(rows, d, generator=g))
-  xr = x.double().requires_grad_(True)
-  sr, br = sc.double().requires_grad_(True), bi.double().requires_grad_(True)
-  yr = O.layer_norm(xr, sr, br)
-  yr.backward(dy.double())
-  y, mean, rstd = ops.layernorm_fwd(x.cuda(), sc.cuda(), bi.cuda())
-  _close(y, yr, 2 ** -7)
-  y32, _, _ = ops.layernorm_fwd(x.cuda(), sc.cuda(), bi.cuda(), out_dtype=torch.float32)
-  _close(y32, yr, 1e-5)
-  ds, db, cs = (torch.zeros(d, device="cuda") for _ in range(3))
-  dx = ops.layernorm_bwd(dy.cuda(), x.cuda(), sc.cuda(), mean, rstd, dres=dres.cuda(), dscale=ds,
-                         dbias=db, dx_colsum=cs)
-  _close(dx, xr.grad + dres.double(), 2 ** -7)
-  _close(ds, sr.grad, 1e-4)
-  _close(db, br.grad, 1e-4)
-  # column sums of dx: the streaming kernel sums the fp32 values, the generic one the stored bf16
-  # values; both are within bf16 rounding noise (~2^-9 / 3) of the exact column sums
-  _close(cs, (xr.grad + dres.double()).sum(0), 3e-3)
+  """Forward and backward for x, y, dy, dx in bf16 and fp32, with and without dres, and each of dscale,
+  dbias, dx_colsum absent in one case; rows offset from zero by up to 16 standard deviations (a
+  residual stream) and scales away from 1.  Element-wise bounds against fp64:
+    * mean and rstd: the summation bound of the fast variance E[x^2] - E[x]^2, chain 8 nch + 6 per lane;
+    * y and dx: 1 ulp of the output dtype at the fp64 value computed from the kernel's own mean and
+      rstd, plus the fp32 roundings of the formula propagated per element (and, for y, 2^-21 of the
+      row's output scale);
+    * dscale, dbias, dx_colsum (accumulated into non-zero initial values): the summation bound over
+      the per-warp strips, the shared-memory and global atomics."""
+  g = torch.Generator(device="cuda").manual_seed(rows * 7 + d)
+  dev = "cuda"
+  sig = torch.rand(rows, 1, generator=g, device=dev) * 1.5 + 0.5
+  off = (torch.rand(rows, 1, generator=g, device=dev) * 32 - 16) * sig
+  x32 = torch.randn(rows, d, generator=g, device=dev) * sig + off
+  sc = torch.randn(d, generator=g, device=dev) * 0.5 + 1.5
+  bi = torch.randn(d, generator=g, device=dev) * 0.3
+  nch = -(-(d // 8) // 32)
+  sms = torch.cuda.get_device_properties(0).multi_processor_count
+  S, Bi = sc.double(), bi.double()
+  stats = {}
+  for xdt in (torch.bfloat16, torch.float32):
+    x = x32.to(xdt)
+    X = x.double()
+    c = 8 * nch + 6
+    m_ref = X.mean(1)
+    e2 = (X * X).mean(1)
+    dmean = c * U32 * X.abs().mean(1) + 2 * U32 * m_ref.abs()
+    dvar = (c + 1) * U32 * e2 + 2 * U32 * e2 + 2 * m_ref.abs() * dmean + 3 * U32 * m_ref * m_ref
+    var = torch.clamp(e2 - m_ref * m_ref, min=0)
+    for ydt in (torch.bfloat16, torch.float32):
+      y, mean, rstd = ops.layernorm_fwd(x, sc, bi, out_dtype=ydt)
+      _check(mean, m_ref, dmean, f"mean x {xdt}")
+      r_ref = torch.rsqrt(var + 1e-6)
+      _check(rstd, r_ref, r_ref * (0.5 * dvar / (var + 1e-6) + 6 * U32), f"rstd x {xdt}")
+      M, R = mean.double()[:, None], rstd.double()[:, None]
+      xh = (X - M) * R
+      yref = xh * S + Bi
+      # the fp32 roundings of each element's formula, and 2^-21 of the row's output scale
+      noise = U32 * (4 * (xh * S).abs() + yref.abs() + Bi.abs()) + 2.0 ** -21 * yref.abs().amax(1, keepdim=True)
+      _check(y, yref, _ulp(yref, ydt) + noise, f"y x {xdt} y {ydt}")
+    stats[xdt] = (x, mean, rstd)
+
+  # longest accumulation chain of dscale / dbias / dx_colsum: a warp's rows (at least min(rows, 8 * sms)
+  # warps share them), one shared atomic per warp (<= 12), one global atomic per block (<= 2 * sms), init
+  chain = -(-rows // min(rows, 8 * sms)) + 12 + 2 * sms + 2
+  bf = torch.bfloat16
+  cases = [(bf, bf, bf, True, ("dscale", "dbias", "dx_colsum")),
+           (bf, bf, bf, False, ("dbias", "dx_colsum")),
+           (bf, torch.float32, torch.float32, True, ("dscale", "dx_colsum")),
+           (torch.float32, bf, torch.float32, False, ("dscale", "dbias"))]
+  for dydt, xdt, dxdt, has_res, sums in cases:
+    what = f"dy {dydt} x {xdt} dx {dxdt} dres {has_res}"
+    x, mean, rstd = stats[xdt]
+    dy = torch.randn(rows, d, generator=g, device=dev).to(dydt)
+    dres = torch.randn(rows, d, generator=g, device=dev).to(dxdt) if has_res else None
+    init = {k: torch.randn(d, generator=g, device=dev) for k in sums}
+    acc = {k: v.clone() for k, v in init.items()}
+    dx = ops.layernorm_bwd(dy, x, sc, mean, rstd, dres=dres, dx_dtype=dxdt, dscale=acc.get("dscale"),
+                           dbias=acc.get("dbias"), dx_colsum=acc.get("dx_colsum"))
+    X, DY = x.double(), dy.double()
+    M, R = mean.double()[:, None], rstd.double()[:, None]
+    xh = (X - M) * R
+    dxh = U32 * (2 * (X.abs() + M.abs()) * R + xh.abs())        # fp32 x * rstd - mean * rstd
+    gy = DY * S
+    c1, c2 = gy.mean(1, keepdim=True), (gy * xh).mean(1, keepdim=True)
+    cl = 8 * nch + 6
+    dc1 = cl * U32 * gy.abs().mean(1, keepdim=True)
+    dc2 = cl * U32 * (gy * xh).abs().mean(1, keepdim=True) + (gy.abs() * dxh).mean(1, keepdim=True)
+    core = R * (gy - c1 - xh * c2)
+    ref = core + (dres.double() if has_res else 0)
+    noise = R * (4 * U32 * (gy.abs() + c1.abs() + (xh * c2).abs()) + dc1 + xh.abs() * dc2 + dxh * c2.abs()) + \
+        2 * U32 * ref.abs()
+    bound = _ulp(ref, dxdt) + noise
+    _check(dx, ref, bound, f"dx {what}")
+    if "dscale" in sums:
+      t = DY * xh
+      _check(acc["dscale"], init["dscale"].double() + t.sum(0),
+             chain * U32 * (init["dscale"].double().abs() + t.abs().sum(0)) + (DY.abs() * dxh).sum(0),
+             f"dscale {what}")
+    if "dbias" in sums:
+      _check(acc["dbias"], init["dbias"].double() + DY.sum(0),
+             chain * U32 * (init["dbias"].double().abs() + DY.abs().sum(0)), f"dbias {what}")
+    if "dx_colsum" in sums:
+      # the generic kernel sums the stored dx, the bf16 streaming one the fp32 values before rounding:
+      # either is within `bound` of ref per element
+      _check(acc["dx_colsum"], init["dx_colsum"].double() + ref.sum(0),
+             chain * U32 * (init["dx_colsum"].double().abs() + ref.abs().sum(0)) + bound.sum(0),
+             f"dx_colsum {what}")
 
 
 def test_layernorm_constant_rows_hit_the_variance_clamp(ops):
