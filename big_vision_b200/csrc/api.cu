@@ -1,5 +1,6 @@
-// extern "C" surface of libbv_b200.so (see include/bv_b200.h).
+// extern "C" surface of libbv_b200.so (see include/bv_b200.h and include/bv_b200_sam.h).
 #include "../../include/bv_b200.h"
+#include "../../include/bv_b200_sam.h"
 
 #include "host_utils.h"
 #include "kernels.h"
@@ -228,6 +229,18 @@ int bv_top1(const void* logits, int logits_dtype, int64_t rows, int32_t C, int64
 int bv_retrieval_ranks(const float* dist, int64_t NI, int64_t NT, int64_t ld, const int32_t* corr,
                        int32_t* rank_t2i, int32_t* rank_i2t, void* stream) {
   return launch_retrieval_ranks(dist, NI, NT, ld, corr, rank_t2i, rank_i2t, S(stream));
+}
+
+int bv_sam_perturb(const float* w, const float* g, const float* g_sumsq, float rho, float eps, int32_t adaptive,
+                   float* w_out, void* w_bf16, int64_t n, void* stream) {
+  return launch_sam_perturb(w, g, g_sumsq, rho, eps, adaptive, w_out, w_bf16, n, S(stream));
+}
+int bv_sam_dots(const float* a, const float* b, float* out, float* ws, int64_t n, void* stream) {
+  return launch_sam_dots(a, b, out, ws, n, S(stream));
+}
+int bv_gsam_combine(float* g_clean, const float* g_robust, const float* dot, const float* norm_sq, float alpha,
+                    int32_t minimize_fp, int64_t n, void* stream) {
+  return launch_gsam_combine(g_clean, g_robust, dot, norm_sq, alpha, minimize_fp, n, S(stream));
 }
 
 }  // extern "C"

@@ -139,4 +139,11 @@ int launch_scale_step(float* params, const float* grads, void* params_bf16, int6
                       float grad_mult, float clip_norm, const float* gnorm_sq, float* upd_sq,
                       float* param_sq, cudaStream_t s);
 
+// ---- GSAM / SAM vector algebra (sam.cu; C ABI in include/bv_b200_sam.h)
+int launch_sam_perturb(const float* w, const float* g, const float* g_sumsq, float rho, float eps, int adaptive,
+                       float* w_out, void* w_bf16, int64_t n, cudaStream_t s);
+int launch_sam_dots(const float* a, const float* b, float* out, float* ws, int64_t n, cudaStream_t s);
+int launch_gsam_combine(float* gc, const float* gr, const float* dot, const float* norm_sq, float alpha,
+                        int minimize_fp, int64_t n, cudaStream_t s);
+
 }  // namespace bv

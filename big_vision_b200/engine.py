@@ -71,6 +71,19 @@ class FlatParams:
     self.half = torch.zeros(self.total, dtype=torch.bfloat16, device=self.device)
     self._views = {}
 
+  def twin(self):
+    """A second parameter set with the same specs, aliases and flat layout but its own zeroed `flat`,
+    `grad` and `half` buffers (10 bytes per element): model code runs on it unchanged, e.g. on the
+    perturbed weights of a GSAM / SAM step."""
+    t = object.__new__(FlatParams)
+    t.specs, t.aliases, t.device = self.specs, self.aliases, self.device
+    t.offsets, t.n_decay, t.total = self.offsets, self.n_decay, self.total
+    t.flat = torch.zeros_like(self.flat)
+    t.grad = torch.zeros_like(self.grad)
+    t.half = torch.zeros_like(self.half)
+    t._views = {}
+    return t
+
   # ---- raw views ------------------------------------------------------------------
   def _view(self, buf, name):
     off, shape = self.offsets[name]

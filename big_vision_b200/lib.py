@@ -110,6 +110,14 @@ SIGNATURES = {
     "bv_device_supported": [],
 }
 
+# include/bv_b200_sam.h (GSAM / SAM), one to one; exported from the same library
+SAM_SIGNATURES = {
+    "bv_sam_perturb": [c_vp, c_vp, c_vp, c_f32, c_f32, c_i32, c_vp, c_vp, c_i64, c_vp],
+    "bv_sam_dots": [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp],
+    "bv_gsam_combine": [c_vp, c_vp, c_vp, c_vp, c_f32, c_i32, c_i64, c_vp],
+}
+SAM_WS_FLOATS = 2048       # BV_SAM_WS_FLOATS
+
 _lib = None
 
 
@@ -127,7 +135,7 @@ def load():
         f"{LIB_PATH} not found: build it with `python -m big_vision_b200.build` "
         "(there is no CPU or eager fallback for the kernels).")
   lib = ctypes.CDLL(LIB_PATH)
-  for name, argtypes in SIGNATURES.items():
+  for name, argtypes in {**SIGNATURES, **SAM_SIGNATURES}.items():
     fn = getattr(lib, name)   # raises AttributeError if the symbol is missing
     fn.argtypes = argtypes
     fn.restype = ctypes.c_int
@@ -147,7 +155,7 @@ def check(rc, what):
 LAUNCHES = [0]
 _LAUNCHES_PER_CALL = {"bv_embed_bwd": 2, "bv_retrieval_ranks": 2, "bv_siglip_loss": 2,
                       "bv_sigmoid_xent": 2, "bv_softmax_xent": 2, "bv_sigmoid_xent_ld": 2, "bv_softmax_xent_ld": 2,
-                      "bv_softmax_contrastive_loss": 2, "bv_adafactor_step": 4}
+                      "bv_softmax_contrastive_loss": 2, "bv_adafactor_step": 4, "bv_sam_dots": 2}
 LOSS_WS_FLOATS = 8192      # BV_LOSS_WS_FLOATS
 
 

@@ -430,6 +430,45 @@ def adafactor_step(P, tens, st, *, decay, eps, beta, lr_eff, wd_eff, grad_mult, 
   L.call("bv_adafactor_step", ctypes.byref(args), _stream())
 
 
+# ---- GSAM / SAM (include/bv_b200_sam.h) --------------------------------------------------------
+def _flat32(*ts):
+  for t in ts:
+    if t.dtype != torch.float32 or not t.is_contiguous():
+      raise L.BvError(f"GSAM kernels take contiguous fp32 buffers, got {t.dtype}")
+
+
+def sam_perturb(w, g, g_sumsq, rho, eps=1e-12, adaptive=False, out=None, out_bf16=None):
+  """out = w + rho * g / (sqrt(g_sumsq) + eps) (times |w| with `adaptive`) and its bf16 shadow, in one pass;
+  g_sumsq is a device scalar [1].  Returns (out, out_bf16)."""
+  _flat32(w, g)
+  out = torch.empty_like(w) if out is None else out
+  out_bf16 = torch.empty(w.shape, dtype=torch.bfloat16, device=w.device) if out_bf16 is None else out_bf16
+  assert out.numel() == out_bf16.numel() == g.numel() == w.numel() and out_bf16.dtype == torch.bfloat16
+  L.call("bv_sam_perturb", _p(w), _p(g), _p(g_sumsq), float(rho), float(eps), int(bool(adaptive)), _p(out),
+         _p(out_bf16), w.numel(), _stream())
+  return out, out_bf16
+
+
+def sam_dots(a, b, out=None, ws=None):
+  """out [2] fp32 on the device = (a . b, b . b), summed in a fixed order (run-to-run identical)."""
+  _flat32(a, b)
+  assert a.numel() == b.numel()
+  out = torch.empty(2, dtype=torch.float32, device=b.device) if out is None else out
+  ws = torch.empty(L.SAM_WS_FLOATS, dtype=torch.float32, device=b.device) if ws is None else ws
+  L.call("bv_sam_dots", _p(a), _p(b), _p(out), _p(ws), b.numel(), _stream())
+  return out
+
+
+def gsam_combine(g_clean, g_robust, dot, norm_sq, alpha, minimize_fp=True):
+  """The GSAM gradient, in place over g_clean; dot = g_c . g_r and norm_sq (||g_r||^2 with minimize_fp,
+  else ||g_c||^2) are device scalars [1]."""
+  _flat32(g_clean, g_robust)
+  assert g_clean.numel() == g_robust.numel()
+  L.call("bv_gsam_combine", _p(g_clean), _p(g_robust), _p(dot), _p(norm_sq), float(alpha), int(bool(minimize_fp)),
+         g_clean.numel(), _stream())
+  return g_clean
+
+
 # ---- integer evaluation paths -------------------------------------------------------------------
 def top1(logits, labels=None, mask=None, want_idx=True):
   """argmax over classes (+ label gather and masked counts).  Returns (idx int32 [rows] or None,
