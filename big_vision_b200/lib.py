@@ -118,6 +118,16 @@ SAM_SIGNATURES = {
 }
 SAM_WS_FLOATS = 2048       # BV_SAM_WS_FLOATS
 
+# include/bv_b200_distill.h (distillation), one to one; exported from the same library
+DISTILL_SIGNATURES = {
+    "bv_distill_loss": [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i32, c_f32, c_f32, c_i32, c_vp, c_i64, c_vp, c_vp,
+                        c_i64, c_i32, c_vp],
+    "bv_distance": [c_vp, c_i64, c_vp, c_i64, c_i32, c_f32, c_f32, c_f32, c_i32, c_vp, c_i64, c_i32, c_vp],
+}
+# BV_DIST_*: the kinds of dist(); BV_DISTILL_*: the outputs of bv_distill_loss, in order
+DIST_KINDS = {"euclidean": 0, "l2": 1, "hard": 2, "kl": 3, "logsoftmax_euclidean": 4, "agree": 5}
+DISTILL_OUTPUTS = ("distance", "entropy_student", "entropy_teacher", "task_loss_student", "task_loss_teacher")
+
 _lib = None
 
 
@@ -135,7 +145,7 @@ def load():
         f"{LIB_PATH} not found: build it with `python -m big_vision_b200.build` "
         "(there is no CPU or eager fallback for the kernels).")
   lib = ctypes.CDLL(LIB_PATH)
-  for name, argtypes in {**SIGNATURES, **SAM_SIGNATURES}.items():
+  for name, argtypes in {**SIGNATURES, **SAM_SIGNATURES, **DISTILL_SIGNATURES}.items():
     fn = getattr(lib, name)   # raises AttributeError if the symbol is missing
     fn.argtypes = argtypes
     fn.restype = ctypes.c_int
@@ -155,7 +165,8 @@ def check(rc, what):
 LAUNCHES = [0]
 _LAUNCHES_PER_CALL = {"bv_embed_bwd": 2, "bv_retrieval_ranks": 2, "bv_siglip_loss": 2,
                       "bv_sigmoid_xent": 2, "bv_softmax_xent": 2, "bv_sigmoid_xent_ld": 2, "bv_softmax_xent_ld": 2,
-                      "bv_softmax_contrastive_loss": 2, "bv_adafactor_step": 4, "bv_sam_dots": 2}
+                      "bv_softmax_contrastive_loss": 2, "bv_adafactor_step": 4, "bv_sam_dots": 2,
+                      "bv_distill_loss": 2}
 LOSS_WS_FLOATS = 8192      # BV_LOSS_WS_FLOATS
 
 

@@ -469,6 +469,52 @@ def gsam_combine(g_clean, g_robust, dot, norm_sq, alpha, minimize_fp=True):
   return g_clean
 
 
+# ---- distillation (include/bv_b200_distill.h) ------------------------------------------------------
+def _logits2d(*ts):
+  for t in ts:
+    if t is not None and (t.dtype != torch.float32 or t.dim() != 2 or t.stride(1) != 1):
+      raise L.BvError(f"distillation kernels take fp32 [n, C] matrices with a contiguous last axis, got "
+                      f"{t.dtype} {tuple(t.shape)} {t.stride()}")
+
+
+def distill_loss(student, teacher, labels=None, kind="kl", t=1.0, ls=0.0, dlogits=None, dlogits_cols=None,
+                 want_grad=True):
+  """One teacher's term of the distillation loss on logits [n, C] (row-strided views allowed).
+
+  Returns (out, rows, dlogits): out fp32 [5] on the device, the batch means named by L.DISTILL_OUTPUTS
+  (distance, the entropies of student and teacher, their task losses against `labels`, 0 without labels),
+  summed in a fixed order; rows [5, n], the same per example; dlogits [n, dlogits_cols or C] =
+  d distance / d student, zero in the columns past C.  Passing `dlogits` (a previous teacher's) adds to it."""
+  _logits2d(student, teacher, labels, dlogits)
+  if kind not in L.DIST_KINDS:
+    raise ValueError(f"Unknown kind of distance {kind}.")
+  n, C = student.shape
+  assert teacher.shape == student.shape and (labels is None or labels.shape == student.shape)
+  accumulate = dlogits is not None
+  if want_grad and dlogits is None:
+    dlogits = torch.empty((n, dlogits_cols or C), dtype=torch.float32, device=student.device)
+  out = torch.empty(len(L.DISTILL_OUTPUTS), dtype=torch.float32, device=student.device)
+  rows = torch.empty((len(L.DISTILL_OUTPUTS), n), dtype=torch.float32, device=student.device)
+  L.call("bv_distill_loss", _p(student), student.stride(0), _p(teacher), teacher.stride(0), _p(labels),
+         labels.stride(0) if labels is not None else 0, L.DIST_KINDS[kind], float(t), float(ls), int(accumulate),
+         _p(dlogits), dlogits.stride(0) if dlogits is not None else 0, _p(out), _p(rows), n, C, _stream())
+  return out, rows, dlogits
+
+
+def distance(student, teacher, kind, epsilon=1e-12, t=1.0, ls=0.0, k=1):
+  """dist() of evaluators/proj/distill/distance.py per row of student / teacher [n, C]: fp32 [n], int32 [n]
+  for `agree`."""
+  _logits2d(student, teacher)
+  if kind not in L.DIST_KINDS:
+    raise ValueError(f"Unknown kind of distance {kind}.")
+  n, C = student.shape
+  assert teacher.shape == student.shape
+  out = torch.empty(n, dtype=torch.int32 if kind == "agree" else torch.float32, device=student.device)
+  L.call("bv_distance", _p(student), student.stride(0), _p(teacher), teacher.stride(0), L.DIST_KINDS[kind],
+         float(epsilon), float(t), float(ls), int(k), _p(out), n, C, _stream())
+  return out
+
+
 # ---- integer evaluation paths -------------------------------------------------------------------
 def top1(logits, labels=None, mask=None, want_idx=True):
   """argmax over classes (+ label gather and masked counts).  Returns (idx int32 [rows] or None,

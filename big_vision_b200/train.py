@@ -15,35 +15,45 @@ from big_vision_b200.trainers.proj.image_text.siglip import Dist
 _LOSSES = {"sigmoid_xent": ops.sigmoid_xent, "softmax_xent": ops.softmax_xent}
 
 
-def loss_and_grads(model, P, images, labels, loss_name="sigmoid_xent", dist_view=None, frozen=None, **fwd_kw):
-  """value_and_grad(loss_fn)(params) of train.py:295-303 on this rank's shard; P.grad holds the
-  LOCAL gradient of the LOCAL-mean loss (callers average across ranks).
+def fwd_loss_bwd(model, P, images, loss_grad, dist_view=None, frozen=None, **fwd_kw):
+  """Forward, `loss_grad`, backward on this rank's shard; P.grad holds the LOCAL gradient (callers average
+  across ranks).  `loss_grad(flat, ld) -> dlogits [rows, ld]` gets the logits as [rows, classes] (row
+  stride ld) and returns d loss / d logits with zeros in the columns past `classes`; the loss itself is
+  its own business.  Returns the logits.
 
   `frozen` (storage names, optax.Chain.frozen()): parameters that get no gradient.  The model's backward
   stages below the lowest trained one run forward-only -- a linear probe (`head/.*` trained, the
   rest None) runs the backbone without a backward -- and the all-reduce covers the trained ranges only."""
-  if loss_name not in _LOSSES:
-    raise NotImplementedError(f"loss {loss_name}")
   ranges = None
   if frozen:
     fwd_kw["frozen"] = frozen
     ranges = P.trained_ranges(frozen)
   P.zero_grad()
   logits, saved = model.fwd(P, images, **fwd_kw)
-  loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
   # unpooled models (pool_type="none") give [n, N, classes]: the losses sum over the class axis and
   # average over all leading axes (utils.py:236-243,276-281), i.e. over the n*N rows.  A head with
   # padded storage returns a view of [rows, Cp] logits; the gradient is written [rows, Cp] with zero
   # padding columns, the layout the head's backward GEMMs take.
   flat = logits.reshape(-1, logits.shape[-1])
   ld = flat.stride(0)
-  dlogits = _LOSSES[loss_name](flat, labels.reshape(flat.shape), loss, dlogits_cols=ld)
-  dlogits = dlogits.view(*logits.shape[:-1], ld)
+  dlogits = loss_grad(flat, ld).view(*logits.shape[:-1], ld)
   if dist_view is None:
     model.bwd(P, dlogits, saved)
   else:      # gradient all-reduce (SUM; callers divide by world) overlapped with the backward
     from big_vision_b200.trainers.proj.image_text.siglip import all_reduce_grads
     all_reduce_grads(P, dist_view, lambda: model.bwd(P, dlogits, saved), ranges=ranges)
+  return logits
+
+
+def loss_and_grads(model, P, images, labels, loss_name="sigmoid_xent", dist_view=None, frozen=None, **fwd_kw):
+  """value_and_grad(loss_fn)(params) of train.py:295-303 on this rank's shard, the LOCAL-mean loss
+  (fwd_loss_bwd)."""
+  if loss_name not in _LOSSES:
+    raise NotImplementedError(f"loss {loss_name}")
+  loss = torch.zeros(1, dtype=torch.float32, device=images.device)
+  logits = fwd_loss_bwd(
+      model, P, images, lambda flat, ld: _LOSSES[loss_name](flat, labels.reshape(flat.shape), loss, dlogits_cols=ld),
+      dist_view, frozen, **fwd_kw)
   return loss, logits
 
 
