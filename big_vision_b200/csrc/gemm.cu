@@ -188,22 +188,24 @@ __device__ __forceinline__ void colsum_add(float* colsum, int N, float s0, float
 }
 
 // Epilogue straight from the registers: fp32 outputs, and bf16 reduce-add outputs (gradient
-// accumulation; never with colsum).
+// accumulation; never with colsum).  Under split-K every unit adds its partial into D, so bias and a
+// residual are added only by the unit of the first split (kb0 == 0); gelu' scales every partial.
 template <int BN, bool OUT_F32, int EF>
 __device__ __forceinline__ void epilogue_regs(const GemmDev& p, const float (&acc)[BN / 2], int m0, int n0,
-                                              int cw) {
+                                              int cw, int kb0) {
   const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
   const int row0 = m0 + cw * 64 + warp * 16 + (lane >> 2);
   const int pM = p.M, pN = p.N;
   const float alpha = p.alpha;
   const bool reduce = p.reduce_out != 0;
+  const bool first = kb0 == 0;
 #pragma unroll
   for (int j = 0; j < BN / 8; ++j) {
     const int col = n0 + 8 * j + 2 * (lane & 3);
     if (col >= pN) continue;
     const bool pair = col + 1 < pN;
     float b0 = 0.f, b1 = 0.f;
-    if (p.bias != nullptr) {
+    if (p.bias != nullptr && first) {
       b0 = __ldg(p.bias + col);
       if (pair) b1 = __ldg(p.bias + col + 1);
     }
@@ -212,7 +214,7 @@ __device__ __forceinline__ void epilogue_regs(const GemmDev& p, const float (&ac
       const int row = row0 + 8 * h;
       if (row >= pM) continue;
       float v0, v1, pre0, pre1, a0 = 0.f, a1 = 0.f;
-      if (EF == EF_RESID || EF == EF_DGELU) aux_global(p, row, col, pair, a0, a1);
+      if ((EF == EF_RESID && first) || EF == EF_DGELU) aux_global(p, row, col, pair, a0, a1);
       epi_math<OUT_F32, EF>(alpha, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], b0, b1, a0, a1, v0, v1, pre0, pre1);
       if (OUT_F32) {
         float* dp = static_cast<float*>(p.d) + row * p.ldd + col;
@@ -237,7 +239,10 @@ __device__ __forceinline__ void epilogue_regs(const GemmDev& p, const float (&ac
 // Epilogue through shared memory for plain bf16 outputs: the warpgroup writes each 64-column
 // sub-tile of its 64 rows into a 128B-swizzled staging buffer (the 16-byte chunk index XOR the row
 // mod 8, so the 8 rows of one store instruction hit different banks), and one thread stores it with
-// TMA, which clips rows >= M and columns >= N.
+// TMA, which clips rows >= M and columns >= N8 = N rounded down to a multiple of 8.  TMA writes the
+// innermost dimension in whole 16-byte chunks, so a map of width N with N % 8 != 0 would write the
+// chunk's columns N .. round_up(N, 8) - 1 of a strided output; the N % 8 columns past N8 are copied
+// from the staging buffer by the threads instead.
 //
 // Without a TMA-loaded aux the two buffers alternate; `nstore` counts the warpgroup's sub-tiles across
 // units, and the issuing thread waits until the store that last read a buffer is done reading before
@@ -254,7 +259,7 @@ __device__ __forceinline__ void epilogue_tma(const GemmDev& p, const CUtensorMap
   const bool leader = (threadIdx.x & 127) == 0;
   const int rl0 = warp * 16 + (lane >> 2);       // row within the warpgroup's 64
   const int row0 = m0 + cw * 64 + rl0;
-  const int pM = p.M, pN = p.N;
+  const int pM = p.M, pN = p.N, pN8 = p.N & ~7;
   const float alpha = p.alpha;
 #pragma unroll
   for (int c = 0; c < BN / 64; ++c) {
@@ -316,11 +321,30 @@ __device__ __forceinline__ void epilogue_tma(const GemmDev& p, const CUtensorMap
     fence_proxy_async();
     named_bar_sync(1 + cw, 128);
     if (leader) {
-      if (n0 + 64 * c < pN && m0 + cw * 64 < pM) {      // sub-tiles wholly past the edge are not stored
+      if (n0 + 64 * c < pN8 && m0 + cw * 64 < pM) {     // sub-tiles wholly past N8 are not stored
         tma_store_2d(tmD, buf, n0 + 64 * c, m0 + cw * 64);
         if (EF == EF_GELU) tma_store_2d(tmD2, buf + SUB_BYTES, n0 + 64 * c, m0 + cw * 64);
       }
       tma_store_commit();
+    }
+    // The sub-tile holding the partial chunk (N % 8 != 0): its N - N8 columns go from the staging
+    // buffer to global memory here, one row of D (and of D2) per thread.  The branch is uniform over
+    // the warpgroup, and its barrier keeps the buffer from being refilled before every read is done.
+    const int tail0 = pN8 - (n0 + 64 * c);
+    if (pN8 < pN && tail0 >= 0 && tail0 < 64) {
+      const int t = threadIdx.x & 127, rl = t & 63, out = t >> 6;
+      const int row = m0 + cw * 64 + rl;
+      if (row < pM && (out == 0 || EF == EF_GELU)) {
+        const uint32_t src = buf + out * SUB_BYTES + rl * 128 + (((tail0 >> 3) ^ (rl & 7)) << 4);
+        uint16_t* dst = reinterpret_cast<uint16_t*>(out ? p.d2 : p.d) + row * (out ? p.ldd2 : p.ldd) + pN8;
+#pragma unroll 1
+        for (int e = 0; e < pN - pN8; ++e) {
+          uint16_t u;
+          asm volatile("ld.shared.u16 %0, [%1];" : "=h"(u) : "r"(src + 2 * e));
+          dst[e] = u;
+        }
+      }
+      named_bar_sync(1 + cw, 128);
     }
     if (!AUX_TMA) ++nstore;
     if (p.colsum != nullptr) {
@@ -445,7 +469,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
     if constexpr (OM == OM_BF16_TMA)
       epilogue_tma<BN, EF, C::BUF_BYTES>(p, &tmD, &tmD2, acc, w.m0, w.n0, cw, staging, nstore, aux_bar, nunit & 1u);
-    else epilogue_regs<BN, OM == OM_F32, EF>(p, acc, w.m0, w.n0, cw);
+    else epilogue_regs<BN, OM == OM_F32, EF>(p, acc, w.m0, w.n0, cw, w.kb0);
   }
   // the staging buffers must outlive every bulk store that reads them
   if (OM == OM_BF16_TMA && (threadIdx.x & 127) == 0) tma_store_wait<0>();
@@ -474,23 +498,25 @@ int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
   p.M = (int)g.M; p.N = (int)g.N;
   p.a_mn = g.a_mn; p.b_mn = g.b_mn; p.reduce_out = g.reduce_out;
   p.alpha = g.alpha;
-  p.bias = g.bias;
+  p.bias = g.epi == EPI_NONE ? nullptr : g.bias;     // EPI_NONE ignores bias (bv_b200.h)
   p.colsum = g.colsum;
   p.aux = reinterpret_cast<const bf16*>(g.aux);
   p.ldaux = g.ldaux;
   p.aux_row_mod = g.aux_row_mod;
   p.d = g.D; p.d2 = g.D2;
   p.ldd = g.ldd; p.ldd2 = g.ldd2;
-  // the output maps span exactly M x N, so TMA leaves the rows past M and the columns past N of a
-  // strided output alone
+  // the output maps span M x N8 (N rounded down to a multiple of 8; epilogue_tma stores the columns
+  // past N8 with plain stores), so TMA leaves the rows past M and the columns past N of a strided
+  // output alone.  With N < 8 there is no map: every column is stored that way.
   memset(&tmD, 0, sizeof(tmD));
   memset(&tmD2, 0, sizeof(tmD2));
   memset(&tmAux, 0, sizeof(tmAux));
-  if (OM == OM_BF16_TMA) {
-    rc = make_tmap_2d(&tmD, bf, g.D, g.N, g.M, g.ldd * 2, 64, 64);
+  const long long n8 = g.N & ~7LL;
+  if (OM == OM_BF16_TMA && n8 > 0) {
+    rc = make_tmap_2d(&tmD, bf, g.D, n8, g.M, g.ldd * 2, 64, 64);
     if (rc) return rc;
     if (EF == EF_GELU) {
-      rc = make_tmap_2d(&tmD2, bf, g.D2, g.N, g.M, g.ldd2 * 2, 64, 64);
+      rc = make_tmap_2d(&tmD2, bf, g.D2, n8, g.M, g.ldd2 * 2, 64, 64);
       if (rc) return rc;
     }
   }

@@ -38,7 +38,7 @@ extern "C" {
 #define BV_BF16 1
 
 /* GEMM epilogues */
-#define BV_EPI_NONE 0        /* D = alpha*acc                                        */
+#define BV_EPI_NONE 0        /* D = alpha*acc  (bias, if given, is ignored)          */
 #define BV_EPI_BIAS 1        /* D = alpha*acc + bias[n]                              */
 #define BV_EPI_BIAS_GELU 2   /* D2 = bf16(alpha*acc + bias); D = gelu_tanh(D2)       */
 #define BV_EPI_BIAS_RESID 3  /* D = bf16(alpha*acc + bias) + aux[m (% aux_row_mod), n] */
@@ -66,7 +66,11 @@ int bv_device_supported(void);
  *     dgrad    dX = dY W^T: A=dY (a_mn=0), B=W[K,N] read as [N'=K rows, K'=N] (b_mn=0)
  *     wgrad    dW = X^T dY: A=X (a_mn=1), B=dY (b_mn=1), out fp32, reduce_out=1
  *   reduce_out : 1 = accumulate into D with atomic adds (split-K / grad accumulation)
- *   splits     : 0 = auto, >1 only with reduce_out
+ *   splits     : 0 = auto (more than one split only with reduce_out, once K >= 2048), >1 only
+ *                with reduce_out.  Under split-K each split's partial goes through the epilogue,
+ *                is rounded to the output dtype and added into D on its own, in no fixed order;
+ *                bias and the BIAS_RESID aux are added once (by the first split), DGELU's
+ *                gelu'(aux) scales every partial.
  *   block_n    : 0 = auto, else 128 or 256
  *   bias (fp32 [N]) and aux (bf16) must be readable up to round_up(N, 8) columns.
  * --------------------------------------------------------------------------------- */

@@ -14,18 +14,28 @@ EXEMPT = {"bv_version", "bv_device_supported", "bv_last_error_string"}
 
 KE = "test_kernel_edges_gpu"
 KG = "test_kernels_gpu"
+GE = "test_gemm_elementwise_gpu"
+AE = "test_attention_elementwise_gpu"
 COVERAGE = {
     "bv_gemm": [f"{KG}::test_dense_forward_epilogues", f"{KG}::test_dense_backward_contractions",
                 "test_gemm_aux_tma_gpu::test_resid_matches_fp32_oracle",
                 f"{KE}::test_gemm_gelu_epilogues_over_every_bf16_input",
-                f"{KE}::test_resid_epilogue_position_embedding_periods"],
+                f"{KE}::test_resid_epilogue_position_embedding_periods",
+                f"{GE}::test_tier1_exact", f"{GE}::test_tier2_bound", f"{GE}::test_colsum_of_the_stored_output",
+                f"{GE}::test_split_k_adds_bias_once"],
     "bv_layernorm_fwd": [f"{KG}::test_layernorm", f"{KG}::test_layernorm_constant_rows_hit_the_variance_clamp"],
     "bv_layernorm_bwd": [f"{KG}::test_layernorm"],
-    "bv_attention_fwd": ["test_head_dim_gpu::test_head_dim_64_through_hd_entry_points_is_bitwise_the_old_path"],
-    "bv_attention_fwd_hd": [f"{KG}::test_attention_forward_backward", "test_head_dim_gpu::test_forward_matches_fp64"],
-    "bv_attention_bwd": ["test_head_dim_gpu::test_head_dim_64_through_hd_entry_points_is_bitwise_the_old_path"],
+    "bv_attention_fwd": ["test_head_dim_gpu::test_head_dim_64_through_hd_entry_points_is_bitwise_the_old_path",
+                         f"{AE}::test_dh64_entry_points_match_the_hd_entry_points"],
+    "bv_attention_fwd_hd": [f"{KG}::test_attention_forward_backward", "test_head_dim_gpu::test_forward_matches_fp64",
+                            f"{AE}::test_zero_queries_average_every_key_once",
+                            f"{AE}::test_dominant_key_gives_its_value",
+                            f"{AE}::test_forward_and_backward_within_bound"],
+    "bv_attention_bwd": ["test_head_dim_gpu::test_head_dim_64_through_hd_entry_points_is_bitwise_the_old_path",
+                         f"{AE}::test_dh64_entry_points_match_the_hd_entry_points"],
     "bv_attention_bwd_hd": [f"{KG}::test_attention_forward_backward",
-                            "test_attention_bwd_split_gpu::test_backward_matches_fp64"],
+                            "test_attention_bwd_split_gpu::test_backward_matches_fp64",
+                            f"{AE}::test_forward_and_backward_within_bound"],
     "bv_patchify": [f"{KG}::test_patchify_embed_pool_l2norm", f"{KE}::test_patchify_layout_and_zero_pad"],
     "bv_patchify_u8": [f"{KG}::test_patchify_u8_fuses_value_range_bit_exactly",
                        f"{KE}::test_patchify_layout_and_zero_pad"],
@@ -113,3 +123,10 @@ def test_every_named_test_exists_as_a_gpu_test():
     assert tests, fn
     for t in tests:
       assert t in known, f"{fn}: {t} is not a GPU test function in tests/"
+
+
+def test_gemm_and_attention_rows_name_an_element_wise_test():
+  """The GEMM and attention entry points are checked per element against fp64, not only against the
+  tensor maximum: each of their rows names a test of the element-wise files."""
+  for fn in ("bv_gemm", "bv_attention_fwd", "bv_attention_fwd_hd", "bv_attention_bwd", "bv_attention_bwd_hd"):
+    assert any(t.split("::")[0] in (GE, AE) for t in COVERAGE[fn]), fn
