@@ -31,7 +31,6 @@
 //   pair, which is cheaper than the HBM traffic of summing per-key-block dQ partials across CTAs.
 #include "common.cuh"
 #include "host_utils.h"
-#include "kernels.h"
 
 namespace bv {
 
@@ -536,7 +535,7 @@ int check_head_dim(int head_dim, const char* who) {
   return BV_ERR_UNSUPPORTED;
 }
 
-int check_attn(const AttnArgs& a, const char* who) {
+int check_attn(const bv_attn_args& a, const char* who) {
   if (a.B <= 0 || a.H <= 0 || a.Nq <= 0 || a.Nk <= 0 || a.Nq > 65536 || a.Nk > 65536) {
     set_error("%s: need 1 <= Nq,Nk <= 65536 and B,H >= 1 (got B=%lld H=%d Nq=%d Nk=%d)", who,
               (long long)a.B, a.H, a.Nq, a.Nk);
@@ -555,7 +554,7 @@ int check_attn(const AttnArgs& a, const char* who) {
 }
 
 template <int DH>
-int attention_fwd(const AttnArgs& a, cudaStream_t s) {
+int attention_fwd(const bv_attn_args& a, cudaStream_t s) {
   using G = Geo<DH>;
   int rc = check_attn(a, "bv_attention_fwd");
   if (rc) return rc;
@@ -580,9 +579,9 @@ int attention_fwd(const AttnArgs& a, cudaStream_t s) {
 }
 
 template <int DH>
-int attention_bwd(const AttnBwdArgs& g, cudaStream_t s) {
+int attention_bwd(const bv_attn_bwd_args& g, cudaStream_t s) {
   using G = Geo<DH>;
-  const AttnArgs& a = g.f;
+  const bv_attn_args& a = g.fwd;
   int rc = check_attn(a, "bv_attention_bwd");
   if (rc) return rc;
   if (a.lse == nullptr) { set_error("bv_attention_bwd: lse required"); return BV_ERR_INVALID; }
@@ -646,10 +645,19 @@ int attention_bwd(const AttnBwdArgs& g, cudaStream_t s) {
 }
 
 }  // namespace
+}  // namespace bv
 
-int launch_attention_fwd(const AttnArgs& a, int head_dim, cudaStream_t s) {
+extern "C" {
+
+int bv_attention_fwd(const bv_attn_args* args, void* stream) { return bv_attention_fwd_hd(args, 64, stream); }
+
+int bv_attention_fwd_hd(const bv_attn_args* args, int32_t head_dim, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!args) { set_error("bv_attention_fwd: null args"); return BV_ERR_INVALID; }
   int rc = check_head_dim(head_dim, "bv_attention_fwd");
   if (rc) return rc;
+  const bv_attn_args& a = *args;
   switch (head_dim) {
     case 72: return attention_fwd<72>(a, s);
     case 80: return attention_fwd<80>(a, s);
@@ -659,9 +667,16 @@ int launch_attention_fwd(const AttnArgs& a, int head_dim, cudaStream_t s) {
   }
 }
 
-int launch_attention_bwd(const AttnBwdArgs& g, int head_dim, cudaStream_t s) {
+int bv_attention_bwd(const bv_attn_bwd_args* args, void* stream) { return bv_attention_bwd_hd(args, 64, stream); }
+
+// args->dq_accum is ignored (kept for the struct layout)
+int bv_attention_bwd_hd(const bv_attn_bwd_args* args, int32_t head_dim, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!args) { set_error("bv_attention_bwd: null args"); return BV_ERR_INVALID; }
   int rc = check_head_dim(head_dim, "bv_attention_bwd");
   if (rc) return rc;
+  const bv_attn_bwd_args& g = *args;
   switch (head_dim) {
     case 72: return attention_bwd<72>(g, s);
     case 80: return attention_bwd<80>(g, s);
@@ -671,4 +686,4 @@ int launch_attention_bwd(const AttnBwdArgs& g, int head_dim, cudaStream_t s) {
   }
 }
 
-}  // namespace bv
+}  // extern "C"

@@ -4,7 +4,6 @@
 // Every kernel streams its operands once with 16-byte accesses where layout allows.
 #include "common.cuh"
 #include "host_utils.h"
-#include "kernels.h"
 
 namespace bv {
 namespace {
@@ -511,9 +510,14 @@ untranspose_add_kernel(const bf16* __restrict__ y, const bf16* __restrict__ res,
 int check_launch(const char* what) { return check_cuda(cudaGetLastError(), what); }
 
 }  // namespace
+}  // namespace bv
 
-int launch_patchify(const float* img, void* out, int64_t n, int H, int W, int C, int P,
-                    cudaStream_t s) {
+extern "C" {
+
+int bv_patchify(const float* img, void* out, int64_t n, int32_t H, int32_t W, int32_t C, int32_t P,
+                void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0 || P <= 0 || H % P || W % P || C <= 0) {
     set_error("bv_patchify: bad geometry n=%lld H=%d W=%d C=%d P=%d", (long long)n, H, W, C, P);
     return BV_ERR_INVALID;
@@ -525,8 +529,10 @@ int launch_patchify(const float* img, void* out, int64_t n, int H, int W, int C,
   return check_launch("patchify_kernel");
 }
 
-int launch_patchify_u8(const uint8_t* img, void* out, int64_t n, int H, int W, int C, int P, float vmin,
-                       float vmax, float in_min, float in_max, int clip, cudaStream_t s) {
+int bv_patchify_u8(const uint8_t* img, void* out, int64_t n, int32_t H, int32_t W, int32_t C, int32_t P,
+                   float vmin, float vmax, float in_min, float in_max, int32_t clip, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0 || P <= 0 || H % P || W % P || C <= 0 || !(in_max > in_min)) {
     set_error("bv_patchify_u8: need n > 0, H,W multiples of P, in_max > in_min");
     return BV_ERR_INVALID;
@@ -543,15 +549,19 @@ int launch_patchify_u8(const uint8_t* img, void* out, int64_t n, int H, int W, i
   return check_cuda(cudaGetLastError(), "patchify_u8_kernel launch");
 }
 
-int launch_embed_fwd(const int32_t* ids, const float* table, const float* pos, void* out,
-                     int out_dtype, int64_t n, int L, int d, int vocab, cudaStream_t s) {
+int bv_embed_fwd(const int32_t* ids, const float* table, const float* pos, void* out, int out_dtype,
+                 int64_t n, int32_t L, int32_t d, int32_t vocab, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (d % 4) { set_error("bv_embed_fwd: d %% 4 != 0"); return BV_ERR_INVALID; }
   embed_fwd_kernel<<<grid_for(n * L * (d / 4), 256, num_sms() * 16), 256, 0, s>>>(ids, table, pos, out,
                                                                          out_dtype, n, L, d, vocab);
   return check_launch("embed_fwd_kernel");
 }
-int launch_embed_bwd(const int32_t* ids, const void* dy, int dy_dtype, float* dtable, float* dpos,
-                     int64_t n, int L, int d, int vocab, cudaStream_t s) {
+int bv_embed_bwd(const int32_t* ids, const void* dy, int dy_dtype, float* dtable, float* dpos, int64_t n,
+                 int32_t L, int32_t d, int32_t vocab, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (dtable) {
     embed_bwd_table_kernel<<<grid_for(n * L * d, 256, num_sms() * 16), 256, 0, s>>>(ids, dy, dy_dtype,
                                                                            dtable, n, L, d, vocab);
@@ -566,8 +576,9 @@ int launch_embed_bwd(const int32_t* ids, const void* dy, int dy_dtype, float* dt
   return BV_OK;
 }
 
-int launch_colsum(const void* x, int x_dtype, float* out, int64_t rows, int64_t cols, int64_t ld,
-                  cudaStream_t s) {
+int bv_colsum(const void* x, int x_dtype, float* out, int64_t rows, int64_t cols, int64_t ld, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (cols % 8 || ld % 8 || (reinterpret_cast<uintptr_t>(x) & 15)) {
     set_error("bv_colsum: cols, ld must be multiples of 8 and x 16B aligned");
     return BV_ERR_INVALID;
@@ -579,71 +590,94 @@ int launch_colsum(const void* x, int x_dtype, float* out, int64_t rows, int64_t 
   return check_launch("colsum_kernel");
 }
 
-int launch_cast(const void* src, int sdt, void* dst, int ddt, int64_t n, cudaStream_t s) {
+int bv_cast(const void* src, int sdt, void* dst, int ddt, int64_t n, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return BV_OK;
   cast_kernel<<<grid_for(n / 4 + 1, 256, num_sms() * 16), 256, 0, s>>>(src, sdt, dst, ddt, n);
   return check_launch("cast_kernel");
 }
 
-int launch_l2norm_fwd(const void* x, int dt, float* z, float* norm, int64_t n, int d, float eps,
-                      cudaStream_t s) {
+int bv_l2norm_fwd(const void* x, int dt, float* z, float* norm, int64_t n, int32_t d, float eps,
+                  void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return BV_OK;
   l2norm_fwd_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(x, dt, z, norm, n, d, eps);
   return check_launch("l2norm_fwd_kernel");
 }
-int launch_l2norm_bwd(const float* dz, const float* z, const float* norm, void* dx, int dt,
-                      int64_t n, int d, float eps, cudaStream_t s) {
+int bv_l2norm_bwd(const float* dz, const float* z, const float* norm, void* dx, int dt, int64_t n, int32_t d,
+                  float eps, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return BV_OK;
   l2norm_bwd_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(dz, z, norm, dx, dt, n, d, eps);
   return check_launch("l2norm_bwd_kernel");
 }
 
-int launch_pool(const void* x, int xdt, void* y, int ydt, int64_t n, int N, int d, int mode,
-                int tok, cudaStream_t s) {
+int bv_pool_fwd(const void* x, int xdt, void* y, int ydt, int64_t n, int32_t N, int32_t d, int32_t mode,
+                int32_t tok, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (mode < 0 || mode > 2) { set_error("bv_pool: mode must be 0 (mean), 1 (token) or 2 (max)"); return BV_ERR_INVALID; }
   if (mode == 1 && (tok < 0 || tok >= N)) { set_error("bv_pool: token index out of range"); return BV_ERR_INVALID; }
   pool_fwd_kernel<<<grid_for(n * d, 256, num_sms() * 16), 256, 0, s>>>(x, xdt, y, ydt, n, N, d, mode, tok);
   return check_launch("pool_fwd_kernel");
 }
-int launch_pool_bwd(const void* dy, int ydt, void* dx, int xdt, int64_t n, int N, int d, int mode,
-                    int tok, cudaStream_t s) {
+int bv_pool_bwd(const void* dy, int ydt, void* dx, int xdt, int64_t n, int32_t N, int32_t d, int32_t mode,
+                int32_t tok, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (mode == 2) { set_error("bv_pool_bwd: the max pool needs its input, use bv_pool_max_bwd"); return BV_ERR_INVALID; }
   if (mode != 0 && (tok < 0 || tok >= N)) { set_error("bv_pool_bwd: token index out of range"); return BV_ERR_INVALID; }
   pool_bwd_kernel<<<grid_for(n * N * d, 256, num_sms() * 16), 256, 0, s>>>(dy, ydt, dx, xdt, n, N, d, mode, tok);
   return check_launch("pool_bwd_kernel");
 }
-int launch_pool_max_bwd(const void* dy, int ydt, const void* x, int xdt, void* dx, int dxdt, int64_t n,
-                        int N, int d, cudaStream_t s) {
+int bv_pool_max_bwd(const void* dy, int ydt, const void* x, int xdt, void* dx, int dxdt, int64_t n, int32_t N,
+                    int32_t d, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0 || N <= 0 || d <= 0) { set_error("bv_pool_max_bwd: empty problem"); return BV_ERR_INVALID; }
   pool_max_bwd_kernel<<<grid_for(n * d, 256, num_sms() * 16), 256, 0, s>>>(dy, ydt, x, xdt, dx, dxdt, n, N, d);
   return check_launch("pool_max_bwd_kernel");
 }
 
-int launch_add_rows(const void* x, int xdt, const float* row, void* y, int ydt, int64_t rows,
-                    int d, cudaStream_t s) {
+int bv_broadcast_row(const void* x, int xdt, const float* row, void* y, int ydt, int64_t rows, int32_t d,
+                     void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   // x holds a single row that is broadcast to `rows` rows (src_rows = 1)
   add_rows_kernel<<<grid_for(rows * d, 256, num_sms() * 16), 256, 0, s>>>(x, xdt, row, y, ydt, rows, d, 1);
   return check_launch("add_rows_kernel");
 }
 
-int launch_tanh_fwd(const void* x, void* y, int dt, int64_t n, cudaStream_t s) {
+int bv_tanh_fwd(const void* x, void* y, int dt, int64_t n, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   map_kernel<MAP_TANH><<<grid_for(n, 256, num_sms() * 16), 256, 0, s>>>(x, nullptr, y, dt, 0.f, 0.f, n);
   return check_launch("tanh_fwd");
 }
-int launch_tanh_bwd(const void* dy, const void* y, void* dx, int dt, int64_t n, cudaStream_t s) {
+int bv_tanh_bwd(const void* dy, const void* y, void* dx, int dt, int64_t n, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   map_kernel<MAP_TANH_BWD><<<grid_for(n, 256, num_sms() * 16), 256, 0, s>>>(dy, y, dx, dt, 0.f, 0.f, n);
   return check_launch("tanh_bwd");
 }
-int launch_gelu_fwd(const void* x, void* y, int dt, int64_t n, cudaStream_t s) {
+int bv_gelu_fwd(const void* x, void* y, int dt, int64_t n, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   map_kernel<MAP_GELU><<<grid_for(n, 256, num_sms() * 16), 256, 0, s>>>(x, nullptr, y, dt, 0.f, 0.f, n);
   return check_launch("gelu_fwd");
 }
-int launch_axpby(const void* x, const void* y, void* out, int dt, float a, float b, int64_t n,
-                 cudaStream_t s) {
+int bv_axpby(const void* x, const void* y, void* out, int dt, float a, float b, int64_t n, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   map_kernel<MAP_AXPBY><<<grid_for(n, 256, num_sms() * 16), 256, 0, s>>>(x, y, out, dt, a, b, n);
   return check_launch("axpby");
 }
-int launch_transpose_tokens(const void* x, void* y, int64_t n, int N, int d, cudaStream_t s) {
+int bv_transpose_tokens(const void* x, void* y, int64_t n, int32_t N, int32_t d, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0 || N <= 0 || d <= 0 || d % 8) { set_error("bv_transpose_tokens: need n,N,d > 0, d %% 8 == 0"); return BV_ERR_INVALID; }
   const int Np = (N + 7) / 8 * 8;
   dim3 grid((Np + TT - 1) / TT, (d + TT - 1) / TT, static_cast<unsigned>(n));
@@ -651,8 +685,10 @@ int launch_transpose_tokens(const void* x, void* y, int64_t n, int N, int d, cud
                                                       reinterpret_cast<bf16*>(y), N, d, Np);
   return check_launch("transpose_tokens_kernel");
 }
-int launch_untranspose_add(const void* y, const void* res, void* out, int64_t n, int N, int d,
-                           cudaStream_t s) {
+int bv_untranspose_add(const void* y, const void* res, void* out, int64_t n, int32_t N, int32_t d,
+                       void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0 || N <= 0 || d <= 0 || d % 8) { set_error("bv_untranspose_add: need n,N,d > 0, d %% 8 == 0"); return BV_ERR_INVALID; }
   const int Np = (N + 7) / 8 * 8;
   dim3 grid((N + TT - 1) / TT, (d + TT - 1) / TT, static_cast<unsigned>(n));
@@ -661,8 +697,10 @@ int launch_untranspose_add(const void* y, const void* res, void* out, int64_t n,
                                                      reinterpret_cast<bf16*>(out), N, d, Np);
   return check_launch("untranspose_add_kernel");
 }
-int launch_row_select(const void* a, const void* b, const float* mask, void* out, int64_t n, int N,
-                      int d, cudaStream_t s) {
+int bv_row_select(const void* a, const void* b, const float* mask, void* out, int64_t n, int32_t N, int32_t d,
+                  void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0 || N <= 0 || d <= 0 || d % 8) { set_error("bv_row_select: need n,N,d > 0, d %% 8 == 0"); return BV_ERR_INVALID; }
   const int64_t per = static_cast<int64_t>(N) * d / 8;
   int64_t blocks = (n * per + 255) / 256;
@@ -673,19 +711,25 @@ int launch_row_select(const void* a, const void* b, const float* mask, void* out
       reinterpret_cast<bf16*>(out), n, per);
   return check_cuda(cudaGetLastError(), "row_select_kernel launch");
 }
-int launch_concat_cls(const void* x, const float* cls, void* out, int64_t n, int N0, int d,
-                      cudaStream_t s) {
+int bv_concat_cls(const void* x, const float* cls, void* out, int64_t n, int32_t N0, int32_t d,
+                  void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (d % 8) { set_error("bv_concat_cls: d %% 8 != 0"); return BV_ERR_INVALID; }
   concat_cls_kernel<<<grid_for(n * (N0 + 1) * (d / 8), 256, num_sms() * 16), 256, 0, s>>>(
       reinterpret_cast<const bf16*>(x), cls, reinterpret_cast<bf16*>(out), n, N0, d);
   return check_launch("concat_cls_kernel");
 }
-int launch_drop_cls(const void* x, void* out, int64_t n, int N0, int d, cudaStream_t s) {
+int bv_drop_cls(const void* x, void* out, int64_t n, int32_t N0, int32_t d, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (d % 8) { set_error("bv_drop_cls: d %% 8 != 0"); return BV_ERR_INVALID; }
   drop_cls_kernel<<<grid_for(n * N0 * (d / 8), 256, num_sms() * 16), 256, 0, s>>>(
       reinterpret_cast<const bf16*>(x), reinterpret_cast<bf16*>(out), n, N0, d);
   return check_launch("drop_cls_kernel");
 }
+
+}  // extern "C"
 
 
 // ---- mixup (K16): utils.py:1146-1158 ---------------------------------------------------------
@@ -694,6 +738,7 @@ int launch_drop_cls(const void* x, void* out, int64_t n, int N0, int d, cudaStre
 // [n, 21843] labels of ImageNet-21k); the rolled operand is the row the neighbouring block has just read,
 // so it is served by L2.  Products and the sum are rounded separately (no FMA contraction): the
 // result is bit-identical to the fp32 expression evaluated left to right.
+namespace bv {
 namespace {
 __device__ __forceinline__ float mix1(float a, float b, float u, float v) {
   return __fadd_rn(__fmul_rn(a, u), __fmul_rn(b, v));
@@ -729,8 +774,13 @@ mixup_scalar_kernel(const float* __restrict__ x, float* __restrict__ out, int64_
   }
 }
 }  // namespace
+}  // namespace bv
 
-int launch_mixup(const float* x, float* out, int64_t n, int64_t row_elems, float a, cudaStream_t s) {
+extern "C" {
+
+int bv_mixup(const float* x, float* out, int64_t n, int64_t row_elems, float a, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0 || row_elems <= 0 || x == out ||
       (reinterpret_cast<uintptr_t>(x) & 3) || (reinterpret_cast<uintptr_t>(out) & 3)) {
     set_error("bv_mixup: need n, row_elems >= 1, 4B-aligned distinct buffers");
@@ -751,4 +801,4 @@ int launch_mixup(const float* x, float* out, int64_t n, int64_t row_elems, float
   return check_cuda(cudaGetLastError(), "mixup_kernel launch");
 }
 
-}  // namespace bv
+}  // extern "C"

@@ -11,7 +11,6 @@
 //    same integers without a sort.  Ties sort by index (a stable argsort).
 #include "common.cuh"
 #include "host_utils.h"
-#include "kernels.h"
 
 #include <limits.h>
 
@@ -151,10 +150,15 @@ rank_i2t_kernel(const float* __restrict__ d, int64_t NI, int64_t NT, int64_t ld,
 }
 
 }  // namespace
+}  // namespace bv
 
-int launch_top1(const void* logits, int dtype, int64_t rows, int C, int64_t ld, int32_t* idx,
-                const float* labels, int64_t ldl, const float* mask, float* top1_correct,
-                float* sums, cudaStream_t s) {
+extern "C" {
+
+int bv_top1(const void* logits, int dtype, int64_t rows, int32_t C, int64_t ld, int32_t* idx,
+            const float* labels, int64_t ldl, const float* mask, float* top1_correct, float* sums,
+            void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (rows < 0 || C <= 0 || ld < C || (labels != nullptr && ldl < C)) {
     set_error("bv_top1: need rows >= 0, C >= 1 and row strides >= C");
     return BV_ERR_INVALID;
@@ -166,8 +170,10 @@ int launch_top1(const void* logits, int dtype, int64_t rows, int C, int64_t ld, 
   return check_cuda(cudaGetLastError(), "top1_kernel launch");
 }
 
-int launch_retrieval_ranks(const float* dist, int64_t NI, int64_t NT, int64_t ld, const int32_t* corr,
-                           int32_t* rank_t2i, int32_t* rank_i2t, cudaStream_t s) {
+int bv_retrieval_ranks(const float* dist, int64_t NI, int64_t NT, int64_t ld, const int32_t* corr,
+                       int32_t* rank_t2i, int32_t* rank_i2t, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (NI <= 0 || NT <= 0 || ld < NT) {
     set_error("bv_retrieval_ranks: need NI, NT >= 1 and ld >= NT");
     return BV_ERR_INVALID;
@@ -184,4 +190,4 @@ int launch_retrieval_ranks(const float* dist, int64_t NI, int64_t NT, int64_t ld
   return BV_OK;
 }
 
-}  // namespace bv
+}  // extern "C"

@@ -25,7 +25,6 @@
 #include "common.cuh"
 #include "gemm_sched.h"
 #include "host_utils.h"
-#include "kernels.h"
 
 #include <atomic>
 
@@ -476,7 +475,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 }
 
 template <int BN, int OM, int EF>
-int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
+int launch_cfg(const bv_gemm_args& g, cudaStream_t stream) {
   using C = Cfg<BN, OM, EF>;
   CUtensorMap tmA, tmB, tmD, tmD2, tmAux;
   int rc;
@@ -498,7 +497,7 @@ int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
   p.M = (int)g.M; p.N = (int)g.N;
   p.a_mn = g.a_mn; p.b_mn = g.b_mn; p.reduce_out = g.reduce_out;
   p.alpha = g.alpha;
-  p.bias = g.epi == EPI_NONE ? nullptr : g.bias;     // EPI_NONE ignores bias (bv_b200.h)
+  p.bias = g.epilogue == BV_EPI_NONE ? nullptr : g.bias;     // BV_EPI_NONE ignores bias (bv_b200.h)
   p.colsum = g.colsum;
   p.aux = reinterpret_cast<const bf16*>(g.aux);
   p.ldaux = g.ldaux;
@@ -521,7 +520,7 @@ int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
     }
   }
   // aux is read through the same M x N window and box as the output it is staged with (the checks in
-  // launch_gemm give TMA's 16-byte base and row-stride alignment)
+  // bv_gemm give TMA's 16-byte base and row-stride alignment)
   if (C::AUX_TMA) {
     rc = make_tmap_2d(&tmAux, bf, g.aux, g.N, g.M, g.ldaux * 2, 64, 64);
     if (rc) return rc;
@@ -549,34 +548,41 @@ int launch_cfg(const GemmArgs& g, cudaStream_t stream) {
 // epilogue.  bf16 reduce-adds (gradient accumulation into bf16, not on the training step's path) run
 // at BN = 128: at 256 their atomics make ptxas spill the accumulators inside the persistent loop.
 template <int BN>
-int dispatch_epi(const GemmArgs& g, cudaStream_t s) {
+int dispatch_epi(const bv_gemm_args& g, cudaStream_t s) {
   const bool f32 = (g.out_dtype == DT_F32), add = !f32 && g.reduce_out;
-  switch (g.epi) {
-    case EPI_NONE:
-    case EPI_BIAS:
+  switch (g.epilogue) {
+    case BV_EPI_NONE:
+    case BV_EPI_BIAS:
       return f32 ? launch_cfg<BN, OM_F32, EF_BIAS>(g, s)
                  : add ? launch_cfg<128, OM_BF16_ADD, EF_BIAS>(g, s) : launch_cfg<BN, OM_BF16_TMA, EF_BIAS>(g, s);
-    case EPI_BIAS_RESID:
+    case BV_EPI_BIAS_RESID:
       if (f32) return launch_cfg<BN, OM_F32, EF_RESID>(g, s);
       if (add) return launch_cfg<128, OM_BF16_ADD, EF_RESID>(g, s);
       return g.aux_row_mod > 0 ? launch_cfg<BN, OM_BF16_TMA, EF_RESID_ROWMOD>(g, s)
                                : launch_cfg<BN, OM_BF16_TMA, EF_RESID>(g, s);
-    case EPI_BIAS_GELU:     // never a reduce-add (refused in launch_gemm)
+    case BV_EPI_BIAS_GELU:     // never a reduce-add (refused in bv_gemm)
       return launch_cfg<BN, OM_BF16_TMA, EF_GELU>(g, s);
-    case EPI_BIAS_GELU_ACT:
+    case BV_EPI_BIAS_GELU_ACT:
       return launch_cfg<BN, OM_BF16_TMA, EF_GELU_ACT>(g, s);
-    case EPI_DGELU:
+    case BV_EPI_DGELU:
       if (f32) { set_error("bv_gemm: DGELU epilogue writes bf16"); return BV_ERR_INVALID; }
       if (g.aux_row_mod > 0) { set_error("bv_gemm: DGELU takes a row-aligned aux"); return BV_ERR_INVALID; }
       return add ? launch_cfg<128, OM_BF16_ADD, EF_DGELU>(g, s) : launch_cfg<BN, OM_BF16_TMA, EF_DGELU>(g, s);
   }
-  set_error("bv_gemm: bad epilogue %d", g.epi);
+  set_error("bv_gemm: bad epilogue %d", g.epilogue);
   return BV_ERR_INVALID;
 }
 
 }  // namespace
+}  // namespace bv
 
-int launch_gemm(const GemmArgs& g, cudaStream_t stream) {
+extern "C" {
+
+int bv_gemm(const bv_gemm_args* args, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!args) { set_error("bv_gemm: null args"); return BV_ERR_INVALID; }
+  const bv_gemm_args& g = *args;
   if (g.M <= 0 || g.N <= 0 || g.K <= 0) { set_error("bv_gemm: empty problem"); return BV_ERR_INVALID; }
   // N need not be a multiple of 8 as long as the row strides are (TMA clips the loads and stores)
   if (g.out_dtype == DT_BF16 && ((reinterpret_cast<uintptr_t>(g.D) & 15) || (g.ldd % 8))) {
@@ -588,11 +594,11 @@ int launch_gemm(const GemmArgs& g, cudaStream_t stream) {
   if (g.M > 0x7fffffffLL || g.N > 0x7fffffffLL || g.K > 0x7fffffffLL) {
     set_error("bv_gemm: dimension exceeds int32"); return BV_ERR_INVALID;
   }
-  if (g.epi < EPI_NONE || g.epi > EPI_BIAS_GELU_ACT) {
-    set_error("bv_gemm: bad epilogue %d", g.epi); return BV_ERR_INVALID;
+  if (g.epilogue < BV_EPI_NONE || g.epilogue > BV_EPI_BIAS_GELU_ACT) {
+    set_error("bv_gemm: bad epilogue %d", g.epilogue); return BV_ERR_INVALID;
   }
-  if ((g.epi == EPI_BIAS_RESID || g.epi == EPI_DGELU) && g.aux == nullptr) {
-    set_error("bv_gemm: epilogue %d needs aux", g.epi); return BV_ERR_INVALID;
+  if ((g.epilogue == BV_EPI_BIAS_RESID || g.epilogue == BV_EPI_DGELU) && g.aux == nullptr) {
+    set_error("bv_gemm: epilogue %d needs aux", g.epilogue); return BV_ERR_INVALID;
   }
   if (g.aux != nullptr && ((reinterpret_cast<uintptr_t>(g.aux) & 15) || (g.ldaux % 8))) {
     set_error("bv_gemm: aux must be 16B aligned with ldaux %% 8 == 0"); return BV_ERR_INVALID;
@@ -600,13 +606,13 @@ int launch_gemm(const GemmArgs& g, cudaStream_t stream) {
   if (g.bias != nullptr && (reinterpret_cast<uintptr_t>(g.bias) & 15)) {
     set_error("bv_gemm: bias must be 16B aligned"); return BV_ERR_INVALID;
   }
-  if (g.epi == EPI_BIAS_GELU && (g.out_dtype != DT_BF16 || g.D2 == nullptr || g.reduce_out)) {
+  if (g.epilogue == BV_EPI_BIAS_GELU && (g.out_dtype != DT_BF16 || g.D2 == nullptr || g.reduce_out)) {
     set_error("bv_gemm: BIAS_GELU needs bf16 output, D2 and no reduce"); return BV_ERR_INVALID;
   }
-  if (g.epi == EPI_BIAS_GELU && ((reinterpret_cast<uintptr_t>(g.D2) & 15) || (g.ldd2 % 8))) {
+  if (g.epilogue == BV_EPI_BIAS_GELU && ((reinterpret_cast<uintptr_t>(g.D2) & 15) || (g.ldd2 % 8))) {
     set_error("bv_gemm: D2 must be 16B aligned with ldd2 %% 8 == 0"); return BV_ERR_INVALID;
   }
-  if (g.epi == EPI_BIAS_GELU_ACT && (g.out_dtype != DT_BF16 || g.reduce_out)) {
+  if (g.epilogue == BV_EPI_BIAS_GELU_ACT && (g.out_dtype != DT_BF16 || g.reduce_out)) {
     set_error("bv_gemm: BIAS_GELU_ACT needs bf16 output and no reduce"); return BV_ERR_INVALID;
   }
   if (g.out_dtype != DT_F32 && g.out_dtype != DT_BF16) { set_error("bv_gemm: bad out dtype"); return BV_ERR_INVALID; }
@@ -615,10 +621,10 @@ int launch_gemm(const GemmArgs& g, cudaStream_t stream) {
   }
   int bn = g.block_n;
   if (bn == 0) bn = (g.N > 128) ? 256 : 128;
-  if (bn == 256) return dispatch_epi<256>(g, stream);
-  if (bn == 128) return dispatch_epi<128>(g, stream);
+  if (bn == 256) return dispatch_epi<256>(g, s);
+  if (bn == 128) return dispatch_epi<128>(g, s);
   set_error("bv_gemm: block_n must be 0, 128 or 256");
   return BV_ERR_INVALID;
 }
 
-}  // namespace bv
+}  // extern "C"

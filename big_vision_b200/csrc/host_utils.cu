@@ -14,7 +14,6 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
-const char* last_error() { return g_err; }
 
 int check_cuda(cudaError_t e, const char* what) {
   if (e == cudaSuccess) return BV_OK;
@@ -94,3 +93,18 @@ int make_tmap(CUtensorMap* out, CUtensorMapDataType dt, int rank, const void* pt
 }
 
 }  // namespace bv
+
+extern "C" {
+
+const char* bv_last_error_string(void) { return bv::g_err; }
+int bv_version(void) { return 100; }
+
+int bv_device_supported(void) {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
+  int major = 0;
+  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
+  return major == 9 ? 1 : 0;
+}
+
+}  // extern "C"

@@ -10,7 +10,6 @@
 namespace bv {
 
 void set_error(const char* fmt, ...);
-const char* last_error();
 int check_cuda(cudaError_t e, const char* what);
 int num_sms();
 

@@ -9,7 +9,6 @@
 // stream, so those need no extra pass over HBM.
 #include "common.cuh"
 #include "host_utils.h"
-#include "kernels.h"
 
 namespace bv {
 namespace {
@@ -460,10 +459,15 @@ int check_ln(int64_t rows, int d, const char* who) {
 }
 
 }  // namespace
+}  // namespace bv
 
-int launch_layernorm_fwd(const void* x, int x_dt, const float* scale, const float* bias, void* y,
-                         int y_dt, float* mean, float* rstd, int64_t rows, int d, float eps,
-                         cudaStream_t s) {
+extern "C" {
+
+int bv_layernorm_fwd(const void* x, int x_dt, const float* scale, const float* bias, void* y,
+                     int y_dt, float* mean, float* rstd, int64_t rows, int32_t d, float eps,
+                     void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   int rc = check_ln(rows, d, "bv_layernorm_fwd");
   if (rc) return rc;
   if (rows == 0) return BV_OK;
@@ -496,10 +500,12 @@ int launch_layernorm_fwd(const void* x, int x_dt, const float* scale, const floa
   return check_cuda(cudaGetLastError(), "ln_fwd_kernel launch");
 }
 
-int launch_layernorm_bwd(const void* dy, int dy_dt, const void* x, int x_dt, const float* scale,
-                         const float* mean, const float* rstd, const void* dres, void* dx,
-                         int dx_dt, float* dscale, float* dbias, float* dx_colsum, int64_t rows,
-                         int d, cudaStream_t s) {
+int bv_layernorm_bwd(const void* dy, int dy_dt, const void* x, int x_dt, const float* scale,
+                     const float* mean, const float* rstd, const void* dres, void* dx,
+                     int dx_dt, float* dscale, float* dbias, float* dx_colsum, int64_t rows,
+                     int32_t d, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   int rc = check_ln(rows, d, "bv_layernorm_bwd");
   if (rc) return rc;
   if (rows == 0) return BV_OK;
@@ -539,4 +545,4 @@ int launch_layernorm_bwd(const void* dy, int dy_dt, const void* x, int x_dt, con
   return check_cuda(cudaGetLastError(), "ln_bwd_kernel launch");
 }
 
-}  // namespace bv
+}  // extern "C"

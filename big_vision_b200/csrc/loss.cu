@@ -10,7 +10,6 @@
 //  * sigmoid_xent / softmax_xent (K15): utils.py:236-243, 276-281.
 #include "common.cuh"
 #include "host_utils.h"
-#include "kernels.h"
 
 namespace bv {
 namespace {
@@ -215,11 +214,16 @@ softmax_xent_kernel(const float* __restrict__ logits, int64_t ldx, const float* 
 }
 
 }  // namespace
+}  // namespace bv
 
-int launch_siglip_loss_ew(const float* dots, int64_t n, int64_t B, int64_t ld, int64_t row_offset,
-                          const float* t_param, const float* b_param, int64_t global_B, void* G,
-                          int64_t ldg, float* loss, float* dt, float* db, float* partials,
-                          cudaStream_t s) {
+extern "C" {
+
+int bv_siglip_loss(const float* dots, int64_t n, int64_t B, int64_t ld, int64_t row_offset,
+                   const float* t_param, const float* b_param, int64_t global_B, void* G,
+                   int64_t ldg, float* loss, float* dt, float* db, float* partials,
+                   void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0 || B <= 0 || B % 4 || ld % 4 || ldg % 4 || global_B <= 0) {
     set_error("bv_siglip_loss: need n,B > 0 and B, ld, ldg multiples of 4");
     return BV_ERR_INVALID;
@@ -237,9 +241,11 @@ int launch_siglip_loss_ew(const float* dots, int64_t n, int64_t B, int64_t ld, i
   return check_cuda(cudaGetLastError(), "finish_sums_kernel launch");
 }
 
-int launch_softmax_contrastive(const float* dots, int64_t n, int64_t B, int64_t ld, int64_t row_offset,
-                               const float* t_param, int64_t global_B, float weight, void* G, int64_t ldg,
-                               float* loss, float* dt, float* ncorrect, float* rows_ws, cudaStream_t s) {
+int bv_softmax_contrastive_loss(const float* dots, int64_t n, int64_t B, int64_t ld, int64_t row_offset,
+                                const float* t_param, int64_t global_B, float weight, void* G, int64_t ldg,
+                                float* loss, float* dt, float* ncorrect, float* rows_ws, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0 || B <= 0 || global_B <= 0 || rows_ws == nullptr) {
     set_error("bv_softmax_contrastive_loss: need n, B > 0 and the [3, n] workspace");
     return BV_ERR_INVALID;
@@ -253,8 +259,19 @@ int launch_softmax_contrastive(const float* dots, int64_t n, int64_t B, int64_t 
   return check_cuda(cudaGetLastError(), "finish_sums_kernel launch");
 }
 
-int launch_sigmoid_xent(const float* logits, int64_t ldx, const float* labels, int64_t ldy, float* loss,
-                        float* dlogits, int64_t ldd, float* row_loss, int64_t n, int C, cudaStream_t s) {
+int bv_sigmoid_xent(const float* logits, const float* labels, float* loss, float* dlogits,
+                    float* row_loss_ws, int64_t n, int32_t C, void* stream) {
+  return bv_sigmoid_xent_ld(logits, C, labels, C, loss, dlogits, C, row_loss_ws, n, C, stream);
+}
+int bv_softmax_xent(const float* logits, const float* labels, float* loss, float* dlogits,
+                    float* row_loss_ws, int64_t n, int32_t C, void* stream) {
+  return bv_softmax_xent_ld(logits, C, labels, C, loss, dlogits, C, row_loss_ws, n, C, stream);
+}
+
+int bv_sigmoid_xent_ld(const float* logits, int64_t ldx, const float* labels, int64_t ldy, float* loss,
+                       float* dlogits, int64_t ldd, float* row_loss, int64_t n, int32_t C, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (ldx < C || ldy < C || ldd < C) {
     set_error("bv_sigmoid_xent_ld: row strides must be >= C (ld_logits %lld, ld_labels %lld, ld_dlogits %lld, C %d)",
               static_cast<long long>(ldx), static_cast<long long>(ldy), static_cast<long long>(ldd), C);
@@ -268,8 +285,10 @@ int launch_sigmoid_xent(const float* logits, int64_t ldx, const float* labels, i
   finish_sums_kernel<<<1, 256, 0, s>>>(row_loss, n, loss, nullptr, nullptr);
   return check_cuda(cudaGetLastError(), "finish_sums_kernel launch");
 }
-int launch_softmax_xent(const float* logits, int64_t ldx, const float* labels, int64_t ldy, float* loss,
-                        float* dlogits, int64_t ldd, float* row_loss, int64_t n, int C, cudaStream_t s) {
+int bv_softmax_xent_ld(const float* logits, int64_t ldx, const float* labels, int64_t ldy, float* loss,
+                       float* dlogits, int64_t ldd, float* row_loss, int64_t n, int32_t C, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (ldx < C || ldy < C || ldd < C) {
     set_error("bv_softmax_xent_ld: row strides must be >= C (ld_logits %lld, ld_labels %lld, ld_dlogits %lld, C %d)",
               static_cast<long long>(ldx), static_cast<long long>(ldy), static_cast<long long>(ldd), C);
@@ -284,4 +303,4 @@ int launch_softmax_xent(const float* logits, int64_t ldx, const float* labels, i
   return check_cuda(cudaGetLastError(), "finish_sums_kernel launch");
 }
 
-}  // namespace bv
+}  // extern "C"

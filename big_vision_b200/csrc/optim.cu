@@ -8,7 +8,6 @@
 // 4+4 (p) + 4 (g) + 2x(2|4) (mu) + 4+4 (nu) + 2 (bf16 shadow) bytes per element.
 #include "common.cuh"
 #include "host_utils.h"
-#include "kernels.h"
 
 namespace bv {
 namespace {
@@ -135,8 +134,15 @@ sumsq_kernel(const float* __restrict__ x, float* __restrict__ out, int64_t n) {
 }
 
 }  // namespace
+}  // namespace bv
 
-int launch_adam(const AdamArgs& a, cudaStream_t s) {
+extern "C" {
+
+int bv_adam_step(const bv_adam_args* args, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!args) { set_error("bv_adam_step: null args"); return BV_ERR_INVALID; }
+  const bv_adam_args& a = *args;
   if (a.n <= 0) return BV_OK;
   if (a.n % 4 != 0 || (reinterpret_cast<uintptr_t>(a.params) & 15) ||
       (reinterpret_cast<uintptr_t>(a.grads) & 15)) {
@@ -151,19 +157,21 @@ int launch_adam(const AdamArgs& a, cudaStream_t s) {
   if (blocks > cap) blocks = cap;
   if (a.mu_dtype == DT_BF16) {
     adam_kernel<true><<<static_cast<unsigned>(blocks), 256, 0, s>>>(
-        a.params, a.grads, a.mu, a.nu, reinterpret_cast<bf16*>(a.params_bf16), a.n, a.lr, a.b1,
-        a.b2, a.eps, a.wd, bc1, bc2, a.gnorm_sq, a.clip_norm, a.grad_scale_host, a.upd_sq, a.param_sq);
+        a.params, a.grads, a.mu, a.nu, reinterpret_cast<bf16*>(a.params_bf16), a.n, a.lr_eff, a.b1,
+        a.b2, a.eps, a.wd_eff, bc1, bc2, a.gnorm_sq, a.clip_norm, a.grad_mult, a.upd_sq, a.param_sq);
   } else {
     adam_kernel<false><<<static_cast<unsigned>(blocks), 256, 0, s>>>(
-        a.params, a.grads, a.mu, a.nu, reinterpret_cast<bf16*>(a.params_bf16), a.n, a.lr, a.b1,
-        a.b2, a.eps, a.wd, bc1, bc2, a.gnorm_sq, a.clip_norm, a.grad_scale_host, a.upd_sq, a.param_sq);
+        a.params, a.grads, a.mu, a.nu, reinterpret_cast<bf16*>(a.params_bf16), a.n, a.lr_eff, a.b1,
+        a.b2, a.eps, a.wd_eff, bc1, bc2, a.gnorm_sq, a.clip_norm, a.grad_mult, a.upd_sq, a.param_sq);
   }
   return check_cuda(cudaGetLastError(), "adam_kernel launch");
 }
 
-int launch_scale_step(float* params, const float* grads, void* params_bf16, int64_t n, float lr, float wd,
-                      float grad_mult, float clip_norm, const float* gnorm_sq, float* upd_sq,
-                      float* param_sq, cudaStream_t s) {
+int bv_scale_step(float* params, const float* grads, void* params_bf16, int64_t n, float lr, float wd,
+                  float grad_mult, float clip_norm, const float* gnorm_sq, float* upd_sq, float* param_sq,
+                  void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return BV_OK;
   int64_t blocks = (n + 255) / 256;
   const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
@@ -174,7 +182,9 @@ int launch_scale_step(float* params, const float* grads, void* params_bf16, int6
   return check_cuda(cudaGetLastError(), "scale_step_kernel launch");
 }
 
-int launch_sumsq(const float* x, float* out, int64_t n, cudaStream_t s) {
+int bv_sumsq(const float* x, float* out, int64_t n, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return BV_OK;
   int64_t blocks = (n / 4 + 255) / 256;
   const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
@@ -183,6 +193,8 @@ int launch_sumsq(const float* x, float* out, int64_t n, cudaStream_t s) {
   sumsq_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(x, out, n);
   return check_cuda(cudaGetLastError(), "sumsq_kernel launch");
 }
+
+}  // extern "C"
 
 
 // =====================================================================================================
@@ -198,6 +210,7 @@ int launch_sumsq(const float* x, float* out, int64_t n, cudaStream_t s) {
 // {d0, d1} = {L, H}): Dense [in, out] = [1, in, 1, out]; DenseGeneral q/k/v [d, h, dh] = [1, d, h, dh];
 // out [h, dh, d] = [h, dh, 1, d]; scan-stacked tensors carry their depth in A.
 // =====================================================================================================
+namespace bv {
 namespace {
 
 struct View4 { int64_t A, L, M, H; int64_t sA, sL, sM; };   // element strides; H has stride 1
@@ -311,8 +324,15 @@ inline unsigned af_blocks(int64_t work) {
 }
 
 }  // namespace
+}  // namespace bv
 
-int launch_adafactor(const AdafactorArgs& a, cudaStream_t s) {
+extern "C" {
+
+int bv_adafactor_step(const bv_adafactor_args* args, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!args) { set_error("bv_adafactor_step: null args"); return BV_ERR_INVALID; }
+  const bv_adafactor_args& a = *args;
   View4 v{a.A, a.L, a.M, a.H, a.sA, a.sL, a.sM};
   if (a.A <= 0 || a.L <= 0 || a.M <= 0 || a.H <= 0 || a.mode < 0 || a.mode > 2) {
     set_error("bv_adafactor_step: bad view or mode");
@@ -336,14 +356,15 @@ int launch_adafactor(const AdafactorArgs& a, cudaStream_t s) {
   if (a.momentum != nullptr) {
     af_apply_kernel<true><<<af_blocks(n), 256, 0, s>>>(
         a.params, a.grads, reinterpret_cast<bf16*>(a.params_bf16), v, a.mode, a.vfull, a.red_h, a.red_l, a.nrm,
-        reinterpret_cast<bf16*>(a.momentum), a.decay, a.eps, a.beta, a.lr, a.wd, a.gnorm_sq, a.clip_norm,
+        reinterpret_cast<bf16*>(a.momentum), a.decay, a.eps, a.beta, a.lr_eff, a.wd_eff, a.gnorm_sq, a.clip_norm,
         a.grad_mult, a.upd_sq, a.param_sq);
   } else {
     af_apply_kernel<false><<<af_blocks(n), 256, 0, s>>>(
         a.params, a.grads, reinterpret_cast<bf16*>(a.params_bf16), v, a.mode, a.vfull, a.red_h, a.red_l, a.nrm,
-        nullptr, a.decay, a.eps, a.beta, a.lr, a.wd, a.gnorm_sq, a.clip_norm, a.grad_mult, a.upd_sq, a.param_sq);
+        nullptr, a.decay, a.eps, a.beta, a.lr_eff, a.wd_eff, a.gnorm_sq, a.clip_norm, a.grad_mult, a.upd_sq,
+        a.param_sq);
   }
   return check_cuda(cudaGetLastError(), "adafactor kernels launch");
 }
 
-}  // namespace bv
+}  // extern "C"

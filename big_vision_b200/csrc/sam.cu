@@ -10,7 +10,6 @@
 
 #include "common.cuh"
 #include "host_utils.h"
-#include "kernels.h"
 
 namespace bv {
 namespace {
@@ -147,9 +146,14 @@ inline unsigned stream_blocks(int64_t n) {
 }
 
 }  // namespace
+}  // namespace bv
 
-int launch_sam_perturb(const float* w, const float* g, const float* g_sumsq, float rho, float eps, int adaptive,
-                       float* w_out, void* w_bf16, int64_t n, cudaStream_t s) {
+extern "C" {
+
+int bv_sam_perturb(const float* w, const float* g, const float* g_sumsq, float rho, float eps, int32_t adaptive,
+                   float* w_out, void* w_bf16, int64_t n, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n < 0 || (n > 0 && (!w || !g || !g_sumsq || !w_out || !w_bf16))) {
     set_error("bv_sam_perturb: null buffer or n < 0");
     return BV_ERR_INVALID;
@@ -164,7 +168,9 @@ int launch_sam_perturb(const float* w, const float* g, const float* g_sumsq, flo
   return check_cuda(cudaGetLastError(), "sam_perturb_kernel launch");
 }
 
-int launch_sam_dots(const float* a, const float* b, float* out, float* ws, int64_t n, cudaStream_t s) {
+int bv_sam_dots(const float* a, const float* b, float* out, float* ws, int64_t n, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n < 0 || !a || !b || !out || !ws) {
     set_error("bv_sam_dots: null buffer or n < 0");
     return BV_ERR_INVALID;
@@ -184,8 +190,10 @@ int launch_sam_dots(const float* a, const float* b, float* out, float* ws, int64
   return check_cuda(cudaGetLastError(), "sam_dots_finish_kernel launch");
 }
 
-int launch_gsam_combine(float* gc, const float* gr, const float* dot, const float* norm_sq, float alpha,
-                        int minimize_fp, int64_t n, cudaStream_t s) {
+int bv_gsam_combine(float* gc, const float* gr, const float* dot, const float* norm_sq, float alpha,
+                    int32_t minimize_fp, int64_t n, void* stream) {
+  using namespace bv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n < 0 || (n > 0 && (!gc || !gr || !dot || !norm_sq))) {
     set_error("bv_gsam_combine: null buffer or n < 0");
     return BV_ERR_INVALID;
@@ -200,4 +208,4 @@ int launch_gsam_combine(float* gc, const float* gr, const float* dot, const floa
   return check_cuda(cudaGetLastError(), "gsam_combine_kernel launch");
 }
 
-}  // namespace bv
+}  // extern "C"

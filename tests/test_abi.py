@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds, loads and exports every symbol include/bv_b200.h declares;
+"""CPU: the C-ABI library builds, loads and exports every symbol include/bv_b200*.h declare;
 argument validation fails loudly (no compute without a GPU)."""
 import ctypes
 import os
@@ -9,12 +9,15 @@ import pytest
 from big_vision_b200 import lib as L
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HEADERS = ("bv_b200.h", "bv_b200_sam.h", "bv_b200_distill.h")
 
 
 def _header_functions():
-  src = open(os.path.join(ROOT, "include", "bv_b200.h")).read()
-  src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-  return sorted(set(re.findall(r"\b(bv_[a-z0-9_]+)\s*\(", src)))
+  names = set()
+  for h in HEADERS:
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", h)).read(), flags=re.S)
+    names |= set(re.findall(r"\b(bv_[a-z0-9_]+)\s*\(", src))
+  return sorted(names)
 
 
 def test_header_symbols_exported():
@@ -22,12 +25,30 @@ def test_header_symbols_exported():
   names = _header_functions()
   assert len(names) >= 25
   for n in names:
-    assert hasattr(lib, n), f"{n} declared in include/bv_b200.h but not exported"
+    assert hasattr(lib, n), f"{n} declared in include/ but not exported"
 
 
 def test_binding_covers_header():
+  """The entry points are defined across the kernel sources, so the three headers together must match the
+  binding one to one."""
   declared = set(_header_functions()) - {"bv_last_error_string"}
-  assert declared == set(L.SIGNATURES), (declared ^ set(L.SIGNATURES))
+  bound = set(L.SIGNATURES) | set(L.SAM_SIGNATURES) | set(L.DISTILL_SIGNATURES)
+  assert declared == bound, declared ^ bound
+
+
+@pytest.mark.parametrize("name,args,message", [
+    ("bv_gemm", (None, None), "bv_gemm: null args"),
+    ("bv_attention_fwd", (None, None), "bv_attention_fwd: null args"),
+    ("bv_attention_fwd_hd", (None, 96, None), "bv_attention_fwd: null args"),
+    ("bv_attention_bwd", (None, None), "bv_attention_bwd: null args"),
+    ("bv_attention_bwd_hd", (None, 96, None), "bv_attention_bwd: null args"),
+    ("bv_adam_step", (None, None), "bv_adam_step: null args"),
+    ("bv_adafactor_step", (None, None), "bv_adafactor_step: null args"),
+])
+def test_null_struct_args_are_refused(name, args, message):
+  lib = L.load()
+  assert getattr(lib, name)(*args) == -1
+  assert lib.bv_last_error_string().decode() == message
 
 
 def test_version_and_no_gpu_support_flag():
