@@ -128,6 +128,12 @@ DISTILL_SIGNATURES = {
 DIST_KINDS = {"euclidean": 0, "l2": 1, "hard": 2, "kl": 3, "logsoftmax_euclidean": 4, "agree": 5}
 DISTILL_OUTPUTS = ("distance", "entropy_student", "entropy_teacher", "task_loss_student", "task_loss_teacher")
 
+# include/bv_b200_flexi.h (FlexiViT resampling), one to one; exported from the same library
+FLEXI_SIGNATURES = {
+    "bv_resample_fwd": [c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp],
+    "bv_resample_bwd": [c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp],
+}
+
 _lib = None
 
 
@@ -145,7 +151,7 @@ def load():
         f"{LIB_PATH} not found: build it with `python -m big_vision_b200.build` "
         "(there is no CPU or eager fallback for the kernels).")
   lib = ctypes.CDLL(LIB_PATH)
-  for name, argtypes in {**SIGNATURES, **SAM_SIGNATURES, **DISTILL_SIGNATURES}.items():
+  for name, argtypes in {**SIGNATURES, **SAM_SIGNATURES, **DISTILL_SIGNATURES, **FLEXI_SIGNATURES}.items():
     fn = getattr(lib, name)   # raises AttributeError if the symbol is missing
     fn.argtypes = argtypes
     fn.restype = ctypes.c_int

@@ -515,6 +515,37 @@ def distance(student, teacher, kind, epsilon=1e-12, t=1.0, ls=0.0, k=1):
   return out
 
 
+# ---- FlexiViT resampling (include/bv_b200_flexi.h) ----------------------------------------------------
+def _resample_args(M, a):
+  for t in (M, a):
+    if t.dtype != torch.float32 or not t.is_contiguous():
+      raise L.BvError(f"resampling takes contiguous fp32 matrices, got {t.dtype} {tuple(t.shape)} {t.stride()}")
+  if M.dim() != 2 or a.dim() != 2:
+    raise L.BvError(f"resampling takes a 2-D matrix and a 2-D operand, got {tuple(M.shape)} and {tuple(a.shape)}")
+  return M.shape[0], M.shape[1], a.shape[1]
+
+
+def resample_fwd(M, x, out=None):
+  """M fp32 [R, K], x fp32 [K, J] -> bf16 [R, J] = M x (fp32 sums in ascending k, one rounding).  `out`: a
+  contiguous bf16 buffer whose first R * J elements receive the result (e.g. a [Kp, d] GEMM operand)."""
+  R, K, J = _resample_args(M, x)
+  assert x.shape[0] == K, (tuple(M.shape), tuple(x.shape))
+  if out is None:
+    out = torch.empty((R, J), dtype=torch.bfloat16, device=x.device)
+  assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.numel() >= R * J
+  L.call("bv_resample_fwd", _p(M), _p(x), _p(out), R, K, J, _stream())
+  return out
+
+
+def resample_bwd(M, dy, dx):
+  """dx fp32 [K, J] += M^T dy for M fp32 [R, K], dy fp32 [R, J] (fp32 sums in ascending r)."""
+  R, K, J = _resample_args(M, dy)
+  assert dy.shape[0] == R and dx.dtype == torch.float32 and dx.is_contiguous() and tuple(dx.shape) == (K, J), \
+      (tuple(M.shape), tuple(dy.shape), tuple(dx.shape))
+  L.call("bv_resample_bwd", _p(M), _p(dy), _p(dx), R, K, J, _stream())
+  return dx
+
+
 # ---- integer evaluation paths -------------------------------------------------------------------
 def top1(logits, labels=None, mask=None, want_idx=True):
   """argmax over classes (+ label gather and masked counts).  Returns (idx int32 [rows] or None,

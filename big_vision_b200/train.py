@@ -63,7 +63,8 @@ def make_update_fn(model, tx, config):
   d = Dist()
   frozen = tx.frozen() if hasattr(tx, "frozen") else frozenset()
 
-  def update_fn(train_state, rng, batch):
+  def update_fn(train_state, rng, batch, **fwd_kw):
+    """`fwd_kw`: extra keyword arguments of the model's forward (a FlexiViT step's seqhw)."""
     P, opt = train_state["params"], train_state["opt"]
     images, labels = batch["image"], batch["labels"]
     if mixup_p:
@@ -74,7 +75,7 @@ def make_update_fn(model, tx, config):
     # stochastic depth (Mixer, mlp_mixer.py:173-177) draws its masks from the step's rng like the
     # reference's `rngs={"dropout": rng}` (train.py:296-299)
     kw = dict(train=True, rng=rng) if getattr(model, "stoch_depth", 0.0) else {}
-    loss, _ = loss_and_grads(model, P, images, labels, loss_name, dist_view=d, frozen=frozen, **kw)
+    loss, _ = loss_and_grads(model, P, images, labels, loss_name, dist_view=d, frozen=frozen, **kw, **fwd_kw)
     # the loss is the mean over the GLOBAL batch: sum the per-rank means and divide by world
     d.all_reduce_sum(loss)
     sc = tx.update(P, opt, grad_mult=1.0 / d.world)
