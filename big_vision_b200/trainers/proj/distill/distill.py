@@ -93,7 +93,8 @@ def make_update_fn(models, tx, config):
   frozen = tx.frozen() if hasattr(tx, "frozen") else frozenset()
   student = models["student"]
 
-  def update_fn(train_state, rng, batch):
+  def update_fn(train_state, rng, batch, **student_kw):
+    """`student_kw`: extra keyword arguments of the student's forward only (a FlexiViT student's seqhw)."""
     params, opt = train_state["params"], train_state["opt"]
     P = params["student"]
     data = dict(batch)
@@ -106,7 +107,8 @@ def make_update_fn(models, tx, config):
       data.update(to_mix)
     # stochastic depth for the student only (`train=name == "student"`, distill.py:226)
     kw = dict(train=True, rng=rng) if getattr(student, "stoch_depth", 0.0) else {}
-    m = loss_and_grads(models, params, data, teachers, kind, distance_kw, dist_view=d, frozen=frozen, **kw)
+    m = loss_and_grads(models, params, data, teachers, kind, distance_kw, dist_view=d, frozen=frozen, **kw,
+                       **student_kw)
     # every measurement is the mean over the GLOBAL batch: sum the per-rank means and divide by world
     names = sorted(m)
     vals = torch.stack([m[k] for k in names])

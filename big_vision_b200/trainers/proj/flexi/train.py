@@ -20,11 +20,10 @@ def flexi_args(config, step, xid=-1, wid=-1):
           for name in sorted(config["flexi"])}
 
 
-def make_update_fn(model, tx, config):
-  """-> update_fn(train_state, rng, batch, **flexi_kw): train.py's step with `flexi_kw` (flexi_args of
-  the step) passed to the model.  Every flexible argument must be given."""
+def demand_flexi_args(step, config):
+  """-> update_fn(train_state, rng, batch, **flexi_kw) = step(...) that refuses a call which does not pass
+  exactly the flexible arguments of `config`."""
   names = sorted(config["flexi"])
-  step = train.make_update_fn(model, tx, config)
 
   def update_fn(train_state, rng, batch, **flexi_kw):
     if sorted(flexi_kw) != names:
@@ -32,6 +31,12 @@ def make_update_fn(model, tx, config):
     return step(train_state, rng, batch, **flexi_kw)
 
   return update_fn
+
+
+def make_update_fn(model, tx, config):
+  """-> update_fn(train_state, rng, batch, **flexi_kw): train.py's step with `flexi_kw` (flexi_args of
+  the step) passed to the model.  Every flexible argument must be given."""
+  return demand_flexi_args(train.make_update_fn(model, tx, config), config)
 
 
 def make_predict_fns(model, config):
