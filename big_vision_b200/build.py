@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libbv_b200.so")
 SOURCES = ["host_utils.cu", "gemm.cu", "attention.cu", "layernorm.cu", "elementwise.cu",
-           "loss.cu", "optim.cu", "eval.cu", "sam.cu", "distill.cu", "flexi.cu"]
+           "loss.cu", "optim.cu", "eval.cu", "sam.cu", "distill.cu", "flexi.cu", "jet.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
@@ -35,6 +35,7 @@ def _headers():
   out.append(os.path.join(os.path.dirname(HERE), "include", "bv_b200_sam.h"))
   out.append(os.path.join(os.path.dirname(HERE), "include", "bv_b200_distill.h"))
   out.append(os.path.join(os.path.dirname(HERE), "include", "bv_b200_flexi.h"))
+  out.append(os.path.join(os.path.dirname(HERE), "include", "bv_b200_jet.h"))
   return out
 
 

@@ -134,6 +134,18 @@ FLEXI_SIGNATURES = {
     "bv_resample_bwd": [c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp],
 }
 
+# include/bv_b200_jet.h (Jet normalizing flow), one to one; exported from the same library
+JET_SIGNATURES = {
+    "bv_jet_dequantize_patchify": [c_vp, c_vp, c_i64, c_i32, c_i32, c_i32, c_i32, ctypes.c_uint64, ctypes.c_uint64,
+                                   c_i64, c_f32, c_vp],
+    "bv_jet_unpatchify": [c_vp, c_vp, c_i64, c_i32, c_i32, c_i32, c_i32, c_vp],
+    "bv_jet_split": [c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp],
+    "bv_jet_coupling_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_f32, c_i32, c_vp],
+    "bv_jet_coupling_bwd": [c_vp, c_vp, c_vp, c_vp, c_f32, c_vp, c_vp, c_i64, c_i32, c_i32, c_f32, c_vp],
+    "bv_jet_merge_grad": [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp],
+    "bv_jet_bits": [c_vp, c_vp, c_vp, c_vp, c_vp, c_f32, c_i64, c_i64, c_vp],
+}
+
 _lib = None
 
 
@@ -151,7 +163,8 @@ def load():
         f"{LIB_PATH} not found: build it with `python -m big_vision_b200.build` "
         "(there is no CPU or eager fallback for the kernels).")
   lib = ctypes.CDLL(LIB_PATH)
-  for name, argtypes in {**SIGNATURES, **SAM_SIGNATURES, **DISTILL_SIGNATURES, **FLEXI_SIGNATURES}.items():
+  for name, argtypes in {**SIGNATURES, **SAM_SIGNATURES, **DISTILL_SIGNATURES, **FLEXI_SIGNATURES,
+                         **JET_SIGNATURES}.items():
     fn = getattr(lib, name)   # raises AttributeError if the symbol is missing
     fn.argtypes = argtypes
     fn.restype = ctypes.c_int
@@ -172,7 +185,7 @@ LAUNCHES = [0]
 _LAUNCHES_PER_CALL = {"bv_embed_bwd": 2, "bv_retrieval_ranks": 2, "bv_siglip_loss": 2,
                       "bv_sigmoid_xent": 2, "bv_softmax_xent": 2, "bv_sigmoid_xent_ld": 2, "bv_softmax_xent_ld": 2,
                       "bv_softmax_contrastive_loss": 2, "bv_adafactor_step": 4, "bv_sam_dots": 2,
-                      "bv_distill_loss": 2}
+                      "bv_distill_loss": 2, "bv_jet_bits": 2}
 LOSS_WS_FLOATS = 8192      # BV_LOSS_WS_FLOATS
 
 

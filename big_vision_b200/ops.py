@@ -546,6 +546,95 @@ def resample_bwd(M, dy, dx):
   return dx
 
 
+# ---- Jet normalizing flow (include/bv_b200_jet.h) -------------------------------------------------------
+def _jet_args(*ts):
+  for t in ts:
+    if t is not None and (t.dtype not in (torch.float32, torch.bfloat16, torch.int32) or not t.is_contiguous()):
+      raise L.BvError(f"Jet kernels take contiguous fp32 / bf16 / int32 buffers, got {t.dtype} {tuple(t.shape)}")
+
+
+def jet_dequantize_patchify(image, ps, seed=0, counter=0, offset=0, noise_scale=1.0 / 127.5, out=None):
+  """image fp32 [n, H, W, C] -> z fp32 [n, T, ps*ps*C] = patchified image + (uniform noise of the global
+  Philox stream at element `offset` on) * noise_scale; noise_scale 0 is a plain patchify."""
+  _jet_args(image, out)
+  n, H, W, C = image.shape
+  assert image.dtype == torch.float32
+  if out is None:
+    out = torch.empty((n, (H // ps) * (W // ps), ps * ps * C), dtype=torch.float32, device=image.device)
+  L.call("bv_jet_dequantize_patchify", _p(image), _p(out), n, H, W, C, ps, int(seed), int(counter), int(offset),
+         float(noise_scale), _stream())
+  return out
+
+
+def jet_unpatchify(z, image_shape, ps, out=None):
+  """z fp32 [n, T, ps*ps*C] -> fp32 [n, H, W, C] (`image_shape`)."""
+  _jet_args(z, out)
+  n, H, W, C = image_shape
+  if out is None:
+    out = torch.empty((n, H, W, C), dtype=torch.float32, device=z.device)
+  L.call("bv_jet_unpatchify", _p(z), _p(out), n, H, W, C, ps, _stream())
+  return out
+
+
+def jet_split(x, idx, T, c, out=None):
+  """x fp32 [n, D] (any shape with n * D elements), idx int32 [D] -> x1 bf16 [n * T, c] = bf16(x[:, idx[:D/2]])."""
+  _jet_args(x, idx, out)
+  n = x.numel() // (2 * T * c)
+  if out is None:
+    out = torch.empty((n * T, c), dtype=torch.bfloat16, device=x.device)
+  L.call("bv_jet_split", _p(x), _p(idx), _p(out), n, T, c, _stream())
+  return out
+
+
+def jet_coupling_fwd(x, idx, br, logdet, T, c, scale_factor=2.0, inverse=False, out=None):
+  """One affine coupling (forward or inverse) of x fp32 [n, D] with br fp32 [n * T, 2c]; adds +-logdet of each
+  image to logdet fp32 [n].  `out` may be x (in place).  Returns out."""
+  _jet_args(x, idx, br, logdet, out)
+  n = x.numel() // (2 * T * c)
+  out = torch.empty_like(x) if out is None else out
+  L.call("bv_jet_coupling_fwd", _p(x), _p(idx), _p(br), _p(out), _p(logdet), n, T, c, float(scale_factor),
+         int(bool(inverse)), _stream())
+  return out
+
+
+def jet_coupling_bwd(dy, x, idx, br, dlogdet, T, c, scale_factor=2.0, dx=None, dbr=None):
+  """Backward of jet_coupling_fwd: -> (dx, dbr).  dx fp32 like x receives d x2 (positions idx[D/2:]; `dx` may be
+  dy), dbr bf16 [n * T, 2c] the gradient of br."""
+  _jet_args(dy, x, idx, br, dx, dbr)
+  n = x.numel() // (2 * T * c)
+  dx = torch.empty_like(x) if dx is None else dx
+  if dbr is None:
+    dbr = torch.empty((n * T, 2 * c), dtype=torch.bfloat16, device=x.device)
+  L.call("bv_jet_coupling_bwd", _p(dy), _p(x), _p(idx), _p(br), float(dlogdet), _p(dx), _p(dbr), n, T, c,
+         float(scale_factor), _stream())
+  return dx, dbr
+
+
+def jet_merge_grad(dy, dx1, idx, T, c, dx=None):
+  """dx[:, idx[:D/2]] = dy[:, idx[:D/2]] + dx1 (fp32 [n * T, c]); `dx` may be dy.  Returns dx."""
+  _jet_args(dy, dx1, idx, dx)
+  n = dy.numel() // (2 * T * c)
+  dx = torch.empty_like(dy) if dx is None else dx
+  L.call("bv_jet_merge_grad", _p(dy), _p(dx1), _p(idx), _p(dx), n, T, c, _stream())
+  return dx
+
+
+def jet_bits(z, logdet, grad_scale=None, dz=None):
+  """z fp32 [n, ...], logdet fp32 [n] -> (rows fp32 [3, n], means fp32 [3]): bits, nll, logdet per dimension
+  (each / (D ln 2)).  With grad_scale, dz (fp32 like z, allocated when None) = grad_scale * z; returns
+  (rows, means, dz)."""
+  _jet_args(z, logdet, dz)
+  n = z.shape[0]
+  D = z.numel() // n
+  rows = torch.empty((3, n), dtype=torch.float32, device=z.device)
+  means = torch.empty(3, dtype=torch.float32, device=z.device)
+  if grad_scale is not None and dz is None:
+    dz = torch.empty_like(z)
+  L.call("bv_jet_bits", _p(z), _p(logdet), _p(rows), _p(means), _p(dz) if grad_scale is not None else None,
+         float(grad_scale or 0.0), n, D, _stream())
+  return (rows, means, dz) if grad_scale is not None else (rows, means)
+
+
 # ---- integer evaluation paths -------------------------------------------------------------------
 def top1(logits, labels=None, mask=None, want_idx=True):
   """argmax over classes (+ label gather and masked counts).  Returns (idx int32 [rows] or None,
