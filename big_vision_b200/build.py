@@ -3,6 +3,7 @@
 nvcc cross-compiles without a GPU, so this also runs on a machine without one.
 The .so and the object directory are build products (git-ignored).
 """
+import glob
 import hashlib
 import os
 import subprocess
@@ -31,12 +32,7 @@ def _digest(paths):
 
 def _headers():
   out = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".h", ".cuh"))]
-  out.append(os.path.join(os.path.dirname(HERE), "include", "bv_b200.h"))
-  out.append(os.path.join(os.path.dirname(HERE), "include", "bv_b200_sam.h"))
-  out.append(os.path.join(os.path.dirname(HERE), "include", "bv_b200_distill.h"))
-  out.append(os.path.join(os.path.dirname(HERE), "include", "bv_b200_flexi.h"))
-  out.append(os.path.join(os.path.dirname(HERE), "include", "bv_b200_jet.h"))
-  return out
+  return out + glob.glob(os.path.join(os.path.dirname(HERE), "include", "bv_b200*.h"))
 
 
 def _compile(src):

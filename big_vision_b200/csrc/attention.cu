@@ -556,7 +556,7 @@ int check_attn(const bv_attn_args& a, const char* who) {
 template <int DH>
 int attention_fwd(const bv_attn_args& a, cudaStream_t s) {
   using G = Geo<DH>;
-  int rc = check_attn(a, "bv_attention_fwd");
+  int rc = check_attn(a, "bv_attention_fwd_hd");
   if (rc) return rc;
   FwdDev p;
   p.H = a.H; p.Nq = a.Nq; p.Nk = a.Nk;
@@ -582,22 +582,23 @@ template <int DH>
 int attention_bwd(const bv_attn_bwd_args& g, cudaStream_t s) {
   using G = Geo<DH>;
   const bv_attn_args& a = g.fwd;
-  int rc = check_attn(a, "bv_attention_bwd");
+  int rc = check_attn(a, "bv_attention_bwd_hd");
   if (rc) return rc;
-  if (a.lse == nullptr) { set_error("bv_attention_bwd: lse required"); return BV_ERR_INVALID; }
+  if (a.lse == nullptr) { set_error("bv_attention_bwd_hd: lse required"); return BV_ERR_INVALID; }
   if (g.delta == nullptr) {
-    set_error("bv_attention_bwd: needs the delta [B,H,Nq] fp32 workspace");
+    set_error("bv_attention_bwd_hd: needs the delta [B,H,Nq] fp32 workspace");
     return BV_ERR_INVALID;
   }
   if ((reinterpret_cast<uintptr_t>(g.d_o) & 15) || (g.lddo % 8) || (g.bsdo % 8)) {
-    set_error("bv_attention_bwd: d_o must be 16B aligned with strides that are multiples of 8");
+    set_error("bv_attention_bwd_hd: d_o must be 16B aligned with strides that are multiples of 8");
     return BV_ERR_INVALID;
   }
   const void* grads[3] = {g.dq, g.dk, g.dv};
   const int64_t lds[3] = {g.lddq, g.lddk, g.lddv}, bss[3] = {g.bsdq, g.bsdk, g.bsdv};
   for (int i = 0; i < 3; ++i) {
     if (grads[i] == nullptr || (reinterpret_cast<uintptr_t>(grads[i]) & 15) || (lds[i] % 8) || (bss[i] % 8)) {
-      set_error("bv_attention_bwd: dq / dk / dv must be non-null, 16B aligned, with strides that are multiples of 8");
+      set_error("bv_attention_bwd_hd: dq / dk / dv must be non-null, 16B aligned, with strides that are multiples "
+                "of 8");
       return BV_ERR_INVALID;
     }
   }
@@ -649,13 +650,11 @@ int attention_bwd(const bv_attn_bwd_args& g, cudaStream_t s) {
 
 extern "C" {
 
-int bv_attention_fwd(const bv_attn_args* args, void* stream) { return bv_attention_fwd_hd(args, 64, stream); }
-
 int bv_attention_fwd_hd(const bv_attn_args* args, int32_t head_dim, void* stream) {
   using namespace bv;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (!args) { set_error("bv_attention_fwd: null args"); return BV_ERR_INVALID; }
-  int rc = check_head_dim(head_dim, "bv_attention_fwd");
+  if (!args) { set_error("bv_attention_fwd_hd: null args"); return BV_ERR_INVALID; }
+  int rc = check_head_dim(head_dim, "bv_attention_fwd_hd");
   if (rc) return rc;
   const bv_attn_args& a = *args;
   switch (head_dim) {
@@ -667,14 +666,11 @@ int bv_attention_fwd_hd(const bv_attn_args* args, int32_t head_dim, void* stream
   }
 }
 
-int bv_attention_bwd(const bv_attn_bwd_args* args, void* stream) { return bv_attention_bwd_hd(args, 64, stream); }
-
-// args->dq_accum is ignored (kept for the struct layout)
 int bv_attention_bwd_hd(const bv_attn_bwd_args* args, int32_t head_dim, void* stream) {
   using namespace bv;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (!args) { set_error("bv_attention_bwd: null args"); return BV_ERR_INVALID; }
-  int rc = check_head_dim(head_dim, "bv_attention_bwd");
+  if (!args) { set_error("bv_attention_bwd_hd: null args"); return BV_ERR_INVALID; }
+  int rc = check_head_dim(head_dim, "bv_attention_bwd_hd");
   if (rc) return rc;
   const bv_attn_bwd_args& g = *args;
   switch (head_dim) {

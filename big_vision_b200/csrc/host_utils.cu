@@ -97,7 +97,7 @@ int make_tmap(CUtensorMap* out, CUtensorMapDataType dt, int rank, const void* pt
 extern "C" {
 
 const char* bv_last_error_string(void) { return bv::g_err; }
-int bv_version(void) { return 100; }
+int bv_version(void) { return 101; }
 
 int bv_device_supported(void) {
   int dev = 0;

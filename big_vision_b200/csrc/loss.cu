@@ -259,15 +259,6 @@ int bv_softmax_contrastive_loss(const float* dots, int64_t n, int64_t B, int64_t
   return check_cuda(cudaGetLastError(), "finish_sums_kernel launch");
 }
 
-int bv_sigmoid_xent(const float* logits, const float* labels, float* loss, float* dlogits,
-                    float* row_loss_ws, int64_t n, int32_t C, void* stream) {
-  return bv_sigmoid_xent_ld(logits, C, labels, C, loss, dlogits, C, row_loss_ws, n, C, stream);
-}
-int bv_softmax_xent(const float* logits, const float* labels, float* loss, float* dlogits,
-                    float* row_loss_ws, int64_t n, int32_t C, void* stream) {
-  return bv_softmax_xent_ld(logits, C, labels, C, loss, dlogits, C, row_loss_ws, n, C, stream);
-}
-
 int bv_sigmoid_xent_ld(const float* logits, int64_t ldx, const float* labels, int64_t ldy, float* loss,
                        float* dlogits, int64_t ldd, float* row_loss, int64_t n, int32_t C, void* stream) {
   using namespace bv;

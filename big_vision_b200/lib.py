@@ -1,4 +1,4 @@
-"""ctypes binding of libbv_b200.so (C ABI declared in include/bv_b200.h).
+"""ctypes binding of libbv_b200.so (C ABI declared in include/bv_b200*.h).
 
 The product path has no fallback: if the library is missing, or a call is made
 without a compute-capability-9.x device, this module raises.
@@ -12,8 +12,14 @@ LIB_PATH = os.environ.get("BV_LIB_PATH") or os.path.join(_HERE, "libbv_b200.so")
 
 c_i32, c_i64, c_f32, c_vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p
 
+# the #defines of include/bv_b200*.h that Python needs
 F32, BF16 = 0, 1
 EPI_NONE, EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_RESID, EPI_DGELU, EPI_BIAS_GELU_ACT = 0, 1, 2, 3, 4, 5
+LOSS_WS_FLOATS = 8192      # BV_LOSS_WS_FLOATS
+SAM_WS_FLOATS = 2048       # BV_SAM_WS_FLOATS
+# BV_DIST_*: the kinds of dist(); BV_DISTILL_*: the outputs of bv_distill_loss, in order
+DIST_KINDS = {"euclidean": 0, "l2": 1, "hard": 2, "kl": 3, "logsoftmax_euclidean": 4, "agree": 5}
+DISTILL_OUTPUTS = ("distance", "entropy_student", "entropy_teacher", "task_loss_student", "task_loss_teacher")
 
 
 class GemmArgs(ctypes.Structure):
@@ -39,7 +45,7 @@ class AttnBwdArgs(ctypes.Structure):
               ("lddq", c_i64), ("lddk", c_i64), ("lddv", c_i64),
               ("bsdq", c_i64), ("bsdk", c_i64), ("bsdv", c_i64),
               ("dq_colsum", c_vp), ("dk_colsum", c_vp), ("dv_colsum", c_vp),
-              ("delta", c_vp), ("dq_accum", c_vp)]
+              ("delta", c_vp)]
 
 
 class AdamArgs(ctypes.Structure):
@@ -60,14 +66,14 @@ class AdafactorArgs(ctypes.Structure):
               ("gnorm_sq", c_vp), ("upd_sq", c_vp), ("param_sq", c_vp)]
 
 
-# name -> argtypes (restype is int unless noted).  Mirrors include/bv_b200.h one to one.
+# name -> argtypes (restype is int).  Mirrors the functions of include/bv_b200*.h one to one, all exported
+# from the same library.
 SIGNATURES = {
+    # include/bv_b200.h
     "bv_gemm": [ctypes.POINTER(GemmArgs), c_vp],
     "bv_layernorm_fwd": [c_vp, c_i32, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_i64, c_i32, c_f32, c_vp],
     "bv_layernorm_bwd": [c_vp, c_i32, c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp,
                          c_vp, c_i64, c_i32, c_vp],
-    "bv_attention_fwd": [ctypes.POINTER(AttnArgs), c_vp],
-    "bv_attention_bwd": [ctypes.POINTER(AttnBwdArgs), c_vp],
     "bv_attention_fwd_hd": [ctypes.POINTER(AttnArgs), c_i32, c_vp],
     "bv_attention_bwd_hd": [ctypes.POINTER(AttnBwdArgs), c_i32, c_vp],
     "bv_patchify": [c_vp, c_vp, c_i64, c_i32, c_i32, c_i32, c_i32, c_vp],
@@ -96,8 +102,6 @@ SIGNATURES = {
                        c_vp, c_vp, c_vp],
     "bv_softmax_contrastive_loss": [c_vp, c_i64, c_i64, c_i64, c_i64, c_vp, c_i64, c_f32, c_vp, c_i64, c_vp, c_vp,
                                     c_vp, c_vp, c_vp],
-    "bv_sigmoid_xent": [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp],
-    "bv_softmax_xent": [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp],
     "bv_sigmoid_xent_ld": [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp],
     "bv_softmax_xent_ld": [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_i32, c_vp],
     "bv_adam_step": [ctypes.POINTER(AdamArgs), c_vp],
@@ -108,34 +112,18 @@ SIGNATURES = {
     "bv_retrieval_ranks": [c_vp, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp],
     "bv_version": [],
     "bv_device_supported": [],
-}
-
-# include/bv_b200_sam.h (GSAM / SAM), one to one; exported from the same library
-SAM_SIGNATURES = {
+    # include/bv_b200_sam.h (GSAM / SAM)
     "bv_sam_perturb": [c_vp, c_vp, c_vp, c_f32, c_f32, c_i32, c_vp, c_vp, c_i64, c_vp],
     "bv_sam_dots": [c_vp, c_vp, c_vp, c_vp, c_i64, c_vp],
     "bv_gsam_combine": [c_vp, c_vp, c_vp, c_vp, c_f32, c_i32, c_i64, c_vp],
-}
-SAM_WS_FLOATS = 2048       # BV_SAM_WS_FLOATS
-
-# include/bv_b200_distill.h (distillation), one to one; exported from the same library
-DISTILL_SIGNATURES = {
+    # include/bv_b200_distill.h (distillation)
     "bv_distill_loss": [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i32, c_f32, c_f32, c_i32, c_vp, c_i64, c_vp, c_vp,
                         c_i64, c_i32, c_vp],
     "bv_distance": [c_vp, c_i64, c_vp, c_i64, c_i32, c_f32, c_f32, c_f32, c_i32, c_vp, c_i64, c_i32, c_vp],
-}
-# BV_DIST_*: the kinds of dist(); BV_DISTILL_*: the outputs of bv_distill_loss, in order
-DIST_KINDS = {"euclidean": 0, "l2": 1, "hard": 2, "kl": 3, "logsoftmax_euclidean": 4, "agree": 5}
-DISTILL_OUTPUTS = ("distance", "entropy_student", "entropy_teacher", "task_loss_student", "task_loss_teacher")
-
-# include/bv_b200_flexi.h (FlexiViT resampling), one to one; exported from the same library
-FLEXI_SIGNATURES = {
+    # include/bv_b200_flexi.h (FlexiViT resampling)
     "bv_resample_fwd": [c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp],
     "bv_resample_bwd": [c_vp, c_vp, c_vp, c_i32, c_i32, c_i64, c_vp],
-}
-
-# include/bv_b200_jet.h (Jet normalizing flow), one to one; exported from the same library
-JET_SIGNATURES = {
+    # include/bv_b200_jet.h (Jet normalizing flow)
     "bv_jet_dequantize_patchify": [c_vp, c_vp, c_i64, c_i32, c_i32, c_i32, c_i32, ctypes.c_uint64, ctypes.c_uint64,
                                    c_i64, c_f32, c_vp],
     "bv_jet_unpatchify": [c_vp, c_vp, c_i64, c_i32, c_i32, c_i32, c_i32, c_vp],
@@ -163,8 +151,7 @@ def load():
         f"{LIB_PATH} not found: build it with `python -m big_vision_b200.build` "
         "(there is no CPU or eager fallback for the kernels).")
   lib = ctypes.CDLL(LIB_PATH)
-  for name, argtypes in {**SIGNATURES, **SAM_SIGNATURES, **DISTILL_SIGNATURES, **FLEXI_SIGNATURES,
-                         **JET_SIGNATURES}.items():
+  for name, argtypes in SIGNATURES.items():
     fn = getattr(lib, name)   # raises AttributeError if the symbol is missing
     fn.argtypes = argtypes
     fn.restype = ctypes.c_int
@@ -182,11 +169,10 @@ def check(rc, what):
 
 # kernels launched by this process through the C ABI (bench.py reports it as gpu_launches)
 LAUNCHES = [0]
-_LAUNCHES_PER_CALL = {"bv_embed_bwd": 2, "bv_retrieval_ranks": 2, "bv_siglip_loss": 2,
-                      "bv_sigmoid_xent": 2, "bv_softmax_xent": 2, "bv_sigmoid_xent_ld": 2, "bv_softmax_xent_ld": 2,
+_LAUNCHES_PER_CALL = {"bv_attention_bwd_hd": 3, "bv_embed_bwd": 2, "bv_retrieval_ranks": 2, "bv_siglip_loss": 2,
+                      "bv_sigmoid_xent_ld": 2, "bv_softmax_xent_ld": 2,
                       "bv_softmax_contrastive_loss": 2, "bv_adafactor_step": 4, "bv_sam_dots": 2,
                       "bv_distill_loss": 2, "bv_jet_bits": 2}
-LOSS_WS_FLOATS = 8192      # BV_LOSS_WS_FLOATS
 
 
 # optional in-situ timing of every C-ABI call (bench.py --profile-calls): list of (name, e0, e1)

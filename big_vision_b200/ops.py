@@ -182,7 +182,6 @@ def attention_bwd(do, q, k, v, o, lse, heads, scale=None, dq=None, dk=None, dv=N
                        dv_colsum=dv_colsum.data_ptr() if dv_colsum is not None else None,
                        delta=delta.data_ptr())
   L.call("bv_attention_bwd_hd", ctypes.byref(args), dh, _stream())
-  L.LAUNCHES[0] += 2            # delta pre-kernel + dQ kernel + dK / dV kernel
   return dq, dk, dv
 
 

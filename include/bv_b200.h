@@ -106,9 +106,8 @@ int bv_layernorm_bwd(const void* dy, int dy_dtype, const void* x, int x_dtype, c
  * (flax MultiHeadDotProductAttention core: models/vit.py:93-98, :176-178).  Keys stream through
  * on-chip memory in 64-key blocks (online combination of per-block softmax statistics), so every
  * sequence length takes the same path.
- * Head dim dh: 64, 72, 80, 96 or 104 (ViT Ti..L, So400m, H, g-opt / G-opt, G).  bv_attention_fwd /
- * bv_attention_bwd are dh = 64; the _hd entry points take dh and refuse any other value with
- * BV_ERR_UNSUPPORTED before touching the device.
+ * Head dim dh: 64, 72, 80, 96 or 104 (ViT Ti..L, So400m, H, g-opt / G-opt, G).  The entry points take
+ * dh and refuse any other value with BV_ERR_UNSUPPORTED before touching the device.
  * q/k/v/o are bf16 strided views: element (b, t, h*dh + j) at
  * base + b*bs + t*ld + h*dh + j  (e.g. column slices of the fused QKV GEMM output).
  * lse [B,H,Nq] fp32 = log sum_j exp(scale * q_i.k_j) is saved for the backward.
@@ -120,7 +119,6 @@ typedef struct bv_attn_args {
   int64_t bsq, bsk, bsv, bso;
   float scale;
 } bv_attn_args;
-int bv_attention_fwd(const bv_attn_args* args, void* stream);
 int bv_attention_fwd_hd(const bv_attn_args* args, int32_t head_dim, void* stream);
 typedef struct bv_attn_bwd_args {
   bv_attn_args fwd;            /* same q,k,v,o,lse as the forward call */
@@ -131,11 +129,9 @@ typedef struct bv_attn_bwd_args {
    * gradients of the projections that produced q / k / v */
   float* dq_colsum; float* dk_colsum; float* dv_colsum;
   /* REQUIRED workspace: delta [B,H,Nq] fp32 = rowsum(O o dO).  dq, dk and dv are each summed in a
-   * fixed order inside one kernel (reproducible bit for bit), with no other workspace.
-   * dq_accum is IGNORED and may be NULL; it is kept so that the struct layout stays the same. */
-  float* delta; float* dq_accum;
+   * fixed order inside one kernel (reproducible bit for bit), with no other workspace. */
+  float* delta;
 } bv_attn_bwd_args;
-int bv_attention_bwd(const bv_attn_bwd_args* args, void* stream);
 int bv_attention_bwd_hd(const bv_attn_bwd_args* args, int32_t head_dim, void* stream);
 
 /* ---------------------------------------------------------------------------------
@@ -239,16 +235,11 @@ int bv_softmax_contrastive_loss(const float* dots, int64_t n, int64_t B, int64_t
                                 const float* t_param, int64_t global_B, float weight, void* G, int64_t ldg,
                                 float* loss, float* dt, float* ncorrect, float* rows_ws, void* stream);
 /* utils.py:236-243 / 276-281 : mean over n rows; loss is accumulated; dlogits may be NULL.
- * row_loss_ws: NULL = atomics; [n] floats = per-row losses + fixed-order sum (deterministic). */
-int bv_sigmoid_xent(const float* logits, const float* labels, float* loss, float* dlogits,
-                    float* row_loss_ws, int64_t n, int32_t C, void* stream);
-int bv_softmax_xent(const float* logits, const float* labels, float* loss, float* dlogits,
-                    float* row_loss_ws, int64_t n, int32_t C, void* stream);
-/* The same losses on row-strided logits [n, ld_logits], labels [n, ld_labels] and dlogits
- * [n, ld_dlogits] (columns 0..C-1 used).  The dlogits columns C..ld_dlogits-1 are written as zeros, so
- * a classifier head stored with padded columns takes the gradient as its GEMM operand unchanged.
- * Any ld < C: BV_ERR_INVALID before any CUDA call.  bv_sigmoid_xent / bv_softmax_xent are these calls
- * with every ld = C. */
+ * row_loss_ws: NULL = atomics; [n] floats = per-row losses + fixed-order sum (deterministic).
+ * Row-strided logits [n, ld_logits], labels [n, ld_labels] and dlogits [n, ld_dlogits] (columns 0..C-1
+ * used).  The dlogits columns C..ld_dlogits-1 are written as zeros, so a classifier head stored with
+ * padded columns takes the gradient as its GEMM operand unchanged.  Any ld < C: BV_ERR_INVALID before
+ * any CUDA call. */
 int bv_sigmoid_xent_ld(const float* logits, int64_t ld_logits, const float* labels, int64_t ld_labels, float* loss,
                        float* dlogits, int64_t ld_dlogits, float* row_loss_ws, int64_t n, int32_t C, void* stream);
 int bv_softmax_xent_ld(const float* logits, int64_t ld_logits, const float* labels, int64_t ld_labels, float* loss,

@@ -1,5 +1,14 @@
-"""Shared tiny configurations for the tests (kept small so the CPU oracle runs in seconds)."""
+"""Shared tiny configurations for the tests (kept small so the CPU oracle runs in seconds), and the parse of
+the C ABI headers."""
+import glob
+import os
+import re
+
 import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+# every header of the C ABI of libbv_b200.so
+HEADERS = sorted(glob.glob(os.path.join(ROOT, "include", "bv_b200*.h")))
 
 TINY = dict(
     image=dict(width=64, depth=2, mlp_dim=128, num_heads=1, patch_size=(16, 16), pool_type="map"),
@@ -34,3 +43,9 @@ def synthetic_batch(image_shape, text_shape, vocab, seed=0):
   for i in range(n):
     text[i, :lens[i]] = rng.integers(2, vocab, size=lens[i])
   return image, text
+
+
+def header_functions(path):
+  """Every `bv_name(` of a C header outside its comments: the functions it declares."""
+  src = re.sub(r"/\*.*?\*/", "", open(path).read(), flags=re.S)
+  return set(re.findall(r"\b(bv_[a-z0-9_]+)\s*\(", src))

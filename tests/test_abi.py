@@ -1,4 +1,5 @@
-"""CPU: the C-ABI library builds, loads and exports every symbol include/bv_b200*.h declare;
+"""CPU: the C-ABI library builds, loads and exports every symbol include/bv_b200*.h declare, the binding
+and the header constants match the headers, each header is plain C that a C program can link against, and
 argument validation fails loudly (no compute without a GPU)."""
 import ctypes
 import os
@@ -7,41 +8,46 @@ import re
 import pytest
 
 from big_vision_b200 import lib as L
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADERS = ("bv_b200.h", "bv_b200_sam.h", "bv_b200_distill.h")
+from common import HEADERS, ROOT, header_functions
 
 
-def _header_functions():
-  names = set()
-  for h in HEADERS:
-    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", h)).read(), flags=re.S)
-    names |= set(re.findall(r"\b(bv_[a-z0-9_]+)\s*\(", src))
-  return sorted(names)
+def _declared():
+  return set().union(*(header_functions(h) for h in HEADERS))
 
 
 def test_header_symbols_exported():
   lib = L.load()
-  names = _header_functions()
-  assert len(names) >= 25
+  names = _declared()
+  assert len(names) >= 50
   for n in names:
     assert hasattr(lib, n), f"{n} declared in include/ but not exported"
 
 
 def test_binding_covers_header():
-  """The entry points are defined across the kernel sources, so the three headers together must match the
-  binding one to one."""
-  declared = set(_header_functions()) - {"bv_last_error_string"}
-  bound = set(L.SIGNATURES) | set(L.SAM_SIGNATURES) | set(L.DISTILL_SIGNATURES)
-  assert declared == bound, declared ^ bound
+  """The entry points are defined across the kernel sources, so the headers together must match the binding
+  one to one."""
+  declared = _declared() - {"bv_last_error_string"}
+  assert declared == set(L.SIGNATURES), declared ^ set(L.SIGNATURES)
+
+
+def test_header_constants_equal_their_python_mirrors():
+  defines = {}
+  for h in HEADERS:
+    defines.update((k, int(v)) for k, v in re.findall(r"#define BV_([A-Z0-9_]+)\s+(\d+)\b", open(h).read()))
+  prefixed = lambda pre: {k[len(pre):].lower(): v for k, v in defines.items() if k.startswith(pre)}
+  for name in ("F32", "BF16", "LOSS_WS_FLOATS", "SAM_WS_FLOATS"):
+    assert defines[name] == getattr(L, name), name
+  assert prefixed("EPI_") == {k[4:].lower(): getattr(L, k) for k in dir(L) if k.startswith("EPI_")}
+  assert prefixed("DIST_") == L.DIST_KINDS
+  outs = prefixed("DISTILL_")
+  assert outs.pop("outputs") == len(L.DISTILL_OUTPUTS)
+  assert outs == {k.replace("task_loss_", "task_"): i for i, k in enumerate(L.DISTILL_OUTPUTS)}
 
 
 @pytest.mark.parametrize("name,args,message", [
     ("bv_gemm", (None, None), "bv_gemm: null args"),
-    ("bv_attention_fwd", (None, None), "bv_attention_fwd: null args"),
-    ("bv_attention_fwd_hd", (None, 96, None), "bv_attention_fwd: null args"),
-    ("bv_attention_bwd", (None, None), "bv_attention_bwd: null args"),
-    ("bv_attention_bwd_hd", (None, 96, None), "bv_attention_bwd: null args"),
+    ("bv_attention_fwd_hd", (None, 96, None), "bv_attention_fwd_hd: null args"),
+    ("bv_attention_bwd_hd", (None, 96, None), "bv_attention_bwd_hd: null args"),
     ("bv_adam_step", (None, None), "bv_adam_step: null args"),
     ("bv_adafactor_step", (None, None), "bv_adafactor_step: null args"),
 ])
@@ -53,7 +59,7 @@ def test_null_struct_args_are_refused(name, args, message):
 
 def test_version_and_no_gpu_support_flag():
   lib = L.load()
-  assert lib.bv_version() == 100
+  assert lib.bv_version() == 101
   assert lib.bv_device_supported() in (0, 1)
 
 
@@ -99,29 +105,63 @@ def test_bench_workloads_cover_the_five_baseline_configs():
   assert model.img.scan and model.txt.scan and model.img.width == 1024 and model.img.patch_size == (14, 14)
 
 
-def test_header_is_plain_c_and_a_c_program_links(tmp_path):
-  """The boundary is a C ABI: include/bv_b200.h must compile as C99 (and C++), and a C program that includes
-  it links against libbv_b200.so and can call the entry points that need no GPU."""
+# header -> (body of the main() of a C program that calls entry points refused before any launch, the integers
+# it prints, a name in the error string it prints after them)
+C_PROGRAMS = {
+    "bv_b200.h": (
+        '  int rc = bv_colsum(NULL, 1, NULL, 4, 7, 7, NULL);   /* 7 columns */\n'
+        '  printf("%d %d %s\\n", bv_version(), rc, bv_last_error_string());\n',
+        [101, -1], "bv_colsum"),
+    "bv_b200_sam.h": (
+        '  int rc = bv_sam_dots(NULL, NULL, NULL, NULL, 8, NULL);\n'
+        '  printf("%d %d %s\\n", BV_SAM_WS_FLOATS, rc, bv_last_error_string());\n',
+        [L.SAM_WS_FLOATS, -1], "bv_sam_dots"),
+    "bv_b200_distill.h": (
+        '  /* a distance without a training kernel, a stride < C */\n'
+        '  int a = bv_distill_loss(NULL, 8, NULL, 8, NULL, 0, BV_DIST_L2, 1.f, 0.f, 0, NULL, 0, NULL, NULL, 4, 8,'
+        ' NULL);\n'
+        '  int b = bv_distance(NULL, 4, NULL, 8, BV_DIST_AGREE, 0.f, 1.f, 0.f, 1, NULL, 4, 8, NULL);\n'
+        '  printf("%d %d %d %s\\n", BV_DISTILL_OUTPUTS, a, b, bv_last_error_string());\n',
+        [len(L.DISTILL_OUTPUTS), -3, -1], "bv_distance"),
+    "bv_b200_flexi.h": (
+        '  /* J not a multiple of 4, a null matrix */\n'
+        '  float m = 1.f;\n'
+        '  int a = bv_resample_fwd(&m, &m, &m, 1, 1, 6, NULL);\n'
+        '  int b = bv_resample_bwd(NULL, &m, &m, 1, 1, 4, NULL);\n'
+        '  printf("%d %d %s\\n", a, b, bv_last_error_string());\n',
+        [-1, -1], "bv_resample_bwd"),
+    "bv_b200_jet.h": (
+        '  /* H not a multiple of ps, a null buffer */\n'
+        '  float m = 1.f;\n'
+        '  int a = bv_jet_unpatchify(&m, &m, 1, 6, 8, 3, 4, NULL);\n'
+        '  int b = bv_jet_bits(&m, NULL, &m, &m, NULL, 1.f, 1, 1, NULL);\n'
+        '  printf("%d %d %s\\n", a, b, bv_last_error_string());\n',
+        [-1, -1], "bv_jet_bits"),
+}
+
+
+@pytest.mark.parametrize("header", [os.path.basename(h) for h in HEADERS])
+def test_header_is_plain_c_and_a_c_program_links(tmp_path, header):
+  """The boundary is a C ABI: each header must compile as C99 (and C++), and a C program that includes it
+  links against libbv_b200.so and can call the entry points that need no GPU."""
   import shutil
   import subprocess
   if shutil.which("gcc") is None:
     pytest.skip("no gcc")
   L.load()
-  hdr = os.path.join(ROOT, "include", "bv_b200.h")
+  hdr = os.path.join(ROOT, "include", header)
   subprocess.run(["gcc", "-std=c99", "-Wall", "-Wextra", "-Werror", "-fsyntax-only", "-x", "c", hdr], check=True)
   subprocess.run(["g++", "-std=c++17", "-fsyntax-only", "-x", "c++", hdr], check=True)
+  body, ints, name = C_PROGRAMS[header]
   src = tmp_path / "main.c"
-  src.write_text('#include <stdio.h>\n#include "bv_b200.h"\n'
-                 'int main(void) {\n'
-                 '  int rc = bv_colsum(NULL, 1, NULL, 4, 7, 7, NULL);   /* 7 columns: rejected before any launch */\n'
-                 '  printf("%d %d %s\\n", bv_version(), rc, bv_last_error_string());\n'
-                 '  return 0;\n}\n')
+  src.write_text(f'#include <stdio.h>\n#include "{header}"\nint main(void) {{\n{body}  return 0;\n}}\n')
   libdir = os.path.dirname(os.path.abspath(L.LIB_PATH))
   exe = tmp_path / "main"
   subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe),
                   "-L", libdir, "-lbv_b200", f"-Wl,-rpath,{libdir}"], check=True)
-  out = subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split(None, 2)
-  assert out[0] == "100" and int(out[1]) < 0 and len(out[2].strip()) > 0
+  out = subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout
+  fields = out.split(None, len(ints))
+  assert [int(v) for v in fields[:-1]] == ints and name in fields[-1], out
 
 
 def test_bench_refuses_to_run_the_product_arm_without_a_gpu():

@@ -1,6 +1,6 @@
 """The attention backward as two kernels that each own their outputs (dQ per query block, dK / dV per
 key block): every head dim against autograd through the fp64 reference on shapes with several key
-blocks and ragged edges, bit-for-bit reproducibility, the raw C ABI with no dq_accum, and the memory
+blocks and ragged edges, bit-for-bit reproducibility, the raw C ABI call, and the memory
 one call allocates (no workspace that grows with the number of key blocks)."""
 import ctypes
 import math
@@ -99,7 +99,7 @@ def test_backward_is_bitwise_reproducible(ops, dh):
 
 @pytest.mark.parametrize("dh", [64, 104])
 def test_raw_abi_without_dq_accum(ops, dh):
-  """bv_attention_bwd_hd with dq_accum = NULL gives the bits of ops.attention_bwd."""
+  """bv_attention_bwd_hd called through the raw C ABI gives the bits of ops.attention_bwd."""
   from big_vision_b200 import lib as L
   B, H, N = 2, 3, 197
   d = H * dh
@@ -113,7 +113,7 @@ def test_raw_abi_without_dq_accum(ops, dh):
   delta = torch.empty(B, H, N, device="cuda")
   a = L.AttnBwdArgs(fwd=f, d_o=do.data_ptr(), lddo=d, bsdo=N * d, dq=dq.data_ptr(), dk=dk.data_ptr(),
                     dv=dv.data_ptr(), lddq=d, lddk=d, lddv=d, bsdq=N * d, bsdk=N * d, bsdv=N * d,
-                    delta=delta.data_ptr(), dq_accum=None)
+                    delta=delta.data_ptr())
   L.call("bv_attention_bwd_hd", ctypes.byref(a), dh, None)
   torch.cuda.synchronize()
   for got, ref in zip((dq, dk, dv), want):

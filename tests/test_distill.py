@@ -1,12 +1,8 @@
 """CPU: distillation (trainers/proj/distill, evaluators/proj/distill) -- its float64 oracle against closed
 forms, config parsing and the refused distances, the choice of each model's input, the evaluator's summary,
-and the C ABI of include/bv_b200_distill.h (exported, bound, covered by a GPU test, plain C)."""
-import ast
+and the refusal of CPU tensors by the distillation ops."""
 import math
 import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -15,14 +11,6 @@ import torch
 import distill_oracle as DO
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "bv_b200_distill.h")
-
-# entry point -> the GPU tests (tests/test_distill_gpu.py) that check it directly
-COVERAGE = {
-    "bv_distill_loss": ["test_distill_loss_elementwise", "test_distill_loss_scalar_path_and_accumulate",
-                        "test_distill_loss_extreme_logits_and_clip", "test_distill_loss_bit_identical_across_runs"],
-    "bv_distance": ["test_distance_every_kind", "test_distance_agree_is_exact_on_ties"],
-}
 
 
 def _logits(n, C, seed, scale=3.0):
@@ -193,40 +181,6 @@ def test_predict_fns_are_the_reference_set():
   assert s.tolist() == [[1.0, 1.0]] and t.tolist() == [pytest.approx([0.0, math.log(3.0)])]
 
 
-# ---- C ABI of include/bv_b200_distill.h ----------------------------------------------------------
-def _header_functions():
-  src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
-  return sorted(set(re.findall(r"\b(bv_[a-z0-9_]+)\s*\(", src)))
-
-
-def test_distill_header_exported_bound_and_covered():
-  from big_vision_b200 import lib as L
-  declared = set(_header_functions())
-  assert declared == {"bv_distill_loss", "bv_distance"}
-  lib = L.load()
-  for n in declared:
-    assert hasattr(lib, n), f"{n} declared in include/bv_b200_distill.h but not exported"
-  assert declared == set(L.DISTILL_SIGNATURES)
-  # the Python-side constants are the header's
-  src = open(HEADER).read()
-  kinds = {m[0].lower(): int(m[1]) for m in re.findall(r"#define BV_DIST_([A-Z0-9_]+) (\d+)", src)}
-  assert kinds == L.DIST_KINDS
-  outs = {m[0].lower(): int(m[1]) for m in re.findall(r"#define BV_DISTILL_([A-Z_]+) (\d+)", src)}
-  assert outs.pop("outputs") == len(L.DISTILL_OUTPUTS)
-  short = lambda k: k.replace("task_loss_", "task_")
-  assert outs == {short(k): i for i, k in enumerate(L.DISTILL_OUTPUTS)}
-  assert set(COVERAGE) == declared
-  tree = ast.parse(open(os.path.join(ROOT, "tests", "test_distill_gpu.py")).read())
-  gpu_file = any(isinstance(n, ast.Assign) and any(getattr(t, "id", "") == "pytestmark" for t in n.targets)
-                 and "gpu" in ast.unparse(n.value) for n in tree.body)
-  assert gpu_file, "tests/test_distill_gpu.py must be marked gpu"
-  tests = {n.name: n for n in tree.body if isinstance(n, ast.FunctionDef) and n.name.startswith("test_")}
-  for fn, names in COVERAGE.items():
-    for t in names:
-      assert t in tests, f"{fn}: {t} is not a test in tests/test_distill_gpu.py"
-      assert fn.replace("bv_", "ops.") in ast.unparse(tests[t]), (fn, t)
-
-
 def test_distill_ops_refuse_cpu_tensors():
   from big_vision_b200 import lib as L
   from big_vision_b200 import ops
@@ -240,27 +194,3 @@ def test_distill_ops_refuse_cpu_tensors():
     dd.dist(x, x, "kl")
   with pytest.raises(ValueError, match="Unknown kind"):
     ops.distance(x, x, "cosine")
-
-
-def test_distill_header_is_plain_c_and_a_c_program_links(tmp_path):
-  from big_vision_b200 import lib as L
-  if shutil.which("gcc") is None:
-    pytest.skip("no gcc")
-  L.load()
-  subprocess.run(["gcc", "-std=c99", "-Wall", "-Wextra", "-Werror", "-fsyntax-only", "-x", "c", HEADER], check=True)
-  subprocess.run(["g++", "-std=c++17", "-fsyntax-only", "-x", "c++", HEADER], check=True)
-  src = tmp_path / "main.c"
-  src.write_text('#include <stdio.h>\n#include "bv_b200_distill.h"\n'
-                 'int main(void) {\n'
-                 '  /* both are rejected before any launch: a distance without a training kernel, a stride < C */\n'
-                 '  int a = bv_distill_loss(NULL, 8, NULL, 8, NULL, 0, BV_DIST_L2, 1.f, 0.f, 0, NULL, 0, NULL, NULL, 4, 8,'
-                 ' NULL);\n'
-                 '  int b = bv_distance(NULL, 4, NULL, 8, BV_DIST_AGREE, 0.f, 1.f, 0.f, 1, NULL, 4, 8, NULL);\n'
-                 '  printf("%d %d %d %s\\n", BV_DISTILL_OUTPUTS, a, b, bv_last_error_string());\n'
-                 '  return 0;\n}\n')
-  libdir = os.path.dirname(os.path.abspath(L.LIB_PATH))
-  exe = tmp_path / "main"
-  subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe),
-                  "-L", libdir, "-lbv_b200", f"-Wl,-rpath,{libdir}"], check=True)
-  out = subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split(None, 3)
-  assert [int(v) for v in out[:3]] == [len(L.DISTILL_OUTPUTS), -3, -1] and "bv_distance" in out[3]

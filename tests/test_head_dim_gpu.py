@@ -1,8 +1,7 @@
 """GPU parity of the attention kernels at head dims 72, 80 and 96 (So400m, H, g-opt) against the fp64
-reference attention, in place in fused QKV buffers, bit for bit reproducible, the head-dim-64 path
-through the _hd entry points, and the So400m geometry through whole models against the fp64 oracle.
+reference attention, in place in fused QKV buffers, bit for bit reproducible, and the So400m geometry through
+whole models against the fp64 oracle.
 Tolerances as in test_attention_gpu.py / test_model_gpu.py / test_precision_gpu.py."""
-import ctypes
 import json
 import math
 
@@ -139,36 +138,6 @@ def test_head_dim_72_is_bitwise_reproducible(ops):
   r = ops.attention_bwd(do, q, k, v, o1, l1, H)
   t = ops.attention_bwd(do, q, k, v, o1, l1, H)
   for a, b in zip(t, r):
-    assert torch.equal(a, b)
-
-
-def test_head_dim_64_through_hd_entry_points_is_bitwise_the_old_path(ops):
-  """bv_attention_fwd_hd / bv_attention_bwd_hd with head_dim 64 give the bits of bv_attention_fwd / _bwd."""
-  from big_vision_b200 import lib as L
-  B, H, N, dh = 2, 12, 197, 64
-  d = H * dh
-  g = torch.Generator().manual_seed(12)
-  c = _bf(torch.randn(B, N, 3 * d, generator=g)).cuda()
-  do = _bf(torch.randn(B, N, d, generator=g)).cuda()
-  q, k, v = c[:, :, 0:d], c[:, :, d:2 * d], c[:, :, 2 * d:]
-  scale = 1 / 8.0
-  outs = []
-  for fwd, bwd, extra in (("bv_attention_fwd", "bv_attention_bwd", ()),
-                          ("bv_attention_fwd_hd", "bv_attention_bwd_hd", (64,))):
-    o = torch.empty(B, N, d, dtype=torch.bfloat16, device="cuda")
-    lse = torch.empty(B, H, N, device="cuda")
-    f = ops._attn_args(q, k, v, o, lse, H, scale)  # pylint: disable=protected-access
-    L.call(fwd, ctypes.byref(f), *extra, None)
-    dq, dk, dv = (torch.empty(B, N, d, dtype=torch.bfloat16, device="cuda") for _ in range(3))
-    delta = torch.empty(B, H, N, device="cuda")
-    acc = torch.empty((N + 63) // 64, B, N, d, device="cuda")
-    a = L.AttnBwdArgs(fwd=f, d_o=do.data_ptr(), lddo=d, bsdo=N * d, dq=dq.data_ptr(), dk=dk.data_ptr(),
-                      dv=dv.data_ptr(), lddq=d, lddk=d, lddv=d, bsdq=N * d, bsdk=N * d, bsdv=N * d,
-                      delta=delta.data_ptr(), dq_accum=acc.data_ptr())
-    L.call(bwd, ctypes.byref(a), *extra, None)
-    torch.cuda.synchronize()
-    outs.append((o, lse, dq, dk, dv))
-  for a, b in zip(*outs):
     assert torch.equal(a, b)
 
 

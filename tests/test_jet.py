@@ -1,12 +1,8 @@
 """CPU: Jet's host side -- the parameter tree of configs/proj/jet/imagenet64.py, the coupling order, the mask
 initialisers, the gather tables against the float64 oracle's einsum split and merge, the noise generator
 against numpy, properties of the oracle itself (invertibility, the log-determinant against an autograd
-Jacobian, bits per dimension against scipy), the refusals and the C ABI of include/bv_b200_jet.h."""
-import ast
+Jacobian, bits per dimension against scipy) and the refusals."""
 import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -15,21 +11,6 @@ import torch
 import jet_oracle as JO
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "bv_b200_jet.h")
-
-# every entry point of include/bv_b200_jet.h and the GPU tests (tests/test_jet_gpu.py) that check it
-COVERAGE = {
-    "bv_jet_dequantize_patchify": ["test_dequantize_patchify_is_numpy_bit_for_bit",
-                                   "test_noise_of_a_global_batch_does_not_depend_on_the_rank_count",
-                                   "test_refusals"],
-    "bv_jet_unpatchify": ["test_unpatchify_and_plain_patchify_are_exact", "test_refusals"],
-    "bv_jet_split": ["test_split_and_merge_grad_are_exact", "test_refusals"],
-    "bv_jet_coupling_fwd": ["test_coupling_fwd_elementwise", "test_logdet_and_bits_are_bit_identical_across_runs",
-                            "test_extreme_raw_scales_stay_finite", "test_refusals"],
-    "bv_jet_coupling_bwd": ["test_coupling_bwd_elementwise", "test_extreme_raw_scales_stay_finite"],
-    "bv_jet_merge_grad": ["test_split_and_merge_grad_are_exact"],
-    "bv_jet_bits": ["test_bits_elementwise", "test_logdet_and_bits_are_bit_identical_across_runs"],
-}
 IMAGENET64 = dict(depth=32, block_depth=2, emb_dim=512, num_heads=8,
                   kinds=("channels", "channels", "channels", "channels", "spatial"),
                   channels_coupling_projs=("random",),
@@ -334,32 +315,6 @@ def test_half_tokens_that_are_not_a_multiple_of_8_are_refused(ps, C):
     jet.Model(**{**TINY, "ps": ps}).specs((16, 16), C)
 
 
-# ---- C ABI of include/bv_b200_jet.h -----------------------------------------------------------------------
-def _header_functions():
-  src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
-  return sorted(set(re.findall(r"\b(bv_[a-z0-9_]+)\s*\(", src)))
-
-
-def test_jet_header_exported_bound_and_covered():
-  from big_vision_b200 import lib as L
-  declared = set(_header_functions())
-  assert len(declared) == 7 and all(n.startswith("bv_jet_") for n in declared)
-  lib = L.load()
-  for n in declared:
-    assert hasattr(lib, n), f"{n} declared in include/bv_b200_jet.h but not exported"
-  assert declared == set(L.JET_SIGNATURES)
-  assert set(COVERAGE) == declared
-  tree = ast.parse(open(os.path.join(ROOT, "tests", "test_jet_gpu.py")).read())
-  gpu_file = any(isinstance(n, ast.Assign) and any(getattr(t, "id", "") == "pytestmark" for t in n.targets)
-                 and "gpu" in ast.unparse(n.value) for n in tree.body)
-  assert gpu_file, "tests/test_jet_gpu.py must be marked gpu"
-  tests = {n.name: n for n in tree.body if isinstance(n, ast.FunctionDef) and n.name.startswith("test_")}
-  for fn, names in COVERAGE.items():
-    for t in names:
-      assert t in tests, f"{fn}: {t} is not a test in tests/test_jet_gpu.py"
-      assert fn.replace("bv_", "ops.") in ast.unparse(tests[t]), (fn, t)
-
-
 def test_jet_ops_refuse_cpu_tensors():
   from big_vision_b200 import lib as L
   from big_vision_b200 import ops
@@ -377,27 +332,3 @@ def test_jet_ops_refuse_cpu_tensors():
       call()
   with pytest.raises(L.BvError, match="contiguous"):
     ops.jet_split(x.double(), idx, 4, 8)
-
-
-def test_jet_header_is_plain_c_and_a_c_program_links(tmp_path):
-  from big_vision_b200 import lib as L
-  if shutil.which("gcc") is None:
-    pytest.skip("no gcc")
-  L.load()
-  subprocess.run(["gcc", "-std=c99", "-Wall", "-Wextra", "-Werror", "-fsyntax-only", "-x", "c", HEADER], check=True)
-  subprocess.run(["g++", "-std=c++17", "-fsyntax-only", "-x", "c++", HEADER], check=True)
-  src = tmp_path / "main.c"
-  src.write_text('#include <stdio.h>\n#include "bv_b200_jet.h"\n'
-                 'int main(void) {\n'
-                 '  /* both are refused before any launch: H not a multiple of ps, a null buffer */\n'
-                 '  float m = 1.f;\n'
-                 '  int a = bv_jet_unpatchify(&m, &m, 1, 6, 8, 3, 4, NULL);\n'
-                 '  int b = bv_jet_bits(&m, NULL, &m, &m, NULL, 1.f, 1, 1, NULL);\n'
-                 '  printf("%d %d %s\\n", a, b, bv_last_error_string());\n'
-                 '  return 0;\n}\n')
-  libdir = os.path.dirname(os.path.abspath(L.LIB_PATH))
-  exe = tmp_path / "main"
-  subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe),
-                  "-L", libdir, "-lbv_b200", f"-Wl,-rpath,{libdir}"], check=True)
-  out = subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split(None, 2)
-  assert [int(v) for v in out[:2]] == [-1, -1] and "bv_jet_bits" in out[2]

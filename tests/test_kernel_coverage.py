@@ -1,12 +1,12 @@
-"""CPU: every entry point of include/bv_b200.h is named here with the GPU test(s) that check it directly
+"""CPU: every entry point of include/bv_b200*.h is named here with the GPU test(s) that check it directly
 against a reference of the same operation (not only through a whole-model test, whose tolerances are far
 too loose to pin one kernel).  A new ABI function without such a test, or a table row that names a test
 that does not exist, fails this file on a machine without a GPU."""
 import ast
 import os
-import re
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from common import HEADERS, ROOT, header_functions
+
 TESTS = os.path.join(ROOT, "tests")
 
 # entry points with nothing to compute on the device
@@ -16,6 +16,10 @@ KE = "test_kernel_edges_gpu"
 KG = "test_kernels_gpu"
 GE = "test_gemm_elementwise_gpu"
 AE = "test_attention_elementwise_gpu"
+SG = "test_gsam_gpu"
+DG = "test_distill_gpu"
+FG = "test_flexi_gpu"
+JG = "test_jet_gpu"
 COVERAGE = {
     "bv_gemm": [f"{KG}::test_dense_forward_epilogues", f"{KG}::test_dense_backward_contractions",
                 "test_gemm_aux_tma_gpu::test_resid_matches_fp32_oracle",
@@ -25,14 +29,10 @@ COVERAGE = {
                 f"{GE}::test_split_k_adds_bias_once"],
     "bv_layernorm_fwd": [f"{KG}::test_layernorm", f"{KG}::test_layernorm_constant_rows_hit_the_variance_clamp"],
     "bv_layernorm_bwd": [f"{KG}::test_layernorm"],
-    "bv_attention_fwd": ["test_head_dim_gpu::test_head_dim_64_through_hd_entry_points_is_bitwise_the_old_path",
-                         f"{AE}::test_dh64_entry_points_match_the_hd_entry_points"],
     "bv_attention_fwd_hd": [f"{KG}::test_attention_forward_backward", "test_head_dim_gpu::test_forward_matches_fp64",
                             f"{AE}::test_zero_queries_average_every_key_once",
                             f"{AE}::test_dominant_key_gives_its_value",
                             f"{AE}::test_forward_and_backward_within_bound"],
-    "bv_attention_bwd": ["test_head_dim_gpu::test_head_dim_64_through_hd_entry_points_is_bitwise_the_old_path",
-                         f"{AE}::test_dh64_entry_points_match_the_hd_entry_points"],
     "bv_attention_bwd_hd": [f"{KG}::test_attention_forward_backward",
                             "test_attention_bwd_split_gpu::test_backward_matches_fp64",
                             f"{AE}::test_forward_and_backward_within_bound"],
@@ -63,8 +63,6 @@ COVERAGE = {
     "bv_siglip_loss": [f"{KG}::test_siglip_loss_slab", f"{KE}::test_siglip_loss_elementwise"],
     "bv_softmax_contrastive_loss": [f"{KG}::test_softmax_contrastive_slab",
                                     f"{KE}::test_softmax_contrastive_at_batch_6144"],
-    "bv_sigmoid_xent": ["test_class_count_gpu::test_xent_ld_with_ld_C_gives_the_bits_of_the_plain_entry_point"],
-    "bv_softmax_xent": ["test_class_count_gpu::test_xent_ld_with_ld_C_gives_the_bits_of_the_plain_entry_point"],
     "bv_sigmoid_xent_ld": [f"{KG}::test_classification_losses", f"{KE}::test_classification_losses_wide_logits"],
     "bv_softmax_xent_ld": [f"{KG}::test_classification_losses", f"{KE}::test_classification_losses_wide_logits"],
     "bv_adam_step": [f"{KG}::test_adam_matches_optax_chain", f"{KE}::test_adam_step_state_and_norms"],
@@ -74,14 +72,33 @@ COVERAGE = {
     "bv_top1": ["test_eval_paths::test_top1_matches_oracle", "test_eval_paths::test_top1_nan_and_zero_shot"],
     "bv_retrieval_ranks": ["test_eval_paths::test_retrieval_ranks_match_stable_argsort",
                            "test_eval_paths::test_retrieval_golden_on_device"],
+    # include/bv_b200_sam.h
+    "bv_sam_perturb": [f"{SG}::test_sam_perturb_elementwise"],
+    "bv_sam_dots": [f"{SG}::test_sam_dots_elementwise", f"{SG}::test_sam_dots_bit_identical_across_runs"],
+    "bv_gsam_combine": [f"{SG}::test_gsam_combine_elementwise", f"{SG}::test_gsam_combine_zero_robust_gradient_is_nan"],
+    # include/bv_b200_distill.h
+    "bv_distill_loss": [f"{DG}::test_distill_loss_elementwise", f"{DG}::test_distill_loss_scalar_path_and_accumulate",
+                        f"{DG}::test_distill_loss_extreme_logits_and_clip",
+                        f"{DG}::test_distill_loss_bit_identical_across_runs"],
+    "bv_distance": [f"{DG}::test_distance_every_kind", f"{DG}::test_distance_agree_is_exact_on_ties"],
+    # include/bv_b200_flexi.h
+    "bv_resample_fwd": [f"{FG}::test_resample_fwd_elementwise", f"{FG}::test_resample_bit_identical_across_runs",
+                        f"{FG}::test_resample_refusals"],
+    "bv_resample_bwd": [f"{FG}::test_resample_bwd_elementwise", f"{FG}::test_resample_bit_identical_across_runs",
+                        f"{FG}::test_resample_refusals"],
+    # include/bv_b200_jet.h
+    "bv_jet_dequantize_patchify": [f"{JG}::test_dequantize_patchify_is_numpy_bit_for_bit",
+                                   f"{JG}::test_noise_of_a_global_batch_does_not_depend_on_the_rank_count",
+                                   f"{JG}::test_refusals"],
+    "bv_jet_unpatchify": [f"{JG}::test_unpatchify_and_plain_patchify_are_exact", f"{JG}::test_refusals"],
+    "bv_jet_split": [f"{JG}::test_split_and_merge_grad_are_exact", f"{JG}::test_refusals"],
+    "bv_jet_coupling_fwd": [f"{JG}::test_coupling_fwd_elementwise",
+                            f"{JG}::test_logdet_and_bits_are_bit_identical_across_runs",
+                            f"{JG}::test_extreme_raw_scales_stay_finite", f"{JG}::test_refusals"],
+    "bv_jet_coupling_bwd": [f"{JG}::test_coupling_bwd_elementwise", f"{JG}::test_extreme_raw_scales_stay_finite"],
+    "bv_jet_merge_grad": [f"{JG}::test_split_and_merge_grad_are_exact"],
+    "bv_jet_bits": [f"{JG}::test_bits_elementwise", f"{JG}::test_logdet_and_bits_are_bit_identical_across_runs"],
 }
-
-
-def _header_functions():
-  """The same parse as test_abi.py: every `bv_name(` outside comments."""
-  src = open(os.path.join(ROOT, "include", "bv_b200.h")).read()
-  src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-  return sorted(set(re.findall(r"\b(bv_[a-z0-9_]+)\s*\(", src)))
 
 
 def _is_gpu_mark(dec):
@@ -92,25 +109,26 @@ def _is_gpu_mark(dec):
 
 
 def _gpu_tests():
-  """module::name of every top-level test function in tests/*_gpu.py, and of those marked gpu in
-  tests/test_eval_paths.py."""
-  out = set()
+  """module::name -> source of every top-level test function in tests/ that is marked gpu, by its module's
+  pytestmark or by its own decorator."""
+  out = {}
   for fn in sorted(os.listdir(TESTS)):
     mod, ext = os.path.splitext(fn)
-    if ext != ".py" or not (mod.endswith("_gpu") or mod == "test_eval_paths"):
+    if ext != ".py" or not mod.startswith("test_"):
       continue
     tree = ast.parse(open(os.path.join(TESTS, fn)).read())
+    gpu_module = any(isinstance(n, ast.Assign) and any(getattr(t, "id", "") == "pytestmark" for t in n.targets)
+                     and _is_gpu_mark(n.value) for n in tree.body)
     for node in tree.body:
-      if isinstance(node, ast.FunctionDef) and node.name.startswith("test_"):
-        if mod == "test_eval_paths" and not any(_is_gpu_mark(d) for d in node.decorator_list):
-          continue
-        out.add(f"{mod}::{node.name}")
+      if isinstance(node, ast.FunctionDef) and node.name.startswith("test_") and (
+          gpu_module or any(_is_gpu_mark(d) for d in node.decorator_list)):
+        out[f"{mod}::{node.name}"] = ast.unparse(node)
   return out
 
 
 def test_table_keys_are_exactly_the_header_entry_points():
-  declared = set(_header_functions()) - EXEMPT
-  assert len(declared) >= 40
+  declared = set().union(*(header_functions(h) for h in HEADERS)) - EXEMPT
+  assert len(declared) >= 50
   missing, extra = declared - set(COVERAGE), set(COVERAGE) - declared
   assert not missing, f"entry points without a direct GPU test in COVERAGE: {sorted(missing)}"
   assert not extra, f"COVERAGE rows for functions the header does not declare: {sorted(extra)}"
@@ -125,8 +143,19 @@ def test_every_named_test_exists_as_a_gpu_test():
       assert t in known, f"{fn}: {t} is not a GPU test function in tests/"
 
 
+def test_feature_header_rows_name_tests_that_call_the_op():
+  """Each entry point of the feature headers (all but bv_b200.h) has one ops function of the same name, and
+  every test its row names calls that function."""
+  known = _gpu_tests()
+  for h in HEADERS:
+    if os.path.basename(h) != "bv_b200.h":
+      for fn in header_functions(h):
+        for t in COVERAGE[fn]:
+          assert fn.replace("bv_", "ops.", 1) in known[t], (fn, t)
+
+
 def test_gemm_and_attention_rows_name_an_element_wise_test():
   """The GEMM and attention entry points are checked per element against fp64, not only against the
   tensor maximum: each of their rows names a test of the element-wise files."""
-  for fn in ("bv_gemm", "bv_attention_fwd", "bv_attention_fwd_hd", "bv_attention_bwd", "bv_attention_bwd_hd"):
+  for fn in ("bv_gemm", "bv_attention_fwd_hd", "bv_attention_bwd_hd"):
     assert any(t.split("::")[0] in (GE, AE) for t in COVERAGE[fn]), fn

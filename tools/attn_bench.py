@@ -1,4 +1,4 @@
-"""Times bv_attention_fwd / bwd at the bench shapes with CUDA events (after warm-up):
+"""Times bv_attention_fwd_hd / bwd_hd at the bench shapes with CUDA events (after warm-up):
   python tools/attn_bench.py [fwd|bwd|both] [--head-dim DH] [--dump DIR]
 env BV_BENCH_SHAPES="B,H,N;..." overrides the shapes.
 FLOPs are counted with the real head dim DH (default 64), not the k16-padded one the kernels compute.
