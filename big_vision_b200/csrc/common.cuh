@@ -46,6 +46,36 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+__device__ __forceinline__ int warp_sum(int v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// CTA sums of N values per thread in the one fixed order of the deterministic reductions (DESIGN.md,
+// "Run-to-run determinism"): a butterfly within each warp, then a butterfly over the warp totals, the
+// lanes past the last warp adding 0.  Every thread gets the same sums.  blockDim.x is a multiple of 32
+// (at most 1024); sh holds 32 * N values and may be reused after the call.
+template <int N, typename T>
+__device__ __forceinline__ void block_sum(T (&v)[N], T* sh) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+#pragma unroll
+  for (int k = 0; k < N; ++k) v[k] = warp_sum(v[k]);
+  if (lane == 0) {
+#pragma unroll
+    for (int k = 0; k < N; ++k) sh[32 * k + warp] = v[k];
+  }
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < N; ++k) v[k] = warp_sum(lane < nw ? sh[32 * k + lane] : T(0));
+  __syncthreads();
+}
+template <typename T>
+__device__ __forceinline__ T block_sum(T v, T* sh) {
+  T a[1] = {v};
+  block_sum(a, sh);
+  return a[0];
+}
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));

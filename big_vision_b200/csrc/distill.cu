@@ -91,29 +91,6 @@ __device__ __forceinline__ Soft block_soft(Soft a, float inv_t, float* sh) {
   return b;
 }
 
-__device__ __forceinline__ float block_sum(float v, float* sh) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  v = warp_sum(v);
-  if (lane == 0) sh[warp] = v;
-  __syncthreads();
-  v = warp_sum(lane < nw ? sh[lane] : 0.f);
-  __syncthreads();
-  return v;
-}
-
-__device__ __forceinline__ int block_sum(int v, int* sh) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if (lane == 0) sh[warp] = v;
-  __syncthreads();
-  v = lane < nw ? sh[lane] : 0;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  return v;
-}
-
 // Block argmax with jnp.argmax's tie rule (the first maximal index), the same in every thread.
 __device__ __forceinline__ int block_argmax(float best, int arg, float* shv, int* shi) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
@@ -271,23 +248,6 @@ distill_loss_kernel(const DistillArgs a) {
   }
 }
 
-// out[k] = (1 / n) sum_i rows[k * n + i] for k = blockIdx.x: thread t sums t, t + 256, ... in index
-// order, then a fixed shared-memory tree.
-__global__ void __launch_bounds__(256)
-distill_finish_kernel(const float* __restrict__ rows, int64_t n, float* __restrict__ out) {
-  __shared__ float sh[256];
-  const int k = blockIdx.x;
-  float acc = 0.f;
-  for (int64_t i = threadIdx.x; i < n; i += 256) acc += rows[k * n + i];
-  sh[threadIdx.x] = acc;
-  __syncthreads();
-  for (int o = 128; o > 0; o >>= 1) {
-    if (static_cast<int>(threadIdx.x) < o) sh[threadIdx.x] += sh[threadIdx.x + o];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) out[k] = sh[0] / static_cast<float>(n);
-}
-
 // The kinds of dist() that are neither `kl` nor `hard`; one CTA of 256 threads per row.
 __global__ void __launch_bounds__(256)
 distance_kernel(const float* __restrict__ sp, int64_t lds, const float* __restrict__ up, int64_t ldu, int kind,
@@ -401,8 +361,9 @@ int bv_distill_loss(const float* student, int64_t ld_student, const float* teach
                          n, C, kind == BV_DIST_HARD ? 1.f : t, ls, accumulate, 1};
   const int lrc = launch_rows(a, kind == BV_DIST_HARD, s);
   if (lrc) return lrc;
-  distill_finish_kernel<<<BV_DISTILL_OUTPUTS, 256, 0, s>>>(rows_ws, n, out);
-  return check_cuda(cudaGetLastError(), "distill_finish_kernel launch");
+  float* outs[BV_DISTILL_OUTPUTS];
+  for (int k = 0; k < BV_DISTILL_OUTPUTS; ++k) outs[k] = out + k;
+  return finish_row_sums(rows_ws, BV_DISTILL_OUTPUTS, n, outs, static_cast<float>(n), false, s);
 }
 
 int bv_distance(const float* student, int64_t ld_student, const float* teacher, int64_t ld_teacher, int32_t kind,

@@ -17,13 +17,6 @@ __device__ __forceinline__ void st_from_float(void* p, int dt, int64_t i, float 
   else reinterpret_cast<float*>(p)[i] = v;
 }
 
-inline unsigned grid_for(int64_t work, int threads, int64_t cap_blocks) {
-  int64_t b = (work + threads - 1) / threads;
-  if (b > cap_blocks) b = cap_blocks;
-  if (b < 1) b = 1;
-  return static_cast<unsigned>(b);
-}
-
 // ---------------------------------------------------------------------------
 // patchify: image [n,H,W,C] fp32 (NHWC) -> patches [n*(H/P)*(W/P), Kp] bf16 with
 // column order (ph, pw, c), the row-major flattening of the HWIO conv kernel
@@ -703,10 +696,7 @@ int bv_row_select(const void* a, const void* b, const float* mask, void* out, in
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0 || N <= 0 || d <= 0 || d % 8) { set_error("bv_row_select: need n,N,d > 0, d %% 8 == 0"); return BV_ERR_INVALID; }
   const int64_t per = static_cast<int64_t>(N) * d / 8;
-  int64_t blocks = (n * per + 255) / 256;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 16;
-  if (blocks > cap) blocks = cap;
-  row_select_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(
+  row_select_kernel<<<grid_for(n * per, 256, num_sms() * 16), 256, 0, s>>>(
       reinterpret_cast<const bf16*>(a), reinterpret_cast<const bf16*>(b), mask,
       reinterpret_cast<bf16*>(out), n, per);
   return check_cuda(cudaGetLastError(), "row_select_kernel launch");
@@ -788,15 +778,12 @@ int bv_mixup(const float* x, float* out, int64_t n, int64_t row_elems, float a, 
   }
   const bool vec = row_elems % 4 == 0 && !(reinterpret_cast<uintptr_t>(x) & 15) &&
                    !(reinterpret_cast<uintptr_t>(out) & 15);
-  const int64_t total = vec ? n * (row_elems / 4) : n * row_elems;
-  int64_t blocks = (total + 255) / 256;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
-  if (blocks > cap) blocks = cap;
+  const unsigned blocks = grid_for(vec ? n * (row_elems / 4) : n * row_elems, 256, num_sms() * 8);
   if (vec) {
-    mixup_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(
-        reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(out), n, row_elems / 4, a);
+    mixup_kernel<<<blocks, 256, 0, s>>>(reinterpret_cast<const float4*>(x), reinterpret_cast<float4*>(out), n,
+                                        row_elems / 4, a);
   } else {
-    mixup_scalar_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(x, out, n, row_elems, a);
+    mixup_scalar_kernel<<<blocks, 256, 0, s>>>(x, out, n, row_elems, a);
   }
   return check_cuda(cudaGetLastError(), "mixup_kernel launch");
 }

@@ -34,6 +34,46 @@ int num_sms() {
   return cached[dev];
 }
 
+namespace {
+struct FinishOuts { float* p[kFinishMaxRows]; };
+
+__global__ void __launch_bounds__(256)
+finish_row_sums_kernel(const float* __restrict__ part, int64_t count, FinishOuts out, float div, int accumulate) {
+  __shared__ float sh[256];
+  static_assert(kFinishMaxRows == 5, "one case per row");
+  float* o;
+  switch (blockIdx.x) {         // out.p[blockIdx.x] would copy out to the stack
+    case 0: o = out.p[0]; break;
+    case 1: o = out.p[1]; break;
+    case 2: o = out.p[2]; break;
+    case 3: o = out.p[3]; break;
+    default: o = out.p[4]; break;
+  }
+  if (o == nullptr) return;     // uniform across the block
+  float acc = 0.f;
+  for (int64_t i = threadIdx.x; i < count; i += 256) acc += part[blockIdx.x * count + i];
+  sh[threadIdx.x] = acc;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if (static_cast<int>(threadIdx.x) < w) sh[threadIdx.x] += sh[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *o = accumulate ? *o + sh[0] : sh[0] / div;
+}
+}  // namespace
+
+int finish_row_sums(const float* part, int K, int64_t count, float* const* out, float div, bool accumulate,
+                    cudaStream_t s) {
+  if (K < 1 || K > kFinishMaxRows) {
+    set_error("finish_row_sums: %d rows, need 1 to %d", K, kFinishMaxRows);
+    return BV_ERR_INVALID;
+  }
+  FinishOuts o = {};
+  for (int k = 0; k < K; ++k) o.p[k] = out[k];
+  finish_row_sums_kernel<<<K, 256, 0, s>>>(part, count, o, div, accumulate ? 1 : 0);
+  return check_cuda(cudaGetLastError(), "finish_row_sums_kernel launch");
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
                                   const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,

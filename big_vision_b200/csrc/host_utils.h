@@ -1,5 +1,6 @@
-// Host-side helpers shared by the launchers: error reporting, TMA descriptor
-// encoding through the driver entry point (no -lcuda link dependency).
+// Host-side helpers shared by the launchers: error reporting, grid sizes, the fixed-order
+// finishing pass, TMA descriptor encoding through the driver entry point (no -lcuda link
+// dependency).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -12,6 +13,23 @@ namespace bv {
 void set_error(const char* fmt, ...);
 int check_cuda(cudaError_t e, const char* what);
 int num_sms();
+
+// Blocks of a grid-stride launch: ceil(work / threads), at most cap_blocks, at least 1.  For a kernel
+// that writes one partial per block this is also the number of partials, so it fixes the summation order.
+inline unsigned grid_for(int64_t work, int threads, int64_t cap_blocks) {
+  int64_t b = (work + threads - 1) / threads;
+  if (b > cap_blocks) b = cap_blocks;
+  if (b < 1) b = 1;
+  return static_cast<unsigned>(b);
+}
+
+// The finishing pass of the deterministic reductions (DESIGN.md, "Run-to-run determinism"), one launch:
+// for each row k < K of part [K, count], thread t of 256 sums entries t, t + 256, ... in index order, a
+// shared-memory tree adds the 256 sums, and then out[k] = sum / div, or out[k] += sum when accumulate.
+// A null out[k] is skipped.  K <= kFinishMaxRows.
+constexpr int kFinishMaxRows = 5;
+int finish_row_sums(const float* part, int K, int64_t count, float* const* out, float div, bool accumulate,
+                    cudaStream_t s);
 
 // Encode a tiled tensor map with 128-byte swizzle (or none).  dims/strides are
 // innermost-first; strides[i] is the byte stride of dim i+1.

@@ -4,9 +4,9 @@
 // is the library's GEMM / attention / LayerNorm path.
 //
 // Determinism: the per-image sums (the coupling log-determinant, the negative log-likelihood) are computed by
-// one CTA per image.  Each thread sums a fixed strided subset of the image in ascending order, the warp
-// reduces with a fixed butterfly and thread 0 adds the warp totals in warp order: no atomics, so every
-// output is the same bit for bit on every run.
+// one CTA per image.  Each thread sums a fixed strided subset of the image in ascending order and block_sum
+// adds the threads' sums in its fixed order; the batch means go through finish_row_sums.  No atomics, so
+// every output is the same bit for bit on every run.
 #include "../../include/bv_b200_jet.h"
 
 #include <cuda_bf16.h>
@@ -108,23 +108,11 @@ __device__ __forceinline__ float sigmoid_stable(float r) {
 // log(sigmoid(r)) = min(r, 0) - log1p(exp(-|r|)): finite for every finite r.
 __device__ __forceinline__ float log_sigmoid_stable(float r) { return fminf(r, 0.f) - log1pf(expf(-fabsf(r))); }
 
-// Sum of v over the CTA in a fixed order; the result is valid in thread 0.
-__device__ __forceinline__ float block_sum(float v, float* warp_tot) {
-  v = warp_sum(v);
-  const int w = threadIdx.x >> 5;
-  if ((threadIdx.x & 31) == 0) warp_tot[w] = v;
-  __syncthreads();
-  float s = 0.f;
-  if (threadIdx.x == 0)
-    for (int i = 0; i < static_cast<int>(blockDim.x >> 5); ++i) s += warp_tot[i];
-  return s;
-}
-
 // One CTA per image b.
 __global__ void __launch_bounds__(kRedThreads)
 coupling_fwd_kernel(const float* x, const int* __restrict__ idx, const float* __restrict__ br, float* y,
                     float* __restrict__ logdet, int T, int c, float scale_factor, float log_scale, int inverse) {
-  __shared__ float warp_tot[kRedThreads / 32];
+  __shared__ float sh[32];
   const int half = T * c;
   const int64_t b = blockIdx.x;
   const float* xb = x + b * 2 * half;
@@ -144,7 +132,7 @@ coupling_fwd_kernel(const float* x, const int* __restrict__ idx, const float* __
     }
     acc += log_sigmoid_stable(raw) + log_scale;
   }
-  const float tot = block_sum(acc, warp_tot);
+  const float tot = block_sum(acc, sh);
   if (threadIdx.x == 0) logdet[b] += inverse ? -tot : tot;
 }
 
@@ -184,7 +172,7 @@ merge_grad_kernel(const float* dy, const float* __restrict__ dx1, const int* __r
 __global__ void __launch_bounds__(kRedThreads)
 bits_rows_kernel(const float* __restrict__ z, const float* __restrict__ logdet, float* __restrict__ rows,
                  float* __restrict__ dz, float grad_scale, int64_t n, int64_t D) {
-  __shared__ float warp_tot[kRedThreads / 32];
+  __shared__ float sh[32];
   const int64_t b = blockIdx.x;
   const float* zb = z + b * D;
   float acc = 0.f;
@@ -193,7 +181,7 @@ bits_rows_kernel(const float* __restrict__ z, const float* __restrict__ logdet, 
     acc = fmaf(v, v, acc);
     if (dz) dz[b * D + k] = grad_scale * v;
   }
-  const float sumsq = block_sum(acc, warp_tot);
+  const float sumsq = block_sum(acc, sh);
   if (threadIdx.x == 0) {
     const double cst = 0.5 * log(2.0 * 3.14159265358979323846) + log(127.5);
     const double norm = static_cast<double>(D) * 0.69314718055994530942;
@@ -202,19 +190,6 @@ bits_rows_kernel(const float* __restrict__ z, const float* __restrict__ logdet, 
     rows[b] = static_cast<float>((nll - ld) / norm);
     rows[n + b] = static_cast<float>(nll / norm);
     rows[2 * n + b] = static_cast<float>(ld / norm);
-  }
-}
-
-// One CTA: the batch means of the three rows, each summed over b in a fixed order.
-__global__ void __launch_bounds__(kRedThreads) bits_means_kernel(const float* __restrict__ rows, float* means,
-                                                                 int64_t n) {
-  __shared__ float warp_tot[kRedThreads / 32];
-  for (int k = 0; k < 3; ++k) {
-    float acc = 0.f;
-    for (int64_t b = threadIdx.x; b < n; b += kRedThreads) acc += rows[k * n + b];
-    const float tot = block_sum(acc, warp_tot);
-    if (threadIdx.x == 0) means[k] = tot / static_cast<float>(n);
-    __syncthreads();     // warp_tot is reused by the next row
   }
 }
 
@@ -327,8 +302,8 @@ int bv_jet_bits(const float* z, const float* logdet, float* rows, float* means, 
   bits_rows_kernel<<<static_cast<unsigned>(n), kRedThreads, 0, s>>>(z, logdet, rows, dz, grad_scale, n, D);
   int rc = check_cuda(cudaGetLastError(), "bits_rows_kernel launch");
   if (rc) return rc;
-  bits_means_kernel<<<1, kRedThreads, 0, s>>>(rows, means, n);
-  return check_cuda(cudaGetLastError(), "bits_means_kernel launch");
+  float* const outs[3] = {means, means + 1, means + 2};
+  return finish_row_sums(rows, 3, n, outs, static_cast<float>(n), false, s);
 }
 
 }  // extern "C"

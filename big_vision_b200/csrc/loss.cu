@@ -20,25 +20,11 @@ __device__ __forceinline__ float log_sigmoid(float y) {
 }
 __device__ __forceinline__ float sigmoid(float y) { return 1.f / (1.f + __expf(-y)); }
 
-__device__ __forceinline__ void block_reduce3(float& a, float& b, float& c, float* sh) {
-  a = warp_sum(a); b = warp_sum(b); c = warp_sum(c);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  if (lane == 0) { sh[warp] = a; sh[32 + warp] = b; sh[64 + warp] = c; }
-  __syncthreads();
-  if (warp == 0) {
-    a = lane < nw ? sh[lane] : 0.f;
-    b = lane < nw ? sh[32 + lane] : 0.f;
-    c = lane < nw ? sh[64 + lane] : 0.f;
-    a = warp_sum(a); b = warp_sum(b); c = warp_sum(c);
-  }
-}
-
 __global__ void __launch_bounds__(256)
 siglip_loss_kernel(const float* __restrict__ dots, int64_t n, int64_t B, int64_t ld,
                    int64_t row_offset, const float* __restrict__ t_param,
                    const float* __restrict__ b_param, float inv_B, bf16* __restrict__ G,
-                   int64_t ldg, float* __restrict__ loss, float* __restrict__ dt,
-                   float* __restrict__ db, float* __restrict__ partials) {
+                   int64_t ldg, float* __restrict__ partials) {
   __shared__ float sh[96];
   const float t = __expf(t_param[0]);
   const float bias = b_param ? b_param[0] : 0.f;
@@ -67,44 +53,14 @@ siglip_loss_kernel(const float* __restrict__ dots, int64_t n, int64_t B, int64_t
     q.y = pack_bf16(g[2], g[3]);
     *reinterpret_cast<uint2*>(G + i * ldg + j0) = q;
   }
-  l_acc *= inv_B;
-  block_reduce3(l_acc, t_acc, b_acc, sh);
+  // one partial per block and scalar, summed in a fixed order by finish_row_sums: the result never
+  // depends on which block finished first (XLA's reductions are run-to-run deterministic too)
+  float sums[3] = {l_acc * inv_B, t_acc, b_acc};
+  block_sum(sums, sh);
   if (threadIdx.x == 0) {
-    if (partials != nullptr) {
-      // deterministic mode: one partial per block, summed in a fixed order by finish_sums_kernel
-      partials[blockIdx.x] = l_acc;
-      partials[gridDim.x + blockIdx.x] = t_acc;
-      partials[2 * gridDim.x + blockIdx.x] = b_acc;
-    } else {
-      atomicAdd(loss, l_acc);
-      if (dt) atomicAdd(dt, t_acc);
-      if (db) atomicAdd(db, b_acc);
-    }
-  }
-}
-
-// Fixed-order finishing pass of the deterministic mode: out[k] += sum_i part[k*count + i].  One
-// block; thread t sums elements t, t+256, ... in index order, then a fixed shared-memory tree.  The
-// result depends only on (count, values), never on which block of the producer finished first --
-// XLA's reductions are run-to-run deterministic and so is this path.
-__global__ void __launch_bounds__(256)
-finish_sums_kernel(const float* __restrict__ part, int64_t count, float* out0, float* out1,
-                   float* out2) {
-  __shared__ float sh[256];
-  float* outs[3] = {out0, out1, out2};
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    if (outs[k] == nullptr) continue;          // uniform across the block
-    float acc = 0.f;
-    for (int64_t i = threadIdx.x; i < count; i += 256) acc += part[k * count + i];
-    sh[threadIdx.x] = acc;
-    __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) {
-      if (static_cast<int>(threadIdx.x) < o) sh[threadIdx.x] += sh[threadIdx.x + o];
-      __syncthreads();
-    }
-    if (threadIdx.x == 0) outs[k][0] += sh[0];
-    __syncthreads();
+    partials[blockIdx.x] = sums[0];
+    partials[gridDim.x + blockIdx.x] = sums[1];
+    partials[2 * gridDim.x + blockIdx.x] = sums[2];
   }
 }
 
@@ -113,7 +69,7 @@ finish_sums_kernel(const float* __restrict__ part, int64_t count, float* out0, f
 //   loss += weight/global_B * sum_i loss_i ;  G_ij = weight/global_B * (softmax_ij - [j == pos]) * exp(t')
 //   dt'  += sum_ij (G_ij / exp(t')) * x_ij ;  ncorrect += #[argmax_j x_ij == pos(i)]   (first max wins)
 // One warp per row; per-row partials (loss, dt', correct) go to `rows_ws` [3, n] and are summed in a
-// fixed order by finish_sums_kernel (deterministic like the other losses).
+// fixed order by finish_row_sums (deterministic like the other losses).
 __global__ void __launch_bounds__(256)
 softmax_contrastive_kernel(const float* __restrict__ dots, int64_t n, int64_t B, int64_t ld, int64_t row_offset,
                            const float* __restrict__ t_param, float scale, bf16* __restrict__ G, int64_t ldg,
@@ -160,7 +116,7 @@ softmax_contrastive_kernel(const float* __restrict__ dots, int64_t n, int64_t B,
 // a head stored with padded columns can feed the [n, ldd] gradient straight to its GEMMs.
 __global__ void __launch_bounds__(256)
 sigmoid_xent_kernel(const float* __restrict__ logits, int64_t ldx, const float* __restrict__ labels, int64_t ldy,
-                    float* __restrict__ loss, float* __restrict__ dlogits, int64_t ldd,
+                    float* __restrict__ dlogits, int64_t ldd,
                     float* __restrict__ row_loss, int64_t n, int C) {
   const int lane = threadIdx.x & 31;
   const int64_t row = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5);
@@ -176,14 +132,12 @@ sigmoid_xent_kernel(const float* __restrict__ logits, int64_t ldx, const float* 
     for (int64_t c = C + lane; c < ldd; c += 32) dlogits[row * ldd + c] = 0.f;
   }
   acc = warp_sum(acc);
-  if (lane == 0) {
-    if (row_loss != nullptr) row_loss[row] = acc * inv_n; else atomicAdd(loss, acc * inv_n);
-  }
+  if (lane == 0) row_loss[row] = acc * inv_n;
 }
 
 __global__ void __launch_bounds__(256)
 softmax_xent_kernel(const float* __restrict__ logits, int64_t ldx, const float* __restrict__ labels, int64_t ldy,
-                    float* __restrict__ loss, float* __restrict__ dlogits, int64_t ldd,
+                    float* __restrict__ dlogits, int64_t ldd,
                     float* __restrict__ row_loss, int64_t n, int C) {
   const int lane = threadIdx.x & 31;
   const int64_t row = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5);
@@ -200,10 +154,7 @@ softmax_xent_kernel(const float* __restrict__ logits, int64_t ldx, const float* 
   se = warp_sum(se); sy = warp_sum(sy); sxy = warp_sum(sxy);
   const float lse = logf(se);
   // -sum y (x - lse) = lse * sum(y) - sum(y x)
-  if (lane == 0) {
-    const float rl = (lse * sy - sxy) * inv_n;
-    if (row_loss != nullptr) row_loss[row] = rl; else atomicAdd(loss, rl);
-  }
+  if (lane == 0) row_loss[row] = (lse * sy - sxy) * inv_n;
   if (dlogits) {
     for (int c = lane; c < C; c += 32) {
       const float x = logits[row * ldx + c] - mx, y = labels[row * ldy + c];
@@ -228,17 +179,19 @@ int bv_siglip_loss(const float* dots, int64_t n, int64_t B, int64_t ld, int64_t 
     set_error("bv_siglip_loss: need n,B > 0 and B, ld, ldg multiples of 4");
     return BV_ERR_INVALID;
   }
-  int64_t blocks = (n * (B / 4) + 255) / 256;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
-  if (blocks > cap) blocks = cap;
+  if (partials == nullptr) {
+    set_error("bv_siglip_loss: need the workspace of BV_LOSS_WS_FLOATS floats");
+    return BV_ERR_INVALID;
+  }
+  unsigned blocks = grid_for(n * (B / 4), 256, num_sms() * 8);
   if (blocks > BV_LOSS_WS_FLOATS / 3) blocks = BV_LOSS_WS_FLOATS / 3;
-  siglip_loss_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(
-      dots, n, B, ld, row_offset, t_param, b_param, 1.0f / static_cast<float>(global_B),
-      reinterpret_cast<bf16*>(G), ldg, loss, dt, db, partials);
+  siglip_loss_kernel<<<blocks, 256, 0, s>>>(dots, n, B, ld, row_offset, t_param, b_param,
+                                            1.0f / static_cast<float>(global_B), reinterpret_cast<bf16*>(G), ldg,
+                                            partials);
   int rc = check_cuda(cudaGetLastError(), "siglip_loss_kernel launch");
-  if (rc || partials == nullptr) return rc;
-  finish_sums_kernel<<<1, 256, 0, s>>>(partials, blocks, loss, dt, db);
-  return check_cuda(cudaGetLastError(), "finish_sums_kernel launch");
+  if (rc) return rc;
+  float* const outs[3] = {loss, dt, db};
+  return finish_row_sums(partials, 3, blocks, outs, 1.f, true, s);
 }
 
 int bv_softmax_contrastive_loss(const float* dots, int64_t n, int64_t B, int64_t ld, int64_t row_offset,
@@ -255,8 +208,8 @@ int bv_softmax_contrastive_loss(const float* dots, int64_t n, int64_t B, int64_t
       rows_ws);
   int rc = check_cuda(cudaGetLastError(), "softmax_contrastive_kernel launch");
   if (rc) return rc;
-  finish_sums_kernel<<<1, 256, 0, s>>>(rows_ws, n, loss, dt, ncorrect);
-  return check_cuda(cudaGetLastError(), "finish_sums_kernel launch");
+  float* const outs[3] = {loss, dt, ncorrect};
+  return finish_row_sums(rows_ws, 3, n, outs, 1.f, true, s);
 }
 
 int bv_sigmoid_xent_ld(const float* logits, int64_t ldx, const float* labels, int64_t ldy, float* loss,
@@ -269,12 +222,15 @@ int bv_sigmoid_xent_ld(const float* logits, int64_t ldx, const float* labels, in
     return BV_ERR_INVALID;
   }
   if (n <= 0) return BV_OK;
-  sigmoid_xent_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(logits, ldx, labels, ldy, loss, dlogits,
-                                                                        ldd, row_loss, n, C);
+  if (row_loss == nullptr) {
+    set_error("bv_sigmoid_xent_ld: need the [n] workspace");
+    return BV_ERR_INVALID;
+  }
+  sigmoid_xent_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(logits, ldx, labels, ldy, dlogits, ldd,
+                                                                        row_loss, n, C);
   int rc = check_cuda(cudaGetLastError(), "sigmoid_xent_kernel launch");
-  if (rc || row_loss == nullptr) return rc;
-  finish_sums_kernel<<<1, 256, 0, s>>>(row_loss, n, loss, nullptr, nullptr);
-  return check_cuda(cudaGetLastError(), "finish_sums_kernel launch");
+  if (rc) return rc;
+  return finish_row_sums(row_loss, 1, n, &loss, 1.f, true, s);
 }
 int bv_softmax_xent_ld(const float* logits, int64_t ldx, const float* labels, int64_t ldy, float* loss,
                        float* dlogits, int64_t ldd, float* row_loss, int64_t n, int32_t C, void* stream) {
@@ -286,12 +242,15 @@ int bv_softmax_xent_ld(const float* logits, int64_t ldx, const float* labels, in
     return BV_ERR_INVALID;
   }
   if (n <= 0) return BV_OK;
-  softmax_xent_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(logits, ldx, labels, ldy, loss, dlogits,
-                                                                        ldd, row_loss, n, C);
+  if (row_loss == nullptr) {
+    set_error("bv_softmax_xent_ld: need the [n] workspace");
+    return BV_ERR_INVALID;
+  }
+  softmax_xent_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(logits, ldx, labels, ldy, dlogits, ldd,
+                                                                        row_loss, n, C);
   int rc = check_cuda(cudaGetLastError(), "softmax_xent_kernel launch");
-  if (rc || row_loss == nullptr) return rc;
-  finish_sums_kernel<<<1, 256, 0, s>>>(row_loss, n, loss, nullptr, nullptr);
-  return check_cuda(cudaGetLastError(), "finish_sums_kernel launch");
+  if (rc) return rc;
+  return finish_row_sums(row_loss, 1, n, &loss, 1.f, true, s);
 }
 
 }  // extern "C"

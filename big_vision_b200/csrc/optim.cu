@@ -12,18 +12,6 @@
 namespace bv {
 namespace {
 
-__device__ __forceinline__ void block_reduce2(float& a, float& b, float* sh) {
-  a = warp_sum(a); b = warp_sum(b);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-  if (lane == 0) { sh[warp] = a; sh[32 + warp] = b; }
-  __syncthreads();
-  if (warp == 0) {
-    a = lane < nw ? sh[lane] : 0.f;
-    b = lane < nw ? sh[32 + lane] : 0.f;
-    a = warp_sum(a); b = warp_sum(b);
-  }
-}
-
 template <bool MU_BF16>
 __global__ void __launch_bounds__(256)
 adam_kernel(float* __restrict__ p, const float* __restrict__ g, void* __restrict__ mu,
@@ -81,10 +69,11 @@ adam_kernel(float* __restrict__ p, const float* __restrict__ g, void* __restrict
       reinterpret_cast<uint2*>(p16)[i] = q;
     }
   }
-  block_reduce2(us, ps, sh);
+  float sums[2] = {us, ps};
+  block_sum(sums, sh);
   if (threadIdx.x == 0) {
-    if (upd_sq) atomicAdd(upd_sq, us);
-    if (param_sq) atomicAdd(param_sq, ps);
+    if (upd_sq) atomicAdd(upd_sq, sums[0]);
+    if (param_sq) atomicAdd(param_sq, sums[1]);
   }
 }
 
@@ -111,17 +100,19 @@ scale_step_kernel(float* __restrict__ p, const float* __restrict__ g, bf16* __re
     p[i] = pp;
     if (p16 != nullptr) p16[i] = __float2bfloat16_rn(pp);
   }
-  block_reduce2(us, ps, sh);
+  float sums[2] = {us, ps};
+  block_sum(sums, sh);
   if (threadIdx.x == 0) {
-    if (upd_sq) atomicAdd(upd_sq, us);
-    if (param_sq) atomicAdd(param_sq, ps);
+    if (upd_sq) atomicAdd(upd_sq, sums[0]);
+    if (param_sq) atomicAdd(param_sq, sums[1]);
   }
 }
 
-__global__ void __launch_bounds__(256)
+// 8 blocks per SM, the grid's cap, all resident at once: at most 32 registers
+__global__ void __launch_bounds__(256, 8)
 sumsq_kernel(const float* __restrict__ x, float* __restrict__ out, int64_t n) {
-  __shared__ float sh[64];
-  float a = 0.f, b = 0.f;
+  __shared__ float sh[32];
+  float a = 0.f;
   const int64_t n4 = n / 4;
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n4;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
@@ -129,7 +120,7 @@ sumsq_kernel(const float* __restrict__ x, float* __restrict__ out, int64_t n) {
     a += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
   }
   if (blockIdx.x == 0 && threadIdx.x < (n & 3)) { const float v = x[n4 * 4 + threadIdx.x]; a += v * v; }
-  block_reduce2(a, b, sh);
+  a = block_sum(a, sh);
   if (threadIdx.x == 0) atomicAdd(out, a);
 }
 
@@ -152,15 +143,13 @@ int bv_adam_step(const bv_adam_args* args, void* stream) {
   if (a.step < 1) { set_error("bv_adam_step: step is 1-based"); return BV_ERR_INVALID; }
   const float bc1 = 1.f - powf(a.b1, static_cast<float>(a.step));
   const float bc2 = 1.f - powf(a.b2, static_cast<float>(a.step));
-  int64_t blocks = (a.n / 4 + 255) / 256;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
-  if (blocks > cap) blocks = cap;
+  const unsigned blocks = grid_for(a.n / 4, 256, num_sms() * 8);
   if (a.mu_dtype == DT_BF16) {
-    adam_kernel<true><<<static_cast<unsigned>(blocks), 256, 0, s>>>(
+    adam_kernel<true><<<blocks, 256, 0, s>>>(
         a.params, a.grads, a.mu, a.nu, reinterpret_cast<bf16*>(a.params_bf16), a.n, a.lr_eff, a.b1,
         a.b2, a.eps, a.wd_eff, bc1, bc2, a.gnorm_sq, a.clip_norm, a.grad_mult, a.upd_sq, a.param_sq);
   } else {
-    adam_kernel<false><<<static_cast<unsigned>(blocks), 256, 0, s>>>(
+    adam_kernel<false><<<blocks, 256, 0, s>>>(
         a.params, a.grads, a.mu, a.nu, reinterpret_cast<bf16*>(a.params_bf16), a.n, a.lr_eff, a.b1,
         a.b2, a.eps, a.wd_eff, bc1, bc2, a.gnorm_sq, a.clip_norm, a.grad_mult, a.upd_sq, a.param_sq);
   }
@@ -173,10 +162,7 @@ int bv_scale_step(float* params, const float* grads, void* params_bf16, int64_t 
   using namespace bv;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return BV_OK;
-  int64_t blocks = (n + 255) / 256;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
-  if (blocks > cap) blocks = cap;
-  scale_step_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(
+  scale_step_kernel<<<grid_for(n, 256, num_sms() * 8), 256, 0, s>>>(
       params, grads, reinterpret_cast<bf16*>(params_bf16), n, lr, wd, gnorm_sq, clip_norm, grad_mult, upd_sq,
       param_sq);
   return check_cuda(cudaGetLastError(), "scale_step_kernel launch");
@@ -186,11 +172,7 @@ int bv_sumsq(const float* x, float* out, int64_t n, void* stream) {
   using namespace bv;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (n <= 0) return BV_OK;
-  int64_t blocks = (n / 4 + 255) / 256;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  sumsq_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(x, out, n);
+  sumsq_kernel<<<grid_for(n / 4, 256, num_sms() * 8), 256, 0, s>>>(x, out, n);
   return check_cuda(cudaGetLastError(), "sumsq_kernel launch");
 }
 
@@ -309,19 +291,15 @@ af_apply_kernel(float* __restrict__ p, const float* __restrict__ g, bf16* __rest
     us += upd * upd;
     ps += pp * pp;
   }
-  block_reduce2(us, ps, sh);
+  float sums[2] = {us, ps};
+  block_sum(sums, sh);
   if (threadIdx.x == 0) {
-    if (upd_sq) atomicAdd(upd_sq, us);
-    if (param_sq) atomicAdd(param_sq, ps);
+    if (upd_sq) atomicAdd(upd_sq, sums[0]);
+    if (param_sq) atomicAdd(param_sq, sums[1]);
   }
 }
 
-inline unsigned af_blocks(int64_t work) {
-  int64_t b = (work + 255) / 256;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
-  if (b > cap) b = cap;
-  return static_cast<unsigned>(b < 1 ? 1 : b);
-}
+inline unsigned af_blocks(int64_t work) { return grid_for(work, 256, num_sms() * 8); }
 
 }  // namespace
 }  // namespace bv

@@ -48,19 +48,6 @@ sam_perturb_kernel(const float* __restrict__ w, const float* __restrict__ g, con
   }
 }
 
-// Block sums of (ab, bb) in a fixed order: warp shuffles, then warp 0 over the warp totals.
-__device__ __forceinline__ void block_sum2(float& a, float& b, float* sh) {
-  a = warp_sum(a); b = warp_sum(b);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) { sh[warp] = a; sh[32 + warp] = b; }
-  __syncthreads();
-  if (warp == 0) {
-    a = lane < kThreads / 32 ? sh[lane] : 0.f;
-    b = lane < kThreads / 32 ? sh[32 + lane] : 0.f;
-    a = warp_sum(a); b = warp_sum(b);
-  }
-}
-
 template <bool SAME>
 __global__ void __launch_bounds__(kThreads)
 sam_dots_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ part, int64_t n) {
@@ -81,29 +68,11 @@ sam_dots_kernel(const float* __restrict__ a, const float* __restrict__ b, float*
     bb += b[i] * b[i];
     if (!SAME) ab += a[i] * b[i];
   }
-  block_sum2(ab, bb, sh);
+  float sums[2] = {ab, bb};
+  block_sum(sums, sh);
   if (threadIdx.x == 0) {
-    part[blockIdx.x] = SAME ? bb : ab;
-    part[gridDim.x + blockIdx.x] = bb;
-  }
-}
-
-// Fixed-order finishing pass: out[k] = sum_i part[k * count + i]; thread t sums t, t + 256, ... in
-// index order, then a fixed shared-memory tree.
-__global__ void __launch_bounds__(kThreads)
-sam_dots_finish_kernel(const float* __restrict__ part, int count, float* __restrict__ out) {
-  __shared__ float sh[kThreads];
-  for (int k = 0; k < 2; ++k) {
-    float acc = 0.f;
-    for (int i = threadIdx.x; i < count; i += kThreads) acc += part[k * count + i];
-    sh[threadIdx.x] = acc;
-    __syncthreads();
-    for (int o = kThreads / 2; o > 0; o >>= 1) {
-      if (static_cast<int>(threadIdx.x) < o) sh[threadIdx.x] += sh[threadIdx.x + o];
-      __syncthreads();
-    }
-    if (threadIdx.x == 0) out[k] = sh[0];
-    __syncthreads();
+    part[blockIdx.x] = SAME ? sums[1] : sums[0];
+    part[gridDim.x + blockIdx.x] = sums[1];
   }
 }
 
@@ -138,12 +107,7 @@ gsam_combine_kernel(float* __restrict__ gc, const float* __restrict__ gr, const 
 
 inline bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
 
-inline unsigned stream_blocks(int64_t n) {
-  int64_t blocks = (n / 4 + kThreads - 1) / kThreads;
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
-  if (blocks > cap) blocks = cap;
-  return static_cast<unsigned>(blocks < 1 ? 1 : blocks);
-}
+inline unsigned stream_blocks(int64_t n) { return grid_for(n / 4, kThreads, num_sms() * 8); }
 
 }  // namespace
 }  // namespace bv
@@ -179,15 +143,13 @@ int bv_sam_dots(const float* a, const float* b, float* out, float* ws, int64_t n
     set_error("bv_sam_dots: a and b must be 16-byte aligned");
     return BV_ERR_INVALID;
   }
-  int64_t blocks = (n / 4 + kThreads - 1) / kThreads;
-  if (blocks > kDotsBlocks) blocks = kDotsBlocks;
-  if (blocks < 1) blocks = 1;
-  if (a == b) sam_dots_kernel<true><<<static_cast<unsigned>(blocks), kThreads, 0, s>>>(a, b, ws, n);
-  else sam_dots_kernel<false><<<static_cast<unsigned>(blocks), kThreads, 0, s>>>(a, b, ws, n);
+  const unsigned blocks = grid_for(n / 4, kThreads, kDotsBlocks);
+  if (a == b) sam_dots_kernel<true><<<blocks, kThreads, 0, s>>>(a, b, ws, n);
+  else sam_dots_kernel<false><<<blocks, kThreads, 0, s>>>(a, b, ws, n);
   int rc = check_cuda(cudaGetLastError(), "sam_dots_kernel launch");
   if (rc) return rc;
-  sam_dots_finish_kernel<<<1, kThreads, 0, s>>>(ws, static_cast<int>(blocks), out);
-  return check_cuda(cudaGetLastError(), "sam_dots_finish_kernel launch");
+  float* const outs[2] = {out, out + 1};
+  return finish_row_sums(ws, 2, blocks, outs, 1.f, false, s);
 }
 
 int bv_gsam_combine(float* gc, const float* gr, const float* dot, const float* norm_sq, float alpha,

@@ -217,9 +217,8 @@ int bv_row_select(const void* a, const void* b, const float* mask, void* out, in
  * _deprecated_contrastive.py:117-141).  row_offset = rank*n locates the positives.
  * Accumulates: loss += sum_ij -loglik_ij / global_B ; dt += dloss/dt' ; db += dloss/db.
  * Writes G[n,B] (bf16) = dloss/ddots.
- * partials_ws: NULL = the three scalars are accumulated with one atomicAdd per block (order of
- * arrival, last-bit differences between runs); a workspace of BV_LOSS_WS_FLOATS floats = per-block
- * partials + a fixed-order finishing pass, i.e. run-to-run deterministic like the reference. */
+ * partials_ws: BV_LOSS_WS_FLOATS floats of per-block partials, summed in a fixed order, so the scalars
+ * are run-to-run deterministic like the reference.  NULL: BV_ERR_INVALID before any CUDA call. */
 #define BV_LOSS_WS_FLOATS 8192
 int bv_siglip_loss(const float* dots, int64_t n, int64_t B, int64_t ld, int64_t row_offset,
                    const float* t_param, const float* b_param, int64_t global_B, void* G,
@@ -235,7 +234,8 @@ int bv_softmax_contrastive_loss(const float* dots, int64_t n, int64_t B, int64_t
                                 const float* t_param, int64_t global_B, float weight, void* G, int64_t ldg,
                                 float* loss, float* dt, float* ncorrect, float* rows_ws, void* stream);
 /* utils.py:236-243 / 276-281 : mean over n rows; loss is accumulated; dlogits may be NULL.
- * row_loss_ws: NULL = atomics; [n] floats = per-row losses + fixed-order sum (deterministic).
+ * row_loss_ws: [n] floats of per-row losses, summed in a fixed order (deterministic).  NULL with n > 0:
+ * BV_ERR_INVALID before any CUDA call.
  * Row-strided logits [n, ld_logits], labels [n, ld_labels] and dlogits [n, ld_dlogits] (columns 0..C-1
  * used).  The dlogits columns C..ld_dlogits-1 are written as zeros, so a classifier head stored with
  * padded columns takes the gradient as its GEMM operand unchanged.  Any ld < C: BV_ERR_INVALID before

@@ -106,37 +106,43 @@ def test_bench_workloads_cover_the_five_baseline_configs():
 
 
 # header -> (body of the main() of a C program that calls entry points refused before any launch, the integers
-# it prints, a name in the error string it prints after them)
+# it prints, the names in the error strings it prints after them)
 C_PROGRAMS = {
     "bv_b200.h": (
-        '  int rc = bv_colsum(NULL, 1, NULL, 4, 7, 7, NULL);   /* 7 columns */\n'
-        '  printf("%d %d %s\\n", bv_version(), rc, bv_last_error_string());\n',
-        [101, -1], "bv_colsum"),
+        '  /* 7 columns; the losses without their workspace */\n'
+        '  char e[2][512];\n'
+        '  int a = bv_colsum(NULL, 1, NULL, 4, 7, 7, NULL);\n'
+        '  snprintf(e[0], sizeof e[0], "%s", bv_last_error_string());\n'
+        '  int b = bv_siglip_loss(NULL, 1, 4, 4, 0, NULL, NULL, 4, NULL, 4, NULL, NULL, NULL, NULL, NULL);\n'
+        '  snprintf(e[1], sizeof e[1], "%s", bv_last_error_string());\n'
+        '  int c = bv_sigmoid_xent_ld(NULL, 8, NULL, 8, NULL, NULL, 8, NULL, 2, 8, NULL);\n'
+        '  printf("%d %d %d %d %s %s %s\\n", bv_version(), a, b, c, e[0], e[1], bv_last_error_string());\n',
+        [101, -1, -1, -1], ("bv_colsum", "bv_siglip_loss", "bv_sigmoid_xent_ld")),
     "bv_b200_sam.h": (
         '  int rc = bv_sam_dots(NULL, NULL, NULL, NULL, 8, NULL);\n'
         '  printf("%d %d %s\\n", BV_SAM_WS_FLOATS, rc, bv_last_error_string());\n',
-        [L.SAM_WS_FLOATS, -1], "bv_sam_dots"),
+        [L.SAM_WS_FLOATS, -1], ("bv_sam_dots",)),
     "bv_b200_distill.h": (
         '  /* a distance without a training kernel, a stride < C */\n'
         '  int a = bv_distill_loss(NULL, 8, NULL, 8, NULL, 0, BV_DIST_L2, 1.f, 0.f, 0, NULL, 0, NULL, NULL, 4, 8,'
         ' NULL);\n'
         '  int b = bv_distance(NULL, 4, NULL, 8, BV_DIST_AGREE, 0.f, 1.f, 0.f, 1, NULL, 4, 8, NULL);\n'
         '  printf("%d %d %d %s\\n", BV_DISTILL_OUTPUTS, a, b, bv_last_error_string());\n',
-        [len(L.DISTILL_OUTPUTS), -3, -1], "bv_distance"),
+        [len(L.DISTILL_OUTPUTS), -3, -1], ("bv_distance",)),
     "bv_b200_flexi.h": (
         '  /* J not a multiple of 4, a null matrix */\n'
         '  float m = 1.f;\n'
         '  int a = bv_resample_fwd(&m, &m, &m, 1, 1, 6, NULL);\n'
         '  int b = bv_resample_bwd(NULL, &m, &m, 1, 1, 4, NULL);\n'
         '  printf("%d %d %s\\n", a, b, bv_last_error_string());\n',
-        [-1, -1], "bv_resample_bwd"),
+        [-1, -1], ("bv_resample_bwd",)),
     "bv_b200_jet.h": (
         '  /* H not a multiple of ps, a null buffer */\n'
         '  float m = 1.f;\n'
         '  int a = bv_jet_unpatchify(&m, &m, 1, 6, 8, 3, 4, NULL);\n'
         '  int b = bv_jet_bits(&m, NULL, &m, &m, NULL, 1.f, 1, 1, NULL);\n'
         '  printf("%d %d %s\\n", a, b, bv_last_error_string());\n',
-        [-1, -1], "bv_jet_bits"),
+        [-1, -1], ("bv_jet_bits",)),
 }
 
 
@@ -152,7 +158,7 @@ def test_header_is_plain_c_and_a_c_program_links(tmp_path, header):
   hdr = os.path.join(ROOT, "include", header)
   subprocess.run(["gcc", "-std=c99", "-Wall", "-Wextra", "-Werror", "-fsyntax-only", "-x", "c", hdr], check=True)
   subprocess.run(["g++", "-std=c++17", "-fsyntax-only", "-x", "c++", hdr], check=True)
-  body, ints, name = C_PROGRAMS[header]
+  body, ints, names = C_PROGRAMS[header]
   src = tmp_path / "main.c"
   src.write_text(f'#include <stdio.h>\n#include "{header}"\nint main(void) {{\n{body}  return 0;\n}}\n')
   libdir = os.path.dirname(os.path.abspath(L.LIB_PATH))
@@ -161,7 +167,7 @@ def test_header_is_plain_c_and_a_c_program_links(tmp_path, header):
                   "-L", libdir, "-lbv_b200", f"-Wl,-rpath,{libdir}"], check=True)
   out = subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout
   fields = out.split(None, len(ints))
-  assert [int(v) for v in fields[:-1]] == ints and name in fields[-1], out
+  assert [int(v) for v in fields[:-1]] == ints and all(name in fields[-1] for name in names), out
 
 
 def test_bench_refuses_to_run_the_product_arm_without_a_gpu():
