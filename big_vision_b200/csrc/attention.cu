@@ -16,6 +16,13 @@
 // zeros, never the next head's columns.  The products whose N is the head dim (O += P V, dV, dK,
 // dQ) are single n = DH wgmmas across both boxes (MN-major operand, leading byte offset = one box).
 //
+// Key-padding mask (dh = 64 only; head_dim | BV_ATTN_KEY_MASK, the mask appended to the arguments,
+// include/bv_b200.h): an optional uint8 [B, Nk] row per batch, nonzero = attend.  The forward
+// and the two backward kernels take it as a template flag MASK; without it they are the unmasked
+// kernels unchanged.  A masked key takes the path of a key past Nk (score -inf in the forward, P = 0 in
+// the backward), wherever it sits in its 64-key block.  A query whose keys are all masked gets O = 0,
+// lse = 0 and zero gradients.
+//
 // Every kernel runs one warpgroup per CTA on 64-row tiles and streams the other operand in 64-row
 // blocks through a two-slot TMA ring, so any sequence length works with the same code:
 //   forward   (b, h, 64 queries):  S = Q K^T (smem x smem), online softmax in registers,
@@ -143,6 +150,16 @@ __device__ __forceinline__ void zero(float (&d)[R]) {
   for (int i = 0; i < R; ++i) d[i] = 0.f;
 }
 
+// the attended keys of the 64-key block at k0, shifted to this thread's columns: bit 8c + e is key
+// k0 + 8c + 2*(lane%4) + e, i.e. accumulator element 4c + e (and 4c + 2 + e) of the S = Q K^T tile.
+// A key is attended when it is below Nk and its mask byte is nonzero.
+__device__ __forceinline__ uint64_t attended_keys(const uint8_t* mask_row, int k0, int Nk, int lane) {
+  const int a = k0 + lane, b = a + 32;
+  const uint32_t lo = __ballot_sync(0xffffffffu, a < Nk && mask_row[a] != 0);
+  const uint32_t hi = __ballot_sync(0xffffffffu, b < Nk && mask_row[b] != 0);
+  return ((static_cast<uint64_t>(hi) << 32) | lo) >> (2 * (lane & 3));
+}
+
 // ============================================================================
 // forward
 // ============================================================================
@@ -152,9 +169,11 @@ struct FwdDev {
   float* lse;
   bf16* o;
   long long ldo, bso;
+  const uint8_t* mask;                     // key mask [B, Nk] (MASK kernels only)
+  long long bsmask;
 };
 
-template <int DH>
+template <int DH, bool MASK>
 __global__ void __launch_bounds__(THREADS)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FwdDev p) {
@@ -200,28 +219,36 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs(s);
-    // online softmax in base 2 over this key block; keys past Nk get probability 0
+    // online softmax in base 2 over this key block; keys past Nk (and masked keys) get probability 0
     const int kbase = j * T + 2 * (lane & 3);
+    uint64_t live = 0;
+    if constexpr (MASK) live = attended_keys(p.mask + b * p.bsmask, j * T, p.Nk, lane);
     float mx[2] = {m[0], m[1]};
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       const int key = kbase + 8 * (i >> 2) + (i & 1);
-      s[i] = key < p.Nk ? s[i] * p.scale_log2 : -INFINITY;
+      bool in;
+      if constexpr (MASK) in = (live >> (8 * (i >> 2) + (i & 1))) & 1;
+      else in = key < p.Nk;
+      s[i] = in ? s[i] * p.scale_log2 : -INFINITY;
       mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
     }
-    float corr[2];
+    float corr[2], base[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
       mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-      corr[r] = ex2(m[r] - mx[r]);       // 0 on the first block (m = -inf)
+      // with a mask, every key so far may be masked (mx = -inf): exponentiate against 0 instead, so
+      // that the probabilities and the correction are 0, not NaN
+      base[r] = MASK && mx[r] == -INFINITY ? 0.f : mx[r];
+      corr[r] = ex2(m[r] - base[r]);     // 0 on the first block (m = -inf)
       m[r] = mx[r];
       l[r] *= corr[r];
     }
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       const int r = (i >> 1) & 1;
-      s[i] = ex2(s[i] - m[r]);
+      s[i] = ex2(s[i] - (MASK ? base[r] : m[r]));
       l[r] += s[i];
       o[i] *= corr[r];
     }
@@ -244,7 +271,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
     l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
   }
-  const float inv[2] = {1.f / l[0], 1.f / l[1]};
+  float inv[2] = {1.f / l[0], 1.f / l[1]};
+  if constexpr (MASK) {                  // l = 0: no attended key, O = 0 and lse = 0
+    inv[0] = l[0] > 0.f ? inv[0] : 0.f;
+    inv[1] = l[1] > 0.f ? inv[1] : 0.f;
+  }
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int q = qt * T + 16 * warp + (lane >> 2) + 8 * r;
@@ -253,7 +284,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
     for (int jj = 0; jj < DH / 8; ++jj)
       *reinterpret_cast<uint32_t*>(orow + 8 * jj) = pack_bf16(o[4 * jj + 2 * r] * inv[r], o[4 * jj + 2 * r + 1] * inv[r]);
-    if ((lane & 3) == 0) p.lse[(static_cast<long long>(b) * p.H + h) * p.Nq + q] = (m[r] + __log2f(l[r])) * LN2;
+    if ((lane & 3) == 0)
+      p.lse[(static_cast<long long>(b) * p.H + h) * p.Nq + q] = MASK && l[r] == 0.f ? 0.f : (m[r] + __log2f(l[r])) * LN2;
   }
 }
 
@@ -268,6 +300,8 @@ struct BwdDev {
   bf16* dq; bf16* dk; bf16* dv;
   long long lddq, bsdq, lddk, bsdk, lddv, bsdv;
   float* dq_colsum; float* dk_colsum; float* dv_colsum;
+  const uint8_t* mask;                     // key mask [B, Nk] (MASK kernels only)
+  long long bsmask;
 };
 
 // column sums of a [64 x DH] accumulator tile's stored (bf16-rounded) rows < nvalid: the eight lanes
@@ -299,7 +333,7 @@ __device__ __forceinline__ void tile_colsum(const float (&d)[R], float mul, int 
 
 // dQ of one (b, h, 64-query) block: the key blocks stream through the K / V ring and their dS K
 // products accumulate in order in one register tile
-template <int DH>
+template <int DH, bool MASK>
 __global__ void __launch_bounds__(THREADS)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const BwdDev p) {
@@ -361,13 +395,19 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     wgmma_wait<0>();
     wgmma_fence_regs(s);
     wgmma_fence_regs(dp);
-    // P = exp(scale S - lse), dS = P o (dP - delta); keys past Nk (zero-filled K rows) get P = 0
+    // P = exp(scale S - lse), dS = P o (dP - delta); keys past Nk (zero-filled K rows) and masked keys
+    // get P = 0
     const int kbase = j * T + 2 * (lane & 3);
+    uint64_t live = 0;
+    if constexpr (MASK) live = attended_keys(p.mask + b * p.bsmask, j * T, p.Nk, lane);
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       const int r = (i >> 1) & 1;
       const int key = kbase + 8 * (i >> 2) + (i & 1);
-      const float pr = key < p.Nk ? ex2(s[i] * p.scale_log2 - lse2[r]) : 0.f;
+      bool in;
+      if constexpr (MASK) in = (live >> (8 * (i >> 2) + (i & 1))) & 1;
+      else in = key < p.Nk;
+      const float pr = in ? ex2(s[i] * p.scale_log2 - lse2[r]) : 0.f;
       dp[i] = pr * (dp[i] - dl[r]);
     }
     uint32_t sf[4][4];
@@ -395,7 +435,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 }
 
 // dK, dV of one (b, h, 64-key) block: the query blocks stream through the Q / dO ring
-template <int DH>
+template <int DH, bool MASK>
 __global__ void __launch_bounds__(THREADS)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const BwdDev p) {
@@ -437,6 +477,14 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   zero(dv);
   const long long bhq = (static_cast<long long>(b) * p.H + h) * p.Nq;
   const int key_row = 16 * warp + (lane >> 2);      // + 8r: this thread's rows of the key block
+  bool live[2] = {true, true};                      // its two keys are attended (MASK)
+  if constexpr (MASK) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int key = kt * T + key_row + 8 * r;
+      live[r] = key < p.Nk && p.mask[b * p.bsmask + key] != 0;
+    }
+  }
   mbar_wait(kv_bar, 0);
   for (int i = 0; i < p.QT; ++i) {
     const int slot = i & 1;
@@ -458,11 +506,13 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     wgmma_wait<0>();
     wgmma_fence_regs(st);
     wgmma_fence_regs(dpt);
-    // P^T = exp(scale S^T - lse), dS^T = P^T o (dP^T - delta)   (the scale of dS is applied at the end)
+    // P^T = exp(scale S^T - lse), dS^T = P^T o (dP^T - delta)   (the scale of dS is applied at the end);
+    // a masked key's row of P^T is 0
 #pragma unroll
     for (int e = 0; e < 32; ++e) {
       const int c = 2 * (e >> 2) + (e & 1);
       st[e] = ex2(st[e] * p.scale_log2 - lse2[c]);
+      if constexpr (MASK) st[e] = live[(e >> 1) & 1] ? st[e] : 0.f;
       dpt[e] = st[e] * (dpt[e] - dl[c]);
     }
     uint32_t pf[4][4], sf[4][4];
@@ -528,11 +578,28 @@ attn_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ d_o, floa
   }
 }
 
-// head dims with kernels; every other one is refused before any CUDA call
-int check_head_dim(int head_dim, const char* who) {
-  if (head_dim == 64 || head_dim == 72 || head_dim == 80 || head_dim == 96 || head_dim == 104) return BV_OK;
-  set_error("%s: head_dim %d is not supported (supported head dims: 64, 72, 80, 96, 104)", who, head_dim);
-  return BV_ERR_UNSUPPORTED;
+// the key mask of a call: head_dim | BV_ATTN_KEY_MASK means the arguments are followed by it
+struct KeyMask {
+  const uint8_t* mask = nullptr;
+  int64_t bs = 0;
+};
+
+// head dims with kernels; every other one is refused before any CUDA call.  The key mask is built at
+// head dim 64 only (BERT-Base and BERT-Large)
+int check_head_dim(int head_dim, bool masked, const KeyMask& m, const char* who) {
+  if (head_dim != 64 && head_dim != 72 && head_dim != 80 && head_dim != 96 && head_dim != 104) {
+    set_error("%s: head_dim %d is not supported (supported head dims: 64, 72, 80, 96, 104)", who, head_dim);
+    return BV_ERR_UNSUPPORTED;
+  }
+  if (masked && head_dim != 64) {
+    set_error("%s: a key mask is supported at head_dim 64 only (got %d)", who, head_dim);
+    return BV_ERR_INVALID;
+  }
+  if (masked && m.mask == nullptr) {
+    set_error("%s: BV_ATTN_KEY_MASK needs a non-null key_mask", who);
+    return BV_ERR_INVALID;
+  }
+  return BV_OK;
 }
 
 int check_attn(const bv_attn_args& a, const char* who) {
@@ -554,7 +621,7 @@ int check_attn(const bv_attn_args& a, const char* who) {
 }
 
 template <int DH>
-int attention_fwd(const bv_attn_args& a, cudaStream_t s) {
+int attention_fwd(const bv_attn_args& a, const KeyMask& km, cudaStream_t s) {
   using G = Geo<DH>;
   int rc = check_attn(a, "bv_attention_fwd_hd");
   if (rc) return rc;
@@ -566,20 +633,25 @@ int attention_fwd(const bv_attn_args& a, cudaStream_t s) {
   p.lse = a.lse;
   p.o = static_cast<bf16*>(a.o);
   p.ldo = a.ldo; p.bso = a.bso;
+  p.mask = km.mask; p.bsmask = km.bs;
   CUtensorMap tmQ, tmK, tmV;
   if ((rc = make_tmap_bnd(&tmQ, a.q, DH, a.H, a.Nq, a.B, a.ldq, a.bsq))) return rc;
   if ((rc = make_tmap_bnd(&tmK, a.k, DH, a.H, a.Nk, a.B, a.ldk, a.bsk))) return rc;
   if ((rc = make_tmap_bnd(&tmV, a.v, DH, a.H, a.Nk, a.B, a.ldv, a.bsv))) return rc;
   const long long grid = a.B * a.H * p.QT;
-  rc = check_cuda(cudaFuncSetAttribute(attn_fwd_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::FWD_SMEM),
+  auto kernel = attn_fwd_kernel<DH, false>;
+  if constexpr (DH == 64) {
+    if (km.mask != nullptr) kernel = attn_fwd_kernel<DH, true>;
+  }
+  rc = check_cuda(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, G::FWD_SMEM),
                   "cudaFuncSetAttribute(attn_fwd)");
   if (rc) return rc;
-  attn_fwd_kernel<DH><<<static_cast<unsigned>(grid), THREADS, G::FWD_SMEM, s>>>(tmQ, tmK, tmV, p);
+  kernel<<<static_cast<unsigned>(grid), THREADS, G::FWD_SMEM, s>>>(tmQ, tmK, tmV, p);
   return check_cuda(cudaGetLastError(), "attn_fwd_kernel launch");
 }
 
 template <int DH>
-int attention_bwd(const bv_attn_bwd_args& g, cudaStream_t s) {
+int attention_bwd(const bv_attn_bwd_args& g, const KeyMask& km, cudaStream_t s) {
   using G = Geo<DH>;
   const bv_attn_args& a = g.fwd;
   int rc = check_attn(a, "bv_attention_bwd_hd");
@@ -625,6 +697,7 @@ int attention_bwd(const bv_attn_bwd_args& g, cudaStream_t s) {
   p.dq = static_cast<bf16*>(g.dq); p.dk = static_cast<bf16*>(g.dk); p.dv = static_cast<bf16*>(g.dv);
   p.lddq = g.lddq; p.bsdq = g.bsdq; p.lddk = g.lddk; p.bsdk = g.bsdk; p.lddv = g.lddv; p.bsdv = g.bsdv;
   p.dq_colsum = g.dq_colsum; p.dk_colsum = g.dk_colsum; p.dv_colsum = g.dv_colsum;
+  p.mask = km.mask; p.bsmask = km.bs;
   CUtensorMap tmQ, tmK, tmV, tmdO;
   if ((rc = make_tmap_bnd(&tmQ, a.q, DH, a.H, a.Nq, a.B, a.ldq, a.bsq))) return rc;
   if ((rc = make_tmap_bnd(&tmK, a.k, DH, a.H, a.Nk, a.B, a.ldk, a.bsk))) return rc;
@@ -632,15 +705,23 @@ int attention_bwd(const bv_attn_bwd_args& g, cudaStream_t s) {
   if ((rc = make_tmap_bnd(&tmdO, g.d_o, DH, a.H, a.Nq, a.B, g.lddo, g.bsdo))) return rc;
   // query blocks of one (b, h) are adjacent in the dQ grid (and key blocks in the dK / dV grid), so the
   // streamed K / V (Q / dO) tiles they share are served from L2
-  rc = check_cuda(cudaFuncSetAttribute(attn_bwd_dq_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::BWD_SMEM),
+  auto dq_kernel = attn_bwd_dq_kernel<DH, false>;
+  auto dkdv_kernel = attn_bwd_dkdv_kernel<DH, false>;
+  if constexpr (DH == 64) {
+    if (km.mask != nullptr) {
+      dq_kernel = attn_bwd_dq_kernel<DH, true>;
+      dkdv_kernel = attn_bwd_dkdv_kernel<DH, true>;
+    }
+  }
+  rc = check_cuda(cudaFuncSetAttribute(dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, G::BWD_SMEM),
                   "cudaFuncSetAttribute(attn_bwd_dq)");
   if (rc) return rc;
-  attn_bwd_dq_kernel<DH><<<static_cast<unsigned>(a.B * a.H * p.QT), THREADS, G::BWD_SMEM, s>>>(tmQ, tmK, tmV, tmdO, p);
+  dq_kernel<<<static_cast<unsigned>(a.B * a.H * p.QT), THREADS, G::BWD_SMEM, s>>>(tmQ, tmK, tmV, tmdO, p);
   if ((rc = check_cuda(cudaGetLastError(), "attn_bwd_dq_kernel launch"))) return rc;
-  rc = check_cuda(cudaFuncSetAttribute(attn_bwd_dkdv_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::BWD_SMEM),
+  rc = check_cuda(cudaFuncSetAttribute(dkdv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, G::BWD_SMEM),
                   "cudaFuncSetAttribute(attn_bwd_dkdv)");
   if (rc) return rc;
-  attn_bwd_dkdv_kernel<DH><<<static_cast<unsigned>(a.B * a.H * p.KT), THREADS, G::BWD_SMEM, s>>>(tmQ, tmK, tmV, tmdO, p);
+  dkdv_kernel<<<static_cast<unsigned>(a.B * a.H * p.KT), THREADS, G::BWD_SMEM, s>>>(tmQ, tmK, tmV, tmdO, p);
   rc = check_cuda(cudaGetLastError(), "attn_bwd_dkdv_kernel launch");
   return rc;
 }
@@ -654,15 +735,23 @@ int bv_attention_fwd_hd(const bv_attn_args* args, int32_t head_dim, void* stream
   using namespace bv;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (!args) { set_error("bv_attention_fwd_hd: null args"); return BV_ERR_INVALID; }
-  int rc = check_head_dim(head_dim, "bv_attention_fwd_hd");
+  const bool masked = (head_dim & BV_ATTN_KEY_MASK) != 0;
+  head_dim &= ~BV_ATTN_KEY_MASK;
+  KeyMask km;
+  if (masked) {     // args is the first member of a bv_attn_masked_args
+    const bv_attn_masked_args* m = reinterpret_cast<const bv_attn_masked_args*>(args);
+    km.mask = m->key_mask;
+    km.bs = m->bsmask;
+  }
+  int rc = check_head_dim(head_dim, masked, km, "bv_attention_fwd_hd");
   if (rc) return rc;
   const bv_attn_args& a = *args;
   switch (head_dim) {
-    case 72: return attention_fwd<72>(a, s);
-    case 80: return attention_fwd<80>(a, s);
-    case 96: return attention_fwd<96>(a, s);
-    case 104: return attention_fwd<104>(a, s);
-    default: return attention_fwd<64>(a, s);
+    case 72: return attention_fwd<72>(a, km, s);
+    case 80: return attention_fwd<80>(a, km, s);
+    case 96: return attention_fwd<96>(a, km, s);
+    case 104: return attention_fwd<104>(a, km, s);
+    default: return attention_fwd<64>(a, km, s);
   }
 }
 
@@ -670,15 +759,23 @@ int bv_attention_bwd_hd(const bv_attn_bwd_args* args, int32_t head_dim, void* st
   using namespace bv;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (!args) { set_error("bv_attention_bwd_hd: null args"); return BV_ERR_INVALID; }
-  int rc = check_head_dim(head_dim, "bv_attention_bwd_hd");
+  const bool masked = (head_dim & BV_ATTN_KEY_MASK) != 0;
+  head_dim &= ~BV_ATTN_KEY_MASK;
+  KeyMask km;
+  if (masked) {     // args is the first member of a bv_attn_masked_bwd_args
+    const bv_attn_masked_bwd_args* m = reinterpret_cast<const bv_attn_masked_bwd_args*>(args);
+    km.mask = m->key_mask;
+    km.bs = m->bsmask;
+  }
+  int rc = check_head_dim(head_dim, masked, km, "bv_attention_bwd_hd");
   if (rc) return rc;
   const bv_attn_bwd_args& g = *args;
   switch (head_dim) {
-    case 72: return attention_bwd<72>(g, s);
-    case 80: return attention_bwd<80>(g, s);
-    case 96: return attention_bwd<96>(g, s);
-    case 104: return attention_bwd<104>(g, s);
-    default: return attention_bwd<64>(g, s);
+    case 72: return attention_bwd<72>(g, km, s);
+    case 80: return attention_bwd<80>(g, km, s);
+    case 96: return attention_bwd<96>(g, km, s);
+    case 104: return attention_bwd<104>(g, km, s);
+    default: return attention_bwd<64>(g, km, s);
   }
 }
 

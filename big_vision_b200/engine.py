@@ -197,11 +197,13 @@ def stage_cut(storages, stages, frozen):
 
 
 class Geom(NamedTuple):
-  """What every stage of one forward sees besides its input: n samples of N tokens each, and the
-  MLP-Mixer's stochastic-depth masks of that forward (None: no residual branch is dropped)."""
+  """What every stage of one forward sees besides its input: n samples of N tokens each, the
+  MLP-Mixer's stochastic-depth masks of that forward (None: no residual branch is dropped) and BERT's
+  key-padding mask [n, N] (None: every key is attended)."""
   n: int
   N: int
   masks: Optional[torch.Tensor] = None
+  key_mask: Optional[torch.Tensor] = None
 
 
 class Stage:

@@ -19,6 +19,7 @@ LOSS_WS_FLOATS = 8192      # BV_LOSS_WS_FLOATS
 SAM_WS_FLOATS = 2048       # BV_SAM_WS_FLOATS
 # BV_DIST_*: the kinds of dist(); BV_DISTILL_*: the outputs of bv_distill_loss, in order
 DIST_KINDS = {"euclidean": 0, "l2": 1, "hard": 2, "kl": 3, "logsoftmax_euclidean": 4, "agree": 5}
+ATTN_KEY_MASK = 65536      # BV_ATTN_KEY_MASK: head_dim flag of a key-masked attention call
 DISTILL_OUTPUTS = ("distance", "entropy_student", "entropy_teacher", "task_loss_student", "task_loss_teacher")
 
 
@@ -46,6 +47,15 @@ class AttnBwdArgs(ctypes.Structure):
               ("bsdq", c_i64), ("bsdk", c_i64), ("bsdv", c_i64),
               ("dq_colsum", c_vp), ("dk_colsum", c_vp), ("dv_colsum", c_vp),
               ("delta", c_vp)]
+
+
+# head_dim | ATTN_KEY_MASK: the attention arguments are the first member of one of these
+class AttnMaskedArgs(ctypes.Structure):
+  _fields_ = [("attn", AttnArgs), ("key_mask", c_vp), ("bsmask", c_i64)]
+
+
+class AttnMaskedBwdArgs(ctypes.Structure):
+  _fields_ = [("attn", AttnBwdArgs), ("key_mask", c_vp), ("bsmask", c_i64)]
 
 
 class AdamArgs(ctypes.Structure):

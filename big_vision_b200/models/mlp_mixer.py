@@ -58,7 +58,7 @@ class MixerBlock(E.Stage):
   def fwd(self, P, x, geom, save=True):
     """save=False (forward only): same output bits; every intermediate is released as soon as the
     next op has consumed it, GELU's pre-activations are not written and saved is None."""
-    n, N, masks = geom
+    n, N, masks = geom.n, geom.N, geom.masks
     d, p, tm = self.d, self.p, self.tm
     y, mean1, rstd1 = ops.layernorm_fwd(x, P.f(p + "LayerNorm_0/scale"), P.f(p + "LayerNorm_0/bias"))
     yt = ops.transpose_tokens(y, n, N, d)                                   # [n*d, Np]
@@ -97,7 +97,7 @@ class MixerBlock(E.Stage):
   def bwd(self, P, dx, saved, geom, sink, need_dx=True):
     """dx: bf16 [n*N, d] grad of the block output.  Returns the grad of the block input; colsum of it is
     accumulated into `sink`.  need_dx changes nothing: LayerNorm_0's gradients need the full chain."""
-    n, N, masks = geom
+    n, N, masks = geom.n, geom.N, geom.masks
     d, p, tm = self.d, self.p, self.tm
     x, mean1, rstd1, yt, hact, hpre, x1, mean2, rstd2, mlp_saved = saved
     # channel mixing

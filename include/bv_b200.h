@@ -102,7 +102,7 @@ int bv_layernorm_bwd(const void* dy, int dy_dtype, const void* x, int x_dtype, c
                      int32_t d, void* stream);
 
 /* ---------------------------------------------------------------------------------
- * Scaled-dot-product attention, no mask, any Nq, Nk >= 1
+ * Scaled-dot-product attention, optional key-padding mask, any Nq, Nk >= 1
  * (flax MultiHeadDotProductAttention core: models/vit.py:93-98, :176-178).  Keys stream through
  * on-chip memory in 64-key blocks (online combination of per-block softmax statistics), so every
  * sequence length takes the same path.
@@ -111,6 +111,12 @@ int bv_layernorm_bwd(const void* dy, int dy_dtype, const void* x, int x_dtype, c
  * q/k/v/o are bf16 strided views: element (b, t, h*dh + j) at
  * base + b*bs + t*ld + h*dh + j  (e.g. column slices of the fused QKV GEMM output).
  * lse [B,H,Nq] fp32 = log sum_j exp(scale * q_i.k_j) is saved for the backward.
+ * Key-padding mask (dh = 64 only; the reference's BERT input_mask, models/proj/flaxformer/bert.py:54):
+ * pass head_dim | BV_ATTN_KEY_MASK, and args then points to a bv_attn_masked_args (forward) or a
+ * bv_attn_masked_bwd_args (backward), which append the mask to the unmasked arguments.  key_mask is
+ * uint8, element (b, k) at key_mask[b*bsmask + k], nonzero = attend; masked keys get probability 0
+ * wherever they sit.  A query with every key masked gets O = 0, lse = 0 and zero gradients.  The flag
+ * at any other head dim, or with a NULL key_mask, is refused with BV_ERR_INVALID before any launch.
  * --------------------------------------------------------------------------------- */
 typedef struct bv_attn_args {
   const void* q; const void* k; const void* v; void* o; float* lse;
@@ -119,6 +125,7 @@ typedef struct bv_attn_args {
   int64_t bsq, bsk, bsv, bso;
   float scale;
 } bv_attn_args;
+#define BV_ATTN_KEY_MASK 65536   /* head_dim flag: args carries a key mask (see above) */
 int bv_attention_fwd_hd(const bv_attn_args* args, int32_t head_dim, void* stream);
 typedef struct bv_attn_bwd_args {
   bv_attn_args fwd;            /* same q,k,v,o,lse as the forward call */
@@ -133,6 +140,14 @@ typedef struct bv_attn_bwd_args {
   float* delta;
 } bv_attn_bwd_args;
 int bv_attention_bwd_hd(const bv_attn_bwd_args* args, int32_t head_dim, void* stream);
+typedef struct bv_attn_masked_args {
+  bv_attn_args attn;
+  const uint8_t* key_mask; int64_t bsmask;
+} bv_attn_masked_args;
+typedef struct bv_attn_masked_bwd_args {
+  bv_attn_bwd_args attn;       /* attn.fwd: the forward call's arguments */
+  const uint8_t* key_mask; int64_t bsmask;   /* the forward call's mask */
+} bv_attn_masked_bwd_args;
 
 /* ---------------------------------------------------------------------------------
  * Data movement / small reductions
