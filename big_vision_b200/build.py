@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libbv_b200.so")
 SOURCES = ["host_utils.cu", "gemm.cu", "attention.cu", "layernorm.cu", "elementwise.cu",
-           "loss.cu", "optim.cu", "eval.cu", "sam.cu", "distill.cu", "flexi.cu", "jet.cu"]
+           "loss.cu", "optim.cu", "eval.cu", "sam.cu", "distill.cu", "flexi.cu", "jet.cu", "dropout.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
@@ -32,7 +32,7 @@ def _digest(paths):
 
 def _headers():
   out = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".h", ".cuh"))]
-  return out + glob.glob(os.path.join(os.path.dirname(HERE), "include", "bv_b200*.h"))
+  return out + glob.glob(os.path.join(os.path.dirname(HERE), "include", "bv_*.h"))
 
 
 def _compile(src):

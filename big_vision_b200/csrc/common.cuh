@@ -289,4 +289,28 @@ __device__ __forceinline__ void tma_store_wait() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
+// ----------------------------------------------------------------------------
+// Philox4x64-10 (Salmon et al., SC'11), the generator of numpy's np.random.Philox: the counter-based
+// stream of Jet's dequantization noise and of the dropout masks.  ctr is replaced by the block's output.
+// ----------------------------------------------------------------------------
+constexpr uint64_t kPhiloxM0 = 0xD2E7470EE14C6C93ull, kPhiloxM1 = 0xCA5A826395121157ull;
+constexpr uint64_t kPhiloxW0 = 0x9E3779B97F4A7C15ull, kPhiloxW1 = 0xBB67AE8584CAA73Bull;
+
+__device__ __forceinline__ void philox4x64_10(uint64_t ctr[4], uint64_t k0, uint64_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r) {
+      k0 += kPhiloxW0;
+      k1 += kPhiloxW1;
+    }
+    const uint64_t hi0 = __umul64hi(kPhiloxM0, ctr[0]), lo0 = kPhiloxM0 * ctr[0];
+    const uint64_t hi1 = __umul64hi(kPhiloxM1, ctr[2]), lo1 = kPhiloxM1 * ctr[2];
+    const uint64_t c1 = ctr[1], c3 = ctr[3];
+    ctr[0] = hi1 ^ c1 ^ k0;
+    ctr[1] = lo1;
+    ctr[2] = hi0 ^ c3 ^ k1;
+    ctr[3] = lo0;
+  }
+}
+
 }  // namespace bv

@@ -20,27 +20,6 @@ namespace {
 constexpr int kThreads = 256;        // element-wise kernels
 constexpr int kRedThreads = 512;     // one CTA per image for the reductions
 
-// ---- Philox4x64-10 (Salmon et al., SC'11), the generator of numpy's np.random.Philox -----------------------
-constexpr uint64_t kPhiloxM0 = 0xD2E7470EE14C6C93ull, kPhiloxM1 = 0xCA5A826395121157ull;
-constexpr uint64_t kPhiloxW0 = 0x9E3779B97F4A7C15ull, kPhiloxW1 = 0xBB67AE8584CAA73Bull;
-
-__device__ __forceinline__ void philox4x64_10(uint64_t ctr[4], uint64_t k0, uint64_t k1) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    if (r) {
-      k0 += kPhiloxW0;
-      k1 += kPhiloxW1;
-    }
-    const uint64_t hi0 = __umul64hi(kPhiloxM0, ctr[0]), lo0 = kPhiloxM0 * ctr[0];
-    const uint64_t hi1 = __umul64hi(kPhiloxM1, ctr[2]), lo1 = kPhiloxM1 * ctr[2];
-    const uint64_t c1 = ctr[1], c3 = ctr[3];
-    ctr[0] = hi1 ^ c1 ^ k0;
-    ctr[1] = lo1;
-    ctr[2] = hi0 ^ c3 ^ k1;
-    ctr[3] = lo0;
-  }
-}
-
 // Thread i owns Philox block (offset / 8 + i): the 8 uniforms of global elements [8 b, 8 b + 8), of which it
 // writes those that fall in this batch.  Block b runs at counter (b + 1, counter, 0, 0): numpy increments the
 // first counter word before each block.

@@ -196,14 +196,60 @@ def stage_cut(storages, stages, frozen):
   return len(stages)
 
 
+class DropoutKey(NamedTuple):
+  """What a training forward's dropout masks are drawn from (include/bv_dropout.h): the run's seed,
+  the optimizer step, the global index of this rank's first sample and the tower of a multi-tower model."""
+  seed: int
+  step: int
+  sample0: int = 0
+  tower: int = 0
+
+
+# Dropout sites: one mask stream per (tower, layer, kind).  Kind EMBED is used at layer 0 only.
+DROP_EMBED, DROP_ATTN, DROP_GELU, DROP_MLP = range(4)
+_LAYERS_PER_TOWER = 1 << 16
+
+
+def dropout_site(tower, layer, kind):
+  """The Philox counter word 2 of a site: >= 1, since 0 is Jet's dequantization noise."""
+  return 1 + kind + 4 * (layer + _LAYERS_PER_TOWER * tower)
+
+
+class Dropout(NamedTuple):
+  """The dropout of one training forward of N tokens per sample."""
+  rate: float
+  key: DropoutKey
+  N: int
+
+  def mask(self, layer, kind):
+    """-> lib.DropoutKey of the site (layer, kind) for this rank's rows."""
+    from big_vision_b200 import lib as L
+    k = self.key
+    return L.DropoutKey(seed=k.seed, step=k.step, site=dropout_site(k.tower, layer, kind), row0=k.sample0 * self.N,
+                        rate=self.rate)
+
+
+def check_dropout_rate(rate):
+  if not 0.0 <= rate < 1.0:
+    raise ValueError(f"dropout rate {rate} outside [0, 1)")
+
+
+def dropout(rate, key, N):
+  """Geom.dropout of a forward: None (no mask is applied) when the rate is 0 or there is no key, which is
+  the evaluation path (train=False)."""
+  return Dropout(float(rate), key, N) if rate and key is not None else None
+
+
 class Geom(NamedTuple):
   """What every stage of one forward sees besides its input: n samples of N tokens each, the
-  MLP-Mixer's stochastic-depth masks of that forward (None: no residual branch is dropped) and BERT's
-  key-padding mask [n, N] (None: every key is attended)."""
+  MLP-Mixer's stochastic-depth masks of that forward (None: no residual branch is dropped), BERT's
+  key-padding mask [n, N] (None: every key is attended) and the ViT / text encoders' Dropout (None: no
+  dropout)."""
   n: int
   N: int
   masks: Optional[torch.Tensor] = None
   key_mask: Optional[torch.Tensor] = None
+  dropout: Optional[Dropout] = None
 
 
 class Stage:

@@ -1,4 +1,4 @@
-"""ctypes binding of libbv_b200.so (C ABI declared in include/bv_b200*.h).
+"""ctypes binding of libbv_b200.so (C ABI declared in include/bv_b200*.h and include/bv_dropout.h).
 
 The product path has no fallback: if the library is missing, or a call is made
 without a compute-capability-9.x device, this module raises.
@@ -56,6 +56,11 @@ class AttnMaskedArgs(ctypes.Structure):
 
 class AttnMaskedBwdArgs(ctypes.Structure):
   _fields_ = [("attn", AttnBwdArgs), ("key_mask", c_vp), ("bsmask", c_i64)]
+
+
+class DropoutKey(ctypes.Structure):
+  _fields_ = [("seed", ctypes.c_uint64), ("step", ctypes.c_uint64), ("site", ctypes.c_uint64), ("row0", c_i64),
+              ("rate", c_f32)]
 
 
 class AdamArgs(ctypes.Structure):
@@ -144,6 +149,13 @@ SIGNATURES = {
     "bv_jet_bits": [c_vp, c_vp, c_vp, c_vp, c_vp, c_f32, c_i64, c_i64, c_vp],
 }
 
+# The same for include/bv_dropout.h, the one header outside the bv_b200*.h set: its functions, binding and C
+# link test are checked by tests/test_dropout.py rather than by the tests of the bv_b200*.h headers.
+DROPOUT_SIGNATURES = {
+    "bv_dropout": [c_vp, c_i64, c_vp, c_i64, c_i64, c_i64, ctypes.POINTER(DropoutKey), c_vp],
+    "bv_dropout_add": [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i64, c_i64, ctypes.POINTER(DropoutKey), c_vp],
+}
+
 _lib = None
 
 
@@ -161,7 +173,7 @@ def load():
         f"{LIB_PATH} not found: build it with `python -m big_vision_b200.build` "
         "(there is no CPU or eager fallback for the kernels).")
   lib = ctypes.CDLL(LIB_PATH)
-  for name, argtypes in SIGNATURES.items():
+  for name, argtypes in {**SIGNATURES, **DROPOUT_SIGNATURES}.items():
     fn = getattr(lib, name)   # raises AttributeError if the symbol is missing
     fn.argtypes = argtypes
     fn.restype = ctypes.c_int

@@ -63,8 +63,7 @@ class _Model(E.Staged):
   name: str = ""
 
   def __post_init__(self):
-    if self.dropout:
-      raise NotImplementedError("dropout > 0 is not on the benchmarked path")
+    E.check_dropout_rate(self.dropout)
     if self.pool_type not in _POOLS:
       raise NotImplementedError(f"Cannot do pooling '{self.pool_type}'")
     vit.check_head_dim(self.width, self.num_heads)
@@ -87,10 +86,12 @@ class _Model(E.Staged):
     specs, aliases = self.specs(text_shape[1])
     return E.FlatParams(specs, aliases, device).init(seed)
 
-  def fwd(self, P, text, frozen=None):
-    """text int32 [n, L] -> (fp32 [n, out], saved); bf16 [n, width] without a head.  `frozen` as in
-    vit._Model.fwd: the stages below the cut run forward-only and save nothing."""
-    return self._stages_fwd(P, text, E.Geom(*text.shape), frozen)
+  def fwd(self, P, text, frozen=None, dropout=None):
+    """text int32 [n, L] -> (fp32 [n, out], saved); bf16 [n, width] without a head.  `frozen` and `dropout`
+    as in vit._Model.fwd: the stages below the cut run forward-only and save nothing.  Dropout applies in
+    the encoder blocks only; the tower has no embedding dropout (text_transformer.py:68-74)."""
+    n, Ln = text.shape
+    return self._stages_fwd(P, text, E.Geom(n, Ln, dropout=E.dropout(self.dropout, dropout, Ln)), frozen)
 
   def bwd(self, P, dout, saved):
     if not self.num_classes:       # the tower's output is bf16
@@ -98,6 +99,8 @@ class _Model(E.Staged):
     self._stages_bwd(P, dout, saved)
 
   def apply(self, variables, text, *, train=False):
+    if train and self.dropout:
+      raise ValueError("apply(train=True) with dropout > 0 has no dropout key; call fwd(..., dropout=key)")
     x, _ = self.fwd(variables["params"], text, frozen=True)     # forward-only, same bits
     return x, {"logits" if self.num_classes else "pre_logits": x}
 

@@ -58,18 +58,23 @@ class Model:
     return (self.img.cut(P, frozen) == len(self.img.stages()),
             self.txt.cut(P, frozen) == len(self.txt.stages()))
 
-  def fwd(self, P, image, text, frozen=None):
+  def fwd(self, P, image, text, frozen=None, dropout=None):
     """-> (zimg fp32 [n,D], ztxt fp32 [n,D], saved).  `frozen` as in vit._Model.fwd; a wholly frozen
-    tower keeps nothing for the backward (its saved entries are None)."""
+    tower keeps nothing for the backward (its saved entries are None).  `dropout`: the engine.DropoutKey of
+    a training forward, or None; the image tower draws its masks as tower 0 and the text tower as tower 1,
+    so no two sites share a stream."""
     saved = {}
     ztxt = zimg = None
+    # only a tower with dropout takes a key (the BERT tower has no dropout)
+    kw = lambda m, tower: ({"dropout": dropout._replace(tower=tower)}
+                           if dropout is not None and getattr(m, "dropout", 0.0) else {})
     if text is not None:
-      e, s = self.txt.fwd(P, text, frozen=frozen)
+      e, s = self.txt.fwd(P, text, frozen=frozen, **kw(self.txt, 1))
       ztxt, nrm = ops.l2norm_fwd(e, eps=1e-8)
       live = self.txt.cut(P, frozen) < len(self.txt.stages())
       saved["txt"], saved["txt_norm"] = (s, (ztxt, nrm)) if live else (None, None)
     if image is not None:
-      e, s = self.img.fwd(P, image, frozen=frozen)
+      e, s = self.img.fwd(P, image, frozen=frozen, **kw(self.img, 0))
       zimg, nrm = ops.l2norm_fwd(e, eps=1e-8)
       live = self.img.cut(P, frozen) < len(self.img.stages())
       saved["img"], saved["img_norm"] = (s, (zimg, nrm)) if live else (None, None)
@@ -90,6 +95,8 @@ class Model:
   def apply(self, variables, image, text=None, **kw):
     """(zimg, ztxt, out) like the flax apply (two_towers.py:39-90); forward-only (same bits as the
     training forward, nothing kept for a backward)."""
+    if kw.get("train") and (getattr(self.img, "dropout", 0.0) or getattr(self.txt, "dropout", 0.0)):
+      raise ValueError("apply(train=True) with dropout > 0 has no dropout key; call fwd(..., dropout=key)")
     P = variables["params"]
     zimg, ztxt, _ = self.fwd(P, image, text, frozen=True)
     out = {"t": P.f("t").exp(), "t/parameter": P.f("t")}

@@ -129,33 +129,47 @@ class Scope:
     return Scope(self.P, self.prefix + rel, self.index)
 
 
-def mlp_fwd(S, y, resid, out_dtype=torch.bfloat16, save=True):
+def mlp_fwd(S, y, resid, out_dtype=torch.bfloat16, save=True, drop=None):
   """resid + Dense_1(gelu(Dense_0(y))) with S the MlpBlock's Scope.  Returns (out, saved).
-  save=False (forward only): GELU's pre-activation is not written at all, saved is None."""
+  save=False (forward only): GELU's pre-activation is not written at all, saved is None.
+  drop: None, or the lib.DropoutKeys (GELU output, MLP output) of the encoder block's dropouts
+  (models/vit.py:76,109): the GELU output is dropped in place, so the saved activation is the dropped one,
+  and the residual add follows the dropped Dense_1 output."""
   if save:
     act, pre = ops.gemm(y, S.h("Dense_0/kernel"), b_mn=True, bias=S.f("Dense_0/bias"),
                         epilogue=L.EPI_BIAS_GELU)
   else:
     act = ops.gemm(y, S.h("Dense_0/kernel"), b_mn=True, bias=S.f("Dense_0/bias"),
                    epilogue=L.EPI_BIAS_GELU_ACT)
-  out = ops.gemm(act, S.h("Dense_1/kernel"), b_mn=True, bias=S.f("Dense_1/bias"),
-                 aux=resid, epilogue=L.EPI_BIAS_RESID if resid is not None else L.EPI_BIAS,
-                 out_dtype=out_dtype)
+  if drop is not None:
+    ops.dropout(act, drop[0], out=act)
+    out = ops.gemm(act, S.h("Dense_1/kernel"), b_mn=True, bias=S.f("Dense_1/bias"))
+    out = ops.dropout_add(resid, out, drop[1], out=out)
+  else:
+    out = ops.gemm(act, S.h("Dense_1/kernel"), b_mn=True, bias=S.f("Dense_1/bias"),
+                   aux=resid, epilogue=L.EPI_BIAS_RESID if resid is not None else L.EPI_BIAS,
+                   out_dtype=out_dtype)
   return out, ((y, act, pre) if save else None)
 
 
-def mlp_bwd(S, dout, saved, want_bias2_grad=True):
+def mlp_bwd(S, dout, saved, want_bias2_grad=True, gelu_drop=None):
   """dout: bf16 [M,d] gradient of the block output.  Returns d(y) (bf16).
 
   The bias gradient of Dense_1 is colsum(dout); callers that already have that column sum
-  from the LayerNorm-backward kernel pass want_bias2_grad=False."""
+  from the LayerNorm-backward kernel pass want_bias2_grad=False.  gelu_drop: the lib.DropoutKey of the
+  forward's GELU-output dropout, or None; its mask is applied to d(GELU pre-activation), which equals
+  masking the GELU output's gradient since both are element-wise products."""
   y, act, pre = saved
   if want_bias2_grad:
     ops.colsum(dout, S.g("Dense_1/bias"))
   ops.gemm(act, dout, a_mn=True, b_mn=True, out=S.g("Dense_1/kernel"), reduce_out=True)
-  # the Dense_0 bias gradient (column sums of dpre) is accumulated by the same GEMM's epilogue
-  dpre = ops.gemm(dout, S.h("Dense_1/kernel"), aux=pre, epilogue=L.EPI_DGELU,
-                  colsum=S.g("Dense_0/bias"))
+  if gelu_drop is not None:
+    dpre = ops.gemm(dout, S.h("Dense_1/kernel"), aux=pre, epilogue=L.EPI_DGELU)
+    ops.dropout(dpre, gelu_drop, out=dpre, colsum_into=S.g("Dense_0/bias"))
+  else:
+    # the Dense_0 bias gradient (column sums of dpre) is accumulated by the same GEMM's epilogue
+    dpre = ops.gemm(dout, S.h("Dense_1/kernel"), aux=pre, epilogue=L.EPI_DGELU,
+                    colsum=S.g("Dense_0/bias"))
   ops.gemm(y, dpre, a_mn=True, b_mn=True, out=S.g("Dense_0/kernel"), reduce_out=True)
   return ops.gemm(dpre, S.h("Dense_0/kernel"))
 
@@ -201,10 +215,12 @@ def mha_specs(p, d, heads, fuse_qkv=True, stack=0):
 
 class EncoderBlock(E.Stage):
   """Encoder1DBlock (models/vit.py:81-112): x + MHSA(LN(x)); x + MLP(LN(x)).
-  `index` = position in the scan-stacked `encoderblock` sub-tree (None: own `encoderblock_{i}`)."""
+  `index` = position in the scan-stacked `encoderblock` sub-tree (None: own `encoderblock_{i}`); `layer` = the
+  block's depth in its encoder, which selects its dropout masks (default: index)."""
 
-  def __init__(self, prefix, d, m, heads, index=None):
+  def __init__(self, prefix, d, m, heads, index=None, layer=None):
     self.p, self.d, self.m, self.heads, self.index = prefix, d, m, heads, index
+    self.layer = index if layer is None else layer
     self.prefixes = (prefix,)
     # every parameter from this block on (in spec order) has its final gradient after its backward: a
     # data-parallel trainer can start reducing them while the earlier blocks are still running
@@ -232,39 +248,57 @@ class EncoderBlock(E.Stage):
     o, lse = ops.attention_fwd(qkv3[:, :, 0:d], qkv3[:, :, d:2 * d], qkv3[:, :, 2 * d:], self.heads)
     if not save:
       del ln1, mean1, rstd1, qkv, qkv3, lse
-    x1 = ops.gemm(o.view(n * N, d), A.h("out_proj/kernel"), b_mn=True,
-                  bias=A.f("out/bias"), aux=x, epilogue=L.EPI_BIAS_RESID)
+    dr = geom.dropout
+    if dr is None:
+      x1 = ops.gemm(o.view(n * N, d), A.h("out_proj/kernel"), b_mn=True,
+                    bias=A.f("out/bias"), aux=x, epilogue=L.EPI_BIAS_RESID)
+    else:    # models/vit.py:100: the attention output is dropped before the residual add
+      x1 = ops.gemm(o.view(n * N, d), A.h("out_proj/kernel"), b_mn=True, bias=A.f("out/bias"))
+      x1 = ops.dropout_add(x, x1, dr.mask(self.layer, E.DROP_ATTN), out=x1)
     if not save:
       del o
     ln2, mean2, rstd2 = ops.layernorm_fwd(x1, S.f("LayerNorm_1/scale"), S.f("LayerNorm_1/bias"))
+    drop = None if dr is None else (dr.mask(self.layer, E.DROP_GELU), dr.mask(self.layer, E.DROP_MLP))
     if not save:
       del mean2, rstd2
-      x2, _ = mlp_fwd(S.sub("MlpBlock_0/"), ln2, x1, save=False)
+      x2, _ = mlp_fwd(S.sub("MlpBlock_0/"), ln2, x1, save=False, drop=drop)
       return x2, None
-    x2, mlp_saved = mlp_fwd(S.sub("MlpBlock_0/"), ln2, x1)
+    x2, mlp_saved = mlp_fwd(S.sub("MlpBlock_0/"), ln2, x1, drop=drop)
     return x2, (x, ln1, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, mlp_saved)
 
   def sink(self, P, geom):
-    """colsum(d block-output) is the gradient of this block's MlpBlock Dense_1 bias."""
-    return self.scope(P).g("MlpBlock_0/Dense_1/bias")
+    """colsum(d block-output) is the gradient of this block's MlpBlock Dense_1 bias.  Under dropout that
+    bias sees the masked gradient, so the block offers no sink and sums it itself (bwd)."""
+    return None if geom.dropout else self.scope(P).g("MlpBlock_0/Dense_1/bias")
 
   def bwd(self, P, dx2, saved, geom, sink, need_dx=True):
-    """dx2: bf16 [M,d] grad of block output; colsum(dx2) has ALREADY been accumulated into
-    this block's Dense_1 bias grad by whoever produced dx2.  Returns dx (grad of block input);
-    colsum(dx) is accumulated into `sink` (the bias gradient of the stage below)."""
+    """dx2: bf16 [M,d] grad of block output; without dropout colsum(dx2) has ALREADY been accumulated
+    into this block's Dense_1 bias grad by whoever produced dx2 (sink).  Returns dx (grad of block input);
+    colsum(dx) is accumulated into `sink` (the bias gradient of the stage below).  Under dropout the
+    gradients entering the MLP and the attention output projection are masked as in the forward; the
+    residual stream's gradient is not."""
     n, N = geom.n, geom.N
     d = self.d
     S = self.scope(P)
     A = S.sub("MultiHeadDotProductAttention_0/")
     x, ln1, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, mlp_saved = saved
-    dln2 = mlp_bwd(S.sub("MlpBlock_0/"), dx2, mlp_saved, want_bias2_grad=False)
+    dr = geom.dropout
+    if dr is None:
+      dln2 = mlp_bwd(S.sub("MlpBlock_0/"), dx2, mlp_saved, want_bias2_grad=False)
+    else:
+      dm = ops.dropout(dx2, dr.mask(self.layer, E.DROP_MLP), colsum_into=S.g("MlpBlock_0/Dense_1/bias"))
+      dln2 = mlp_bwd(S.sub("MlpBlock_0/"), dm, mlp_saved, want_bias2_grad=False,
+                     gelu_drop=dr.mask(self.layer, E.DROP_GELU))
+      del dm
     dx1 = ops.layernorm_bwd(dln2, x1, S.f("LayerNorm_1/scale"), mean2, rstd2, dres=dx2,
                             dscale=S.g("LayerNorm_1/scale"), dbias=S.g("LayerNorm_1/bias"),
-                            dx_colsum=A.g("out/bias"))
+                            dx_colsum=A.g("out/bias") if dr is None else None)
     del dln2
+    da = dx1 if dr is None else ops.dropout(dx1, dr.mask(self.layer, E.DROP_ATTN), colsum_into=A.g("out/bias"))
     o2 = o.view(n * N, d)
-    ops.gemm(o2, dx1, a_mn=True, b_mn=True, out=A.g("out_proj/kernel"), reduce_out=True)
-    do = ops.gemm(dx1, A.h("out_proj/kernel"))
+    ops.gemm(o2, da, a_mn=True, b_mn=True, out=A.g("out_proj/kernel"), reduce_out=True)
+    do = ops.gemm(da, A.h("out_proj/kernel"))
+    del da
     qkv3 = qkv.view(n, N, 3 * d)
     dqkv = torch.empty_like(qkv)
     dqkv3 = dqkv.view(n, N, 3 * d)
@@ -325,7 +359,7 @@ def encoder_stages(prefix, depth, d, m, heads, scan=False, remat_policy="nothing
   (models/vit.py:151-158), or one ScanEncoder with scan=True."""
   if scan:
     return [ScanEncoder(prefix, depth, d, m, heads, remat_policy)]
-  return [EncoderBlock(f"{prefix}encoderblock_{i}/", d, m, heads) for i in range(depth)]
+  return [EncoderBlock(f"{prefix}encoderblock_{i}/", d, m, heads, layer=i) for i in range(depth)]
 
 
 class NormPool(E.Stage):
@@ -500,16 +534,21 @@ class PatchEmbedding(E.Stage):
     if self.cls:
       # cls token is prepended AFTER the position embedding was added (models/vit.py:223-225)
       x = ops.concat_cls(x, P.f(self.p + "cls").view(self.d), n, N0)
+    if geom.dropout is not None:     # models/vit.py:228
+      ops.dropout(x, geom.dropout.mask(0, E.DROP_EMBED), out=x)
     return x, saved
 
   def sink(self, P, geom):
     # the column sum of the gradient reaching the embedding output is the patch-embed bias gradient
-    # (models/vit.py:212-214); with [cls] it is summed over the patch tokens only (bwd)
-    return None if self.cls else P.g(self.w + "bias")
+    # (models/vit.py:212-214); with [cls] it is summed over the patch tokens only, and under dropout over
+    # the masked gradient (bwd)
+    return None if self.cls or geom.dropout else P.g(self.w + "bias")
 
   def bwd(self, P, dx, patches, geom, sink=None, need_dx=False):
     n, N = geom.n, geom.N
     d, p = self.d, self.p
+    if geom.dropout is not None:
+      dx = ops.dropout(dx, geom.dropout.mask(0, E.DROP_EMBED), colsum_into=None if self.cls else P.g(self.w + "bias"))
     if self.cls:
       # batch-sum of the gradient at every token position: row 0 is d cls, the rest d pos_embedding;
       # the patch-embed bias gradient is the sum of the latter over positions
@@ -554,8 +593,7 @@ class _Model(E.Staged):
   name: str = ""
 
   def __post_init__(self):
-    if self.dropout:
-      raise NotImplementedError("dropout > 0 is not on the benchmarked path (reference configs use 0)")
+    E.check_dropout_rate(self.dropout)
     if self.pool_type not in _POOLS:
       raise ValueError(f"Unknown pool type: '{self.pool_type}'")
     check_head_dim(self.width, self.num_heads)
@@ -587,15 +625,17 @@ class _Model(E.Staged):
     return E.FlatParams(specs, aliases, device).init(seed)
 
   # ---- forward / backward ----------------------------------------------------------------
-  def fwd(self, P, image, frozen=None):
+  def fwd(self, P, image, frozen=None, dropout=None):
     """image [n,H,W,C] fp32 in [-1,1] (the shape given to specs()) -> (x fp32 [n, out], saved).  With a
     class head whose storage is padded (common.Dense) x is the [n, num_classes] view of the padded logits.
 
     `frozen`: storage names that receive no gradient (optax.Chain.frozen()), or True for all of them
     (inference).  Stages below the cut (see cut()) run forward-only and save nothing; the output is
-    bit-identical either way."""
+    bit-identical either way.  `dropout`: the engine.DropoutKey of a training forward; without one (or at
+    rate 0) no dropout is applied, as with train=False.  Frozen stages drop too."""
     n, N = image.shape[0], self._stages[0].tokens
-    out, saved = self._stages_fwd(P, image, E.Geom(n, N), frozen)
+    geom = E.Geom(n, N, dropout=E.dropout(self.dropout, dropout, N))
+    out, saved = self._stages_fwd(P, image, geom, frozen)
     if self.pool_type == "none":
       # no pooling (models/vit.py:252-253): pre_logits / head run on every token, out is [n, N, .]
       if out.dtype != torch.float32:
@@ -613,7 +653,10 @@ class _Model(E.Staged):
 
   # ---- reference-style entry points --------------------------------------------------------
   def apply(self, variables, image, *, train=False):
-    """(x, out) like flax apply (models/vit.py:206-276); `out` holds what this path keeps."""
+    """(x, out) like flax apply (models/vit.py:206-276); `out` holds what this path keeps.  train=True
+    with dropout needs a key, which apply() has no argument for: use fwd(..., dropout=key)."""
+    if train and self.dropout:
+      raise ValueError("apply(train=True) with dropout > 0 has no dropout key; call fwd(..., dropout=key)")
     P = variables["params"]
     x, _ = self.fwd(P, image, frozen=True)     # no backward follows: forward-only, same bits
     out = {"head_input": x} if not (self.rep_size or self.num_classes) else {}

@@ -359,6 +359,37 @@ def drop_cls(x, n, N0):
   return out
 
 
+def _bf16_2d(*ts):
+  for t in ts:
+    if t.dtype != torch.bfloat16 or t.dim() != 2 or t.stride(1) != 1:
+      raise L.BvError(f"dropout takes bf16 [rows, cols] matrices with a contiguous last axis, got "
+                      f"{t.dtype} {tuple(t.shape)} {t.stride()}")
+
+
+def dropout(x, key, out=None, colsum_into=None):
+  """out = dropout(x) under `key` (lib.DropoutKey) for bf16 [rows, cols] (row-strided views allowed; `out`
+  may be x).  colsum_into: None, or fp32 [cols] += the column sums of out (a bias gradient).  Returns out."""
+  out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device) if out is None else out
+  _bf16_2d(x, out)
+  assert out.shape == x.shape, (tuple(x.shape), tuple(out.shape))
+  L.call("bv_dropout", _p(x), x.stride(0), _p(out), out.stride(0), x.shape[0], x.shape[1], ctypes.byref(key),
+         _stream())
+  if colsum_into is not None:
+    colsum(out, colsum_into)
+  return out
+
+
+def dropout_add(resid, y, key, out=None):
+  """out = resid + dropout(y) under `key` for bf16 [rows, cols] (row-strided views allowed; `out` may be
+  resid or y).  Returns out."""
+  out = torch.empty(y.shape, dtype=torch.bfloat16, device=y.device) if out is None else out
+  _bf16_2d(resid, y, out)
+  assert resid.shape == y.shape == out.shape, (tuple(resid.shape), tuple(y.shape), tuple(out.shape))
+  L.call("bv_dropout_add", _p(resid), resid.stride(0), _p(y), y.stride(0), _p(out), out.stride(0), y.shape[0],
+         y.shape[1], ctypes.byref(key), _stream())
+  return out
+
+
 def siglip_loss(dots, row_offset, t_param, b_param, global_b, loss, dt, db):
   n, B = dots.shape
   # G feeds two GEMMs through TMA: its row stride must be a multiple of 16 bytes (8 bf16) even when the

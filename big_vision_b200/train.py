@@ -9,6 +9,7 @@ loss+gradient kernels.
 """
 import torch
 
+from big_vision_b200 import engine as E
 from big_vision_b200 import ops
 from big_vision_b200.trainers.proj.image_text.siglip import Dist
 
@@ -57,11 +58,19 @@ def loss_and_grads(model, P, images, labels, loss_name="sigmoid_xent", dist_view
   return loss, logits
 
 
+def dropout_key(seed, opt, d, n):
+  """The engine.DropoutKey of a training step on this rank's n samples: config.seed, the optimizer's step
+  count and the rank's first sample in the global batch, taken as the Jet trainer takes its noise key, so
+  a step draws the masks of one rank running the global batch."""
+  return E.DropoutKey(seed, int(opt["count"]), d.rank * n)
+
+
 def make_update_fn(model, tx, config):
   mixup_p = (config.get("mixup") or {}).get("p")
   loss_name = config.get("loss", "sigmoid_xent")
   d = Dist()
   frozen = tx.frozen() if hasattr(tx, "frozen") else frozenset()
+  seed = int(config.get("seed", 0))
 
   def update_fn(train_state, rng, batch, **fwd_kw):
     """`fwd_kw`: extra keyword arguments of the model's forward (a FlexiViT step's seqhw)."""
@@ -75,6 +84,8 @@ def make_update_fn(model, tx, config):
     # stochastic depth (Mixer, mlp_mixer.py:173-177) draws its masks from the step's rng like the
     # reference's `rngs={"dropout": rng}` (train.py:296-299)
     kw = dict(train=True, rng=rng) if getattr(model, "stoch_depth", 0.0) else {}
+    if getattr(model, "dropout", 0.0):
+      kw["dropout"] = dropout_key(seed, opt, d, images.shape[0])
     loss, _ = loss_and_grads(model, P, images, labels, loss_name, dist_view=d, frozen=frozen, **kw, **fwd_kw)
     # the loss is the mean over the GLOBAL batch: sum the per-rank means and divide by world
     d.all_reduce_sum(loss)

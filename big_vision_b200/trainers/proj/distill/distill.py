@@ -92,6 +92,7 @@ def make_update_fn(models, tx, config):
   d = Dist()
   frozen = tx.frozen() if hasattr(tx, "frozen") else frozenset()
   student = models["student"]
+  seed = int(config.get("seed", 0))
 
   def update_fn(train_state, rng, batch, **student_kw):
     """`student_kw`: extra keyword arguments of the student's forward only (a FlexiViT student's seqhw)."""
@@ -107,6 +108,8 @@ def make_update_fn(models, tx, config):
       data.update(to_mix)
     # stochastic depth for the student only (`train=name == "student"`, distill.py:226)
     kw = dict(train=True, rng=rng) if getattr(student, "stoch_depth", 0.0) else {}
+    if getattr(student, "dropout", 0.0):      # the teachers run train=False: no dropout
+      kw["dropout"] = train.dropout_key(seed, opt, d, getfirst(data, "student", "image").shape[0])
     m = loss_and_grads(models, params, data, teachers, kind, distance_kw, dist_view=d, frozen=frozen, **kw,
                        **student_kw)
     # every measurement is the mean over the GLOBAL batch: sum the per-rank means and divide by world

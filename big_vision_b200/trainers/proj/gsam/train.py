@@ -7,6 +7,7 @@
 The learning rate that sets rho is `sched_fns[0](count) * lr` at the count the optimizer evaluates its
 own schedule with.  Measurements: the CLEAN loss, l2_grads of the averaged g, l2_params, l2_updates.
 """
+from big_vision_b200 import train as T
 from big_vision_b200.trainers.proj.gsam import gsam as G
 from big_vision_b200.trainers.proj.image_text.siglip import Dist
 
@@ -23,6 +24,7 @@ def make_update_fn(model, tx, config):
     raise NotImplementedError("GSAM supports one global learning-rate schedule (train.py:182)")
   d = Dist()
   twin = {}
+  seed = int(config.get("seed", 0))
 
   def update_fn(train_state, rng, batch):
     P, opt = train_state["params"], train_state["opt"]
@@ -38,6 +40,8 @@ def make_update_fn(model, tx, config):
       if rng is None:
         raise ValueError("stoch_depth > 0 in training needs an rng (numpy Generator)")
       fwd_kw["masks"] = model.draw_masks(rng, images.shape[0], images.device)
+    if getattr(model, "dropout", 0.0):      # one key for both passes, as for the masks above
+      fwd_kw["dropout"] = T.dropout_key(seed, opt, d, images.shape[0])
     if "P" not in twin or twin["P"][0] is not P:
       twin["P"] = (P, P.twin())
     lr = tx.sched_fns[0](opt["count"]) * tx.lr

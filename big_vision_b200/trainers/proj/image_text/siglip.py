@@ -19,6 +19,7 @@ import os
 import torch
 import torch.distributed as dist
 
+from big_vision_b200 import engine as E
 from big_vision_b200 import ops
 
 
@@ -285,8 +286,10 @@ def make_update_fn(model, tx, config=None):
   frozen = tx.frozen() if hasattr(tx, "frozen") else frozenset()
   plan = {}
 
+  seed = int((config or {}).get("seed", 0))
+
   def update_fn(train_state, rng, batch):
-    del rng  # dropout is 0 on this path; nothing stochastic in the step
+    del rng  # the dropout masks come from config.seed and the step count
     P, opt = train_state["params"], train_state["opt"]
     images, labels = batch["image"], batch["labels"]
     if id(P) not in plan:
@@ -295,7 +298,8 @@ def make_update_fn(model, tx, config=None):
     fz, ranges, (img_frozen, txt_frozen) = plan[id(P)]
     P.zero_grad()
     scal = torch.zeros(4, dtype=torch.float32, device=P.flat.device)
-    zimg, ztxt, saved = model.fwd(P, images, labels, frozen=fz)
+    key = E.DropoutKey(seed, int(opt["count"]), d.rank * images.shape[0])
+    zimg, ztxt, saved = model.fwd(P, images, labels, frozen=fz, dropout=key)
     dzimg, dztxt = loss_fwd_bwd(P, zimg, ztxt, d, scal, img_grad=not img_frozen, txt_grad=not txt_frozen)
     # C3 (+ dt, db inside the flat buffer), bucketed and overlapped with the backward
     all_reduce_grads(P, d, lambda: model.bwd(P, dzimg, dztxt, saved), ranges=ranges)
@@ -320,16 +324,17 @@ def _frozen_plan(model, P, frozen):
   return frozen, P.trained_ranges(frozen), model.tower_frozen(P, frozen)
 
 
-def loss_and_grads(model, P, images, labels, loss_fn="sigmoid", frozen=None):
+def loss_and_grads(model, P, images, labels, loss_fn="sigmoid", frozen=None, dropout=None):
   """value_and_grad(loss_fn)(params) of siglip.py:287-311 without the optimizer: returns the
   global loss (device scalar) with P.grad holding d loss / d params (summed over ranks).  `frozen`
-  (storage names, optax.Chain.frozen()) as in make_update_fn: their gradients are not computed."""
+  (storage names, optax.Chain.frozen()) as in make_update_fn: their gradients are not computed.
+  `dropout`: the step's engine.DropoutKey, or None (no dropout)."""
   d = Dist()
   sigmoid_loss_fwd_bwd = _loss_fn({"loss_fn": loss_fn})   # pylint: disable=redefined-outer-name
   fz, ranges, (img_frozen, txt_frozen) = _frozen_plan(model, P, frozen)
   P.zero_grad()
   scal = torch.zeros(4, dtype=torch.float32, device=P.flat.device)
-  zimg, ztxt, saved = model.fwd(P, images, labels, frozen=fz)
+  zimg, ztxt, saved = model.fwd(P, images, labels, frozen=fz, dropout=dropout)
   dzimg, dztxt = sigmoid_loss_fwd_bwd(P, zimg, ztxt, d, scal, img_grad=not img_frozen,
                                       txt_grad=not txt_frozen)
   all_reduce_grads(P, d, lambda: model.bwd(P, dzimg, dztxt, saved), ranges=ranges)
