@@ -16,12 +16,15 @@
 // The grid is persistent: min(work units, SMs) CTAs, each running a static sequence of work units
 // (one 128 x BN output tile x one K split; gemm_sched.h).  Roles (384 threads): warpgroup 0 is the
 // TMA producer (one thread issues, the rest give their registers back with setmaxnreg), warpgroups
-// 1 and 2 each run m64 x BN x 16 wgmma on their half of the rows from a STAGES-deep ring of shared
-// memory.  The ring's barriers live for the whole CTA and the producer runs ahead across units, so
-// the next tile's loads overlap this tile's epilogue.  Plain bf16 outputs leave through shared
-// memory and TMA stores; a row-aligned aux operand (residual, gelu' pre-activation) arrives by TMA
-// into the same staging buffers during the main loop.  fp32 and bf16 reduce-add outputs store from
-// the registers.
+// 1 and 2 are the consumers, fed from a STAGES-deep ring of shared memory.  At BN = 128 they
+// ping-pong: the CTA's units alternate between them, a warpgroup runs all 128 rows of its unit
+// (two m64 x 128 x 16 wgmma per k16 step), and one warpgroup's epilogue runs while the other's MMAs
+// keep the tensor cores busy.  At BN = 256 they cooperate: both run every unit, each m64 x 256 x 16 on
+// its half of the rows.  The ring's barriers live for the whole CTA and the producer runs ahead
+// across units, so the next tile's loads overlap this tile's epilogue.  Plain bf16 outputs leave
+// through shared memory and TMA stores; a row-aligned aux operand (residual, gelu' pre-activation)
+// arrives by TMA into the same staging buffers during the main loop.  fp32 and bf16 reduce-add
+// outputs store from the registers.
 #include "common.cuh"
 #include "gemm_sched.h"
 #include "host_utils.h"
@@ -35,7 +38,7 @@ namespace bv {
 
 namespace {
 
-constexpr int BM = 128;          // rows per tile (two consumer warpgroups of 64)
+constexpr int BM = 128;          // rows per tile: two 64-row halves
 constexpr int BK = 64;           // 64 bf16 = 128 B = one swizzle row
 constexpr int A_STAGE_BYTES = BM * BK * 2;   // 16 KB
 constexpr int NUM_THREADS = 384;
@@ -53,27 +56,33 @@ enum : int { OM_F32 = 0, OM_BF16_ADD = 1, OM_BF16_TMA = 2 };
 
 template <int BN, int OM, int EF>
 struct Cfg {
+  // BN = 128: ping-pong, each consumer warpgroup runs both 64-row halves of its own units.
+  // BN = 256: cooperative, each consumer warpgroup runs one half of every unit.
+  static constexpr bool PINGPONG = BN == 128;
+  static constexpr int HALVES = PINGPONG ? 2 : 1;
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  // TMA-store staging of bf16 outputs, each buffer holding one sub-tile of every output (GELU writes
-  // two).  Per consumer warpgroup either two buffers (one fills while the other's store is in
-  // flight), or, when aux is loaded by TMA, one buffer per sub-tile of the unit, so that the whole
-  // unit's aux is prefetched during its main loop.
+  // TMA-store staging of bf16 outputs, each buffer holding one 64 x 64 sub-tile of every output (GELU
+  // writes two).  Per consumer warpgroup either two buffers (one fills while the other's store is in
+  // flight), or, when aux is loaded by TMA, one buffer per sub-tile of the warpgroup's part of the
+  // unit, so that the whole unit's aux is prefetched during its main loop.
   static constexpr bool AUX_TMA = OM == OM_BF16_TMA && (EF == EF_RESID || EF == EF_DGELU);
   static constexpr int OUTS = OM != OM_BF16_TMA ? 0 : (EF == EF_GELU ? 2 : 1);
   static constexpr int BUF_BYTES = OUTS * SUB_BYTES;
-  static constexpr int BUFS = AUX_TMA ? BN / 64 : 2;
+  static constexpr int BUFS = AUX_TMA ? HALVES * BN / 64 : 2;
   static constexpr int STAGING_BYTES = 2 * BUFS * BUF_BYTES;
   static constexpr int SMEM_LIMIT = 232448 - 2048;         // 227 KB minus barriers / align slack
   static constexpr int STAGES_FIT = (SMEM_LIMIT - STAGING_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
   static constexpr int STAGING_OFFSET = STAGES * STAGE_BYTES;
   static constexpr int BAR_OFFSET = STAGING_OFFSET + STAGING_BYTES;
-  // barriers: full and empty per stage, then (AUX_TMA) one per staging buffer of each warpgroup
+  // barriers: full and empty per stage, then (AUX_TMA) one per staging buffer of each warpgroup, then
+  // (PINGPONG) one per warpgroup that completes a phase when all of its unit's k blocks have landed
   static constexpr int AUX_BAR = 2 * STAGES;
+  static constexpr int ISSUED_BAR = AUX_BAR + (AUX_TMA ? 2 * BUFS : 0);
   static constexpr int SMEM_BYTES = BAR_OFFSET + 256 + 1024;  // + barriers + align slack
   static_assert(STAGES >= 3, "shared-memory budget leaves fewer than 3 stages");
-  static_assert(8 * (AUX_BAR + (AUX_TMA ? 2 * BUFS : 0)) <= 256, "barriers overflow their 256 bytes");
+  static_assert(8 * (ISSUED_BAR + 2) <= 256, "barriers overflow their 256 bytes");
 };
 
 struct GemmDev {
@@ -90,36 +99,49 @@ struct GemmDev {
   int aux_row_mod;
 };
 
-// The consumer warpgroup's main loop over one unit's k blocks.  `ps` is the running ring position,
-// carried from unit to unit.  The transpose bits of wgmma are immediates, so each operand layout pair
-// is its own instantiation (a branch between wgmma issues would make ptxas serialise them).
-// `after_first` runs once, after the first k block's MMAs are committed, so that whatever it waits
-// for overlaps them.
-template <int BN, int STAGES, int STAGE_BYTES, int TA, int TB, typename F>
-__device__ __forceinline__ void mainloop(float (&acc)[BN / 2], uint32_t base, uint32_t bar_base, int cw,
-                                         PipeState& ps, int kb0, int kb1, F&& after_first) {
+// The consumer warpgroup's main loop over one unit's k blocks, for the H 64-row halves h0 .. h0 + H - 1
+// of the tile; acc[h] holds half h0 + h.  `ps` is the running ring position, carried from unit to
+// unit.  The transpose bits of wgmma are immediates, so each operand layout pair is its own
+// instantiation (a branch between wgmma issues would make ptxas serialise them).  `after_first` runs
+// once, after the first k block's MMAs are committed, so that whatever it waits for overlaps them;
+// `after_last` runs once, after the last k block's MMAs are committed.
+template <int BN, int H, int STAGES, int STAGE_BYTES, int TA, int TB, typename F, typename G>
+__device__ __forceinline__ void mainloop(float (&acc)[H][BN / 2], uint32_t base, uint32_t bar_base, int h0,
+                                         PipeState& ps, int kb0, int kb1, F&& after_first, G&& after_last) {
   // 128B-swizzled operand tiles: K-major rows of 128 B (8-row groups 1024 B apart, K step 32 B);
-  // MN-major boxes of 64 (M|N) x 64 (K), 8 KB each (K step 16 rows = 2048 B)
+  // MN-major boxes of 64 (M|N) x 64 (K), 8 KB each (K step 16 rows = 2048 B).  Either way rows
+  // 64 .. 127 of the A tile start 8 KB after row 0.
   constexpr uint32_t a_lbo = TA ? 8192u : 16u, b_lbo = TB ? 8192u : 16u;
   constexpr uint32_t a_kstep = TA ? 2048u : 32u, b_kstep = TB ? 2048u : 32u;
   int prev_stage = -1;
   for (int kb = kb0; kb < kb1; ++kb) {
     mbar_wait(bar_base + 8u * ps.stage, ps.phase);
-    const uint32_t a_s = base + ps.stage * STAGE_BYTES + cw * 8192;
+    const uint32_t a_s = base + ps.stage * STAGE_BYTES + h0 * 8192;
     const uint32_t b_s = base + ps.stage * STAGE_BYTES + A_STAGE_BYTES;
-    const uint64_t adesc = wgmma_desc_sw128(a_s, a_lbo, 1024u), bdesc = wgmma_desc_sw128(b_s, b_lbo, 1024u);
-    wgmma_fence_regs(acc);
+    const uint64_t bdesc = wgmma_desc_sw128(b_s, b_lbo, 1024u);
+    uint64_t adesc[H];
+#pragma unroll
+    for (int h = 0; h < H; ++h) {
+      adesc[h] = wgmma_desc_sw128(a_s + h * 8192, a_lbo, 1024u);
+      wgmma_fence_regs(acc[h]);
+    }
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < BK / 16; ++k) {
-      const uint64_t a = adesc + k * (a_kstep >> 4), b = bdesc + k * (b_kstep >> 4);
+      const uint64_t b = bdesc + k * (b_kstep >> 4);
       const int accumulate = (kb > kb0 || k > 0) ? 1 : 0;    // the first MMA overwrites the registers
-      if constexpr (BN == 256) wgmma_ss_n256<TA, TB>(acc, a, b, accumulate);
-      else wgmma_ss_n128<TA, TB>(acc, a, b, accumulate);
+#pragma unroll
+      for (int h = 0; h < H; ++h) {
+        const uint64_t a = adesc[h] + k * (a_kstep >> 4);
+        if constexpr (BN == 256) wgmma_ss_n256<TA, TB>(acc[h], a, b, accumulate);
+        else wgmma_ss_n128<TA, TB>(acc[h], a, b, accumulate);
+      }
     }
     wgmma_commit();
-    wgmma_fence_regs(acc);
+#pragma unroll
+    for (int h = 0; h < H; ++h) wgmma_fence_regs(acc[h]);
     if (kb == kb0) after_first();
+    if (kb == kb1 - 1) after_last();
     // keep this k block's MMAs in flight; the previous one has retired -> its slot is free
     wgmma_wait<1>();
     if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_base + 8u * (STAGES + prev_stage));
@@ -128,7 +150,8 @@ __device__ __forceinline__ void mainloop(float (&acc)[BN / 2], uint32_t base, ui
   }
   // every MMA of the unit has retired, so the last slot is free before the epilogue starts
   wgmma_wait<0>();
-  wgmma_fence_regs(acc);
+#pragma unroll
+  for (int h = 0; h < H; ++h) wgmma_fence_regs(acc[h]);
   if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(bar_base + 8u * (STAGES + prev_stage));
 }
 
@@ -189,11 +212,12 @@ __device__ __forceinline__ void colsum_add(float* colsum, int N, float s0, float
 // Epilogue straight from the registers: fp32 outputs, and bf16 reduce-add outputs (gradient
 // accumulation; never with colsum).  Under split-K every unit adds its partial into D, so bias and a
 // residual are added only by the unit of the first split (kb0 == 0); gelu' scales every partial.
+// r0 is the first row of the warpgroup's 64-row half.
 template <int BN, bool OUT_F32, int EF>
-__device__ __forceinline__ void epilogue_regs(const GemmDev& p, const float (&acc)[BN / 2], int m0, int n0,
-                                              int cw, int kb0) {
+__device__ __forceinline__ void epilogue_regs(const GemmDev& p, const float (&acc)[BN / 2], int r0, int n0,
+                                              int kb0) {
   const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
-  const int row0 = m0 + cw * 64 + warp * 16 + (lane >> 2);
+  const int row0 = r0 + warp * 16 + (lane >> 2);
   const int pM = p.M, pN = p.N;
   const float alpha = p.alpha;
   const bool reduce = p.reduce_out != 0;
@@ -226,18 +250,29 @@ __device__ __forceinline__ void epilogue_regs(const GemmDev& p, const float (&ac
           *dp = v0;
         }
       } else {
+        // the pair, or (last column of an odd N) its low half, as one predicated reduction: two branches
+        // here, one per case, make ptxas spill the 128 accumulators of a ping-pong unit
         bf16* dp = static_cast<bf16*>(p.d) + row * p.ldd + col;
-        const __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
-        if (pair) atomicAdd(reinterpret_cast<__nv_bfloat162*>(dp), o);
-        else atomicAdd(dp, o.x);
+        const uint32_t o = pack_bf16(v0, v1);
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            ".reg .b16 lo, hi;\n"
+            "setp.ne.u32 p, %2, 0;\n"
+            "mov.b32 {lo, hi}, %1;\n"
+            "@p red.global.add.noftz.bf16x2 [%0], %1;\n"
+            "@!p red.global.add.noftz.bf16 [%0], lo;\n"
+            "}\n" ::"l"(dp), "r"(o), "r"(pair ? 1u : 0u)
+            : "memory");
       }
     }
   }
 }
 
-// Epilogue through shared memory for plain bf16 outputs: the warpgroup writes each 64-column
-// sub-tile of its 64 rows into a 128B-swizzled staging buffer (the 16-byte chunk index XOR the row
-// mod 8, so the 8 rows of one store instruction hit different banks), and one thread stores it with
+// Epilogue through shared memory for plain bf16 outputs, for one 64-row half of the tile (first row
+// r0): the warpgroup writes each 64-column sub-tile of those rows into a 128B-swizzled staging buffer
+// (the 16-byte chunk index XOR the row mod 8, so the 8 rows of one store instruction hit different
+// banks), and one thread stores it with
 // TMA, which clips rows >= M and columns >= N8 = N rounded down to a multiple of 8.  TMA writes the
 // innermost dimension in whole 16-byte chunks, so a map of width N with N % 8 != 0 would write the
 // chunk's columns N .. round_up(N, 8) - 1 of a strided output; the N % 8 columns past N8 are copied
@@ -245,19 +280,19 @@ __device__ __forceinline__ void epilogue_regs(const GemmDev& p, const float (&ac
 //
 // Without a TMA-loaded aux the two buffers alternate; `nstore` counts the warpgroup's sub-tiles across
 // units, and the issuing thread waits until the store that last read a buffer is done reading before
-// the buffer is refilled.  With one (EF_RESID, EF_DGELU), sub-tile c uses buffer c, which already
-// holds the aux sub-tile (issue_aux_loads, same swizzle): each thread waits on the buffer's barrier
-// (phase `aux_parity`), reads its aux pair at the offset where it then writes its output pair, and the
-// output overwrites the aux in place.
+// the buffer is refilled.  With one (EF_RESID, EF_DGELU), sub-tile c of the half uses buffer c after
+// `staging`, which already holds the aux sub-tile (issue_aux_loads, same swizzle): each thread waits
+// on the buffer's barrier (phase `aux_parity`), reads its aux pair at the offset where it then writes
+// its output pair, and the output overwrites the aux in place.
 template <int BN, int EF, int BUF_BYTES>
 __device__ __forceinline__ void epilogue_tma(const GemmDev& p, const CUtensorMap* tmD, const CUtensorMap* tmD2,
-                                             const float (&acc)[BN / 2], int m0, int n0, int cw, uint32_t staging,
+                                             const float (&acc)[BN / 2], int r0, int n0, int cw, uint32_t staging,
                                              uint32_t& nstore, uint32_t aux_bar, uint32_t aux_parity) {
   constexpr bool AUX_TMA = (EF == EF_RESID || EF == EF_DGELU);
   const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
   const bool leader = (threadIdx.x & 127) == 0;
-  const int rl0 = warp * 16 + (lane >> 2);       // row within the warpgroup's 64
-  const int row0 = m0 + cw * 64 + rl0;
+  const int rl0 = warp * 16 + (lane >> 2);       // row within the half
+  const int row0 = r0 + rl0;
   const int pM = p.M, pN = p.N, pN8 = p.N & ~7;
   const float alpha = p.alpha;
 #pragma unroll
@@ -320,9 +355,9 @@ __device__ __forceinline__ void epilogue_tma(const GemmDev& p, const CUtensorMap
     fence_proxy_async();
     named_bar_sync(1 + cw, 128);
     if (leader) {
-      if (n0 + 64 * c < pN8 && m0 + cw * 64 < pM) {     // sub-tiles wholly past N8 are not stored
-        tma_store_2d(tmD, buf, n0 + 64 * c, m0 + cw * 64);
-        if (EF == EF_GELU) tma_store_2d(tmD2, buf + SUB_BYTES, n0 + 64 * c, m0 + cw * 64);
+      if (n0 + 64 * c < pN8 && r0 < pM) {     // sub-tiles wholly past N8 are not stored
+        tma_store_2d(tmD, buf, n0 + 64 * c, r0);
+        if (EF == EF_GELU) tma_store_2d(tmD2, buf + SUB_BYTES, n0 + 64 * c, r0);
       }
       tma_store_commit();
     }
@@ -332,7 +367,7 @@ __device__ __forceinline__ void epilogue_tma(const GemmDev& p, const CUtensorMap
     const int tail0 = pN8 - (n0 + 64 * c);
     if (pN8 < pN && tail0 >= 0 && tail0 < 64) {
       const int t = threadIdx.x & 127, rl = t & 63, out = t >> 6;
-      const int row = m0 + cw * 64 + rl;
+      const int row = r0 + rl;
       if (row < pM && (out == 0 || EF == EF_GELU)) {
         const uint32_t src = buf + out * SUB_BYTES + rl * 128 + (((tail0 >> 3) ^ (rl & 7)) << 4);
         uint16_t* dst = reinterpret_cast<uint16_t*>(out ? p.d2 : p.d) + row * (out ? p.ldd2 : p.ldd) + pN8;
@@ -355,23 +390,29 @@ __device__ __forceinline__ void epilogue_tma(const GemmDev& p, const CUtensorMap
 }
 
 // Run by the warpgroup's leader thread, which owns the warpgroup's bulk-store groups: once every store
-// of the previous unit has finished reading its staging buffer, TMA-load this unit's aux sub-tiles
-// (64 rows x 64 columns, 128B-swizzled like the outputs) into buffers 0 .. BN/64 - 1.  A sub-tile
-// wholly past N, or a warpgroup whose 64 rows are all past M, is never stored, so its aux is not
-// loaded; a plain arrival completes the barrier's phase instead, which keeps every barrier's phase
-// equal to the unit count and the consumers' wait unconditional.
-template <int BN>
-__device__ __forceinline__ void issue_aux_loads(const CUtensorMap* tmAux, int M, int N, int m0, int n0, int cw,
+// of the warpgroup's previous unit has finished reading its staging buffer, TMA-load the aux sub-tiles
+// (64 rows x 64 columns, 128B-swizzled like the outputs) of the H halves h0 .. h0 + H - 1 of this unit
+// into buffers 0 .. H * BN/64 - 1, half by half.  A sub-tile wholly past N, or a half whose 64 rows
+// are all past M, is never stored, so its aux is not loaded; a plain arrival completes the barrier's
+// phase instead, which keeps every barrier's phase equal to the warpgroup's unit count and the
+// consumers' wait unconditional.
+template <int BN, int H>
+__device__ __forceinline__ void issue_aux_loads(const CUtensorMap* tmAux, int M, int N, int m0, int n0, int h0,
                                                 uint32_t staging, uint32_t aux_bar) {
   tma_store_wait_read<0>();
 #pragma unroll
-  for (int c = 0; c < BN / 64; ++c) {
-    const uint32_t bar = aux_bar + 8u * c;
-    if (n0 + 64 * c < N && m0 + cw * 64 < M) {
-      mbar_expect_tx(bar, SUB_BYTES);        // the full box, zero fill included
-      tma_load_2d(staging + c * SUB_BYTES, tmAux, bar, n0 + 64 * c, m0 + cw * 64);
-    } else {
-      mbar_arrive(bar);
+  for (int h = 0; h < H; ++h) {
+    const int r0 = m0 + 64 * (h0 + h);
+#pragma unroll
+    for (int c = 0; c < BN / 64; ++c) {
+      const int b = h * (BN / 64) + c;
+      const uint32_t bar = aux_bar + 8u * b;
+      if (n0 + 64 * c < N && r0 < M) {
+        mbar_expect_tx(bar, SUB_BYTES);        // the full box, zero fill included
+        tma_load_2d(staging + b * SUB_BYTES, tmAux, bar, n0 + 64 * c, r0);
+      } else {
+        mbar_arrive(bar);
+      }
     }
   }
 }
@@ -398,10 +439,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (C::AUX_TMA) tma_prefetch_desc(&tmAux);
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 2);     // one arrival per consumer warpgroup
+      mbar_init(empty_bar(s), C::PINGPONG ? 1 : 2);     // one arrival per warpgroup that reads the stage
     }
     if (C::AUX_TMA) {
       for (int b = 0; b < 2 * C::BUFS; ++b) mbar_init(bar_base + 8u * (C::AUX_BAR + b), 1);
+    }
+    if (C::PINGPONG) {
+      for (int b = 0; b < 2; ++b) mbar_init(bar_base + 8u * (C::ISSUED_BAR + b), 1);
     }
     fence_barrier_init();
   }
@@ -442,36 +486,60 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
   // ========================= consumers: warpgroups 1, 2 =========================
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-  const int cw = wg - 1;                        // which 64-row half of the tile
+  const int cw = wg - 1;
+  constexpr int H = C::HALVES;
+  const int h0 = C::PINGPONG ? 0 : cw;          // the warpgroup's first 64-row half of a tile
   const uint32_t staging = base + C::STAGING_OFFSET + cw * C::BUFS * C::BUF_BYTES;
   const uint32_t aux_bar = bar_base + 8u * (C::AUX_BAR + cw * C::BUFS);
   const bool leader = (threadIdx.x & 127) == 0;
-  uint32_t nstore = 0, nunit = 0;
+  uint32_t nstore = 0;
   PipeState ps;
+  ConsumerWalk walk(blockIdx.x, gridDim.x, C::PINGPONG ? cw : -1);
+  WorkUnit w;
   constexpr int S = C::STAGES, SB = C::STAGE_BYTES;
-  for (int u = blockIdx.x; u < units; u += gridDim.x, ++nunit) {
-    const WorkUnit w = gemm_work_unit(p.s, u, BM, BN);
+  for (int j = 0; walk.next(p.s, BM, BN, S, ps, w); ++j) {
+    // Ping-pong: this warpgroup's ring position skipped the other warpgroup's previous unit without
+    // waiting, and a parity wait on a full barrier is only sound once that barrier's previous phase has
+    // completed.  So wait until every k block of that unit has landed (the other warpgroup's
+    // (j + cw - 1)-th unit; warpgroup 0's first unit has none).  This also orders the two main loops.
+    if constexpr (C::PINGPONG) {
+      const int prev = j + cw - 1;
+      if (prev >= 0) mbar_wait(bar_base + 8u * (C::ISSUED_BAR + 1 - cw), prev & 1);
+    }
     // the leader's wait for the previous unit's stores overlaps the first k block's MMAs
     auto after_first = [&]() {
       if constexpr (C::AUX_TMA) {
-        if (leader) issue_aux_loads<BN>(&tmAux, p.M, p.N, w.m0, w.n0, cw, staging, aux_bar);
+        if (leader) issue_aux_loads<BN, H>(&tmAux, p.M, p.N, w.m0, w.n0, h0, staging, aux_bar);
       }
     };
-    float acc[BN / 2];
+    auto after_last = [&]() {
+      if constexpr (C::PINGPONG) {
+        if (leader) mbar_arrive(bar_base + 8u * (C::ISSUED_BAR + cw));
+      }
+    };
+    float acc[H][BN / 2];
     if (p.a_mn) {
-      if (p.b_mn) mainloop<BN, S, SB, 1, 1>(acc, base, bar_base, cw, ps, w.kb0, w.kb1, after_first);
-      else mainloop<BN, S, SB, 1, 0>(acc, base, bar_base, cw, ps, w.kb0, w.kb1, after_first);
+      if (p.b_mn) mainloop<BN, H, S, SB, 1, 1>(acc, base, bar_base, h0, ps, w.kb0, w.kb1, after_first, after_last);
+      else mainloop<BN, H, S, SB, 1, 0>(acc, base, bar_base, h0, ps, w.kb0, w.kb1, after_first, after_last);
     } else {
-      if (p.b_mn) mainloop<BN, S, SB, 0, 1>(acc, base, bar_base, cw, ps, w.kb0, w.kb1, after_first);
-      else mainloop<BN, S, SB, 0, 0>(acc, base, bar_base, cw, ps, w.kb0, w.kb1, after_first);
+      if (p.b_mn) mainloop<BN, H, S, SB, 0, 1>(acc, base, bar_base, h0, ps, w.kb0, w.kb1, after_first, after_last);
+      else mainloop<BN, H, S, SB, 0, 0>(acc, base, bar_base, h0, ps, w.kb0, w.kb1, after_first, after_last);
     }
 
-    if constexpr (OM == OM_BF16_TMA)
-      epilogue_tma<BN, EF, C::BUF_BYTES>(p, &tmD, &tmD2, acc, w.m0, w.n0, cw, staging, nstore, aux_bar, nunit & 1u);
-    else epilogue_regs<BN, OM == OM_F32, EF>(p, acc, w.m0, w.n0, cw, w.kb0);
+#pragma unroll
+    for (int h = 0; h < H; ++h) {
+      const int r0 = w.m0 + 64 * (h0 + h);
+      if constexpr (OM == OM_BF16_TMA) {
+        const int b = C::AUX_TMA ? h * (BN / 64) : 0;
+        epilogue_tma<BN, EF, C::BUF_BYTES>(p, &tmD, &tmD2, acc[h], r0, w.n0, cw, staging + b * C::BUF_BYTES, nstore,
+                                           aux_bar + 8u * b, j & 1);
+      } else {
+        epilogue_regs<BN, OM == OM_F32, EF>(p, acc[h], r0, w.n0, w.kb0);
+      }
+    }
   }
   // the staging buffers must outlive every bulk store that reads them
-  if (OM == OM_BF16_TMA && (threadIdx.x & 127) == 0) tma_store_wait<0>();
+  if (OM == OM_BF16_TMA && leader) tma_store_wait<0>();
 }
 
 template <int BN, int OM, int EF>
@@ -546,7 +614,8 @@ int launch_cfg(const bv_gemm_args& g, cudaStream_t stream) {
 
 // Plain bf16 outputs leave by TMA store; fp32 outputs and bf16 reduce-add outputs keep the register
 // epilogue.  bf16 reduce-adds (gradient accumulation into bf16, not on the training step's path) run
-// at BN = 128: at 256 their atomics make ptxas spill the accumulators inside the persistent loop.
+// the ping-pong kernel (BN = 128) whatever BN is asked for: cooperative at 256, their atomics make
+// ptxas spill the accumulators inside the persistent loop.
 template <int BN>
 int dispatch_epi(const bv_gemm_args& g, cudaStream_t s) {
   const bool f32 = (g.out_dtype == DT_F32), add = !f32 && g.reduce_out;
@@ -619,8 +688,13 @@ int bv_gemm(const bv_gemm_args* args, void* stream) {
   if (g.colsum != nullptr && (g.out_dtype != DT_BF16 || g.reduce_out)) {
     set_error("bv_gemm: colsum needs a plain bf16 output"); return BV_ERR_INVALID;
   }
+  // The tile width picks the kernel's structure (Cfg): 128 ping-pongs, 256 is cooperative.  Ping-pong
+  // hides each tile's epilogue under the other warpgroup's MMAs, but its 128 x 128 tiles bring a third
+  // more operand bytes from L2 per FLOP than 128 x 256.  The fp32 outputs (split-K weight gradients,
+  // K ~ 10^5 with a light register epilogue) lose more by that than they gain, so they run cooperative
+  // at 256 (DESIGN §5); every bf16 output ping-pongs.  N <= 128 is one 128-wide tile.
   int bn = g.block_n;
-  if (bn == 0) bn = (g.N > 128) ? 256 : 128;
+  if (bn == 0) bn = (g.N > 128 && g.out_dtype == DT_F32) ? 256 : 128;
   if (bn == 256) return dispatch_epi<256>(g, s);
   if (bn == 128) return dispatch_epi<128>(g, s);
   set_error("bv_gemm: block_n must be 0, 128 or 256");

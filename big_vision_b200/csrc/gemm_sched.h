@@ -1,10 +1,12 @@
 // Work decomposition of the persistent GEMM (csrc/gemm.cu), shared by the host launcher, the
-// kernel's producer and consumers, and the CPU test that checks it (tests/test_gemm_sched.py).
+// kernel's producer and consumers, and the CPU tests that check it (tests/test_gemm_sched.py,
+// tests/test_gemm_pingpong_sched.py).
 //
 // A work unit is one 128 x BN output tile times one K split.  Units are numbered n-tile fastest,
 // then m-tile, then split (so the CTAs that run at the same time share the A row-panel in L2), and
-// CTA b of a grid of G runs units b, b + G, b + 2G, ...  The producer and the consumers walk the same
-// units and keep one running k-block counter across them; its (stage, phase) is a PipeState.
+// CTA b of a grid of G runs units b, b + G, b + 2G, ...  The producer loads every unit of its CTA and
+// keeps one running k-block counter across them; its (stage, phase) is a PipeState.  The consumer
+// warpgroups walk the same units (ConsumerWalk) and keep the same counter.
 #pragma once
 
 #ifdef __CUDACC__
@@ -80,6 +82,30 @@ struct PipeState {
   unsigned phase = 0;
   BV_HD void advance(int stages) {
     if (++stage == stages) { stage = 0; phase ^= 1u; }
+  }
+  // n k blocks at once
+  BV_HD void advance(int stages, int n) {
+    const int t = stage + n;
+    phase ^= static_cast<unsigned>(t / stages) & 1u;
+    stage = t % stages;
+  }
+};
+
+// The units of CTA `cta` (of `grid`) that one consumer warpgroup runs.  Ping-pong (`cw` = 0 or 1): the
+// CTA's i-th unit is warpgroup i % 2's, so the two warpgroups alternate.  Cooperative (`cw` < 0): the
+// warpgroup runs every unit.  next() returns the warpgroup's next unit in `w` (its index in `unit`) and
+// moves `ps` past the k blocks of the other warpgroup's units on the way, without waiting on them, so
+// that at every k block the warpgroup runs, its (stage, phase) is the producer's.
+struct ConsumerWalk {
+  int unit, i, grid, cw;
+  BV_HD ConsumerWalk(int cta, int grid_, int cw_) : unit(cta - grid_), i(-1), grid(grid_), cw(cw_) {}
+  BV_HD bool next(const GemmSched& s, int bm, int bn, int stages, PipeState& ps, WorkUnit& w) {
+    for (unit += grid, ++i; unit < s.units; unit += grid, ++i) {
+      w = gemm_work_unit(s, unit, bm, bn);
+      if (cw < 0 || (i & 1) == cw) return true;
+      ps.advance(stages, w.kb1 - w.kb0);
+    }
+    return false;
   }
 };
 

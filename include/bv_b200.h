@@ -71,7 +71,10 @@ int bv_device_supported(void);
  *                is rounded to the output dtype and added into D on its own, in no fixed order;
  *                bias and the BIAS_RESID aux are added once (by the first split), DGELU's
  *                gelu'(aux) scales every partial.
- *   block_n    : 0 = auto, else 128 or 256
+ *   block_n    : output tile width, 0 = auto, else 128 or 256.  128 runs the two consumer
+ *                warpgroups ping-pong on alternate tiles, 256 runs them together on each tile;
+ *                the output bits are the same.  Auto: 256 for fp32 outputs with N > 128, else
+ *                128.  bf16 reduce-adds (reduce_out with a bf16 output) are fixed at 128.
  *   bias (fp32 [N]) and aux (bf16) must be readable up to round_up(N, 8) columns.
  * --------------------------------------------------------------------------------- */
 typedef struct bv_gemm_args {
