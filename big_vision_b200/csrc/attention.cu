@@ -23,6 +23,14 @@
 // the backward), wherever it sits in its 64-key block.  A query whose keys are all masked gets O = 0,
 // lse = 0 and zero gradients.
 //
+// Attention-probability dropout (key-masked dh = 64 only; head_dim | BV_ATTN_KEY_MASK | BV_ATTN_DROPOUT,
+// include/bv_dropout.h): template flag DROP.  The mask is regenerated in each of the forward, dQ and dK / dV
+// kernels from the Philox stream of the header, never stored.  A warp's 64 x 64 tile needs 64 Philox blocks
+// (one per row and 16-key group); each lane draws two and turns them into 16-bit keep masks, and the lanes
+// exchange those by shuffle (keep_rows, keep_cols).  The forward keeps l and lse of the undropped softmax,
+// multiplies V by P o Z and divides O by l (1 - rate); the backward applies Z / (1 - rate) to dP (dQ, dK) and
+// to P (dV).  Without DROP the kernels are unchanged.
+//
 // Every kernel runs one warpgroup per CTA on 64-row tiles and streams the other operand in 64-row
 // blocks through a two-slot TMA ring, so any sequence length works with the same code:
 //   forward   (b, h, 64 queries):  S = Q K^T (smem x smem), online softmax in registers,
@@ -36,6 +44,10 @@
 //             dV += P^T dO, dK += dS^T Q (register A operands).
 //   S and dP are computed twice, once per kernel: 7 instead of 5 64 x 64 x DH products per tile
 //   pair, which is cheaper than the HBM traffic of summing per-key-block dQ partials across CTAs.
+#include "../../include/bv_dropout.h"
+
+#include <math.h>
+
 #include "common.cuh"
 #include "host_utils.h"
 
@@ -160,6 +172,67 @@ __device__ __forceinline__ uint64_t attended_keys(const uint8_t* mask_row, int k
   return ((static_cast<uint64_t>(hi) << 32) | lo) >> (2 * (lane & 3));
 }
 
+// the attention dropout of a DROP kernel (include/bv_dropout.h)
+struct DropDev {
+  uint64_t seed, step, site;
+  long long row0;                          // global row of (b, h, q) = (0, 0, 0)
+  uint32_t thresh;                         // a probability is dropped when its 16-bit lane < thresh
+  float keep, rkeep;                       // 1 - rate and 1 / (1 - rate), fp32
+};
+
+// keep bits of the 16 keys 16 kblk .. 16 kblk + 15 of global row `row`: bit t = key 16 kblk + t is kept
+__device__ __forceinline__ uint32_t keep16(const DropDev& d, long long row, int kblk) {
+  uint64_t w[4] = {static_cast<uint64_t>(kblk) + 1, d.step, d.site, static_cast<uint64_t>(row) + 1};
+  philox4x64_10(w, d.seed, 0);
+  uint32_t bits = 0;
+#pragma unroll
+  for (int t = 0; t < 16; ++t)
+    bits |= static_cast<uint32_t>(((w[t >> 2] >> (16 * (t & 3))) & 0xffffu) >= d.thresh) << t;
+  return bits;
+}
+
+// keep bits of this thread's 32 elements of a 64 x 64 tile whose rows are queries (S in the forward and the
+// dQ kernel): bit i is element i, row `row` + 8 ((i >> 1) & 1), key 64 kb + 8 (i >> 2) + 2 (lane % 4) + (i & 1).
+// Lane g of a quad draws key group g (16 keys) for the quad's two rows, and the quad shares them by shuffle.
+__device__ __forceinline__ uint32_t keep_rows(const DropDev& d, long long row, int kb, int lane) {
+  const int g = lane & 3;
+  const uint32_t mine = keep16(d, row, 4 * kb + g) | (keep16(d, row + 8, 4 * kb + g) << 16);
+  uint32_t keep = 0;
+#pragma unroll
+  for (int gg = 0; gg < 4; ++gg) {
+    // bit 16 r + 8 h + e: key 16 gg + 8 h + 2 (lane % 4) + e of row r, i.e. element 8 gg + 4 h + 2 r + e
+    const uint32_t m = __shfl_sync(0xffffffffu, mine, (lane & ~3) | gg) >> (2 * g);
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int r = 0; r < 2; ++r)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) keep |= ((m >> (16 * r + 8 * h + e)) & 1u) << (8 * gg + 4 * h + 2 * r + e);
+  }
+  return keep;
+}
+
+// keep bits of this thread's 32 elements of a 64 x 64 tile whose rows are keys (S^T in the dK / dV kernel;
+// the warp's 16 keys are the key group kblk): bit e is element e, key 16 kblk + lane / 4 + 8 ((e >> 1) & 1),
+// query row0q + 8 (e >> 2) + 2 (lane % 4) + (e & 1).  Lane l draws queries l and l + 32, and each thread gathers
+// its bits from the 8 lanes that drew its queries.
+__device__ __forceinline__ uint32_t keep_cols(const DropDev& d, long long row0q, int kblk, int lane) {
+  const uint32_t mine = keep16(d, row0q + lane, kblk) | (keep16(d, row0q + lane + 32, kblk) << 16);
+  uint32_t keep = 0;
+#pragma unroll
+  for (int c = 0; c < 4; ++c)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      // bit 16 hi + 8 r: key lane / 4 + 8 r of query 8 (c + 4 hi) + 2 (lane % 4) + e
+      const uint32_t m = __shfl_sync(0xffffffffu, mine, 8 * c + 2 * (lane & 3) + e) >> (lane >> 2);
+#pragma unroll
+      for (int hi = 0; hi < 2; ++hi)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) keep |= ((m >> (16 * hi + 8 * r)) & 1u) << (4 * (c + 4 * hi) + 2 * r + e);
+    }
+  return keep;
+}
+
 // ============================================================================
 // forward
 // ============================================================================
@@ -171,9 +244,10 @@ struct FwdDev {
   long long ldo, bso;
   const uint8_t* mask;                     // key mask [B, Nk] (MASK kernels only)
   long long bsmask;
+  DropDev drop;                            // DROP kernels only
 };
 
-template <int DH, bool MASK>
+template <int DH, bool MASK, bool DROP>
 __global__ void __launch_bounds__(THREADS)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FwdDev p) {
@@ -210,6 +284,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   float o[G::R], s[32];
   zero(o);
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  // DROP: the global dropout row of this thread's first query
+  const long long drow = DROP ? p.drop.row0 + static_cast<long long>(bh) * p.Nq + qt * T + 16 * warp + (lane >> 2) : 0;
   mbar_wait(q_bar, 0);
   for (int j = 0; j < p.NB; ++j) {
     const int slot = j & 1;
@@ -217,6 +293,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     wgmma_fence();
     mma_tile_kk<DH>(s, q_s, k_s + slot * TILE_BYTES);
     wgmma_commit();
+    uint32_t keep = 0;                   // drawn while the MMAs run
+    if constexpr (DROP) keep = keep_rows(p.drop, drow, j, lane);
     wgmma_wait<0>();
     wgmma_fence_regs(s);
     // online softmax in base 2 over this key block; keys past Nk (and masked keys) get probability 0
@@ -254,6 +332,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     }
 #pragma unroll
     for (int i = 32; i < G::R; ++i) o[i] *= corr[(i >> 1) & 1];
+    if constexpr (DROP) {                // l stays the undropped sum; P V takes P o Z
+#pragma unroll
+      for (int i = 0; i < 32; ++i) s[i] = (keep >> i) & 1u ? s[i] : 0.f;
+    }
     uint32_t pf[4][4];
     to_frags(s, pf);
     wgmma_fence_regs(o);
@@ -272,6 +354,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
   }
   float inv[2] = {1.f / l[0], 1.f / l[1]};
+  if constexpr (DROP) {                  // O = (P o Z) V / (l (1 - rate))
+    inv[0] = 1.f / (l[0] * p.drop.keep);
+    inv[1] = 1.f / (l[1] * p.drop.keep);
+  }
   if constexpr (MASK) {                  // l = 0: no attended key, O = 0 and lse = 0
     inv[0] = l[0] > 0.f ? inv[0] : 0.f;
     inv[1] = l[1] > 0.f ? inv[1] : 0.f;
@@ -302,6 +388,7 @@ struct BwdDev {
   float* dq_colsum; float* dk_colsum; float* dv_colsum;
   const uint8_t* mask;                     // key mask [B, Nk] (MASK kernels only)
   long long bsmask;
+  DropDev drop;                            // DROP kernels only
 };
 
 // column sums of a [64 x DH] accumulator tile's stored (bf16-rounded) rows < nvalid: the eight lanes
@@ -333,7 +420,7 @@ __device__ __forceinline__ void tile_colsum(const float (&d)[R], float mul, int 
 
 // dQ of one (b, h, 64-query) block: the key blocks stream through the K / V ring and their dS K
 // products accumulate in order in one register tile
-template <int DH, bool MASK>
+template <int DH, bool MASK, bool DROP>
 __global__ void __launch_bounds__(THREADS)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const BwdDev p) {
@@ -382,6 +469,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     lse2[r] = q < p.Nq ? p.lse[bhq + q] * LOG2E : INFINITY;
     dl[r] = q < p.Nq ? p.delta[bhq + q] : 0.f;
   }
+  const long long drow = DROP ? p.drop.row0 + bhq + q0 : 0;   // DROP: global dropout row of query q0
   mbar_wait(q_bar, 0);
   for (int j = 0; j < p.KT; ++j) {
     const int slot = j & 1;
@@ -392,6 +480,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     mma_tile_kk<DH>(s, q_s, kj);          // S  = Q K^T
     mma_tile_kk<DH>(dp, do_s, vj);        // dP = dO V^T
     wgmma_commit();
+    uint32_t keep = 0;                    // drawn while the MMAs run
+    if constexpr (DROP) keep = keep_rows(p.drop, drow, j, lane);
     wgmma_wait<0>();
     wgmma_fence_regs(s);
     wgmma_fence_regs(dp);
@@ -408,6 +498,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       if constexpr (MASK) in = (live >> (8 * (i >> 2) + (i & 1))) & 1;
       else in = key < p.Nk;
       const float pr = in ? ex2(s[i] * p.scale_log2 - lse2[r]) : 0.f;
+      if constexpr (DROP) dp[i] = (keep >> i) & 1u ? dp[i] * p.drop.rkeep : 0.f;   // Z o dP / (1 - rate)
       dp[i] = pr * (dp[i] - dl[r]);
     }
     uint32_t sf[4][4];
@@ -435,7 +526,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 }
 
 // dK, dV of one (b, h, 64-key) block: the query blocks stream through the Q / dO ring
-template <int DH, bool MASK>
+template <int DH, bool MASK, bool DROP>
 __global__ void __launch_bounds__(THREADS)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const BwdDev p) {
@@ -503,6 +594,8 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       lse2[c] = q < p.Nq ? p.lse[bhq + q] * LOG2E : INFINITY;   // +inf -> P = 0 for queries past Nq
       dl[c] = q < p.Nq ? p.delta[bhq + q] : 0.f;
     }
+    uint32_t keep = 0;
+    if constexpr (DROP) keep = keep_cols(p.drop, p.drop.row0 + bhq + i * T, 4 * kt + warp, lane);
     wgmma_wait<0>();
     wgmma_fence_regs(st);
     wgmma_fence_regs(dpt);
@@ -513,7 +606,13 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       const int c = 2 * (e >> 2) + (e & 1);
       st[e] = ex2(st[e] * p.scale_log2 - lse2[c]);
       if constexpr (MASK) st[e] = live[(e >> 1) & 1] ? st[e] : 0.f;
-      dpt[e] = st[e] * (dpt[e] - dl[c]);
+      if constexpr (DROP) {              // dS^T from Z o dP^T / (1 - rate); dV from Z o P^T / (1 - rate)
+        const bool kept = (keep >> e) & 1u;
+        dpt[e] = st[e] * ((kept ? dpt[e] * p.drop.rkeep : 0.f) - dl[c]);
+        st[e] = kept ? st[e] * p.drop.rkeep : 0.f;
+      } else {
+        dpt[e] = st[e] * (dpt[e] - dl[c]);
+      }
     }
     uint32_t pf[4][4], sf[4][4];
     to_frags(st, pf);
@@ -584,6 +683,47 @@ struct KeyMask {
   int64_t bs = 0;
 };
 
+// the attention dropout of a call: head_dim | BV_ATTN_DROPOUT means the masked arguments are followed by a
+// bv_dropout_key
+struct AttnDrop {
+  bool on = false;
+  DropDev dev{};
+};
+
+// the dropout flag is accepted with the key mask at head dim 64 only, with a key that bv_dropout would accept
+int check_drop(bool dropped, bool masked, int head_dim, const bv_dropout_key& k, AttnDrop* d, const char* who) {
+  if (!dropped) return BV_OK;
+  if (!masked) {
+    set_error("%s: BV_ATTN_DROPOUT needs BV_ATTN_KEY_MASK", who);
+    return BV_ERR_INVALID;
+  }
+  if (head_dim != 64) {
+    set_error("%s: BV_ATTN_DROPOUT is supported at head_dim 64 only (got %d)", who, head_dim);
+    return BV_ERR_INVALID;
+  }
+  if (!(k.rate >= 0.f && k.rate < 1.f)) {
+    set_error("%s: dropout rate %g outside [0, 1)", who, static_cast<double>(k.rate));
+    return BV_ERR_INVALID;
+  }
+  if (k.site == 0) {
+    set_error("%s: dropout site 0 is Jet's noise stream; dropout sites start at 1", who);
+    return BV_ERR_INVALID;
+  }
+  if (k.row0 < 0) {
+    set_error("%s: dropout row0 must be >= 0 (got %lld)", who, static_cast<long long>(k.row0));
+    return BV_ERR_INVALID;
+  }
+  d->on = true;
+  d->dev.seed = k.seed;
+  d->dev.step = k.step;
+  d->dev.site = k.site;
+  d->dev.row0 = k.row0;
+  d->dev.thresh = static_cast<uint32_t>(nearbyint(static_cast<double>(k.rate) * 65536.0));
+  d->dev.keep = 1.f - k.rate;
+  d->dev.rkeep = 1.f / d->dev.keep;
+  return BV_OK;
+}
+
 // head dims with kernels; every other one is refused before any CUDA call.  The key mask is built at
 // head dim 64 only (BERT-Base and BERT-Large)
 int check_head_dim(int head_dim, bool masked, const KeyMask& m, const char* who) {
@@ -621,7 +761,7 @@ int check_attn(const bv_attn_args& a, const char* who) {
 }
 
 template <int DH>
-int attention_fwd(const bv_attn_args& a, const KeyMask& km, cudaStream_t s) {
+int attention_fwd(const bv_attn_args& a, const KeyMask& km, const AttnDrop& dr, cudaStream_t s) {
   using G = Geo<DH>;
   int rc = check_attn(a, "bv_attention_fwd_hd");
   if (rc) return rc;
@@ -634,14 +774,15 @@ int attention_fwd(const bv_attn_args& a, const KeyMask& km, cudaStream_t s) {
   p.o = static_cast<bf16*>(a.o);
   p.ldo = a.ldo; p.bso = a.bso;
   p.mask = km.mask; p.bsmask = km.bs;
+  p.drop = dr.dev;
   CUtensorMap tmQ, tmK, tmV;
   if ((rc = make_tmap_bnd(&tmQ, a.q, DH, a.H, a.Nq, a.B, a.ldq, a.bsq))) return rc;
   if ((rc = make_tmap_bnd(&tmK, a.k, DH, a.H, a.Nk, a.B, a.ldk, a.bsk))) return rc;
   if ((rc = make_tmap_bnd(&tmV, a.v, DH, a.H, a.Nk, a.B, a.ldv, a.bsv))) return rc;
   const long long grid = a.B * a.H * p.QT;
-  auto kernel = attn_fwd_kernel<DH, false>;
+  auto kernel = attn_fwd_kernel<DH, false, false>;
   if constexpr (DH == 64) {
-    if (km.mask != nullptr) kernel = attn_fwd_kernel<DH, true>;
+    if (km.mask != nullptr) kernel = dr.on ? attn_fwd_kernel<DH, true, true> : attn_fwd_kernel<DH, true, false>;
   }
   rc = check_cuda(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, G::FWD_SMEM),
                   "cudaFuncSetAttribute(attn_fwd)");
@@ -651,7 +792,7 @@ int attention_fwd(const bv_attn_args& a, const KeyMask& km, cudaStream_t s) {
 }
 
 template <int DH>
-int attention_bwd(const bv_attn_bwd_args& g, const KeyMask& km, cudaStream_t s) {
+int attention_bwd(const bv_attn_bwd_args& g, const KeyMask& km, const AttnDrop& dr, cudaStream_t s) {
   using G = Geo<DH>;
   const bv_attn_args& a = g.fwd;
   int rc = check_attn(a, "bv_attention_bwd_hd");
@@ -698,6 +839,7 @@ int attention_bwd(const bv_attn_bwd_args& g, const KeyMask& km, cudaStream_t s) 
   p.lddq = g.lddq; p.bsdq = g.bsdq; p.lddk = g.lddk; p.bsdk = g.bsdk; p.lddv = g.lddv; p.bsdv = g.bsdv;
   p.dq_colsum = g.dq_colsum; p.dk_colsum = g.dk_colsum; p.dv_colsum = g.dv_colsum;
   p.mask = km.mask; p.bsmask = km.bs;
+  p.drop = dr.dev;
   CUtensorMap tmQ, tmK, tmV, tmdO;
   if ((rc = make_tmap_bnd(&tmQ, a.q, DH, a.H, a.Nq, a.B, a.ldq, a.bsq))) return rc;
   if ((rc = make_tmap_bnd(&tmK, a.k, DH, a.H, a.Nk, a.B, a.ldk, a.bsk))) return rc;
@@ -705,12 +847,15 @@ int attention_bwd(const bv_attn_bwd_args& g, const KeyMask& km, cudaStream_t s) 
   if ((rc = make_tmap_bnd(&tmdO, g.d_o, DH, a.H, a.Nq, a.B, g.lddo, g.bsdo))) return rc;
   // query blocks of one (b, h) are adjacent in the dQ grid (and key blocks in the dK / dV grid), so the
   // streamed K / V (Q / dO) tiles they share are served from L2
-  auto dq_kernel = attn_bwd_dq_kernel<DH, false>;
-  auto dkdv_kernel = attn_bwd_dkdv_kernel<DH, false>;
+  auto dq_kernel = attn_bwd_dq_kernel<DH, false, false>;
+  auto dkdv_kernel = attn_bwd_dkdv_kernel<DH, false, false>;
   if constexpr (DH == 64) {
-    if (km.mask != nullptr) {
-      dq_kernel = attn_bwd_dq_kernel<DH, true>;
-      dkdv_kernel = attn_bwd_dkdv_kernel<DH, true>;
+    if (km.mask != nullptr && dr.on) {
+      dq_kernel = attn_bwd_dq_kernel<DH, true, true>;
+      dkdv_kernel = attn_bwd_dkdv_kernel<DH, true, true>;
+    } else if (km.mask != nullptr) {
+      dq_kernel = attn_bwd_dq_kernel<DH, true, false>;
+      dkdv_kernel = attn_bwd_dkdv_kernel<DH, true, false>;
     }
   }
   rc = check_cuda(cudaFuncSetAttribute(dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, G::BWD_SMEM),
@@ -735,23 +880,28 @@ int bv_attention_fwd_hd(const bv_attn_args* args, int32_t head_dim, void* stream
   using namespace bv;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (!args) { set_error("bv_attention_fwd_hd: null args"); return BV_ERR_INVALID; }
-  const bool masked = (head_dim & BV_ATTN_KEY_MASK) != 0;
-  head_dim &= ~BV_ATTN_KEY_MASK;
+  const bool masked = (head_dim & BV_ATTN_KEY_MASK) != 0, dropped = (head_dim & BV_ATTN_DROPOUT) != 0;
+  head_dim &= ~(BV_ATTN_KEY_MASK | BV_ATTN_DROPOUT);
   KeyMask km;
   if (masked) {     // args is the first member of a bv_attn_masked_args
     const bv_attn_masked_args* m = reinterpret_cast<const bv_attn_masked_args*>(args);
     km.mask = m->key_mask;
     km.bs = m->bsmask;
   }
-  int rc = check_head_dim(head_dim, masked, km, "bv_attention_fwd_hd");
+  AttnDrop dr;      // with the dropout flag, that is the first member of a bv_attn_dropout_args
+  int rc = check_drop(dropped, masked, head_dim,
+                      dropped ? reinterpret_cast<const bv_attn_dropout_args*>(args)->drop : bv_dropout_key{}, &dr,
+                      "bv_attention_fwd_hd");
+  if (rc) return rc;
+  rc = check_head_dim(head_dim, masked, km, "bv_attention_fwd_hd");
   if (rc) return rc;
   const bv_attn_args& a = *args;
   switch (head_dim) {
-    case 72: return attention_fwd<72>(a, km, s);
-    case 80: return attention_fwd<80>(a, km, s);
-    case 96: return attention_fwd<96>(a, km, s);
-    case 104: return attention_fwd<104>(a, km, s);
-    default: return attention_fwd<64>(a, km, s);
+    case 72: return attention_fwd<72>(a, km, dr, s);
+    case 80: return attention_fwd<80>(a, km, dr, s);
+    case 96: return attention_fwd<96>(a, km, dr, s);
+    case 104: return attention_fwd<104>(a, km, dr, s);
+    default: return attention_fwd<64>(a, km, dr, s);
   }
 }
 
@@ -759,23 +909,28 @@ int bv_attention_bwd_hd(const bv_attn_bwd_args* args, int32_t head_dim, void* st
   using namespace bv;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (!args) { set_error("bv_attention_bwd_hd: null args"); return BV_ERR_INVALID; }
-  const bool masked = (head_dim & BV_ATTN_KEY_MASK) != 0;
-  head_dim &= ~BV_ATTN_KEY_MASK;
+  const bool masked = (head_dim & BV_ATTN_KEY_MASK) != 0, dropped = (head_dim & BV_ATTN_DROPOUT) != 0;
+  head_dim &= ~(BV_ATTN_KEY_MASK | BV_ATTN_DROPOUT);
   KeyMask km;
   if (masked) {     // args is the first member of a bv_attn_masked_bwd_args
     const bv_attn_masked_bwd_args* m = reinterpret_cast<const bv_attn_masked_bwd_args*>(args);
     km.mask = m->key_mask;
     km.bs = m->bsmask;
   }
-  int rc = check_head_dim(head_dim, masked, km, "bv_attention_bwd_hd");
+  AttnDrop dr;      // with the dropout flag, that is the first member of a bv_attn_dropout_bwd_args
+  int rc = check_drop(dropped, masked, head_dim,
+                      dropped ? reinterpret_cast<const bv_attn_dropout_bwd_args*>(args)->drop : bv_dropout_key{}, &dr,
+                      "bv_attention_bwd_hd");
+  if (rc) return rc;
+  rc = check_head_dim(head_dim, masked, km, "bv_attention_bwd_hd");
   if (rc) return rc;
   const bv_attn_bwd_args& g = *args;
   switch (head_dim) {
-    case 72: return attention_bwd<72>(g, km, s);
-    case 80: return attention_bwd<80>(g, km, s);
-    case 96: return attention_bwd<96>(g, km, s);
-    case 104: return attention_bwd<104>(g, km, s);
-    default: return attention_bwd<64>(g, km, s);
+    case 72: return attention_bwd<72>(g, km, dr, s);
+    case 80: return attention_bwd<80>(g, km, dr, s);
+    case 96: return attention_bwd<96>(g, km, dr, s);
+    case 104: return attention_bwd<104>(g, km, dr, s);
+    default: return attention_bwd<64>(g, km, dr, s);
   }
 }
 

@@ -228,6 +228,15 @@ class Dropout(NamedTuple):
     return L.DropoutKey(seed=k.seed, step=k.step, site=dropout_site(k.tower, layer, kind), row0=k.sample0 * self.N,
                         rate=self.rate)
 
+  def probs(self, layer, heads):
+    """-> lib.DropoutKey of the attention probabilities of `layer` (BERT): the site (layer, DROP_ATTN), whose
+    attention stream never meets the attention output's (include/bv_dropout.h), and this rank's first
+    (sample, head, query) row."""
+    from big_vision_b200 import lib as L
+    k = self.key
+    return L.DropoutKey(seed=k.seed, step=k.step, site=dropout_site(k.tower, layer, DROP_ATTN),
+                        row0=k.sample0 * heads * self.N, rate=self.rate)
+
 
 def check_dropout_rate(rate):
   if not 0.0 <= rate < 1.0:
@@ -243,13 +252,14 @@ def dropout(rate, key, N):
 class Geom(NamedTuple):
   """What every stage of one forward sees besides its input: n samples of N tokens each, the
   MLP-Mixer's stochastic-depth masks of that forward (None: no residual branch is dropped), BERT's
-  key-padding mask [n, N] (None: every key is attended) and the ViT / text encoders' Dropout (None: no
-  dropout)."""
+  key-padding mask [n, N] (None: every key is attended), the ViT / text / BERT encoders' Dropout (None: no
+  dropout) and BERT's attention-probability Dropout (None: none)."""
   n: int
   N: int
   masks: Optional[torch.Tensor] = None
   key_mask: Optional[torch.Tensor] = None
   dropout: Optional[Dropout] = None
+  attn_dropout: Optional[Dropout] = None
 
 
 class Stage:

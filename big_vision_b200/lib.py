@@ -20,6 +20,7 @@ SAM_WS_FLOATS = 2048       # BV_SAM_WS_FLOATS
 # BV_DIST_*: the kinds of dist(); BV_DISTILL_*: the outputs of bv_distill_loss, in order
 DIST_KINDS = {"euclidean": 0, "l2": 1, "hard": 2, "kl": 3, "logsoftmax_euclidean": 4, "agree": 5}
 ATTN_KEY_MASK = 65536      # BV_ATTN_KEY_MASK: head_dim flag of a key-masked attention call
+ATTN_DROPOUT = 131072      # BV_ATTN_DROPOUT (include/bv_dropout.h): head_dim flag of attention-probability dropout
 DISTILL_OUTPUTS = ("distance", "entropy_student", "entropy_teacher", "task_loss_student", "task_loss_teacher")
 
 
@@ -61,6 +62,15 @@ class AttnMaskedBwdArgs(ctypes.Structure):
 class DropoutKey(ctypes.Structure):
   _fields_ = [("seed", ctypes.c_uint64), ("step", ctypes.c_uint64), ("site", ctypes.c_uint64), ("row0", c_i64),
               ("rate", c_f32)]
+
+
+# head_dim | ATTN_KEY_MASK | ATTN_DROPOUT: the masked arguments are the first member of one of these
+class AttnDropoutArgs(ctypes.Structure):
+  _fields_ = [("masked", AttnMaskedArgs), ("drop", DropoutKey)]
+
+
+class AttnDropoutBwdArgs(ctypes.Structure):
+  _fields_ = [("masked", AttnMaskedBwdArgs), ("drop", DropoutKey)]
 
 
 class AdamArgs(ctypes.Structure):

@@ -65,9 +65,8 @@ class Model:
     so no two sites share a stream."""
     saved = {}
     ztxt = zimg = None
-    # only a tower with dropout takes a key (the BERT tower has no dropout)
-    kw = lambda m, tower: ({"dropout": dropout._replace(tower=tower)}
-                           if dropout is not None and getattr(m, "dropout", 0.0) else {})
+    # only a tower with dropout takes a key
+    kw = lambda m, tower: {"dropout": dropout._replace(tower=tower)} if dropout is not None and _drops(m) else {}
     if text is not None:
       e, s = self.txt.fwd(P, text, frozen=frozen, **kw(self.txt, 1))
       ztxt, nrm = ops.l2norm_fwd(e, eps=1e-8)
@@ -95,7 +94,7 @@ class Model:
   def apply(self, variables, image, text=None, **kw):
     """(zimg, ztxt, out) like the flax apply (two_towers.py:39-90); forward-only (same bits as the
     training forward, nothing kept for a backward)."""
-    if kw.get("train") and (getattr(self.img, "dropout", 0.0) or getattr(self.txt, "dropout", 0.0)):
+    if kw.get("train") and (_drops(self.img) or _drops(self.txt)):
       raise ValueError("apply(train=True) with dropout > 0 has no dropout key; call fwd(..., dropout=key)")
     P = variables["params"]
     zimg, ztxt, _ = self.fwd(P, image, text, frozen=True)
@@ -103,6 +102,11 @@ class Model:
     if self.bias_init is not None:
       out["b"] = P.f("b")
     return zimg, ztxt, out
+
+
+def _drops(tower):
+  """Whether a tower trains with dropout: the ViT and text towers' `dropout`, BERT's two rates."""
+  return any(getattr(tower, k, 0.0) for k in ("dropout", "dropout_rate", "attention_dropout_rate"))
 
 
 # which entry of `init_files` feeds which part of the model: (part, accepted keys)

@@ -134,7 +134,8 @@ def mlp_fwd(S, y, resid, out_dtype=torch.bfloat16, save=True, drop=None):
   save=False (forward only): GELU's pre-activation is not written at all, saved is None.
   drop: None, or the lib.DropoutKeys (GELU output, MLP output) of the encoder block's dropouts
   (models/vit.py:76,109): the GELU output is dropped in place, so the saved activation is the dropped one,
-  and the residual add follows the dropped Dense_1 output."""
+  and the residual add follows the dropped Dense_1 output.  A GELU key of None leaves the GELU output as it
+  is (BERT drops the MLP output only)."""
   if save:
     act, pre = ops.gemm(y, S.h("Dense_0/kernel"), b_mn=True, bias=S.f("Dense_0/bias"),
                         epilogue=L.EPI_BIAS_GELU)
@@ -142,7 +143,8 @@ def mlp_fwd(S, y, resid, out_dtype=torch.bfloat16, save=True, drop=None):
     act = ops.gemm(y, S.h("Dense_0/kernel"), b_mn=True, bias=S.f("Dense_0/bias"),
                    epilogue=L.EPI_BIAS_GELU_ACT)
   if drop is not None:
-    ops.dropout(act, drop[0], out=act)
+    if drop[0] is not None:
+      ops.dropout(act, drop[0], out=act)
     out = ops.gemm(act, S.h("Dense_1/kernel"), b_mn=True, bias=S.f("Dense_1/bias"))
     out = ops.dropout_add(resid, out, drop[1], out=out)
   else:

@@ -132,17 +132,24 @@ def _attn_args(q, k, v, o, lse, heads, scale):
                     scale=scale)
 
 
-def _attn_call(name, args, masked_type, key_mask, B, Nk, dh):
+def _attn_call(name, args, masked_type, key_mask, B, Nk, dh, dropout=None, dropout_type=None):
   """Calls `name` on `args`; with a key mask, on a `masked_type` that appends it, and head_dim | ATTN_KEY_MASK
-  (the arguments are its first member, so the pointer is the same)."""
+  (the arguments are its first member, so the pointer is the same); with a dropout key too, on a
+  `dropout_type` that appends the key to that, and head_dim | ATTN_KEY_MASK | ATTN_DROPOUT."""
   if key_mask is None:
+    if dropout is not None:
+      raise L.BvError("attention: dropout is built for key-masked attention only; pass a key_mask")
     L.call(name, ctypes.byref(args), dh, _stream())
     return
   if key_mask.dtype not in (torch.uint8, torch.bool) or tuple(key_mask.shape) != (B, Nk) or key_mask.stride(1) != 1:
     raise L.BvError(f"attention: key_mask must be uint8 or bool [B, Nk] = [{B}, {Nk}] with unit key stride, got "
                     f"{key_mask.dtype} {tuple(key_mask.shape)}")
   m = masked_type(attn=args, key_mask=_p(key_mask), bsmask=key_mask.stride(0))
-  L.call(name, ctypes.byref(m.attn), dh | L.ATTN_KEY_MASK, _stream())
+  if dropout is None:
+    L.call(name, ctypes.byref(m.attn), dh | L.ATTN_KEY_MASK, _stream())
+    return
+  d = dropout_type(masked=m, drop=dropout)
+  L.call(name, ctypes.byref(d.masked.attn), dh | L.ATTN_KEY_MASK | L.ATTN_DROPOUT, _stream())
 
 
 # head dims the attention kernels are built for (bv_attention_fwd_hd / bv_attention_bwd_hd)
@@ -155,11 +162,13 @@ def _head_dim(cols, heads):
   return cols // heads
 
 
-def attention_fwd(q, k, v, heads, scale=None, key_mask=None):
+def attention_fwd(q, k, v, heads, scale=None, key_mask=None, dropout=None):
   """q:[B,Nq,H*dh] k,v:[B,Nk,H*dh] bf16 (strided views allowed) -> o [B,Nq,H*dh], lse [B,H,Nq].
 
   dh is one of ATTN_HEAD_DIMS; the library refuses any other.  key_mask: None, or uint8 / bool [B, Nk],
-  nonzero = attend (head dim 64 only); a query with every key masked gets o = 0 and lse = 0."""
+  nonzero = attend (head dim 64 only); a query with every key masked gets o = 0 and lse = 0.  dropout: None, or
+  the lib.DropoutKey of attention-probability dropout (with a key_mask only; row0 = the global index of sample 0
+  times H * Nq, include/bv_dropout.h); lse stays that of the undropped softmax."""
   B, Nq, cols = q.shape
   dh = _head_dim(cols, heads)
   if scale is None:
@@ -167,13 +176,13 @@ def attention_fwd(q, k, v, heads, scale=None, key_mask=None):
   o = torch.empty((B, Nq, cols), dtype=torch.bfloat16, device=q.device)
   lse = torch.empty((B, heads, Nq), dtype=torch.float32, device=q.device)
   args = _attn_args(q, k, v, o, lse, heads, scale)
-  _attn_call("bv_attention_fwd_hd", args, L.AttnMaskedArgs, key_mask, B, k.shape[1], dh)
+  _attn_call("bv_attention_fwd_hd", args, L.AttnMaskedArgs, key_mask, B, k.shape[1], dh, dropout, L.AttnDropoutArgs)
   return o, lse
 
 
 def attention_bwd(do, q, k, v, o, lse, heads, scale=None, dq=None, dk=None, dv=None,
-                  dq_colsum=None, dk_colsum=None, dv_colsum=None, key_mask=None):
-  """Gradients of attention_fwd (the same key_mask): -> dq, dk, dv; masked keys get dk = dv = 0."""
+                  dq_colsum=None, dk_colsum=None, dv_colsum=None, key_mask=None, dropout=None):
+  """Gradients of attention_fwd (the same key_mask and dropout key): -> dq, dk, dv; masked keys get dk = dv = 0."""
   dh = _head_dim(q.shape[2], heads)
   if scale is None:
     scale = 1.0 / math.sqrt(dh)
@@ -196,7 +205,8 @@ def attention_bwd(do, q, k, v, o, lse, heads, scale=None, dq=None, dk=None, dv=N
                        dk_colsum=dk_colsum.data_ptr() if dk_colsum is not None else None,
                        dv_colsum=dv_colsum.data_ptr() if dv_colsum is not None else None,
                        delta=delta.data_ptr())
-  _attn_call("bv_attention_bwd_hd", args, L.AttnMaskedBwdArgs, key_mask, B, k.shape[1], dh)
+  _attn_call("bv_attention_bwd_hd", args, L.AttnMaskedBwdArgs, key_mask, B, k.shape[1], dh, dropout,
+             L.AttnDropoutBwdArgs)
   return dq, dk, dv
 
 

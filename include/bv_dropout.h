@@ -1,5 +1,6 @@
 /* bv_dropout.h -- C ABI of the dropout kernels in libbv_b200.so (flax nn.Dropout in models/vit.py and
- * models/proj/image_text/text_transformer.py of the reference).
+ * models/proj/image_text/text_transformer.py of the reference), and the attention-probability dropout flag of
+ * the attention entry points of bv_b200.h (BERT, models/proj/flaxformer/bert.py).
  *
  * Exported from the same library as bv_b200.h and following its conventions:
  *  - every pointer is a DEVICE pointer; the caller owns all buffers;
@@ -57,6 +58,41 @@ int bv_dropout(const void* x, int64_t ldx, void* y, int64_t ldy, int64_t rows, i
 /* out = resid + dropout(y): the residual add after a dropped branch (models/vit.py:100,109). */
 int bv_dropout_add(const void* resid, int64_t ldr, const void* y, int64_t ldy, void* out, int64_t ldo,
                    int64_t rows, int64_t cols, const bv_dropout_key* key, void* stream);
+
+/* ---------------------------------------------------------------------------------
+ * Attention-probability dropout (BERT's attention_probs_dropout_prob; flaxformer's BertEncoder with
+ * enable_dropout, models/proj/flaxformer/bert.py:55): the key-masked attention of bv_b200.h drops each
+ * softmax probability P[b, h, q, k] with probability `rate` and scales the kept ones by 1 / (1 - rate).
+ * Built for key-masked attention at head dim 64 only: pass head_dim = 64 | BV_ATTN_KEY_MASK | BV_ATTN_DROPOUT to
+ * bv_attention_fwd_hd / bv_attention_bwd_hd, with args pointing to a bv_attn_dropout_args /
+ * bv_attn_dropout_bwd_args.  The backward must be given the forward's key.  The flag without
+ * BV_ATTN_KEY_MASK, at any other head dim, with a NULL args pointer, site 0, row0 < 0 or a rate outside [0, 1)
+ * is refused with BV_ERR_INVALID before any launch.
+ *
+ * The mask is never stored: the forward, dQ and dK/dV kernels each regenerate it.  Its stream is the
+ * generator of bv_dropout, Philox4x64-10 under key (seed, 0).  Probability (b, h, q, k) belongs to the global
+ * row r = row0 + (b * H + h) * Nq + q (a data-parallel rank whose batch starts at global sample sample0
+ * passes row0 = sample0 * H * Nq) and uses the 16-bit lane k % 16 of the block at counter
+ * (k / 16 + 1, step, site, r + 1), i.e. numpy's
+ * np.random.Philox(key=seed, counter=[0, step, site, r + 1]).random_raw(4 * ceil(Nk / 16)), lanes as above.  It
+ * is dropped when that lane is below T = round(rate * 65536), as in bv_dropout.  Counter word 3 is >= 1
+ * here and 0 in every bv_dropout counter, so the two streams never meet, even at the same site.
+ *
+ * Maths, with Z the keep mask and kappa = 1 - rate in fp32: lse and the row sums l are those of the
+ * undropped softmax, and O = ((P o Z) V) / (l * kappa).  The backward's delta = rowsum(dO o O) is unchanged;
+ * dS = P o (Z o dP / kappa - delta) with dP = dO V^T, and dV = (Z o P / kappa)^T dO.  Masked keys and keys
+ * past Nk keep P = 0 whatever their mask bits.  At rate 0 the results are the bits of the call without the
+ * flag.
+ * --------------------------------------------------------------------------------- */
+#define BV_ATTN_DROPOUT 131072   /* head_dim flag: args carries a dropout key (with BV_ATTN_KEY_MASK) */
+typedef struct bv_attn_dropout_args {
+  bv_attn_masked_args masked;
+  bv_dropout_key drop;
+} bv_attn_dropout_args;
+typedef struct bv_attn_dropout_bwd_args {
+  bv_attn_masked_bwd_args masked;   /* masked.attn.fwd and the mask: the forward call's */
+  bv_dropout_key drop;              /* the forward call's key */
+} bv_attn_dropout_bwd_args;
 
 #ifdef __cplusplus
 }
