@@ -15,7 +15,8 @@ CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libbv_b200.so")
 SOURCES = ["host_utils.cu", "gemm.cu", "attention.cu", "layernorm.cu", "elementwise.cu",
-           "loss.cu", "optim.cu", "eval.cu", "sam.cu", "distill.cu", "flexi.cu", "jet.cu", "dropout.cu"]
+           "loss.cu", "optim.cu", "eval.cu", "sam.cu", "distill.cu", "flexi.cu", "jet.cu", "dropout.cu",
+           "conv.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]

@@ -26,10 +26,12 @@
 // arrives by TMA into the same staging buffers during the main loop.  fp32 and bf16 reduce-add
 // outputs store from the registers.
 #include "common.cuh"
+#include "conv_gemm.h"
 #include "gemm_sched.h"
 #include "host_utils.h"
 
 #include <atomic>
+#include <type_traits>
 
 #include <stdlib.h>
 #include <string.h>
@@ -98,6 +100,32 @@ struct GemmDev {
   float* colsum;         // optional bias-gradient accumulator (bf16 outputs only)
   int aux_row_mod;
 };
+
+// What the producer loads per k block (template parameter).  PROD_GEMM: the 2-D tiles of A and B.  The
+// convolution modes (conv_gemm.h) read A from an NHWC activation by TMA in im2col mode, so no im2col matrix
+// is ever written: PROD_CONV is the forward / data gradient, whose k block (tap, 64-channel block) loads 128
+// output pixels x 64 channels of the tap-shifted input (A K-major) and the tap's rows of the kernel (B);
+// PROD_WGRAD is the kernel gradient, whose M rows are (tap, input channel) and whose k block is 64 output
+// pixels: A is two 64-pixel x 64-channel im2col boxes (MN-major), B the 64 pixels' rows of dy (MN-major).
+enum : int { PROD_GEMM = 0, PROD_CONV = 1, PROD_WGRAD = 2 };
+
+struct ConvDev {
+  int gh, gw;              // the output-pixel grid whose row-major order (img, y, x) the pixel index runs over
+  int lw, lh, es;          // input base position of grid point (x, y) = (lw + es * x, lh + es * y)
+  int cblocks, cin;        // 64-channel blocks per tap (PROD_CONV); channels per tap of M (PROD_WGRAD)
+  int ntaps;
+  uint16_t offw[kConvMaxTaps], offh[kConvMaxTaps];   // the tap's shift of the base position
+  int brow[kConvMaxTaps];  // PROD_CONV: first row of the tap's kernel slice in the 2-D map of B
+};
+
+// the input base position (w, h) and image of output pixel m
+__device__ __forceinline__ void conv_base(const ConvDev& cv, int m, int& img, int& bw, int& bh) {
+  const int t = m / cv.gw, x = m - t * cv.gw;
+  img = t / cv.gh;
+  const int y = t - img * cv.gh;
+  bw = cv.lw + cv.es * x;
+  bh = cv.lh + cv.es * y;
+}
 
 // The consumer warpgroup's main loop over one unit's k blocks, for the H 64-row halves h0 .. h0 + H - 1
 // of the tile; acc[h] holds half h0 + h.  `ps` is the running ring position, carried from unit to
@@ -417,11 +445,16 @@ __device__ __forceinline__ void issue_aux_loads(const CUtensorMap* tmAux, int M,
   }
 }
 
-template <int BN, int OM, int EF>
+// The convolution modes take a ConvDev; the plain GEMM an empty placeholder.
+struct NoConv {};
+template <int PROD>
+using ConvParam = std::conditional_t<PROD == PROD_GEMM, NoConv, ConvDev>;
+
+template <int BN, int OM, int EF, int PROD>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmD2,
-            const __grid_constant__ CUtensorMap tmAux, const GemmDev p) {
+            const __grid_constant__ CUtensorMap tmAux, const GemmDev p, const __grid_constant__ ConvParam<PROD> cv) {
   using C = Cfg<BN, OM, EF>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -458,26 +491,61 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       PipeState ps;
       for (int u = blockIdx.x; u < units; u += gridDim.x) {
         const WorkUnit w = gemm_work_unit(p.s, u, BM, BN);
-        for (int kb = w.kb0; kb < w.kb1; ++kb) {
-          mbar_wait(empty_bar(ps.stage), ps.phase ^ 1u);
-          const uint32_t a_s = base + ps.stage * C::STAGE_BYTES;
-          const uint32_t b_s = a_s + A_STAGE_BYTES;
-          const uint32_t fb = full_bar(ps.stage);
-          mbar_expect_tx(fb, C::STAGE_BYTES);
-          const int k0 = kb * BK;
-          if (p.a_mn) {
+        if constexpr (PROD == PROD_GEMM) {
+          for (int kb = w.kb0; kb < w.kb1; ++kb) {
+            mbar_wait(empty_bar(ps.stage), ps.phase ^ 1u);
+            const uint32_t a_s = base + ps.stage * C::STAGE_BYTES;
+            const uint32_t b_s = a_s + A_STAGE_BYTES;
+            const uint32_t fb = full_bar(ps.stage);
+            mbar_expect_tx(fb, C::STAGE_BYTES);
+            const int k0 = kb * BK;
+            if (p.a_mn) {
 #pragma unroll
-            for (int j = 0; j < BM / 64; ++j) tma_load_2d(a_s + j * 8192, &tmA, fb, w.m0 + 64 * j, k0);
-          } else {
-            tma_load_2d(a_s, &tmA, fb, k0, w.m0);
-          }
-          if (p.b_mn) {
+              for (int j = 0; j < BM / 64; ++j) tma_load_2d(a_s + j * 8192, &tmA, fb, w.m0 + 64 * j, k0);
+            } else {
+              tma_load_2d(a_s, &tmA, fb, k0, w.m0);
+            }
+            if (p.b_mn) {
 #pragma unroll
-            for (int j = 0; j < BN / 64; ++j) tma_load_2d(b_s + j * 8192, &tmB, fb, w.n0 + 64 * j, k0);
-          } else {
-            tma_load_2d(b_s, &tmB, fb, k0, w.n0);
+              for (int j = 0; j < BN / 64; ++j) tma_load_2d(b_s + j * 8192, &tmB, fb, w.n0 + 64 * j, k0);
+            } else {
+              tma_load_2d(b_s, &tmB, fb, k0, w.n0);
+            }
+            ps.advance(C::STAGES);
           }
-          ps.advance(C::STAGES);
+        } else {
+          int img = 0, bw = 0, bh = 0;
+          if constexpr (PROD == PROD_CONV) conv_base(cv, w.m0, img, bw, bh);
+          for (int kb = w.kb0; kb < w.kb1; ++kb) {
+            mbar_wait(empty_bar(ps.stage), ps.phase ^ 1u);
+            const uint32_t a_s = base + ps.stage * C::STAGE_BYTES;
+            const uint32_t b_s = a_s + A_STAGE_BYTES;
+            const uint32_t fb = full_bar(ps.stage);
+            mbar_expect_tx(fb, C::STAGE_BYTES);
+            const int k0 = kb * BK;
+            if constexpr (PROD == PROD_CONV) {
+              const int tap = kb / cv.cblocks, c0 = (kb - tap * cv.cblocks) * BK, brow = cv.brow[tap];
+              tma_load_im2col_4d(a_s, &tmA, fb, c0, bw, bh, img, cv.offw[tap], cv.offh[tap]);
+              if (p.b_mn) {
+#pragma unroll
+                for (int j = 0; j < BN / 64; ++j) tma_load_2d(b_s + j * 8192, &tmB, fb, w.n0 + 64 * j, brow + c0);
+              } else {
+                tma_load_2d(b_s, &tmB, fb, c0, brow + w.n0);
+              }
+            } else {
+              conv_base(cv, k0, img, bw, bh);
+#pragma unroll
+              for (int j = 0; j < BM / 64; ++j) {
+                // a box past the last tap (M = taps x cin is a multiple of 64) loads tap 0; its rows are not stored
+                const int m = w.m0 + 64 * j, t = m / cv.cin, tap = t < cv.ntaps ? t : 0;
+                tma_load_im2col_4d(a_s + j * 8192, &tmA, fb, m - t * cv.cin, bw, bh, img, cv.offw[tap],
+                                   cv.offh[tap]);
+              }
+#pragma unroll
+              for (int j = 0; j < BN / 64; ++j) tma_load_2d(b_s + j * 8192, &tmB, fb, w.n0 + 64 * j, k0);
+            }
+            ps.advance(C::STAGES);
+          }
         }
       }
     }
@@ -542,6 +610,25 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (OM == OM_BF16_TMA && leader) tma_store_wait<0>();
 }
 
+// The dynamic-shared-memory opt-in is a per-DEVICE attribute of the kernel: cache it per device and
+// instantiation (one process may drive several GPUs from several host threads; the flags are atomics and a
+// duplicate set by two racing threads is harmless).
+template <int BN, int OM, int EF, int PROD>
+int opt_in_smem() {
+  auto kern = gemm_kernel<BN, OM, EF, PROD>;
+  const int bytes = Cfg<BN, OM, EF>::SMEM_BYTES;
+  static std::atomic<bool> attr_set[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = -1;
+  if (dev < 0 || !attr_set[dev].load(std::memory_order_acquire)) {
+    const int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes),
+                              "cudaFuncSetAttribute(gemm)");
+    if (rc) return rc;
+    if (dev >= 0) attr_set[dev].store(true, std::memory_order_release);
+  }
+  return BV_OK;
+}
+
 template <int BN, int OM, int EF>
 int launch_cfg(const bv_gemm_args& g, cudaStream_t stream) {
   using C = Cfg<BN, OM, EF>;
@@ -594,21 +681,11 @@ int launch_cfg(const bv_gemm_args& g, cudaStream_t stream) {
     if (rc) return rc;
   }
 
-  auto kern = gemm_kernel<BN, OM, EF>;
-  // The dynamic-shared-memory opt-in is a per-DEVICE attribute of the kernel: cache it per device
-  // (one process may drive several GPUs from several host threads; the flags are atomics and a
-  // duplicate set by two racing threads is harmless).
-  static std::atomic<bool> attr_set[64];
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = -1;
-  if (dev < 0 || !attr_set[dev].load(std::memory_order_acquire)) {
-    rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES),
-                    "cudaFuncSetAttribute(gemm)");
-    if (rc) return rc;
-    if (dev >= 0) attr_set[dev].store(true, std::memory_order_release);
-  }
+  auto kern = gemm_kernel<BN, OM, EF, PROD_GEMM>;
+  rc = opt_in_smem<BN, OM, EF, PROD_GEMM>();
+  if (rc) return rc;
   const int grid = p.s.units < num_sms() ? p.s.units : num_sms();
-  kern<<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(tmA, tmB, tmD, tmD2, tmAux, p);
+  kern<<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(tmA, tmB, tmD, tmD2, tmAux, p, NoConv{});
   return check_cuda(cudaGetLastError(), "gemm_kernel launch");
 }
 
@@ -642,7 +719,81 @@ int dispatch_epi(const bv_gemm_args& g, cudaStream_t s) {
   return BV_ERR_INVALID;
 }
 
+template <int BN, int OM, int EF, int PROD>
+int launch_conv_cfg(const ConvGemm& g, cudaStream_t stream) {
+  using C = Cfg<BN, OM, EF>;
+  const bool wgrad = PROD == PROD_WGRAD;
+  const long long pixels = g.n * g.gh * g.gw;
+  const long long M = wgrad ? (long long)g.ntaps * g.c : pixels;
+  const long long K = wgrad ? pixels : (long long)g.ntaps * g.c;
+  const CUtensorMapDataType bf = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  CUtensorMap tmA, tmB, tmD, tmD2, tmAux;
+  memset(&tmD, 0, sizeof(tmD));
+  memset(&tmD2, 0, sizeof(tmD2));
+  memset(&tmAux, 0, sizeof(tmAux));
+  int rc = make_tmap_im2col_nhwc(&tmA, g.x, g.n, g.h, g.w, g.c, g.lw, g.lh, g.lw + g.stride * (g.gw - 1) - (g.w - 1),
+                                 g.lh + g.stride * (g.gh - 1) - (g.h - 1), g.stride, wgrad ? 64 : BM);
+  if (rc) return rc;
+  if (wgrad || g.b_mn) rc = make_tmap_2d(&tmB, bf, g.b, g.b_cols, g.b_rows, (uint64_t)g.b_cols * 2, 64, 64);
+  else rc = make_tmap_2d(&tmB, bf, g.b, g.b_cols, g.b_rows, (uint64_t)g.b_cols * 2, 64, BN);
+  if (rc) return rc;
+
+  GemmDev p;
+  if ((M + BM - 1) / BM * ((g.N + BN - 1) / BN) * ((K + BK - 1) / BK) > 0x7fffffffLL || M > 0x7fffffffLL) {
+    set_error("bv_conv: problem too large");
+    return BV_ERR_INVALID;
+  }
+  gemm_make_sched(M, g.N, K, BM, BN, BK, wgrad ? 0 : 1, wgrad, num_sms(), &p.s);
+  p.M = (int)M; p.N = g.N;
+  p.a_mn = wgrad ? 1 : 0;
+  p.b_mn = wgrad ? 1 : g.b_mn;
+  p.reduce_out = wgrad ? 1 : 0;
+  p.alpha = 1.f;
+  p.bias = nullptr;
+  p.colsum = nullptr;
+  p.aux = reinterpret_cast<const bf16*>(g.resid);
+  p.ldaux = g.N;
+  p.aux_row_mod = 0;
+  p.d = g.out; p.d2 = nullptr;
+  p.ldd = g.N; p.ldd2 = 0;
+  if (OM == OM_BF16_TMA) {
+    rc = make_tmap_2d(&tmD, bf, g.out, g.N, M, (uint64_t)g.N * 2, 64, 64);
+    if (rc) return rc;
+  }
+  if (C::AUX_TMA) {
+    rc = make_tmap_2d(&tmAux, bf, g.resid, g.N, M, (uint64_t)g.N * 2, 64, 64);
+    if (rc) return rc;
+  }
+  ConvDev cv;
+  memset(&cv, 0, sizeof(cv));
+  cv.gh = g.gh; cv.gw = g.gw; cv.lw = g.lw; cv.lh = g.lh; cv.es = g.stride;
+  cv.cblocks = g.c / BK; cv.cin = g.c; cv.ntaps = g.ntaps;
+  for (int t = 0; t < g.ntaps; ++t) {
+    cv.offw[t] = (uint16_t)g.taps[t].ow;
+    cv.offh[t] = (uint16_t)g.taps[t].oh;
+    cv.brow[t] = g.taps[t].brow;
+  }
+  auto kern = gemm_kernel<BN, OM, EF, PROD>;
+  rc = opt_in_smem<BN, OM, EF, PROD>();
+  if (rc) return rc;
+  const int grid = p.s.units < num_sms() ? p.s.units : num_sms();
+  kern<<<grid, NUM_THREADS, C::SMEM_BYTES, stream>>>(tmA, tmB, tmD, tmD2, tmAux, p, cv);
+  return check_cuda(cudaGetLastError(), "gemm_kernel (convolution) launch");
+}
+
 }  // namespace
+
+// Forward and data gradient: bf16 outputs on the ping-pong kernel, with the residual epilogue when resid is
+// given.  Kernel gradient: fp32 reduce-add, cooperative at BN = 256 when N > 128, as bv_gemm's fp32 outputs.
+int conv_gemm(const ConvGemm& g, cudaStream_t s) {
+  if (g.wgrad) {
+    return g.N > 128 ? launch_conv_cfg<256, OM_F32, EF_BIAS, PROD_WGRAD>(g, s)
+                     : launch_conv_cfg<128, OM_F32, EF_BIAS, PROD_WGRAD>(g, s);
+  }
+  return g.resid ? launch_conv_cfg<128, OM_BF16_TMA, EF_RESID, PROD_CONV>(g, s)
+                 : launch_conv_cfg<128, OM_BF16_TMA, EF_BIAS, PROD_CONV>(g, s);
+}
+
 }  // namespace bv
 
 extern "C" {

@@ -132,6 +132,43 @@ int make_tmap(CUtensorMap* out, CUtensorMapDataType dt, int rank, const void* pt
   return BV_OK;
 }
 
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                   const cuuint64_t*, const int*, const int*, cuuint32_t, cuuint32_t,
+                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+int make_tmap_im2col_nhwc(CUtensorMap* out, const void* ptr, int64_t n, int h, int w, int c, int lower_w,
+                          int lower_h, int upper_w, int upper_h, int stride, int pixels) {
+  static EncodeIm2colFn enc = nullptr;
+  if (!enc) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &p, cudaEnableDefault, &qres);
+    if (e != cudaSuccess || qres != cudaDriverEntryPointSuccess || p == nullptr) {
+      set_error("cuTensorMapEncodeIm2col entry point unavailable (no CUDA driver?)");
+      return BV_ERR_CUDA;
+    }
+    enc = reinterpret_cast<EncodeIm2colFn>(p);
+  }
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0) {
+    set_error("TMA base pointer %p not 16-byte aligned", ptr);
+    return BV_ERR_INVALID;
+  }
+  const cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
+  const cuuint64_t strides[3] = {(cuuint64_t)c * 2, (cuuint64_t)w * c * 2, (cuuint64_t)h * w * c * 2};
+  const int lower[2] = {lower_w, lower_h}, upper[2] = {upper_w, upper_h};
+  const cuuint32_t es[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, lower, upper, 64,
+                   (cuuint32_t)pixels, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeIm2col failed (CUresult %d; n %lld h %d w %d c %d corners %d,%d / %d,%d stride %d)",
+              (int)r, (long long)n, h, w, c, lower_w, lower_h, upper_w, upper_h, stride);
+    return BV_ERR_CUDA;
+  }
+  return BV_OK;
+}
+
 }  // namespace bv
 
 extern "C" {

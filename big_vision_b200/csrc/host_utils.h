@@ -37,6 +37,12 @@ int make_tmap(CUtensorMap* out, CUtensorMapDataType dt, int rank, const void* pt
               const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box,
               bool swizzle128);
 
+// Encode an im2col-mode map of a bf16 NHWC tensor [n, h, w, c] with 128-byte swizzle: a load yields
+// `pixels` rows of 64 channels (128 B).  The base positions a load may start from span
+// [lower, dim - 1 + upper] in w and h, stepped by `stride`.
+int make_tmap_im2col_nhwc(CUtensorMap* out, const void* ptr, int64_t n, int h, int w, int c, int lower_w,
+                          int lower_h, int upper_w, int upper_h, int stride, int pixels);
+
 inline int make_tmap_2d(CUtensorMap* out, CUtensorMapDataType dt, const void* ptr, uint64_t inner,
                         uint64_t outer, uint64_t row_stride_bytes, uint32_t box_inner,
                         uint32_t box_outer) {

@@ -1,4 +1,5 @@
-"""ctypes binding of libbv_b200.so (C ABI declared in include/bv_b200*.h and include/bv_dropout.h).
+"""ctypes binding of libbv_b200.so (C ABI declared in include/bv_b200*.h, include/bv_dropout.h and
+include/bv_conv.h).
 
 The product path has no fallback: if the library is missing, or a call is made
 without a compute-capability-9.x device, this module raises.
@@ -71,6 +72,17 @@ class AttnDropoutArgs(ctypes.Structure):
 
 class AttnDropoutBwdArgs(ctypes.Structure):
   _fields_ = [("masked", AttnMaskedBwdArgs), ("drop", DropoutKey)]
+
+
+# include/bv_conv.h
+STEM_K, STEM_K_PAD = 147, 152   # BV_STEM_K, BV_STEM_K_PAD
+
+
+class ConvArgs(ctypes.Structure):
+  _fields_ = [("x", c_vp), ("kernel", c_vp), ("dy", c_vp), ("y", c_vp), ("dx", c_vp), ("dkernel", c_vp),
+              ("resid", c_vp), ("workspace", c_vp), ("n", c_i64),
+              ("h", c_i32), ("w", c_i32), ("cin", c_i32), ("cout", c_i32), ("k", c_i32), ("stride", c_i32),
+              ("accumulate", c_i32)]
 
 
 class AdamArgs(ctypes.Structure):
@@ -166,6 +178,21 @@ DROPOUT_SIGNATURES = {
     "bv_dropout_add": [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i64, c_i64, ctypes.POINTER(DropoutKey), c_vp],
 }
 
+# include/bv_conv.h (BiT ResNet-v2), also outside the bv_b200*.h set; checked by tests/test_conv.py.
+CONV_SIGNATURES = {
+    "bv_conv_fwd": [ctypes.POINTER(ConvArgs), c_vp],
+    "bv_conv_dgrad": [ctypes.POINTER(ConvArgs), c_vp],
+    "bv_conv_wgrad": [ctypes.POINTER(ConvArgs), c_vp],
+    "bv_weight_std_fwd": [c_vp, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp],
+    "bv_weight_std_bwd": [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp],
+    "bv_groupnorm_fwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i32, c_i32, c_vp],
+    "bv_groupnorm_bwd": [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_i64, c_i32, c_i32,
+                         c_vp],
+    "bv_maxpool_fwd": [c_vp, c_vp, c_i64, c_i32, c_i32, c_i32, c_vp],
+    "bv_maxpool_bwd": [c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_i32, c_vp],
+    "bv_stem_im2col": [c_vp, c_vp, c_i64, c_i32, c_i32, c_vp],
+}
+
 _lib = None
 
 
@@ -183,7 +210,7 @@ def load():
         f"{LIB_PATH} not found: build it with `python -m big_vision_b200.build` "
         "(there is no CPU or eager fallback for the kernels).")
   lib = ctypes.CDLL(LIB_PATH)
-  for name, argtypes in {**SIGNATURES, **DROPOUT_SIGNATURES}.items():
+  for name, argtypes in {**SIGNATURES, **DROPOUT_SIGNATURES, **CONV_SIGNATURES}.items():
     fn = getattr(lib, name)   # raises AttributeError if the symbol is missing
     fn.argtypes = argtypes
     fn.restype = ctypes.c_int

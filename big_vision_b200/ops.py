@@ -724,3 +724,169 @@ def retrieval_ranks(dist, corr, t2i=True, i2t=True):
   r_i2t = torch.empty(NI, dtype=torch.int32, device=dist.device) if i2t else None
   L.call("bv_retrieval_ranks", _p(dist), NI, NT, ld, _p(corr), _p(r_t2i), _p(r_i2t), _stream())
   return r_t2i, r_i2t
+
+
+# ---------------------------------------------------------------------------------------------------------
+# BiT ResNet-v2 (include/bv_conv.h): NHWC bf16 activations, HWIO kernels.
+
+def conv_out_size(h, k, stride):
+  """Output size of the reference's k x k convolution with symmetric padding k // 2."""
+  return (h + 2 * (k // 2) - k) // stride + 1
+
+
+def _contig(*ts):
+  for t in ts:
+    if t is not None:
+      assert t.is_contiguous(), "convolution operands must be contiguous"
+
+
+def _conv_args(n, h, w, cin, cout, k, stride, **ptrs):
+  a = L.ConvArgs(n=n, h=h, w=w, cin=cin, cout=cout, k=k, stride=stride)
+  for name, t in ptrs.items():
+    setattr(a, name, _p(t))
+  return a
+
+
+def conv_fwd(x, kernel, stride=1, resid=None):
+  """y = conv(x, kernel) (+ resid): x bf16 [n, h, w, cin], kernel bf16 [k, k, cin, cout] (the standardised
+  kernel).  Returns bf16 [n, ho, wo, cout].  A 1 x 1 stride-1 convolution is bv_gemm on [n h w, cin]; every
+  other one is bv_conv_fwd."""
+  n, h, w, cin = x.shape
+  k, _, _, cout = kernel.shape
+  _contig(x, kernel, resid)
+  if k == 1 and stride == 1:     # a plain GEMM on [n h w, cin]
+    aux = None if resid is None else resid.view(-1, cout)
+    y = gemm(x.view(-1, cin), kernel.view(cin, cout), b_mn=True, aux=aux,
+             epilogue=L.EPI_NONE if resid is None else L.EPI_BIAS_RESID)
+    return y.view(n, h, w, cout)
+  y = torch.empty((n, conv_out_size(h, k, stride), conv_out_size(w, k, stride), cout), dtype=torch.bfloat16,
+                  device=x.device)
+  a = _conv_args(n, h, w, cin, cout, k, stride, x=x, kernel=kernel, y=y, resid=resid)
+  L.call("bv_conv_fwd", ctypes.byref(a), _stream())
+  return y
+
+
+def conv_dgrad(dy, kernel, h, w, stride=1, resid=None):
+  """The input gradient [n, h, w, cin] (bf16) of conv_fwd for output gradient dy (+ resid)."""
+  n, _, _, cout = dy.shape
+  k, _, cin, _ = kernel.shape
+  _contig(dy, kernel, resid)
+  if k == 1 and stride == 1:
+    aux = None if resid is None else resid.view(-1, cin)
+    dx = gemm(dy.view(-1, cout), kernel.view(cin, cout), aux=aux,
+              epilogue=L.EPI_NONE if resid is None else L.EPI_BIAS_RESID)
+    return dx.view(n, h, w, cin)
+  dx = torch.empty((n, h, w, cin), dtype=torch.bfloat16, device=dy.device)
+  ws = torch.empty_like(dx) if stride == 2 else None
+  a = _conv_args(n, h, w, cin, cout, k, stride, dy=dy, kernel=kernel, dx=dx, resid=resid, workspace=ws)
+  L.call("bv_conv_dgrad", ctypes.byref(a), _stream())
+  return dx
+
+
+def conv_wgrad(x, dy, k, stride=1, out=None):
+  """The kernel gradient fp32 [k, k, cin, cout] of conv_fwd; added into `out` when given."""
+  n, h, w, cin = x.shape
+  cout = dy.shape[-1]
+  _contig(x, dy, out)
+  acc = out is not None
+  if k == 1 and stride == 1:
+    dk = gemm(x.view(-1, cin), dy.view(-1, cout), a_mn=True, b_mn=True, out_dtype=torch.float32, reduce_out=True,
+              out=None if out is None else out.view(cin, cout))
+    return dk.view(1, 1, cin, cout)
+  out = torch.empty((k, k, cin, cout), dtype=torch.float32, device=x.device) if out is None else out
+  a = _conv_args(n, h, w, cin, cout, k, stride, x=x, dy=dy, dkernel=out)
+  a.accumulate = int(acc)
+  L.call("bv_conv_wgrad", ctypes.byref(a), _stream())
+  return out
+
+
+def weight_std_fwd(kernel):
+  """bit_paper.standardize of an fp32 HWIO kernel: (bf16 standardised kernel, mean [cout], rstd [cout])."""
+  _contig(kernel)
+  cout = kernel.shape[-1]
+  rows = kernel.numel() // cout
+  ws = torch.empty(kernel.shape, dtype=torch.bfloat16, device=kernel.device)
+  mean = torch.empty(cout, dtype=torch.float32, device=kernel.device)
+  rstd = torch.empty_like(mean)
+  L.call("bv_weight_std_fwd", _p(kernel), rows, cout, _p(ws), _p(mean), _p(rstd), _stream())
+  return ws, mean, rstd
+
+
+def weight_std_bwd(kernel, mean, rstd, g):
+  """fp32 gradient of the kernel from g, the fp32 gradient of its standardised copy."""
+  _contig(kernel, g)
+  cout = kernel.shape[-1]
+  dw = torch.empty_like(kernel)
+  L.call("bv_weight_std_bwd", _p(kernel), _p(mean), _p(rstd), _p(g), kernel.numel() // cout, cout, _p(dw),
+         _stream())
+  return dw
+
+
+def groupnorm_fwd(x, scale, bias, relu=True):
+  """bit_paper.GroupNorm (32 groups) and an optional ReLU on bf16 NHWC x; returns (y, mean, rstd), the
+  statistics fp32 [n, 32]."""
+  _contig(x)
+  n, c = x.shape[0], x.shape[-1]
+  y = torch.empty_like(x)
+  mean = torch.empty((n, 32), dtype=torch.float32, device=x.device)
+  rstd = torch.empty_like(mean)
+  L.call("bv_groupnorm_fwd", _p(x), _p(scale), _p(bias), _p(y), _p(mean), _p(rstd), n, x.numel() // (n * c), c,
+         int(relu), _stream())
+  return y, mean, rstd
+
+
+def groupnorm_bwd(dy, x, scale, bias, mean, rstd, dscale, dbias, relu=True, dx_add=None):
+  """dx (bf16, + dx_add when given) of groupnorm_fwd; dscale and dbias (fp32 [c]) are added into."""
+  _contig(dy, x, dx_add)
+  n, c = x.shape[0], x.shape[-1]
+  dx = torch.empty_like(x)
+  L.call("bv_groupnorm_bwd", _p(x), _p(dy), _p(scale), _p(bias), _p(mean), _p(rstd), _p(dx_add), _p(dx),
+         _p(dscale), _p(dbias), n, x.numel() // (n * c), c, int(relu), _stream())
+  return dx
+
+
+def maxpool_fwd(x):
+  """3 x 3 / 2 max pool with -inf padding (1, 1) of bf16 NHWC x."""
+  _contig(x)
+  n, h, w, c = x.shape
+  y = torch.empty((n, (h - 1) // 2 + 1, (w - 1) // 2 + 1, c), dtype=torch.bfloat16, device=x.device)
+  L.call("bv_maxpool_fwd", _p(x), _p(y), n, h, w, c, _stream())
+  return y
+
+
+def maxpool_bwd(dy, x):
+  _contig(dy, x)
+  n, h, w, c = x.shape
+  dx = torch.empty_like(x)
+  L.call("bv_maxpool_bwd", _p(x), _p(dy), _p(dx), n, h, w, c, _stream())
+  return dx
+
+
+def stem_im2col(image):
+  """The root convolution's 7 x 7 / 2 patches of an fp32 NHWC image [n, h, w, 3]: bf16
+  [n * ho * wo, STEM_K_PAD] (columns past STEM_K are zero)."""
+  _contig(image)
+  n, h, w, _ = image.shape
+  ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+  cols = torch.empty((n * ho * wo, L.STEM_K_PAD), dtype=torch.bfloat16, device=image.device)
+  L.call("bv_stem_im2col", _p(image), _p(cols), n, h, w, _stream())
+  return cols
+
+
+def stem_conv_fwd(image, kernel):
+  """The root block's 7 x 7 / 2 convolution (padding 3) of an fp32 image with the bf16 standardised kernel
+  [7, 7, 3, cout]: bv_stem_im2col, then one GEMM with K = 147.  Returns bf16 [n, ho, wo, cout]."""
+  n, h, w, _ = image.shape
+  cout = kernel.shape[-1]
+  cols = stem_im2col(image)
+  y = gemm(cols[:, :L.STEM_K], kernel.reshape(L.STEM_K, cout), b_mn=True)
+  return y.view(n, (h - 1) // 2 + 1, (w - 1) // 2 + 1, cout)
+
+
+def stem_conv_wgrad(image, dy):
+  """fp32 [7, 7, 3, cout] kernel gradient of stem_conv_fwd (the patches are extracted again)."""
+  cout = dy.shape[-1]
+  cols = stem_im2col(image)
+  dk = gemm(cols[:, :L.STEM_K], dy.reshape(-1, cout), a_mn=True, b_mn=True, out_dtype=torch.float32,
+            reduce_out=True)
+  return dk.view(7, 7, 3, cout)

@@ -13,9 +13,7 @@ trained):
 P, ...}; only the student is trained.
 """
 import functools
-import importlib
 
-from big_vision_b200 import utils
 from big_vision_b200.trainers.proj.distill import distill
 from big_vision_b200.trainers.proj.flexi import common as flexi
 from big_vision_b200.trainers.proj.flexi.train import demand_flexi_args, flexi_args  # pylint: disable=unused-import
@@ -43,37 +41,6 @@ def make_predict_fns(models, config):
   return {**student_fns, **teacher_fns, **pairs}
 
 
-def _model_module(config, name):
-  return importlib.import_module(f"big_vision_b200.models.{config[f'{name}_name']}")
-
-
-def init_params(params, config):
-  """Initialises params {name: FlatParams} in place after model.init, as flexi/distill.py:273-314 does:
-    - `init_head_bias` first fills every model's head bias, as the distillation trainer's init does
-      (distill/distill.py:186-189): the i21k config's -10, so the loss starts small.  A loaded head
-      replaces it;
-    - each teacher loads `<name>_init` through its model module's `load` (config["<name>_name"]), with
-      config[name] as the model config and config["<name>_load"] as keyword arguments.  Teachers are
-      never checkpointed, so each must have one;
-    - then the student loads `student_init` the same way, if the config has one.  For a FlexiViT student
-      that is models/proj/flexi/vit.py:load, which takes a plain ViT checkpoint of any grid and patch
-      size: it resizes the position embedding and resamples the patch-embedding kernel."""
-  if "init_head_bias" in config:
-    for P in params.values():
-      views = P.tree("f")
-      if "head/bias" in views:
-        views["head/bias"].fill_(config["init_head_bias"])
-        P.sync_half()
-  teachers = tuple(config["teachers"])
-  for name in teachers + ("student",):
-    init = config.get(f"{name}_init")
-    if not init:
-      if name != "student":
-        raise ValueError(f"teacher '{name}' has no {name}_init: teachers are never trained or checkpointed")
-      continue
-    P = params[name]
-    tree = utils.recover_tree(*zip(*P.numpy_tree("f").items()))
-    tree = _model_module(config, name).load(tree, init, dict(config.get(name) or {}),
-                                            **config.get(f"{name}_load", {}))
-    P.load_tree(dict(utils.tree_flatten_with_names(tree)[0]))
-  return params
+# the config-driven initialisation is the plain distillation trainer's (trainers/proj/distill)
+_model_module = distill._model_module
+init_params = distill.init_params
