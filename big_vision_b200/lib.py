@@ -1,5 +1,4 @@
-"""ctypes binding of libbv_b200.so (C ABI declared in include/bv_b200*.h, include/bv_dropout.h and
-include/bv_conv.h).
+"""ctypes binding of libbv_b200.so (C ABI declared in include/bv_*.h).
 
 The product path has no fallback: if the library is missing, or a call is made
 without a compute-capability-9.x device, this module raises.
@@ -13,7 +12,7 @@ LIB_PATH = os.environ.get("BV_LIB_PATH") or os.path.join(_HERE, "libbv_b200.so")
 
 c_i32, c_i64, c_f32, c_vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_void_p
 
-# the #defines of include/bv_b200*.h that Python needs
+# the #defines of include/bv_*.h that Python needs
 F32, BF16 = 0, 1
 EPI_NONE, EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_RESID, EPI_DGELU, EPI_BIAS_GELU_ACT = 0, 1, 2, 3, 4, 5
 LOSS_WS_FLOATS = 8192      # BV_LOSS_WS_FLOATS
@@ -103,8 +102,8 @@ class AdafactorArgs(ctypes.Structure):
               ("gnorm_sq", c_vp), ("upd_sq", c_vp), ("param_sq", c_vp)]
 
 
-# name -> argtypes (restype is int).  Mirrors the functions of include/bv_b200*.h one to one, all exported
-# from the same library.
+# name -> argtypes (restype is int).  Mirrors the functions of include/bv_*.h one to one, all exported from the
+# same library.
 SIGNATURES = {
     # include/bv_b200.h
     "bv_gemm": [ctypes.POINTER(GemmArgs), c_vp],
@@ -169,17 +168,10 @@ SIGNATURES = {
     "bv_jet_coupling_bwd": [c_vp, c_vp, c_vp, c_vp, c_f32, c_vp, c_vp, c_i64, c_i32, c_i32, c_f32, c_vp],
     "bv_jet_merge_grad": [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_vp],
     "bv_jet_bits": [c_vp, c_vp, c_vp, c_vp, c_vp, c_f32, c_i64, c_i64, c_vp],
-}
-
-# The same for include/bv_dropout.h, the one header outside the bv_b200*.h set: its functions, binding and C
-# link test are checked by tests/test_dropout.py rather than by the tests of the bv_b200*.h headers.
-DROPOUT_SIGNATURES = {
+    # include/bv_dropout.h (dropout)
     "bv_dropout": [c_vp, c_i64, c_vp, c_i64, c_i64, c_i64, ctypes.POINTER(DropoutKey), c_vp],
     "bv_dropout_add": [c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i64, c_i64, ctypes.POINTER(DropoutKey), c_vp],
-}
-
-# include/bv_conv.h (BiT ResNet-v2), also outside the bv_b200*.h set; checked by tests/test_conv.py.
-CONV_SIGNATURES = {
+    # include/bv_conv.h (BiT ResNet-v2)
     "bv_conv_fwd": [ctypes.POINTER(ConvArgs), c_vp],
     "bv_conv_dgrad": [ctypes.POINTER(ConvArgs), c_vp],
     "bv_conv_wgrad": [ctypes.POINTER(ConvArgs), c_vp],
@@ -210,7 +202,7 @@ def load():
         f"{LIB_PATH} not found: build it with `python -m big_vision_b200.build` "
         "(there is no CPU or eager fallback for the kernels).")
   lib = ctypes.CDLL(LIB_PATH)
-  for name, argtypes in {**SIGNATURES, **DROPOUT_SIGNATURES, **CONV_SIGNATURES}.items():
+  for name, argtypes in SIGNATURES.items():
     fn = getattr(lib, name)   # raises AttributeError if the symbol is missing
     fn.argtypes = argtypes
     fn.restype = ctypes.c_int

@@ -1,14 +1,16 @@
-"""Shared tiny configurations for the tests (kept small so the CPU oracle runs in seconds), and the parse of
-the C ABI headers."""
+"""Shared tiny configurations for the tests (kept small so the CPU oracle runs in seconds), the parse of
+the C ABI headers, and C programs built against them."""
 import glob
 import os
 import re
+import shutil
+import subprocess
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-# every header of the C ABI of libbv_b200.so
-HEADERS = sorted(glob.glob(os.path.join(ROOT, "include", "bv_b200*.h")))
+# every header of the C ABI of libbv_b200.so (the headers big_vision_b200.build hashes)
+HEADERS = sorted(glob.glob(os.path.join(ROOT, "include", "bv_*.h")))
 
 TINY = dict(
     image=dict(width=64, depth=2, mlp_dim=128, num_heads=1, patch_size=(16, 16), pool_type="map"),
@@ -49,3 +51,23 @@ def header_functions(path):
   """Every `bv_name(` of a C header outside its comments: the functions it declares."""
   src = re.sub(r"/\*.*?\*/", "", open(path).read(), flags=re.S)
   return set(re.findall(r"\b(bv_[a-z0-9_]+)\s*\(", src))
+
+
+def run_c(tmp_path, source, cxx=False, link=False):
+  """Writes `source` as a C99 (or, with cxx, C++17) program, compiles it with -Wall -Werror against include/
+  (and, with link, libbv_b200.so), runs it and returns its stdout.  Skips the test without the compiler."""
+  import pytest   # smoke() imports this module and must not need pytest
+  cc = "g++" if cxx else "gcc"
+  if shutil.which(cc) is None:
+    pytest.skip(f"no {cc}")
+  src, exe = tmp_path / ("main.cc" if cxx else "main.c"), tmp_path / "main"
+  src.write_text(source)
+  cmd = [cc, "-std=c++17" if cxx else "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"),
+         str(src), "-o", str(exe)]
+  if link:
+    from big_vision_b200 import lib
+    lib.load()
+    libdir = os.path.dirname(os.path.abspath(lib.LIB_PATH))
+    cmd += ["-L", libdir, "-lbv_b200", f"-Wl,-rpath,{libdir}"]
+  subprocess.run(cmd, check=True)
+  return subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout

@@ -1,16 +1,14 @@
-"""CPU: BERT dropout.  The attention-dropout arguments of include/bv_dropout.h (their layout against a C program,
-the BV_ATTN_DROPOUT flag mirrored, every refusal before any launch), the numpy restatement of the
-attention mask stream (numpy's Philox in 16-bit lanes, its realized rate, and its separation from every
-bv_dropout counter and from Jet's), the float64 BERT oracle with given masks pinned against
-`transformers.BertModel` in train mode with the same masks, and what the BERT tower launches and keeps with
-dropout, recorded by tests/golden/make_model_traces.py's recorder."""
+"""CPU: BERT dropout.  The attention-dropout arguments of include/bv_dropout.h (every refusal before any
+launch; their layout and the BV_ATTN_DROPOUT mirror are checked with the other headers' in
+tests/test_abi.py), the numpy restatement of the attention mask stream (numpy's Philox in 16-bit lanes, its
+realized rate, and its separation from every bv_dropout counter and from Jet's), the float64 BERT oracle
+with given masks pinned against `transformers.BertModel` in train mode with the same masks, and what the
+BERT tower launches and keeps with dropout, recorded by tests/golden/make_model_traces.py's recorder."""
 import ctypes
 import importlib.util
 import math
 import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -24,36 +22,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 # ---- the C ABI -------------------------------------------------------------------------------------------
-def test_the_flag_is_mirrored_and_distinct_from_the_key_mask_flag():
-  from big_vision_b200 import lib as L
-  src = open(os.path.join(ROOT, "include", "bv_dropout.h")).read()
-  assert f"#define BV_ATTN_DROPOUT {L.ATTN_DROPOUT} " in src
-  assert L.ATTN_DROPOUT & 0xffff == 0 and L.ATTN_DROPOUT & L.ATTN_KEY_MASK == 0
-
-
-@pytest.mark.skipif(shutil.which("gcc") is None, reason="no gcc")
-def test_dropout_struct_layout_matches_the_header(tmp_path):
-  from big_vision_b200 import lib as L
-  prog = tmp_path / "layout.c"
-  prog.write_text("""#include <stddef.h>
-#include <stdio.h>
-#include "bv_dropout.h"
-int main(void) {
-  printf("%zu %zu %zu %zu %zu %zu\\n", sizeof(bv_attn_dropout_args), offsetof(bv_attn_dropout_args, masked),
-         offsetof(bv_attn_dropout_args, drop), sizeof(bv_attn_dropout_bwd_args),
-         offsetof(bv_attn_dropout_bwd_args, masked), offsetof(bv_attn_dropout_bwd_args, drop));
-  return 0;
-}
-""")
-  exe = tmp_path / "layout"
-  subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), str(prog), "-o",
-                  str(exe)], check=True)
-  got = [int(x) for x in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
-  F, B = L.AttnDropoutArgs, L.AttnDropoutBwdArgs
-  assert got == [ctypes.sizeof(F), F.masked.offset, F.drop.offset, ctypes.sizeof(B), B.masked.offset,
-                 B.drop.offset]
-
-
 def _key(**kw):
   from big_vision_b200 import lib as L
   return L.DropoutKey(**{"seed": 1, "step": 2, "site": 3, "row0": 0, "rate": 0.1, **kw})

@@ -1,89 +1,21 @@
-"""CPU: dropout for the ViT and text towers.  The C ABI of include/bv_dropout.h (its functions exported and
-bound one to one, plain C that a C program links against, each entry point named with the GPU tests that
-call its ops function), the numpy restatement of the mask stream (its realized rate, its independence across
-sites, steps, seeds and rows, and its separation from Jet's noise), the refusals of the entry points and of
-the models, the key struct's layout against a C program, and what the models launch and keep with dropout,
-recorded by tests/golden/make_model_traces.py's recorder."""
+"""CPU: dropout for the ViT and text towers.  The numpy restatement of the mask stream (its realized rate,
+its independence across sites, steps, seeds and rows, and its separation from Jet's noise), the refusals of
+the entry points of include/bv_dropout.h and of the models, and what the models launch and keep with
+dropout, recorded by tests/golden/make_model_traces.py's recorder.  The header's binding, layout and C
+program are checked with the other headers' in tests/test_abi.py."""
 import ctypes
 import importlib.util
 import math
 import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
 import dropout_oracle as D
-from common import header_functions
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HEADER = os.path.join(ROOT, "include", "bv_dropout.h")
-
-# entry point -> the GPU tests of tests/test_dropout_gpu.py that check it directly against numpy / float64
-COVERAGE = {
-    "bv_dropout": ["test_dropout_is_numpy_bit_for_bit", "test_column_sums_match_fp64_and_runs_repeat",
-                   "test_realized_rate_at_b16_shapes"],
-    "bv_dropout_add": ["test_dropout_add_is_numpy_bit_for_bit"],
-}
-
-
-# ---- the C ABI of include/bv_dropout.h ------------------------------------------------------------------
-def test_header_functions_are_exported_and_bound_one_to_one():
-  from big_vision_b200 import lib as L
-  declared = header_functions(HEADER)
-  assert declared == set(L.DROPOUT_SIGNATURES) == set(COVERAGE)
-  assert not declared & set(L.SIGNATURES)
-  lib = L.load()
-  for name in declared:
-    assert tuple(getattr(lib, name).argtypes) == tuple(L.DROPOUT_SIGNATURES[name])
-
-
-def test_every_entry_point_has_gpu_tests_that_call_its_op():
-  import ast
-  tree = ast.parse(open(os.path.join(ROOT, "tests", "test_dropout_gpu.py")).read())
-  gpu_module = any(isinstance(n, ast.Assign) and any(getattr(t, "id", "") == "pytestmark" for t in n.targets)
-                   and ast.unparse(n.value) == "pytest.mark.gpu" for n in tree.body)
-  assert gpu_module
-  tests = {n.name: ast.unparse(n) for n in tree.body if isinstance(n, ast.FunctionDef) and n.name.startswith("test_")}
-  for fn, names in COVERAGE.items():
-    for t in names:
-      assert t in tests, (fn, t)
-      assert fn.replace("bv_", "ops.", 1) + "(" in tests[t], (fn, t)
-
-
-@pytest.mark.skipif(shutil.which("gcc") is None, reason="no gcc")
-def test_header_is_plain_c_and_a_c_program_links(tmp_path):
-  """The header compiles as C99 and C++, and a C program that includes it links against libbv_b200.so and
-  gets the refusals that need no GPU."""
-  from big_vision_b200 import lib as L
-  L.load()
-  subprocess.run(["gcc", "-std=c99", "-Wall", "-Wextra", "-Werror", "-fsyntax-only", "-x", "c", HEADER], check=True)
-  subprocess.run(["g++", "-std=c++17", "-fsyntax-only", "-x", "c++", HEADER], check=True)
-  src = tmp_path / "main.c"
-  src.write_text("""#include <stdio.h>
-#include "bv_dropout.h"
-int main(void) {
-  /* a rate of 1, then site 0 */
-  unsigned short buf[64];
-  bv_dropout_key key = {1, 2, 3, 0, 1.f};
-  int a = bv_dropout(buf, 8, buf, 8, 4, 8, &key, NULL);
-  key.rate = 0.1f;
-  key.site = 0;
-  int b = bv_dropout_add(buf, 8, buf, 8, buf, 8, 4, 8, &key, NULL);
-  printf("%d %d %s\\n", a, b, bv_last_error_string());
-  return 0;
-}
-""")
-  libdir = os.path.dirname(os.path.abspath(L.LIB_PATH))
-  exe = tmp_path / "main"
-  subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe),
-                  "-L", libdir, "-lbv_b200", f"-Wl,-rpath,{libdir}"], check=True)
-  out = subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split(None, 2)
-  assert [int(v) for v in out[:2]] == [-1, -1] and "bv_dropout_add" in out[2] and "site 0" in out[2], out
-
 
 # ---- the mask stream ------------------------------------------------------------------------------------
 @pytest.mark.parametrize("rate", [0.1, 0.5, 0.03])
@@ -201,27 +133,6 @@ def test_apply_train_with_dropout_has_no_key():
                         text=dict(width=64, depth=1, mlp_dim=128, num_heads=1, dropout=0.1))
   with pytest.raises(ValueError, match="dropout key"):
     tt.apply({"params": None}, None, None, train=True)
-
-
-@pytest.mark.skipif(shutil.which("gcc") is None, reason="no gcc")
-def test_key_struct_layout_matches_the_header(tmp_path):
-  from big_vision_b200 import lib as L
-  prog = tmp_path / "layout.c"
-  prog.write_text("""#include <stddef.h>
-#include <stdio.h>
-#include "bv_dropout.h"
-int main(void) {
-  printf("%zu %zu %zu %zu %zu %zu\\n", sizeof(bv_dropout_key), offsetof(bv_dropout_key, seed),
-         offsetof(bv_dropout_key, step), offsetof(bv_dropout_key, site), offsetof(bv_dropout_key, row0),
-         offsetof(bv_dropout_key, rate));
-  return 0;
-}
-""")
-  exe = tmp_path / "layout"
-  subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(prog), "-o", str(exe)], check=True)
-  got = [int(x) for x in subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()]
-  K = L.DropoutKey
-  assert got == [ctypes.sizeof(K), K.seed.offset, K.step.offset, K.site.offset, K.row0.offset, K.rate.offset]
 
 
 # ---- what the models launch and keep --------------------------------------------------------------------

@@ -1,4 +1,4 @@
-"""CPU: every entry point of include/bv_b200*.h is named here with the GPU test(s) that check it directly
+"""CPU: every entry point of include/bv_*.h is named here with the GPU test(s) that check it directly
 against a reference of the same operation (not only through a whole-model test, whose tolerances are far
 too loose to pin one kernel).  A new ABI function without such a test, or a table row that names a test
 that does not exist, fails this file on a machine without a GPU."""
@@ -20,6 +20,8 @@ SG = "test_gsam_gpu"
 DG = "test_distill_gpu"
 FG = "test_flexi_gpu"
 JG = "test_jet_gpu"
+DR = "test_dropout_gpu"
+CV = "test_conv_gpu"
 COVERAGE = {
     "bv_gemm": [f"{KG}::test_dense_forward_epilogues", f"{KG}::test_dense_backward_contractions",
                 "test_gemm_aux_tma_gpu::test_resid_matches_fp32_oracle",
@@ -98,7 +100,24 @@ COVERAGE = {
     "bv_jet_coupling_bwd": [f"{JG}::test_coupling_bwd_elementwise", f"{JG}::test_extreme_raw_scales_stay_finite"],
     "bv_jet_merge_grad": [f"{JG}::test_split_and_merge_grad_are_exact"],
     "bv_jet_bits": [f"{JG}::test_bits_elementwise", f"{JG}::test_logdet_and_bits_are_bit_identical_across_runs"],
+    # include/bv_dropout.h
+    "bv_dropout": [f"{DR}::test_dropout_is_numpy_bit_for_bit", f"{DR}::test_column_sums_match_fp64_and_runs_repeat",
+                   f"{DR}::test_realized_rate_at_b16_shapes"],
+    "bv_dropout_add": [f"{DR}::test_dropout_add_is_numpy_bit_for_bit"],
+    # include/bv_conv.h
+    "bv_conv_fwd": [f"{CV}::test_convolutions_match_fp64"],
+    "bv_conv_dgrad": [f"{CV}::test_convolutions_match_fp64"],
+    "bv_conv_wgrad": [f"{CV}::test_convolutions_match_fp64"],
+    "bv_weight_std_fwd": [f"{CV}::test_weight_standardisation_matches_fp64"],
+    "bv_weight_std_bwd": [f"{CV}::test_weight_standardisation_matches_fp64"],
+    "bv_groupnorm_fwd": [f"{CV}::test_groupnorm_relu_matches_fp64"],
+    "bv_groupnorm_bwd": [f"{CV}::test_groupnorm_relu_matches_fp64"],
+    "bv_maxpool_fwd": [f"{CV}::test_maxpool_forward_and_first_max_backward"],
+    "bv_maxpool_bwd": [f"{CV}::test_maxpool_forward_and_first_max_backward"],
+    "bv_stem_im2col": [f"{CV}::test_stem_convolution_matches_fp64"],
 }
+# entry points whose op is reached through another ops function of the same family
+VIA = {"bv_stem_im2col": "ops.stem_conv_fwd("}
 
 
 def _is_gpu_mark(dec):
@@ -144,14 +163,14 @@ def test_every_named_test_exists_as_a_gpu_test():
 
 
 def test_feature_header_rows_name_tests_that_call_the_op():
-  """Each entry point of the feature headers (all but bv_b200.h) has one ops function of the same name, and
-  every test its row names calls that function."""
+  """Each entry point of the feature headers (all but bv_b200.h) has one ops function of the same name (or
+  the one VIA names), and every test its row names calls that function."""
   known = _gpu_tests()
   for h in HEADERS:
     if os.path.basename(h) != "bv_b200.h":
       for fn in header_functions(h):
         for t in COVERAGE[fn]:
-          assert fn.replace("bv_", "ops.", 1) in known[t], (fn, t)
+          assert VIA.get(fn, fn.replace("bv_", "ops.", 1) + "(") in known[t], (fn, t)
 
 
 def test_gemm_and_attention_rows_name_an_element_wise_test():
