@@ -2,8 +2,9 @@
 // 1-query attention, K10).  Reference: flax.linen.MultiHeadDotProductAttention as called at
 // models/vit.py:93-98 (self-attention, no mask, no dropout) and models/vit.py:176-178 (MAPHead
 // probe attention): q is scaled by 1/sqrt(dh), softmax over keys, weights times v.  Head dims 64,
-// 72, 80, 96 and 104 are built (the size table of models/vit.py:284-303: 64 for Ti, S, M, B and L,
-// 72 for So400m, 80 for H, 96 for g-opt and G-opt, 104 for G); mu (16), g (88) and e (112) are not.
+// 72, 80, 96, 104 and 112 are built (the size table of models/vit.py:284-303: 64 for Ti, S, M, B and
+// L, 72 for So400m, 80 for H, 96 for g-opt and G-opt, 104 for G, 112 for e); mu (16) and g (88) are
+// not.
 // Every kernel is a template on the head dim DH.
 //
 // q/k/v/o are strided views into the fused QKV GEMM output: element (b, t, h*DH+j) at
@@ -66,7 +67,8 @@ constexpr int THREADS = 128;
 // kernel K, V and two Q / dO slots.
 template <int DH>
 struct Geo {
-  static_assert(DH == 64 || DH == 72 || DH == 80 || DH == 96 || DH == 104, "head dims 64, 72, 80, 96, 104");
+  static_assert(DH == 64 || DH == 72 || DH == 80 || DH == 96 || DH == 104 || DH == 112,
+                "head dims 64, 72, 80, 96, 104, 112");
   static constexpr int TILE_BYTES = DH > 64 ? 2 * BOX_BYTES : BOX_BYTES;   // a [64 rows x DH] tile
   static constexpr int KSTEPS = (DH + 15) / 16;                            // k16 steps over the head dim
   static_assert(KSTEPS >= 4 && KSTEPS <= 8, "one or two 64-column boxes");
@@ -121,7 +123,8 @@ __device__ __forceinline__ void wgmma_rs_dh(float (&d)[R], const uint32_t (&a)[4
   else if constexpr (R == 36) wgmma_rs_n72<TB>(d, a, b, scale_d);
   else if constexpr (R == 40) wgmma_rs_n80<TB>(d, a, b, scale_d);
   else if constexpr (R == 48) wgmma_rs_n96<TB>(d, a, b, scale_d);
-  else wgmma_rs_n104<TB>(d, a, b, scale_d);
+  else if constexpr (R == 52) wgmma_rs_n104<TB>(d, a, b, scale_d);
+  else wgmma_rs_n112<TB>(d, a, b, scale_d);
 }
 
 // S[64 x 64] = A B^T over the head dimension (zero-padded to a multiple of 16), both tiles K-major
@@ -727,8 +730,8 @@ int check_drop(bool dropped, bool masked, int head_dim, const bv_dropout_key& k,
 // head dims with kernels; every other one is refused before any CUDA call.  The key mask is built at
 // head dim 64 only (BERT-Base and BERT-Large)
 int check_head_dim(int head_dim, bool masked, const KeyMask& m, const char* who) {
-  if (head_dim != 64 && head_dim != 72 && head_dim != 80 && head_dim != 96 && head_dim != 104) {
-    set_error("%s: head_dim %d is not supported (supported head dims: 64, 72, 80, 96, 104)", who, head_dim);
+  if (head_dim != 64 && head_dim != 72 && head_dim != 80 && head_dim != 96 && head_dim != 104 && head_dim != 112) {
+    set_error("%s: head_dim %d is not supported (supported head dims: 64, 72, 80, 96, 104, 112)", who, head_dim);
     return BV_ERR_UNSUPPORTED;
   }
   if (masked && head_dim != 64) {
@@ -901,6 +904,7 @@ int bv_attention_fwd_hd(const bv_attn_args* args, int32_t head_dim, void* stream
     case 80: return attention_fwd<80>(a, km, dr, s);
     case 96: return attention_fwd<96>(a, km, dr, s);
     case 104: return attention_fwd<104>(a, km, dr, s);
+    case 112: return attention_fwd<112>(a, km, dr, s);
     default: return attention_fwd<64>(a, km, dr, s);
   }
 }
@@ -930,6 +934,7 @@ int bv_attention_bwd_hd(const bv_attn_bwd_args* args, int32_t head_dim, void* st
     case 80: return attention_bwd<80>(g, km, dr, s);
     case 96: return attention_bwd<96>(g, km, dr, s);
     case 104: return attention_bwd<104>(g, km, dr, s);
+    case 112: return attention_bwd<112>(g, km, dr, s);
     default: return attention_bwd<64>(g, km, dr, s);
   }
 }

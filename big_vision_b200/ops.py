@@ -153,7 +153,7 @@ def _attn_call(name, args, masked_type, key_mask, B, Nk, dh, dropout=None, dropo
 
 
 # head dims the attention kernels are built for (bv_attention_fwd_hd / bv_attention_bwd_hd)
-ATTN_HEAD_DIMS = (64, 72, 80, 96, 104)
+ATTN_HEAD_DIMS = (64, 72, 80, 96, 104, 112)
 
 
 def _head_dim(cols, heads):

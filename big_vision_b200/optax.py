@@ -46,6 +46,8 @@ class _AdafactorTensor:
         self.dims, self.strides = (1, 1, 1, self.numel), (0, 0, 0)
       elif len(shape) == 2 and stride[1] == 1:
         self.dims, self.strides = (1, shape[0], 1, shape[1]), (0, stride[0], 0)
+      elif len(shape) == 3 and stride[2] == 1:     # e.g. a scan-stacked q / k / v bias [depth, heads, dh]
+        self.dims, self.strides = (shape[0], shape[1], 1, shape[2]), (stride[0], stride[1], 0)
       else:
         raise NotImplementedError(f"adafactor: unfactored strided tensor {name} {shape} {stride}")
       return

@@ -109,7 +109,7 @@ int bv_layernorm_bwd(const void* dy, int dy_dtype, const void* x, int x_dtype, c
  * (flax MultiHeadDotProductAttention core: models/vit.py:93-98, :176-178).  Keys stream through
  * on-chip memory in 64-key blocks (online combination of per-block softmax statistics), so every
  * sequence length takes the same path.
- * Head dim dh: 64, 72, 80, 96 or 104 (ViT Ti..L, So400m, H, g-opt / G-opt, G).  The entry points take
+ * Head dim dh: 64, 72, 80, 96, 104 or 112 (ViT Ti..L, So400m, H, g-opt / G-opt, G, e).  The entry points take
  * dh and refuse any other value with BV_ERR_UNSUPPORTED before touching the device.
  * q/k/v/o are bf16 strided views: element (b, t, h*dh + j) at
  * base + b*bs + t*ld + h*dh + j  (e.g. column slices of the fused QKV GEMM output).

@@ -4,12 +4,17 @@ recompute.  Head dim 104 (1664 / 16) and a class count that is not a multiple of
 stored padded (models/common.py Dense, pad=True).  1,930.4 M parameters: the flat fp32 parameter and
 gradient buffers are 7.2 GiB each.
 
+`--variant e/14` times the same config switched to `e/14` instead (`scaling_laws_vit_e14`): width 1792,
+depth 56, MLP 15360, head dim 112, 3,926.4 M parameters, so the flat buffers hold more than 2^31
+elements (14.6 GiB each in fp32).
+
 Registers `scaling_laws_vit_G14` into bench.WORKLOADS and sets bench.OPT_CONFIG to the config's
 optimizer, in this process only, then reuses bench.py's measurement and JSON line; bench.py's own
 workload list and optimizer stay the BASELINE.json ones.  Mixup is not on the timed path (bench.py
 steps with rng=None).
 
-  python tools/bench_vit_G14.py [--steps 8] [--warmup 3] [--per-gpu-batch N] [--profile-calls]
+  python tools/bench_vit_G14.py [--variant {G/14,e/14}] [--steps 8] [--warmup 3] [--per-gpu-batch N]
+                                [--profile-calls]
 
 Prints one JSON line: our arm as bench.py prints it plus parameter counts, with the labelled PyTorch
 stand-in (baseline/torch_gpu.py: fused AdamW, not Adafactor) measured in its own process in
@@ -61,23 +66,41 @@ WORKLOAD = dict(
          "per-block recompute (models/vit.py:129-148 nn.remat, nothing_saveable)")
 
 
-def register():
-  bench.WORKLOADS[NAME] = WORKLOAD
+E_NAME = "scaling_laws_vit_e14"
+# per-GPU batch 256: the largest power of two that fits an 80 GB H100 (DESIGN.md section 5)
+E_WIDTH, E_DEPTH, E_MLP = 1792, 56, 15360
+E_WORKLOAD = dict(
+    WORKLOAD, metric="vit_e14_cls_img_per_sec", per_gpu_batch=256,
+    flops=image_train_flops(d=E_WIDTH, m=E_MLP, depth=E_DEPTH),
+    model_kw=dict(WORKLOAD["model_kw"], variant=f"e/{PATCH}"), oracle=dict(WORKLOAD["oracle"], depth=E_DEPTH),
+    desc="ViT-e/14 (configs/proj/scaling_laws/train_vit_g.py switched to e/14: 256 tokens, map pool, head dim 112, "
+         "29593 classes, sigmoid_xent, BV-Adafactor, grad_clip_norm 1, wd_mults), 224x224, full update_fn with "
+         "per-block recompute (models/vit.py:129-148 nn.remat, nothing_saveable)")
+
+# --variant -> (workload name, workload)
+VARIANTS = {"G/14": (NAME, WORKLOAD), "e/14": (E_NAME, E_WORKLOAD)}
+
+
+def register(variant="G/14"):
+  name, wl = VARIANTS[variant]
+  bench.WORKLOADS[name] = wl
   bench.OPT_CONFIG = OPT_CONFIG
-  return WORKLOAD
+  return wl
 
 
 def main():
   ap = argparse.ArgumentParser()
+  ap.add_argument("--variant", default="G/14", choices=sorted(VARIANTS))
   ap.add_argument("--steps", type=int, default=8)
   ap.add_argument("--warmup", type=int, default=3)
-  ap.add_argument("--per-gpu-batch", type=int, default=0, help=f"0 = {WORKLOAD['per_gpu_batch']}")
+  ap.add_argument("--per-gpu-batch", type=int, default=0, help="0 = the variant's per_gpu_batch (G/14: "
+                  f"{WORKLOAD['per_gpu_batch']}, e/14: {E_WORKLOAD['per_gpu_batch']})")
   ap.add_argument("--impl", default="ours", choices=["ours", "torch_gpu"])
   ap.add_argument("--profile-calls", action="store_true")
   ap.add_argument("--no-gpu-baseline", action="store_true")
   args = ap.parse_args()
-  register()
-  argv = ["bench.py", "--workload", NAME, "--steps", str(args.steps), "--warmup", str(args.warmup),
+  wl = register(args.variant)
+  argv = ["bench.py", "--workload", VARIANTS[args.variant][0], "--steps", str(args.steps), "--warmup", str(args.warmup),
           "--per-gpu-batch", str(args.per_gpu_batch)]
   if args.impl == "torch_gpu":
     sys.argv = argv + ["--impl", "torch_gpu"]
@@ -88,11 +111,12 @@ def main():
   with contextlib.redirect_stdout(buf):
     bench.main()
   line = json.loads(buf.getvalue().strip().splitlines()[-1])
-  line["config"]["params"] = param_counts()
+  line["config"]["params"] = param_counts(wl)
   line["config"]["optimizer"] = "big_vision.scale_by_adafactor (train_vit_g.py)"
   if not args.no_gpu_baseline:
     # the stand-in in its own process (this one's device memory is released when it exits)
-    cmd = [sys.executable, os.path.abspath(__file__), "--impl", "torch_gpu", "--steps", str(min(args.steps, 6)),
+    cmd = [sys.executable, os.path.abspath(__file__), "--variant", args.variant, "--impl", "torch_gpu",
+           "--steps", str(min(args.steps, 6)),
            "--warmup", "3", "--per-gpu-batch", str(args.per_gpu_batch)]
     try:
       out = subprocess.run(cmd, capture_output=True, text=True, timeout=1800)
@@ -103,10 +127,10 @@ def main():
   print(json.dumps(line), flush=True)
 
 
-def param_counts():
+def param_counts(wl=WORKLOAD):
   """Parameter counts under the reference names and shapes (nothing allocated)."""
   from big_vision_b200 import engine as E
-  model = bench.build_model(WORKLOAD)
+  model = bench.build_model(wl)
   specs, aliases = model.specs((RES, RES), 3)
   tree = E.FlatParams(specs, aliases, "meta").tree("f")
   head = sum(v.numel() for k, v in tree.items() if k.startswith("head/"))
