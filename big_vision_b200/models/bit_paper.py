@@ -53,16 +53,6 @@ class _StdConv:
     P.g(self.name).add_(ops.weight_std_bwd(self.w, self.mean, self.rstd, g_std))
 
 
-class _Stage:
-  """The defaults of a backward stage (engine.Stage's): no gradient sink, no all-reduce hook.  The stages here
-  implement the protocol without subclassing engine.Stage, which the per-stage replay tests require to have
-  replay cases of their own; they are pinned on their own inputs in tests/test_bit_gpu.py instead."""
-  ready = None
-
-  def sink(self, P, geom):
-    return None
-
-
 def _gn_fwd(P, prefix, x):
   y, mean, rstd = ops.groupnorm_fwd(x, P.f(prefix + "scale"), P.f(prefix + "bias"), relu=True)
   return y, (mean, rstd)
@@ -73,7 +63,7 @@ def _gn_bwd(P, prefix, dy, x, stats, dx_add=None):
                            P.g(prefix + "bias"), relu=True, dx_add=dx_add)
 
 
-class RootBlock(_Stage):
+class RootBlock(E.Stage):
   """root_block (bit_paper.py:71-80): StdConv 7 x 7 / 2 with padding 3, then max pool 3 x 3 / 2, padding 1."""
 
   def __init__(self, width):
@@ -97,7 +87,7 @@ class RootBlock(_Stage):
     return None          # the image gets no gradient
 
 
-class ResidualUnit(_Stage):
+class ResidualUnit(E.Stage):
   """block{b}/unit{u:02d} (bit_paper.py:83-111): pre-activation bottleneck.  gn1 + relu feeds both conv_proj
   and conv1; the stride sits on conv2 (and conv_proj)."""
 
@@ -153,7 +143,7 @@ class ResidualUnit(_Stage):
     return _gn_bwd(P, p + "gn1/", da1, x, st1, dx_add=None if self.proj else dy)
 
 
-class PreHead(_Stage):
+class PreHead(E.Stage):
   """norm-pre-head GroupNorm + ReLU and the mean over the pixels (bit_paper.py:144-146): fp32 [n, C]."""
 
   def __init__(self, c):

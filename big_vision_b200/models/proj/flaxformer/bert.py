@@ -62,14 +62,9 @@ def trunc_normal(std):
   return init
 
 
-# The three stages below implement engine.Staged's stage protocol directly instead of subclassing
-# engine.Stage: every engine.Stage subclass under models/ must have a per-stage replay case in
-# tests/test_stage_replay_gpu.py (tests/test_stage_oracle.py), and BERT's are not written yet.  The tower
-# is checked as a whole against tests/bert_oracle.py instead.
-class _Embed:
+class _Embed(E.Stage):
   """Token + position + segment-0 embeddings, then the embedding LayerNorm and its dropout.  The position
   table has MAX_POSITIONS rows; a forward of N tokens reads rows 0..N-1."""
-  ready = None
 
   def __init__(self, prefix, d, vocab_size):
     self.p, self.d, self.vocab_size = prefix + "embedder/", d, vocab_size
@@ -93,9 +88,6 @@ class _Embed:
       ops.dropout(y, geom.dropout.mask(0, E.DROP_EMBED), out=y)
     return y, ((text, x, mean, rstd) if save else None)
 
-  def sink(self, P, geom):
-    return None
-
   def bwd(self, P, dy, saved, geom, sink=None, need_dx=False):
     N, p = geom.N, self.p
     text, x, mean, rstd = saved
@@ -110,7 +102,7 @@ class _Embed:
     ops.colsum(dpos, P.g(p + "embedders_segment_ids/embedding")[0])
 
 
-class _Layer:
+class _Layer(E.Stage):
   """One post-LN encoder layer: x1 = LN(x + Attn(x)), x2 = LN(x1 + MLP(x1)), with the forward's key
   mask (geom.key_mask) in the attention.  Under dropout, x1 = LN(x + drop(Attn(x))) with the attention
   probabilities dropped too (geom.attn_dropout), and x2 = LN(x1 + drop(MLP(x1)))."""
@@ -119,9 +111,6 @@ class _Layer:
     self.p, self.d, self.m, self.heads, self.layer = prefix, d, m, heads, layer
     self.prefixes = (prefix,)
     self.ready = prefix + "self_attention/qkv/kernel"      # its first spec: see vit.EncoderBlock
-
-  def sink(self, P, geom):
-    return None
 
   def specs(self):
     s, a = vit.mha_specs(self.p + "self_attention/", self.d, self.heads)
@@ -205,12 +194,9 @@ class _Layer:
     return ops.gemm(dqkv, A.h("qkv/kernel"), aux=dh1, epilogue=L.EPI_BIAS_RESID)    # + the residual
 
 
-class _ClsPool:
+class _ClsPool(E.Stage):
   """x[:, 0]: the [CLS] token of the last layer (bert.py:58).  No parameters."""
-  prefixes, ready = (), None
-
-  def sink(self, P, geom):
-    return None
+  prefixes = ()
 
   def specs(self):
     return [], []

@@ -1,18 +1,29 @@
 """TEST INFRASTRUCTURE: one float64 reference per kind of backward stage (engine.Stage) of the models, built
-from oracle/bv_oracle.py's pieces with mm="float32" (plain high-precision math).  Each function takes the
-stage's input and its parameters, `p`: a dict of float64 tensors under the reference names relative to the
-stage's root (the stage's own prefix, or the model prefix for the embeddings), and returns the stage's output;
-torch autograd then gives d input and the parameter gradients under the same names.
+from the pieces of oracle/bv_oracle.py (mm="float32": plain high-precision math) and of tests/bit_oracle.py
+(in its float64 mode).  Each function takes the stage's input and its parameters, `p`: a dict of float64
+tensors under the reference names relative to the stage's root (the stage's own prefix, or the model prefix
+for the embeddings), and returns the stage's output; torch autograd then gives d input and the parameter
+gradients under the same names.
 
 Chained bottom-up they are the whole models of the oracle (tests/test_stage_oracle.py checks that), so a stage
 checked against its reference on the inputs the CUDA path actually gave it is checked against the pinned
-oracle, one stage at a time."""
-import torch
+oracle, one stage at a time.
 
+Where a stage's discrete decision (a ReLU's sign, a max pool's route) is taken on a value the kernels rounded
+to bf16 inside the stage, a reference can be handed that decision instead of taking its own: within a bf16
+rounding of the threshold the two would decide differently and move a whole gradient term, which says nothing
+about the kernels.  Without it each reference decides on its own float64 values."""
+import math
+
+import torch
+import torch.nn.functional as F
+
+import bit_oracle as BO
 import flexi_oracle as FO
 from oracle import bv_oracle as O
 
 MM = "float32"
+BERT_EPS = 1e-12      # models/proj/flaxformer/bert.py LN_EPS
 
 
 def patch_embedding(image, p, name, pos=None, cls=False):
@@ -100,6 +111,97 @@ def dense(x, p, tanh=False):
   """common.Dense: x [rows, fan_in] -> [rows, fan_out] (tanh(x W + b) with `tanh`)."""
   y = O.dense(x, p["kernel"], p["bias"], MM)
   return torch.tanh(y) if tanh else y
+
+
+# ---- BERT (models/proj/flaxformer/bert.py) ----------------------------------------------------------------
+def bert_embed(ids, p, keep=None):
+  """bert._Embed: ids [n, N] -> the token row + position row (< N) + segment row 0, then the embedding
+  LayerNorm (eps 1e-12) -> [n, N, d]; `keep` (the scaled EMBED dropout mask [n, N, d]) multiplies it."""
+  N = ids.shape[1]
+  x = (p["embedders_token_ids/embedding"][ids.long()] + p["embedders_position_ids/embedding"][:N]
+       + p["embedders_segment_ids/embedding"][0])
+  y = O.layer_norm(x, p["layer_norm/scale"], p["layer_norm/bias"], eps=BERT_EPS)
+  return y if keep is None else y * keep
+
+
+def bert_attention(x, p, heads, key_mask, probs=None):
+  """BERT's self-attention of x [n, N, d] with the key mask [n, N] (True = attend; every sample attends at
+  least one key) and `probs` (the scaled dropout mask [n, heads, N, N] of the probabilities, or None).  The
+  softmax is torch.softmax of the -inf-masked scores, where ScoreGrad finds it."""
+  n, N, d = x.shape
+  dh = d // heads
+
+  def proj(name):
+    y = O.dense(x, p[name + "/kernel"].reshape(d, d), p[name + "/bias"].reshape(d), MM)
+    return y.reshape(n, N, heads, dh).transpose(1, 2)
+
+  q, k, v = proj("query"), proj("key"), proj("value")
+  s = (q @ k.transpose(-1, -2)) / math.sqrt(dh)
+  w = torch.softmax(s.masked_fill(~key_mask[:, None, None, :], -math.inf), dim=-1)
+  if probs is not None:
+    w = w * probs
+  o = (w @ v).transpose(1, 2).reshape(n, N, d)
+  return O.dense(o, p["out/kernel"].reshape(d, d), p["out/bias"], MM)
+
+
+def bert_layer(x, p, heads, key_mask, masks=None):
+  """bert._Layer: x [n, N, d] -> the post-LN layer x1 = LN(x + Attn(x)), LN(x1 + MLP(x1)).  `masks`: None, or
+  the scaled dropout masks (probabilities [n, heads, N, N], attention output [n, N, d], MLP output [n, N, d])."""
+  probs, attn, mlp = (None, None, None) if masks is None else masks
+  y = bert_attention(x, O.sub(p, "self_attention/"), heads, key_mask, probs)
+  if attn is not None:
+    y = y * attn
+  x = O.layer_norm(x + y, p["attention_layer_norm/scale"], p["attention_layer_norm/bias"], eps=BERT_EPS)
+  y = O.mlp_block(x, O.sub(p, "mlp/"), MM)
+  if mlp is not None:
+    y = y * mlp
+  return O.layer_norm(x + y, p["output_layer_norm/scale"], p["output_layer_norm/bias"], eps=BERT_EPS)
+
+
+def cls_pool(x):
+  """bert._ClsPool: x [n, N, d] -> the [CLS] token x[:, 0]."""
+  return x[:, 0]
+
+
+# ---- BiT ResNet-v2 (models/bit_paper.py) -------------------------------------------------------------------
+def _windows(t, ho, wo):
+  """The 3 x 3 / 2 windows of t [n, h + 2, w + 2, C] (padded by one): [9, n, ho, wo, C], row-major order."""
+  return torch.stack([t[:, i:i + 2 * ho - 1:2, j:j + 2 * wo - 1:2] for i in range(3) for j in range(3)])
+
+
+def bit_root(image, p, route=None):
+  """bit_paper.RootBlock: image [n, H, W, 3] -> StdConv 7 x 7 / 2 (padding 3), then the -inf-padded 3 x 3 / 2
+  max pool -> [n, ho, wo, C].  Each window takes its first maximum in row-major window order of `route`
+  [n, h, w, C] (default: the convolution output itself); the CUDA path routes by its bf16 convolution output."""
+  y = BO.std_conv(image, p["conv_root/kernel"], 2, 3)
+  h, w = y.shape[1], y.shape[2]
+  ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+  pad = lambda t: F.pad(t, (0, 0, 1, 1, 1, 1), value=-math.inf)
+  first = _windows(pad((y if route is None else route).detach()), ho, wo).argmax(0)   # the first maximum
+  return _windows(pad(y), ho, wo).gather(0, first[None])[0]
+
+
+def _gn_relu(x, p, prefix, keep=None):
+  """The GroupNorm under `prefix` of x, then the ReLU, or the given ReLU decision `keep` (True = positive)."""
+  y = BO.group_norm(x, p[prefix + "scale"], p[prefix + "bias"])
+  return torch.relu(y) if keep is None else y * keep
+
+
+def bit_unit(x, p, stride, relu_masks=None):
+  """bit_paper.ResidualUnit: x [n, h, w, cin] -> the pre-activation bottleneck [n, ho, wo, 4 nmid], with the
+  projection when p has conv_proj.  `relu_masks`: None, or the ReLU decisions of gn2 and gn3 (bool, shaped like
+  their outputs); the CUDA path decides them on its bf16 conv1 and conv2 outputs."""
+  m2, m3 = (None, None) if relu_masks is None else relu_masks
+  a1 = _gn_relu(x, p, "gn1/")
+  res = BO.std_conv(a1, p["conv_proj/kernel"], stride, 0) if "conv_proj/kernel" in p else x
+  h = _gn_relu(BO.std_conv(a1, p["conv1/kernel"], 1, 0), p, "gn2/", m2)
+  h = _gn_relu(BO.std_conv(h, p["conv2/kernel"], stride, 1), p, "gn3/", m3)
+  return BO.std_conv(h, p["conv3/kernel"], 1, 0) + res
+
+
+def bit_prehead(x, p):
+  """bit_paper.PreHead: x [n, h, w, C] -> GroupNorm + ReLU, then the mean over the pixels -> [n, C]."""
+  return _gn_relu(x, p, "").mean(dim=(1, 2))
 
 
 class Tap(torch.overrides.TorchFunctionMode):

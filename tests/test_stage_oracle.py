@@ -1,7 +1,7 @@
 """CPU: the per-stage float64 references of tests/stage_oracle.py, chained bottom-up, are the whole-model
-oracle (O.vit_forward, O.mixer_forward, O.text_forward and the FlexiViT forward), outputs and autograd
-gradients to 1e-12; and every backward stage class of the models is named with the replay cases of
-tests/test_stage_replay_gpu.py that check it."""
+oracle (O.vit_forward, O.mixer_forward, O.text_forward, the FlexiViT forward, the BERT tower with and without
+dropout, and the BiT ResNet-v2), outputs and autograd gradients to 1e-12; and every backward stage class of the
+models is named with the replay cases of tests/test_stage_replay_gpu.py that check it."""
 import importlib
 import pkgutil
 
@@ -26,18 +26,21 @@ def _tree(specs_aliases, seed):
   return O.to_f64_tree(tree, requires_grad=True)
 
 
-def _assert_same(chain, ref, p, inputs):
-  """The two forwards agree, and so do their gradients w.r.t. every parameter (and input) for one cotangent."""
+def _assert_same(chain, ref, p, inputs, scale_of=None):
+  """The two forwards agree, and so do their gradients w.r.t. every parameter (and input) for one cotangent.
+  `scale_of` {name: other name}: a gradient that is zero in exact arithmetic, held to the other's scale."""
   assert chain.shape == ref.shape
   assert float((chain - ref).abs().max()) <= 1e-12 * float(ref.detach().abs().max())
   leaves = list(p.values()) + list(inputs)
   dy = torch.randn(ref.shape, dtype=F64, generator=torch.Generator().manual_seed(0))
   g1 = torch.autograd.grad(chain, leaves, dy, allow_unused=True)
   g2 = torch.autograd.grad(ref, leaves, dy, allow_unused=True)
+  grads = dict(zip(list(p) + ["input"] * len(inputs), g2))
   for name, a, b in zip(list(p) + ["input"] * len(inputs), g1, g2):
     assert (a is None) == (b is None), name
     if a is not None:
-      assert float((a - b).abs().max()) <= 1e-12 * max(float(b.abs().max()), 1e-300), name
+      scale = grads[(scale_of or {}).get(name, name)]
+      assert float((a - b).abs().max()) <= 1e-12 * max(float(scale.abs().max()), 1e-300), name
 
 
 # (O.vit_forward pool_type -> the NormPool pool)
@@ -109,6 +112,77 @@ def test_text_chain_is_the_text_oracle(pool, head):
     x = S.dense(x, sub(p, "head/"))
   cfg = dict(depth=2, num_heads=1, pool_type=pool, num_classes=C)
   _assert_same(x, O.text_forward(p, ids, cfg), p, [])
+
+
+BERT_TINY = dict(width=128, depth=2, num_heads=2, mlp_dim=96, vocab_size=20)
+
+
+@pytest.mark.parametrize("head,dropout", [(True, False), (False, False), (True, True), (False, True)])
+def test_bert_chain_is_the_bert_oracle(head, dropout):
+  """Without masks the chain is bert_oracle.bert_forward; under given dropout masks (the embedding, each
+  layer's probabilities, attention output and MLP output) it is bert_dropout_oracle.bert_forward."""
+  import bert_dropout_oracle as BDO
+  import bert_oracle as BO
+  from big_vision_b200 import engine as E
+  from big_vision_b200.models.proj.flaxformer import bert
+  C, n, N, d, H = (5 if head else None), 3, 7, 128, 2
+  model = bert.Model(BERT_TINY, num_classes=C)
+  p = _tree(model.specs(N), 5)
+  ids = torch.from_numpy(BO.padded_text(n, N, 20, seed=6))
+  assert (ids == 0).any()
+  key_mask = ids != 0
+  masks = None
+  if dropout:
+    rng = np.random.default_rng(7)
+    keep = lambda *shape: torch.from_numpy(rng.random(shape) >= 0.1).to(F64) / 0.9
+    masks = BDO.GivenMasks({(i, k): keep(n, N, d) for i in range(2) for k in (E.DROP_EMBED, E.DROP_ATTN, E.DROP_MLP)},
+                           [keep(n, H, N, N) for _ in range(2)])
+  x = S.bert_embed(ids, sub(p, "BertEncoder_0/embedder/"), masks and masks.h[(0, E.DROP_EMBED)])
+  for i in range(2):
+    m = masks and (masks.p[i], masks.h[(i, E.DROP_ATTN)], masks.h[(i, E.DROP_MLP)])
+    x = S.bert_layer(x, sub(p, f"BertEncoder_0/encoder_layer_{i}/"), H, key_mask, m)
+  x = S.cls_pool(x)
+  if head:
+    x = S.dense(x, sub(p, "head/"))
+  cfg = dict(depth=2, num_heads=H, num_classes=C)
+  ref = BO.bert_forward(p, ids.long(), cfg) if masks is None else BDO.bert_forward(p, ids.long(), cfg, masks)
+  # the key bias (softmax is invariant to a per-query shift) at the value bias's scale: the two softmax forms
+  # round differently
+  _assert_same(x, ref, p, [], {k: k.replace("key/bias", "value/bias") for k in p if k.endswith("key/bias")})
+
+
+@pytest.mark.parametrize("head", [True, False])
+def test_bit_chain_is_the_bit_oracle(head):
+  """Depth [2, 1, 1, 1]: a projection unit and an identity unit in block 1, stride 2 on odd sizes after."""
+  import bit_oracle as BO
+  from big_vision_b200.models import bit_paper
+  depth = [2, 1, 1, 1]
+  model = bit_paper.Model(5 if head else None, width=0.5, depth=depth)
+  p = _tree(model.specs((26, 22), 3), 15)
+  image = torch.empty(2, 26, 22, 3, dtype=F64).uniform_(-1, 1, generator=torch.Generator().manual_seed(16))
+  x = S.bit_root(image, sub(p, "root_block/"))
+  for b, size in enumerate(depth):
+    for u in range(size):
+      x = S.bit_unit(x, sub(p, f"block{b + 1}/unit{u + 1:02d}/"), 2 if (b > 0 and u == 0) else 1)
+  x = S.bit_prehead(x, sub(p, "norm-pre-head/"))
+  if head:
+    x = S.dense(x, sub(p, "head/"))
+  _assert_same(x, BO.forward(p, image, depth), p, [])
+
+
+def test_bit_root_routes_to_the_first_maximum_of_route():
+  """With a `route` whose windows tie, each window takes its first maximum in row-major order."""
+  import bit_oracle as BO
+  y = torch.randn(1, 5, 5, 2, dtype=F64, generator=torch.Generator().manual_seed(17))
+  route = torch.zeros_like(y)          # every window ties: the first in-image element of each window wins
+  kernel = torch.randn(7, 7, 3, 2, dtype=F64, generator=torch.Generator().manual_seed(18))
+  image = torch.randn(1, 10, 10, 3, dtype=F64, generator=torch.Generator().manual_seed(19))
+  out = S.bit_root(image, {"conv_root/kernel": kernel}, route=route)
+  conv = BO.std_conv(image, kernel, 2, 3)
+  assert out.shape == (1, 3, 3, 2)
+  # window (i, j) covers rows 2i - 1 .. 2i + 1: its first in-image element is (max(2i - 1, 0), max(2j - 1, 0))
+  first = [0, 1, 3]
+  assert torch.equal(out, conv[:, first][:, :, first])
 
 
 def test_max_pool_splits_ties_like_amax():
@@ -214,6 +288,12 @@ COVERAGE = {
     "big_vision_b200.models.mlp_mixer.MixerBlock": ["mixer", "mixer_stoch"],
     "big_vision_b200.models.proj.image_text.text_transformer._Embed": ["text_last", "text_max", "text_frozen_cut"],
     "big_vision_b200.models.proj.flexi.vit.FlexiPatchEmbedding": ["flexi_resample", "flexi_base_sincos"],
+    "big_vision_b200.models.proj.flaxformer.bert._Embed": ["bert", "bert_dropout", "bert_nohead"],
+    "big_vision_b200.models.proj.flaxformer.bert._Layer": ["bert", "bert_dropout", "bert_nohead", "bert_frozen_cut"],
+    "big_vision_b200.models.proj.flaxformer.bert._ClsPool": ["bert", "bert_dropout", "bert_nohead", "bert_frozen_cut"],
+    "big_vision_b200.models.bit_paper.RootBlock": ["bit", "bit_nohead"],
+    "big_vision_b200.models.bit_paper.ResidualUnit": ["bit", "bit_nohead", "bit_frozen_cut"],
+    "big_vision_b200.models.bit_paper.PreHead": ["bit", "bit_nohead", "bit_frozen_cut"],
 }
 
 
@@ -234,7 +314,7 @@ def _stage_classes():
 
 def test_every_stage_class_is_named_with_replay_cases():
   found = _stage_classes()
-  assert len(found) >= 9
+  assert len(found) >= 15
   missing, extra = found - set(COVERAGE), set(COVERAGE) - found
   assert not missing, f"backward stages without a per-stage replay case: {sorted(missing)}"
   assert not extra, f"COVERAGE rows for classes that are not stages under models/: {sorted(extra)}"

@@ -24,6 +24,7 @@ import numpy as np
 import pytest
 import torch
 
+import dropout_oracle as D
 import stage_oracle as S
 
 pytestmark = pytest.mark.gpu
@@ -40,6 +41,12 @@ TOL = {
     "NormPool": (2 ** -7, 2 ** -6),                # 2.4e-3, 4.5e-3
     "MAPHead": (2 ** -6, 2 ** -5),                 # 8.4e-3, 1.1e-2
     "Dense": (2 ** -7, 2 ** -7),                   # 2.4e-3, 2.8e-3
+    "bert._Embed": (2 ** -20, 2 ** -21),           # 3.3e-7, 2.2e-7 (under dropout: on its bf16 masked dy, see _check)
+    "bert._Layer": (2 ** -6, 2 ** -5),             # 1.1e-2, 1.1e-2
+    "bert._ClsPool": (0.0, 0.0),                   # 0, 0: a copy of the [CLS] rows
+    "RootBlock": (2 ** -8, 2 ** -8),               # 1.6e-3, 1.5e-3 (max pool routed by the bf16 convolution output)
+    "ResidualUnit": (2 ** -6, 2 ** -6),            # 6.8e-3, 7.4e-3 (gn2 / gn3 ReLUs decided by the bf16 a2, a3)
+    "PreHead": (2 ** -7, 2 ** -7),                 # 2.4e-3, 4.0e-3
 }
 ZERO_FLOOR = 2 ** -6
 # gradients that are zero in exact arithmetic -> the per-row shape of the tap that gives their floor: the key
@@ -50,6 +57,7 @@ EXACT_ZERO = {
     "EncoderBlock": (KEY_BIAS, lambda st, n, N: (n, N, st.d)),
     "MAPHead": (KEY_BIAS, lambda st, n, N: (n, N, st.d)),
     "MixerBlock": ("token_mixing/Dense_1/bias", lambda st, n, N: (n, st.d, N)),
+    "bert._Layer": ("self_attention/key/bias", lambda st, n, N: (n, N, st.d)),
 }
 
 # the gradients computed from the attention backward's dq and dk, which get the bound of stage_oracle.ScoreGrad
@@ -64,6 +72,8 @@ QK_FLOOR = ("EncoderBlock", "MAPHead")
 
 NC = 13      # C % 8 != 0: the padded class head
 TINY = dict(width=64, depth=2, mlp_dim=128, num_heads=1)
+BERT = dict(width=128, depth=2, num_heads=2, mlp_dim=256, vocab_size=97)
+BERT_DROPOUT = dict(BERT, dropout_rate=0.1, attention_dropout_rate=0.1)
 
 # name -> (model kind, model keyword arguments, input shape, extra)
 CASES = {
@@ -90,6 +100,16 @@ CASES = {
     "flexi_base_sincos": ("flexi", dict(pool_type="gap", posemb="sincos2d"), (4, 56, 56, 3), dict(seqhw=7)),
     "vit_frozen_cut": ("vit", dict(pool_type="gap"), (4, 40, 40, 3), dict(frozen=1)),
     "text_frozen_cut": ("text", dict(pool_type="last"), (4, 16), dict(frozen=1)),
+    # zero-padded captions (bert_oracle.padded_text): the key mask, and the embedding rows no token reads.  BERT's
+    # head is a tower projection, stored unpadded like the text towers': its width is a multiple of 8
+    "bert": ("bert", dict(config=BERT), (4, 16), {}),
+    "bert_dropout": ("bert", dict(config=BERT_DROPOUT), (4, 16), dict(dropout=True)),
+    "bert_nohead": ("bert", dict(config=BERT, num_classes=None), (4, 16), {}),
+    "bert_frozen_cut": ("bert", dict(config=BERT), (4, 16), dict(frozen=1)),
+    # identity and projection units; stride 2 on odd sizes (13 -> 7, 11 -> 6); a non-square image
+    "bit": ("bit", dict(depth=[2, 1, 1, 1]), (4, 52, 44, 3), {}),
+    "bit_nohead": ("bit", dict(depth=[1, 1, 1, 1], num_classes=None), (4, 40, 40, 3), {}),
+    "bit_frozen_cut": ("bit", dict(depth=[2, 1, 1, 1]), (4, 52, 44, 3), dict(frozen=1)),
 }
 
 
@@ -110,6 +130,14 @@ def build_model(case):
     from big_vision_b200.models.proj.image_text import text_transformer
     model = text_transformer.Model(**{"num_classes": 32, **kw}, **TINY, vocab_size=64)
     model.specs(shape[1])
+  elif kind == "bert":
+    from big_vision_b200.models.proj.flaxformer import bert
+    model = bert.Model(**{"num_classes": 32, "head_zeroinit": False, **kw})
+    model.specs(shape[1])
+  elif kind == "bit":
+    from big_vision_b200.models import bit_paper
+    model = bit_paper.Model(**{"num_classes": NC, "head_zeroinit": False, **kw})
+    model.specs(shape[1:3], shape[3])
   else:
     from big_vision_b200.models.proj.flexi import vit as fv
     model = fv.Model(NC, patch_size=(8, 8), **{**TINY, **kw})
@@ -119,14 +147,19 @@ def build_model(case):
 
 # ---- set-up -------------------------------------------------------------------------------------------
 def _params(model, case, seed=0):
-  """FlatParams with every all-zero initial tensor replaced by small random values (padding stays zero)."""
+  """FlatParams with every all-zero initial tensor replaced by small random values (padding stays zero); in
+  BERT and BiT the LayerNorm / GroupNorm scales also moved away from 1, so the terms of dz * scale count."""
   from big_vision_b200 import engine as E
-  _, _, shape, extra = CASES[case]
-  specs, aliases = (model.specs(shape[1]) if CASES[case][0] == "text" else model.specs(shape[1:3], shape[3]))
+  kind, _, shape, extra = CASES[case]
+  specs, aliases = (model.specs(shape[1]) if kind in ("text", "bert") else model.specs(shape[1:3], shape[3]))
   P = E.FlatParams(specs, aliases, "cuda").init(seed)
   rng = np.random.default_rng(seed + 1)
   tree = {k: ((rng.standard_normal(v.shape) * 0.05).astype(np.float32) if not np.any(v) else v)
           for k, v in P.numpy_tree("f").items()}
+  if kind in ("bert", "bit"):
+    for k in tree:
+      if k.endswith("scale"):
+        tree[k] = tree[k] + (0.3 * rng.standard_normal(tree[k].shape)).astype(np.float32)
   if extra.get("ties"):            # tokens 4 and 9 identical in every layer: exact ties in the max pool
     tree["pos_embedding"][:, 9] = tree["pos_embedding"][:, 4]
   P.load_tree(tree)
@@ -134,8 +167,15 @@ def _params(model, case, seed=0):
 
 
 def _inputs(model, case, seed=0):
-  kind, _, shape, extra = CASES[case]
+  from big_vision_b200 import engine as E
+  kind, kw_model, shape, extra = CASES[case]
   rng = np.random.default_rng(seed + 2)
+  if kind == "bert":
+    import bert_oracle
+    ids = bert_oracle.padded_text(*shape, kw_model["config"]["vocab_size"], seed=seed + 2)
+    assert (ids == 0).any()
+    kw = dict(dropout=E.DropoutKey(seed=seed + 5, step=3, sample0=1)) if extra.get("dropout") else {}
+    return torch.from_numpy(ids).cuda(), kw
   if kind == "text":
     ids = rng.integers(0, 64, size=shape).astype(np.int32)
     if extra.get("ties"):
@@ -228,6 +268,46 @@ def _flat(t):
   if isinstance(t, (tuple, list)):
     return [u for v in t for u in _flat(v)]
   return [t]
+
+
+def _kind(st):
+  """The stage kind that TOL, EXACT_ZERO and the worst values are keyed by: the class name, qualified by the
+  module for BERT's (text_transformer has an _Embed too)."""
+  name = type(st).__name__
+  return "bert." + name if type(st).__module__.endswith(".flaxformer.bert") else name
+
+
+def _live_rows(st, N):
+  """{name relative to the stage's root: the rows of that table whose gradient a forward of N tokens reaches}.
+  BERT's embedding: the position rows < N, segment row 0 and every token row but the pad token's (row 0, whose
+  positions no attended key or [CLS] depends on).  The other rows are not the stage's to write: check 4 holds
+  them at the seed, bit for bit."""
+  from big_vision_b200.models.proj.flaxformer import bert
+  if isinstance(st, bert._Embed):   # pylint: disable=protected-access
+    return {"embedders_position_ids/embedding": slice(0, N), "embedders_segment_ids/embedding": slice(0, 1),
+            "embedders_token_ids/embedding": slice(bert.PAD_ID + 1, None)}
+  return {}
+
+
+def _hidden_keep(geom, layer, kind, d):
+  """The scaled dropout mask [n, N, d] of BERT's hidden site (layer, kind) under geom.dropout, restated by
+  tests/dropout_oracle.py (None: no dropout)."""
+  dr = geom.dropout
+  if dr is None:
+    return None
+  keep = D.key_mask(dr.mask(layer, kind), dr.rate, geom.n * geom.N, d).reshape(geom.n, geom.N, d)
+  return (torch.from_numpy(keep).to(F64) / float(D.keep_divisor(dr.rate))).cuda()
+
+
+def _probs_keep(st, geom):
+  """The scaled dropout mask [n, heads, N, N] of a BERT layer's attention probabilities, restated by
+  tests/bert_dropout_oracle.py (None: no attention dropout)."""
+  import bert_dropout_oracle as BDO
+  key = st.probs_key(geom)
+  if key is None:
+    return None
+  keep = BDO.attn_keep_of(key, geom.n, st.heads, geom.N, geom.N)
+  return BDO.scaled(keep, geom.attn_dropout.rate).cuda()
 
 
 def _sink_of(st, P, geom):
@@ -433,8 +513,9 @@ class Replay:
                                f"(tau_max {tau_max:.3g})")
 
   def _names(self, st):
-    """(root, {name relative to the stage's root: flat-buffer indices}) of the tree names the stage owns."""
-    root = st.p
+    """(root, {name relative to the stage's root: flat-buffer indices}) of the tree names the stage owns.  The
+    root of a stage without `p`: its first prefix (the BiT root block), or "" when it owns nothing."""
+    root = getattr(st, "p", st.prefixes[0] if st.prefixes else "")
     own = {}
     for name, ix in self.idx.items():
       if name.startswith(st.prefixes):
@@ -444,11 +525,13 @@ class Replay:
     return root, own
 
   def _check(self, label, st, x, geom, dy, saved, sink, want_sink, need_dx, dx):
-    from big_vision_b200.models import common, mlp_mixer, vit
+    from big_vision_b200 import engine as E
+    from big_vision_b200.models import bit_paper, common, mlp_mixer, vit
+    from big_vision_b200.models.proj.flaxformer import bert
     from big_vision_b200.models.proj.flexi import vit as fv
     from big_vision_b200.models.proj.image_text import text_transformer as tt
     P, n, N = self.P, geom.n, geom.N
-    kind = type(st).__name__
+    kind = _kind(st)
     root, own = self._names(st)
     g = P.grad.to(F64)
     # --- the reference, on what the kernels read
@@ -458,10 +541,13 @@ class Replay:
       resampled = x.shape[1] // seqhw != st.patch_size[0] or (seqhw, seqhw) != st.posemb_size
     h = P.tree("h")
     f = P.tree("f")
+    # BiT's convolutions standardise the fp32 master (bv_weight_std_fwd); every GEMM reads the bf16 shadow
+    std_conv = isinstance(st, (bit_paper.RootBlock, bit_paper.ResidualUnit))
 
     def value(rel):
       full = root + rel
-      use_h = rel.endswith("kernel") or rel == "probe" or (rel == "pos_embedding" and isinstance(st, vit.PatchEmbedding))
+      use_h = not std_conv and (rel.endswith("kernel") or rel == "probe" or
+                                (rel == "pos_embedding" and isinstance(st, vit.PatchEmbedding)))
       t = (f if resampled or not use_h else h)[full]
       if getattr(st, "index", None) is not None:
         t = t[st.index]
@@ -474,8 +560,10 @@ class Replay:
     if kind in EXACT_ZERO:
       zname, zshape = EXACT_ZERO[kind]
       tap = S.Tap(p[zname], zshape(st, n, N))
-    if isinstance(st, (vit.PatchEmbedding, tt._Embed)):     # pylint: disable=protected-access
-      xin = x if isinstance(st, tt._Embed) else x.to(torch.bfloat16).to(F64)   # pylint: disable=protected-access
+    if isinstance(st, (tt._Embed, bert._Embed)):     # pylint: disable=protected-access
+      xin = x
+    elif isinstance(st, (vit.PatchEmbedding, bit_paper.RootBlock)):    # the kernels read the image in bf16
+      xin = x.to(torch.bfloat16).to(F64)
     else:
       xin = (common.to16(x) if isinstance(st, common.Dense) else x).to(F64).requires_grad_(True)
     if isinstance(st, fv.FlexiPatchEmbedding):
@@ -506,6 +594,29 @@ class Replay:
     elif isinstance(st, common.Dense):
       y = S.dense(xin, p, st.tanh)
       dy = dy[:, :st.C]
+    elif isinstance(st, bert._Embed):   # pylint: disable=protected-access
+      y = S.bert_embed(xin, p)
+      keep = _hidden_keep(geom, 0, E.DROP_EMBED, st.d)
+      if keep is not None:
+        # The backward's dropout (ops.dropout) stores dy / (1 - rate) in bf16 before the LayerNorm's backward
+        # reads it: one rounding of unit roundoff 2^-9, which against the float64 dy * mask made 1.5e-3 of this
+        # stage's error (1e3 times its error without dropout).  So the reference's cotangent is that bf16 product,
+        # on the restated mask, and the embedding's bound stays that of its fp32 sums.
+        q = dy.float() / float(D.keep_divisor(geom.dropout.rate))
+        dy = torch.where(keep.reshape(q.shape) != 0, q, torch.zeros_like(q)).to(torch.bfloat16)
+    elif isinstance(st, bert._Layer):   # pylint: disable=protected-access
+      masks = (_probs_keep(st, geom), _hidden_keep(geom, st.layer, E.DROP_ATTN, st.d),
+               _hidden_keep(geom, st.layer, E.DROP_MLP, st.d))
+      with tap:
+        y = S.bert_layer(xin.view(n, N, -1), p, st.heads, geom.key_mask, masks)
+    elif isinstance(st, bert._ClsPool):   # pylint: disable=protected-access
+      y = S.cls_pool(xin.view(n, N, -1))
+    elif isinstance(st, bit_paper.RootBlock):      # the max pool routes by the bf16 convolution output
+      y = S.bit_root(xin, p, route=saved[2].to(F64))
+    elif isinstance(st, bit_paper.ResidualUnit):   # gn2's and gn3's ReLUs decide on the bf16 a2, a3
+      y = S.bit_unit(xin, p, st.s, relu_masks=(saved[6] > 0, saved[10] > 0))
+    elif isinstance(st, bit_paper.PreHead):
+      y = S.bit_prehead(xin, p)
     else:
       raise NotImplementedError(f"no reference for stage {kind}")
     y.backward(dy.to(F64).reshape(y.shape))
@@ -528,10 +639,13 @@ class Replay:
         self._fail(1, label, "no dx returned")
       else:
         self._compare(1, label, kind, "dx", dx, dx_ref)
-    # 2. own parameters
+    # 2. own parameters (the rows of them the stage can reach)
     allowed = torch.zeros_like(self.final)
+    live = _live_rows(st, N)
     for rel, ix in own.items():
       ref = p[rel].grad if p[rel].grad is not None else torch.zeros_like(p[rel])
+      if rel in live:
+        ix, ref = ix[live[rel]], ref[live[rel]]
       got = g[ix] - self.seed64[ix]
       if tap is not None and rel == EXACT_ZERO[kind][0]:
         e, fl = (got - ref).abs(), ZERO_FLOOR * tap.floor()
@@ -584,14 +698,16 @@ def test_every_stage_matches_its_fp64_reference(case):
   rep = _replay(case)
   _report(case, rep)
   assert not rep.failures, rep.failures[:10]
-  kinds = {type(s).__name__ for s in rep.stages[rep.cut:]}
+  kinds = {_kind(s) for s in rep.stages[rep.cut:]}
   assert set(rep.worst) >= kinds - {"ScanEncoder"}, (kinds, set(rep.worst))
 
 
 def test_siglip_two_tower_ready_announcements_hold_their_final_bits():
   """Both towers in one FlatParams (spec order: image, text, t, b): every slice announced during
-  siglip.loss_and_grads' backward is final."""
+  siglip.loss_and_grads' backward is final.  Then SigLiT (test_bert_gpu._siglit_model): the BERT text tower
+  trained under a frozen ViT image tower, its announcements restricted to the trained ranges."""
   import common
+  import test_bert_gpu
   from big_vision_b200.models.proj.image_text import two_towers
   from big_vision_b200.trainers.proj.image_text import siglip
   model = two_towers.Model(**common.TINY)
@@ -603,6 +719,15 @@ def test_siglip_two_tower_ready_announcements_hold_their_final_bits():
   rec.finish()
   torch.cuda.synchronize()
   assert len(rec.snaps) >= 4           # two blocks per tower, then the rest
+  assert not rec.broken()
+
+  model, P, image, text, frozen = test_bert_gpu._siglit_model()   # pylint: disable=protected-access
+  rec = ready_recorder(P, P.trained_ranges(frozen))
+  rec.begin()
+  siglip.loss_and_grads(model, P, image, text, frozen=frozen)
+  rec.finish()
+  torch.cuda.synchronize()
+  assert len(rec.snaps) >= 3           # the two BERT layers, then the rest
   assert not rec.broken()
 
 
@@ -695,3 +820,34 @@ def test_fault_mixer_sink_kept_under_stochastic_depth_is_caught():
   # and numerically, not only by which buffer was handed over
   assert any(c == 2 and lbl == "2" and m.startswith("channel_mixing/Dense_1/bias:") for c, lbl, m in rep.failures), \
       rep.failures
+
+
+def test_fault_bit_missing_residual_gradient_is_caught():
+  """The identity unit of `bit` (stage 2): gn1's backward without dx_add, the gradient of the residual."""
+  rep = _replay("bit", op_fault={"2": ("groupnorm_bwd", _once(lambda kw: kw.get("dx_add") is not None,
+                                                             lambda fn, a, kw: fn(*a, **{**kw, "dx_add": None})))})
+  assert 1 in _checks(rep), rep.failures
+
+
+def test_fault_bit_groupnorm_overwriting_its_parameter_gradients_is_caught():
+  """gn3 of stage 2 (its first GroupNorm backward) with dscale and dbias zeroed first, so the kernel's sum
+  replaces the buffer's value.  Without the seed this fault is invisible: the buffer would start at zero."""
+  def overwrite(fn, a, kw):
+    a[6].zero_()      # dscale
+    a[7].zero_()      # dbias
+    return fn(*a, **kw)
+  rep = _replay("bit", op_fault={"2": ("groupnorm_bwd", _once(lambda kw: True, overwrite))})
+  assert 2 in _checks(rep), rep.failures
+
+
+def test_fault_bert_mlp_mask_of_another_step_is_caught():
+  """The top layer of `bert_dropout` (stage 2) regenerates its MLP-output mask (its first masked gradient in
+  the backward) under the next optimizer step instead of the forward's."""
+  from big_vision_b200 import lib as L
+
+  def other_step(fn, a, kw):
+    k = a[1]
+    return fn(a[0], L.DropoutKey(seed=k.seed, step=k.step + 1, site=k.site, row0=k.row0, rate=k.rate), *a[2:], **kw)
+  rep = _replay("bert_dropout", op_fault={"2": ("dropout", _once(lambda kw: kw.get("colsum_into") is not None,
+                                                                 other_step))})
+  assert _checks(rep) & {1, 2}, rep.failures
